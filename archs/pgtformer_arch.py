@@ -1,4 +1,4 @@
-"""Drop-in `archs/pgtformer_arch.py`: the reference's model surface over the B200 engine.
+"""Drop-in `archs/pgtformer_arch.py`: the reference's model surface over the H100 engine.
 
 Same import path, constructor keywords and forward contract as the reference class
 (`archs/pgtformer_arch.py:490-714`, built from `options/release_test_stage_IIII_*.yml ->
@@ -107,7 +107,7 @@ class _B200Model(nn.Module):
             from pgtformer_b200.engine import Engine
             dev = next(self.parameters()).device
             if dev.type != 'cuda':
-                raise RuntimeError('pgtformer_b200: no CPU path — move the model to a CUDA (sm_100a) device first')
+                raise RuntimeError('pgtformer_b200: no CPU path — move the model to a CUDA (sm_90a) device first')
             self.__dict__['_engine'] = Engine(self._network_g, self.state_dict(), dev)
         return self.__dict__['_engine']
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — clips/s of the PGTFormer forward path (BASELINE.json metric) on N B200s.
+"""bench.py — clips/s of the PGTFormer forward path (BASELINE.json metric) on N H100s.
 
 A "step" is one `PGTFormer.forward` over `--clips` synthetic 3-frame 512x512 clips per GPU
 (default 16 = BASELINE configs[2] at N=1, configs[3] at N=8: weak scaling, clips are independent).
@@ -7,11 +7,12 @@ A "step" is one `PGTFormer.forward` over `--clips` synthetic 3-frame 512x512 cli
   e2e         the same metric through the drop-in `PGTFormer.__call__` with HOST (pinned) inputs:
               H2D copy of the clips and D2H copy of `out` every step inside the timed region (on their own
               streams, overlapping the neighbouring step's compute as a serving loop would)
-  roofline    dominant kernel (tcgen05 implicit-GEMM conv / GEMM): algorithmic FLOPs / live per-launch
+  roofline    dominant kernel (wgmma implicit-GEMM conv / GEMM): algorithmic FLOPs / live per-launch
               device time (CUDA events on the launching stream, separate profiled pass of the same steps)
   cpu_baseline  the CPU oracle (port of the reference's PyTorch path) on the host cores, N=1 rank 0 only
-`--impl reference` times that CPU path alone (the reference has no CUDA code of its own and cannot
-travel to the GPU box; `oracle/pgt_oracle.py` is pinned to it by tests/golden/).
+`--impl reference` times that CPU path alone (the reference has no CUDA code of its own;
+`oracle/pgt_oracle.py` is pinned to it by tests/golden/).
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (see dump_outputs).
 """
 import argparse
 import json
@@ -55,7 +56,37 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, 'measured'
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback'
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 — not measured, and not reached
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0}, 'data-sheet'
+
+
+DUMP_BUDGET = 60 << 20          # bytes of array data written by --dump-outputs (all arrays together, under 64 MB)
+
+
+def dump_outputs(directory, arrays):
+    """Writes `arrays` (name -> device tensor, the outputs of the last timed step) as DIR/<name>.npy in float32.  An array
+    larger than its share of DUMP_BUDGET is replaced by a fixed sample: the elements at sorted flat indices drawn with
+    numpy seed 0, so two builds run with the same arguments write comparable files.  DIR/manifest.json records shapes,
+    dtypes and which arrays were sampled."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    share = DUMP_BUDGET // max(len(arrays), 1)
+    manifest = {}
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        entry = {'shape': list(a.shape), 'source_dtype': str(t.dtype).replace('torch.', ''), 'dtype': 'float32'}
+        flat = a.reshape(-1)
+        k = share // 4
+        if flat.size > k:
+            idx = np.sort(np.random.default_rng(0).choice(flat.size, size=k, replace=False))
+            flat = flat[idx]
+            entry['sampled'] = {'elements': int(k), 'of': int(a.size), 'index': 'sorted numpy default_rng(0).choice'}
+            np.save(os.path.join(directory, name + '.npy'), flat)
+        else:
+            np.save(os.path.join(directory, name + '.npy'), a)
+        manifest[name] = entry
+    with open(os.path.join(directory, 'manifest.json'), 'w') as f:
+        json.dump(manifest, f, indent=1)
 
 
 class ClockSampler:
@@ -113,7 +144,7 @@ def cpu_oracle_clips_per_s(H, warmup, steps):
     from oracle import pgt_oracle as O
     from pgtformer_b200.spec import build_spec
     from pgtformer_b200.weights import synth_state_dict
-    # all the host threads that help: on the 2x32-core GPU boxes oneDNN/OpenMP is fastest at 16-32 threads and
+    # all the host threads that help: on a 2x32-core host oneDNN/OpenMP is fastest at 16-32 threads and
     # collapses (100x slower) at 128 — measured with tools/cpu_threads.py (256^2 clip: 1.5 s @16-32, 2.5 s @64, 118 s @128)
     torch.set_num_threads(min(os.cpu_count() or 1, 32))
     arch, spec = build_spec(load_network_g())
@@ -130,8 +161,8 @@ def cpu_oracle_clips_per_s(H, warmup, steps):
 
 
 def load_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel class, from the committed ncu
-    capture of this command (profiles/r2_traffic.json, written by tools/summarize_profiles.py); None if absent."""
+    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel class, from an ncu capture of this
+    command stored as profiles/r2_traffic.json; None if absent."""
     p = os.path.join(ROOT, 'profiles', 'r2_traffic.json')
     if os.path.exists(p):
         try:
@@ -239,6 +270,8 @@ def main():
     ap.add_argument('--gather', default='middle_u8', choices=['middle_u8', 'full'],
                     help='N > 1: what the end-of-step all-gather carries (restored middle frames as rgb24, or every fp32 frame)')
     ap.add_argument('--no-parity', action='store_true', help='skip the golden-vector parity block of the JSON line')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the last step\'s outputs (out, logits, lq_feat) as DIR/<name>.npy')
     args = ap.parse_args()
     if args.impl == 'reference':
         return run_reference(args)
@@ -277,8 +310,12 @@ def main():
             return out
         return gather_frames(out, world * b) if args.gather == 'full' else gather_restored(out, world * b)
 
+    last = {}
+
     def step_resident():
-        return collective(model(x_dev, w=1, adain=True)[0])
+        out, logits, lq = model(x_dev, w=1, adain=True)
+        last['out'], last['logits'], last['lq_feat'] = out, logits, lq
+        return collective(out)
 
     # end to end as a serving loop would run it: the pinned-host -> device copy of step k+1 and the device -> host copy
     # of step k's result ride their own streams and overlap the compute of the neighbouring step; every step still does
@@ -342,6 +379,8 @@ def main():
     launches = ops.launch_count() if not args.graph else launches_per_forward * args.steps
     clocks = sampler.stop() if rank == 0 else None
     value = world * b * args.steps / (ms / 1000.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)              # before any other forward rewrites (graph-static) outputs
 
     for _ in range(2):
         step_e2e()
@@ -367,7 +406,7 @@ def main():
     if rank == 0:
         work, pms, n = prof['gemm_tc']
         achieved = work / (pms / 1000.0) / 1e12 if pms > 0 else 0.0
-        peak = float(peaks.get('bf16_tflops_sustained', 1400.0))
+        peak = float(peaks.get('bf16_tflops_sustained', 989.0))
         total_ms = sum(v[1] for v in prof.values())
         breakdown = {k: {'ms_per_step': v[1] / args.steps, 'launches_per_step': v[2] / args.steps,
                          'work_per_step': v[0] / args.steps} for k, v in prof.items() if v[2] > 0}
@@ -378,13 +417,13 @@ def main():
             'config': {'workload': 'PGTFormer.forward on %d clips/GPU of 3x%dx%d (%s), w=1, adain, '
                                    'random-init pgtformer-base' % (b, H, H, config_label(b, H, world)),
                        'clips_per_gpu': b, 'size': H, 'global_clips': world * b, 'parallelism': 'dp%d' % world,
-                       'l2_policy': 'inputs and activations (GBs per step) exceed the 126 MB L2; no flush needed',
+                       'l2_policy': 'inputs and activations (GBs per step) exceed the 50 MB L2; no flush needed',
                        'flops_per_clip': flops_per_clip(H), 'cuda_graph': bool(args.graph)},
             'e2e': {'value': e2e_val, 'unit': 'clips/s', 'ms_per_step': ms_e2e / args.steps,
                     'h2d_bytes_per_step': x_host.numel() * 4, 'd2h_bytes_per_step': out_host.numel() * 4},
             'gpu_launches': launches,
             'clocks': clocks,
-            'roofline': {'bound': 'tensor', 'kernel': 'gemm_tc_kernel (tcgen05 implicit-GEMM conv / GEMM)',
+            'roofline': {'bound': 'tensor', 'kernel': 'gemm_tc_kernel (wgmma implicit-GEMM conv / GEMM)',
                          'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak,
                          'peak_kind': peak_kind + ' bf16_tflops_sustained', 'traffic': None,
                          'launches_per_step': n / args.steps, 'kernel_ms_per_step': pms / args.steps,

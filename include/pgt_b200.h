@@ -1,9 +1,9 @@
-/* pgt_b200.h — C ABI of libpgt_b200.so: the hand-written sm_100a kernels behind
+/* pgt_b200.h — C ABI of libpgt_b200.so: the hand-written sm_90a kernels behind
  * PGTFormer.forward.
  *
  * The reference (kepengxu/PGTFormer) exposes a Python class and no FFI (SURVEY.md 8b); these
  * entry points are what a `torch.ops`/ctypes binding for the hot path would bind.  Each entry
- * cites the reference code it replaces (paths relative to /root/reference).
+ * cites the reference code it replaces (paths relative to the reference repository).
  *
  * Conventions
  *  - every function returns 0 (PGT_OK) or a negative pgt_status; it never throws, never
@@ -28,7 +28,7 @@ typedef enum pgt_status {
   PGT_OK = 0,
   PGT_ERR_INVALID = -1,      /* bad shape / alignment / null pointer                      */
   PGT_ERR_CUDA = -2,         /* a CUDA runtime call failed (see pgt_last_cuda_error)       */
-  PGT_ERR_UNSUPPORTED = -3,  /* valid request the sm_100a kernels do not cover            */
+  PGT_ERR_UNSUPPORTED = -3,  /* valid request the sm_90a kernels do not cover             */
   PGT_ERR_DRIVER = -4        /* cuTensorMapEncodeTiled unavailable / failed               */
 } pgt_status;
 
@@ -84,7 +84,7 @@ int pgt_profile_end(double* work, double* ms, int64_t* launches);
 /* same, and also writes one CSV row per launch (class, description, work, ms) to `path` (host string). */
 int pgt_profile_end_csv(const char* path, double* work, double* ms, int64_t* launches);
 
-/* ---- tcgen05 GEMM:  out[M,N] = epilogue(A[M,K] * W[N,K]^T)
+/* ---- wgmma GEMM:  out[M,N] = epilogue(A[M,K] * W[N,K]^T)
  * Replaces nn.Linear / 1x1 Conv2d call sites: WindowAttention3D q/kv/proj
  * (modules/rstt_layers.py:210-212,231), Mlp fc1/fc2 (:126-131), nn.MultiheadAttention in/out
  * projections and linear1/linear2 (archs/codeformer_arch.py:105-108,127-136), feat_emb /
@@ -94,7 +94,7 @@ int pgt_profile_end_csv(const char* path, double* work, double* ms, int64_t* lau
 int pgt_linear_bf16(const void* A, int lda, const void* W, int ldw, int M, int N, int K,
                     const pgt_epilogue* ep, void* stream);
 
-/* ---- tcgen05 implicit-GEMM convolution on NHWC bf16.
+/* ---- wgmma implicit-GEMM convolution on NHWC bf16.
  * ksize in {1,3}; stride in {1,2}; pad_lo = zero rows/cols before the first input row/col
  * (3x3 s1: 1; Downsample pad(0,1,0,1): 0; ResNet 3x3 s2: 1), the far side is zero-filled as
  * needed.  Output is [F, Hout, Wout, Cout], Hout = Hin/stride.
@@ -104,7 +104,7 @@ int pgt_linear_bf16(const void* A, int lda, const void* W, int ldw, int M, int N
 int pgt_conv_bf16(const void* x, int F, int Hin, int Win, int Cin, int ldx, const void* Wp, int ldw,
                   int Cout, int ksize, int stride, int pad_lo, const pgt_epilogue* ep, void* stream);
 
-/* ---- decoder tail: GroupNorm(32) -> SiLU -> 3x3 conv to <= 3 channels -> fp32 NCHW, one tcgen05 kernel (conv_out.cu).
+/* ---- decoder tail: GroupNorm(32) -> SiLU -> 3x3 conv to <= 3 channels -> fp32 NCHW, one wgmma kernel (conv_out.cu).
  * x: RAW (pre-norm) bf16 [F, H, W, 64]; gn_ab: fp32 [F][2][64] from pgt_groupnorm_ab; Wp: packed [Cout, 9*64] bf16;
  * out: fp32 [F, Cout, H, W].  Replaces norm_out / nonlinearity / conv_out at the end of the decoder
  * (archs/pgtformer_arch.py:707-710, archs/tdcrqvae3_arch.py:700-706).  PGT_ERR_UNSUPPORTED unless Cin == 64,
@@ -185,7 +185,7 @@ int pgt_ln_linear_bf16(const void* x, int ldx, int T, int C, const float* ln_g, 
                        const void* W, int ldw, int N, const float* bias, void* out, int ldo, void* stream);
 
 /* ---- fused Swin MLP half-block (C = 256):  out = x + fc2(GELU(fc1(LayerNorm(x)))) in ONE kernel — the hidden tile
- * stays in shared memory / TMEM, x is read once and out written once.  W1, W2: bf16 [C, C] row-major ([out, in]);
+ * stays in shared memory / registers, x is read once and out written once.  W1, W2: bf16 [C, C] row-major ([out, in]);
  * gn_stats: optional GroupNorm partials of `out` as in pgt_epilogue.  ln_g == ln_b == NULL: plain normalisation (the
  * caller folded gamma / beta into W1 / b1, as for pgt_ln_linear_bf16).  Returns PGT_ERR_UNSUPPORTED for C != 256.
  * Replaces norm2 + Mlp + residual of VSTSREncoderTransformerBlock (modules/rstt_layers.py:116-132,335-336). */
@@ -203,9 +203,9 @@ int pgt_swin_mlp_bf16(const void* x, int ldx, int T, int C, const float* ln_g, c
 int pgt_window_attention(const void* qkv, int ldqkv, int clips, int H, int W, int C, int heads, int shift,
                          const float* bias_tab, void* out, int ldo, void* stream);
 
-/* The same core on TMA + tcgen05 (window_attn_tc.cu): a window's q / k / v rows of a 64-column chunk are one 5-D TMA box
- * of the qkv matrix (wrapped windows of a shifted block: 2 or 4 partial boxes), QK^T and PV run as tcgen05.mma with S / O
- * in TMEM, results leave through TMA stores of the same boxes.  tab: fp16 [4][heads][6][48][8] bias / mask tables
+/* The same core on TMA + wgmma (window_attn_tc.cu): a window's q / k / v rows of a 64-column chunk are one 5-D TMA box
+ * of the qkv matrix (wrapped windows of a shifted block: 2 or 4 partial boxes), QK^T and PV run as wgmma with S / P / O
+ * in registers, results are stored to the tokens' output rows.  tab: fp16 [4][heads][6][48][8] bias / mask tables
  * (pgtformer_b200/ops.py::window_tables — relative-position bias and the {0,-100} shift mask in the row order of the
  * four box layouts, times log2 e).  mode_n64: for d = 32 run P V with N = 64 instead of a half-atom N = 32 operand view.
  * Returns PGT_ERR_UNSUPPORTED unless heads == 8, d in {32, 64}, C % 128 == 0, shift in {0, 2}. */
@@ -244,7 +244,7 @@ int pgt_argmax_gather(const float* logits, int T, int K, const float* codebook, 
                       int64_t* idx, void* quant, int ldq, int quant_dtype, void* stream);
 int pgt_l2_argmin(const float* z, int T, int E, const float* codebook, int K, int64_t* idx, float* quant,
                   void* stream);
-/* The same result on tcgen05 (l2_argmin_tc.cu): bf16 tensor-core scores of all K codes + a rigorous error window
+/* The same result on wgmma (l2_argmin_tc.cu): bf16 tensor-core scores of all K codes + a rigorous error window
  * around the approximate minimum; the window's members are re-evaluated exactly (fp32, fp64 when closer than the fp32
  * bound), tokens whose window does not fit go through the exhaustive kernel above — equal to an fp64 argmin with
  * first-index tie-break for every input.

@@ -1,11 +1,12 @@
 """TEST INFRASTRUCTURE ONLY — mints tests/golden/* by running the UNMODIFIED reference
-(/root/reference, imported through oracle/reference_loader.py) on seeded inputs with the
+(a reference checkout, imported through oracle/reference_loader.py) on seeded inputs with the
 deterministic synthetic checkpoint (pgtformer_b200.weights.synth_state_dict, seed 0).
 
-Run in the build container (the reference does not exist on the GPU box):
-    python -m oracle.make_golden            # 128^2 fixtures (full tensors)
+Run where the reference checkout is available (PGT_REFERENCE_ROOT); the tests only read tests/golden/*:
+    python -m oracle.make_golden            # 128^2 fixtures
     python -m oracle.make_golden --full     # 512^2 (the reference's native size, NO size patch) and 1024^2 (size patch)
-    python -m oracle.make_golden --video    # first 8 frames of assets/inputdemovideo.mp4 through inference.py's loop
+    python -m oracle.make_golden --video    # first 8 frames of assets/inputdemovideo.mp4, downscaled to 128^2, through
+                                            # inference.py's loop
     python -m oracle.make_golden --swin     # the Video-Swin BasicLayer of modules/swin.py (TDRQVAE) on stand-in weights
 Inputs are not stored: `golden_input(seed, b, H)` regenerates them bit-exactly.
 
@@ -13,6 +14,8 @@ The full-size fixtures are stored compactly (the raw outputs are 50-200 MB): eve
 logit values of every token (the margin that decides whether a code flip is a real error), full logit rows for a
 seeded sample of tokens, lq_feat as fp16 (at 1024^2: every other token in y and x), the middle output frame as fp16
 (that is what `inference.py:15` consumes), the L2-argmin codes of `TDCRQVAE3.get_codes`, and per-tensor max|ref|.
+Every fixture stays below 1 MB: large tensors are kept as `t.reshape(-1)[::stride]` with key_shape / key_stride /
+key_absmax beside them (`sample_into`), and the tests take the same sample of their own output.
 """
 import argparse
 import os
@@ -27,7 +30,11 @@ sys.path.insert(0, ROOT)
 GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 OPT = os.path.join(ROOT, 'options', 'release_test_stage_IIII_dont_need_align_version.yml')
 DEMO_VIDEO = 'assets/inputdemovideo.mp4'          # relative to the reference root
-N_LOGIT_ROWS = 384
+N_LOGIT_ROWS = 384               # seeded token sample; a compact fixture keeps every LOGIT_ROW_STEP-th of them
+LOGIT_ROW_STEP = 4
+SMALL_STRIDES = {'out': 2, 'logits': 4, 'lq_feat': 2, 'vq_out': 4}     # x b (clips) at 128^2
+COMPACT_STRIDES = {512: (8, 12), 1024: (16, 48)}                       # (lq_feat, out_mid) flat sample strides
+DEMO_SIZE = 128
 
 
 def load_network_g():
@@ -44,6 +51,22 @@ def sampled_rows(T, seed):
     """Token rows whose full logit vectors a compact fixture keeps."""
     g = torch.Generator().manual_seed(1000 + seed)
     return torch.randperm(T, generator=g)[:N_LOGIT_ROWS].sort().values
+
+
+def sample_into(rec, key, t, stride):
+    """rec[key] = the strided flat sample of t, with its full shape, stride and max|t|."""
+    rec[key] = t.reshape(-1)[::stride].contiguous()
+    rec[key + '_shape'] = tuple(t.shape)
+    rec[key + '_stride'] = stride
+    rec[key + '_absmax'] = t.abs().max().item()
+
+
+def small_record(out, logits, lq, vq_out, vq_loss, vq_codes, seed, b, H):
+    rec = {'seed': seed, 'b': b, 'H': H, 'w': 1.0, 'adain': True, 'codes': logits.argmax(-1),
+           'vq_loss': vq_loss, 'vq_codes': vq_codes}
+    for key, t in (('out', out), ('logits', logits), ('lq_feat', lq.contiguous()), ('vq_out', vq_out)):
+        sample_into(rec, key, t.float(), SMALL_STRIDES[key] * b)
+    return rec
 
 
 def _reference_model():
@@ -64,20 +87,24 @@ def small():
     for (seed, b, H) in ((1, 1, 128), (2, 2, 128)):
         x = golden_input(seed, b, H)
         out, logits, lq = reference_forward(m, x, w=1.0, adain=True)
-        rec = {'out': out, 'logits': logits, 'lq_feat': lq.contiguous(), 'seed': seed, 'b': b, 'H': H,
-               'w': 1.0, 'adain': True}
         # the registered TDCRQVAE3.forward (L2-argmin path) on the same module / weights
         vq = []
         with torch.no_grad():
             for i in range(b):
                 generalise_size(m, H, H)
                 vq.append(ref_mod.TDCRQVAE3.forward(m, x[i * 3:(i + 1) * 3]))
-        rec['vq_out'] = torch.cat([v[0] for v in vq], 0)
-        rec['vq_loss'] = torch.stack([v[1] for v in vq])
-        rec['vq_codes'] = torch.cat([v[2] for v in vq], 0)
+        rec = small_record(out, logits, lq, torch.cat([v[0] for v in vq], 0), torch.stack([v[1] for v in vq]),
+                           torch.cat([v[2] for v in vq], 0), seed, b, H)
         path = os.path.join(GOLDEN, 'pgtformer_ref_b%d_%d_seed%d.pt' % (b, H, seed))
         torch.save(rec, path)
         print('wrote', path, {k: tuple(v.shape) for k, v in rec.items() if torch.is_tensor(v)})
+    # 64^2, small enough to keep whole
+    seed, H = 7, 64
+    out, logits, lq = reference_forward(m, golden_input(seed, 1, H), w=1.0, adain=True)
+    path = os.path.join(GOLDEN, 'pgtformer_ref_b1_%d_seed%d.pt' % (H, seed))
+    torch.save({'seed': seed, 'b': 1, 'H': H, 'w': 1.0, 'adain': True, 'out': out, 'logits': logits,
+                'lq_feat': lq.contiguous()}, path)
+    print('wrote', path)
 
 
 def compact_record(out, logits, lq, seed, H, lq_stride):
@@ -85,15 +112,18 @@ def compact_record(out, logits, lq, seed, H, lq_stride):
     T = logits.numel() // logits.shape[-1]
     lo = logits.reshape(T, -1)
     top2 = lo.topk(2, dim=-1)
-    rows = sampled_rows(T, seed)
-    return {'seed': seed, 'b': Fr // 3, 'H': H, 'w': 1.0, 'adain': True, 'compact': True,
-            'codes': lo.argmax(-1).to(torch.int16).view(Fr, H // 16, H // 16),
-            'top2': top2.values.float().view(Fr, H // 16, H // 16, 2).contiguous(),
-            'logit_rows_idx': rows.to(torch.int32), 'logit_rows': lo[rows].float().contiguous(),
-            'logits_absmax': lo.abs().max().item(),
-            'lq_feat': lq[:, ::lq_stride, ::lq_stride].to(torch.float16).contiguous(), 'lq_stride': lq_stride,
-            'lq_absmax': lq.abs().max().item(),
-            'out_mid': out[1::3].to(torch.float16).contiguous(), 'out_absmax': out.abs().max().item()}
+    rows = sampled_rows(T, seed)[::LOGIT_ROW_STEP]
+    lq_flat, out_flat = COMPACT_STRIDES[H]
+    rec = {'seed': seed, 'b': Fr // 3, 'H': H, 'w': 1.0, 'adain': True, 'compact': True,
+           'codes': lo.argmax(-1).to(torch.int16).view(Fr, H // 16, H // 16),
+           'top2': top2.values.float().view(Fr, H // 16, H // 16, 2).contiguous(),
+           'logit_rows_idx': rows.to(torch.int32), 'logit_rows': lo[rows].float().contiguous(),
+           'logits_absmax': lo.abs().max().item(), 'lq_stride': lq_stride}
+    sample_into(rec, 'lq_feat', lq[:, ::lq_stride, ::lq_stride].to(torch.float16), lq_flat)
+    rec['lq_absmax'] = lq.abs().max().item()                  # of the whole tensor, not only the y / x subsample
+    sample_into(rec, 'out_mid', out[1::3].to(torch.float16), out_flat)
+    rec['out_absmax'] = out.abs().max().item()
+    return rec
 
 
 def full():
@@ -135,12 +165,16 @@ def read_demo_frames(n):
 
 
 def video(n=8):
-    """`inference.py:12-19,37-76` on the first n frames of assets/inputdemovideo.mp4 with the reference model (CPU): the
-    input frames and the reference's uint8 outputs are stored, so the GPU test needs neither the video nor the reference."""
+    """`inference.py:12-19,37-76` on the first n frames of assets/inputdemovideo.mp4, downscaled to DEMO_SIZE^2 (area
+    filter), with the reference model (CPU): the input frames and the reference's uint8 outputs are stored, so the GPU
+    test needs neither the video nor the reference."""
+    import cv2
     import numpy as np
     from oracle import video_oracle as VO
+    from oracle.reference_loader import generalise_size
     m = _reference_model()
-    frames = read_demo_frames(n)
+    generalise_size(m, DEMO_SIZE, DEMO_SIZE)
+    frames = np.stack([cv2.resize(f, (DEMO_SIZE, DEMO_SIZE), interpolation=cv2.INTER_AREA) for f in read_demo_frames(n)])
 
     def apply_window(win):                               # apply_net_to_frames without the .cuda()
         x = torch.from_numpy(VO.rgbnp2tensor(win))
@@ -174,6 +208,12 @@ def swin():
         path = os.path.join(GOLDEN, 'swin3d_%s.pt' % name)
         torch.save({'case': name, 'out': y.to(torch.float16), 'out_absmax': y.abs().max().item()}, path)
         print('wrote', path, tuple(y.shape), '%.1f KB' % (os.path.getsize(path) / 1e3))
+    # the reference layer's state dict layout (names, shapes, dtypes) and relative position index, for the drop-in
+    ref = mod.BasicLayer(256, 4, 8, (5, 5, 5)).state_dict()
+    path = os.path.join(GOLDEN, 'swin3d_state_dict_spec.pt')
+    torch.save({'spec': {k: (tuple(v.shape), str(v.dtype)) for k, v in ref.items()},
+                'relative_position_index': ref['blocks.0.attn.relative_position_index'].to(torch.int16)}, path)
+    print('wrote', path)
 
 
 if __name__ == '__main__':

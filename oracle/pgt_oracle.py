@@ -4,11 +4,10 @@ of the reference algorithm for the PGTFormer forward path.  It is the *checker*:
 The product path (pgtformer_b200/, archs/) never does and fails loudly without its CUDA library.
 
 Pinning: the reference ships no golden vectors or tests (SURVEY 4, 8c).  This restatement is
-pinned instead against the reference itself, imported in the build container
-(oracle/reference_loader.py): tests/test_oracle.py checks agreement with the live reference at
-128x128 when /root/reference is present, and tests/golden/* hold outputs *of the reference*
-(minted by oracle/make_golden.py: 128x128 in full, 512x512 — its unpatched native size — and
-1024x1024 compactly) that this file is checked against everywhere else.
+pinned instead against the reference itself (oracle/reference_loader.py imports a reference
+checkout): tests/golden/* hold outputs *of the reference* (minted by oracle/make_golden.py: 64x64
+in full, 128x128, 512x512 — its unpatched native size — and 1024x1024 as bounded samples) that
+tests/test_oracle.py checks this file against.
 
 Every function cites the reference lines it restates.  Unlike the reference it is size-general
 (H, W multiples of 64) and batch-general (b clips of 3 frames); SURVEY F4/F5 explain why the

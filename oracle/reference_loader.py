@@ -1,8 +1,7 @@
-"""TEST INFRASTRUCTURE ONLY — imports the *unmodified* reference (read-only at /root/reference)
-as a CPU oracle.  Never imported by product code; never runs on the GPU box (the reference
-does not exist there).  Used in THIS container to (a) pin oracle/pgt_oracle.py against the real
-reference and (b) mint the committed golden vectors under tests/golden/ (see
-oracle/make_golden.py).
+"""TEST INFRASTRUCTURE ONLY — imports the *unmodified* reference (a read-only checkout of
+kepengxu/PGTFormer at PGT_REFERENCE_ROOT) as a CPU oracle.  Never imported by product code or by the
+tests.  Used to mint the committed golden vectors under tests/golden/ (see oracle/make_golden.py),
+which pin oracle/pgt_oracle.py and the CUDA path against the real reference.
 
 Recipe (SURVEY.md Appendix C):
   * two shim packages (oracle/shims/{basicsr,timm}) stand in for the absent imports
@@ -17,12 +16,12 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get('PGT_REFERENCE_ROOT', '/root/reference')
+REFERENCE_ROOT = os.environ.get('PGT_REFERENCE_ROOT', '')     # a checkout of kepengxu/PGTFormer
 _SHIMS = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'shims')
 
 
 def reference_available():
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, 'archs', 'pgtformer_arch.py'))
+    return bool(REFERENCE_ROOT) and os.path.isfile(os.path.join(REFERENCE_ROOT, 'archs', 'pgtformer_arch.py'))
 
 
 def _ensure_paths():
@@ -32,9 +31,9 @@ def _ensure_paths():
 
 
 def import_reference():
-    """Returns the reference's `archs.pgtformer_arch` module (imported from /root/reference)."""
+    """Returns the reference's `archs.pgtformer_arch` module (imported from REFERENCE_ROOT)."""
     if not reference_available():
-        raise RuntimeError('reference tree not present at %s' % REFERENCE_ROOT)
+        raise RuntimeError('reference tree not present at %r (set PGT_REFERENCE_ROOT)' % REFERENCE_ROOT)
     _ensure_paths()
     # The product repo also has a top-level `archs` package (the drop-in). Make sure the name
     # `archs` resolves to the reference's while importing it, then restore.

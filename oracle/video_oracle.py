@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — CPU restatement of the reference's streaming frame loop, used only by tests/ as the checker
 for pgtformer_b200/video.py.  Not a product path.
 
-Restates `/root/reference/inference.py`:
+Restates the reference's `inference.py`:
   * `rgbnp2tensor` (:6-10)            rgb24 frames -> float32 [t,3,h,w] via numpy's double division
   * `apply_net_to_frames` (:12-19)    model(window)[0][1] -> clamp -> * 255 -> uint8 (truncation)
   * `process_video_ffmpeg` (:37-76)   the three-frame buffer: first frame duplicated, one window per new frame, last

@@ -1,7 +1,7 @@
-"""Builds libpgt_b200.so (all hand-written sm_100a kernels + the C ABI) in-tree with nvcc.
+"""Builds libpgt_b200.so (all hand-written sm_90a kernels + the C ABI) in-tree with nvcc.
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the
-gpurun snapshot.  `python -m pgtformer_b200.build [--force]`.
+nvcc cross-compiles without a GPU; the .so is git-ignored and rebuilt whenever a source, the
+header or the flags change.  `python -m pgtformer_b200.build [--force]`.
 """
 import hashlib
 import os
@@ -14,7 +14,8 @@ LIB_DIR = os.path.join(HERE, 'lib')
 LIB_PATH = os.path.join(LIB_DIR, 'libpgt_b200.so')
 STAMP = os.path.join(LIB_DIR, 'build.stamp')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']          # H100 (Hopper): wgmma, TMA, mbarrier
+FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
@@ -82,9 +83,8 @@ def build(force=False, verbose=False):
     if not force and os.path.exists(LIB_PATH) and os.path.exists(STAMP) and open(STAMP).read() == fp:
         return LIB_PATH
     if not os.path.exists(NVCC):
-        if os.path.exists(LIB_PATH):
-            return LIB_PATH           # GPU box without a toolchain change: use the shipped build
-        raise RuntimeError('nvcc not found at %s and no prebuilt %s' % (NVCC, LIB_PATH))
+        # a library from other sources or flags must not be loaded in place of these kernels
+        raise RuntimeError('nvcc not found at %s and %s is missing or was built from other sources' % (NVCC, LIB_PATH))
     objs = []
     procs = []
     for src in _sources():
@@ -98,7 +98,7 @@ def build(force=False, verbose=False):
             raise RuntimeError('nvcc failed for %s:\n%s' % (src, out))
         if verbose:
             sys.stderr.write(out)
-    link = [NVCC, '-shared', '-o', LIB_PATH] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart']
+    link = [NVCC, '-shared', '-o', LIB_PATH] + objs + ARCH + ['-lcudart']
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n' + r.stdout)

@@ -18,10 +18,10 @@ void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int num_sms() {
   static std::atomic<int> per_dev[64];                 // per device: a process may drive several GPUs
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   int n = per_dev[dev].load(std::memory_order_relaxed);
   if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     per_dev[dev].store(n, std::memory_order_relaxed);
   }
   return n;
@@ -90,7 +90,7 @@ extern "C" const char* pgt_strerror(int status) {
     case PGT_OK: return "ok";
     case PGT_ERR_INVALID: return "invalid argument (shape / alignment / null pointer)";
     case PGT_ERR_CUDA: return "CUDA runtime error (see pgt_last_cuda_error)";
-    case PGT_ERR_UNSUPPORTED: return "configuration not covered by the sm_100a kernels";
+    case PGT_ERR_UNSUPPORTED: return "configuration not covered by the sm_90a kernels";
     case PGT_ERR_DRIVER: return "cuTensorMapEncodeTiled unavailable or failed";
     default: return "unknown status";
   }

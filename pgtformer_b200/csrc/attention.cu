@@ -1,4 +1,4 @@
-// Attention cores (round-1 implementation on the warp-level mma.sync path; the tcgen05 fused
+// Attention cores (round-1 implementation on the warp-level mma.sync path; the wgmma fused
 // Swin-block kernel replaces the window kernel in a later round — see DESIGN.md):
 //   * shifted-window spatio-temporal attention, 3x4x4 windows (N = 48), roll / partition / reverse and the
 //     {0,-100} shift mask done as index math, relative-position bias from a [heads,48,48] table;
@@ -298,7 +298,7 @@ mha_fwd_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16
 }
 
 int mha_tc_launch(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, int clips, int L, int heads,
-                  int d, void* out, int ldo, cudaStream_t stream);      // mha_tc.cu (tcgen05 path)
+                  int d, void* out, int ldo, cudaStream_t stream);      // mha_tc.cu (wgmma path)
 
 }  // namespace pgt
 
@@ -347,7 +347,7 @@ extern "C" int pgt_mha_fwd(const void* q, int ldq, const void* k, int ldk, const
   if (!no_tc) {
     ProfScope pst(PGT_PROF_MHA, 4.0 * (double)L * L * d * heads * clips, static_cast<cudaStream_t>(stream), "mha_tc");
     const int rc = mha_tc_launch(q, ldq, k, ldk, v, ldv, clips, L, heads, d, out, ldo, static_cast<cudaStream_t>(stream));
-    if (rc != PGT_ERR_UNSUPPORTED) return rc;        // shapes the tcgen05 kernel does not cover use the mma.sync kernel
+    if (rc != PGT_ERR_UNSUPPORTED) return rc;        // shapes the wgmma kernel does not cover use the mma.sync kernel
   }
   dim3 grid(ceil_div(L, FA_BM), heads, clips);
   const size_t smem = (size_t)4 * FA_BN * (64 + 8) * 2;

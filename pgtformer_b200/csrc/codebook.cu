@@ -1,5 +1,5 @@
 // RQ-VAE codebook kernels: row argmax + embedding gather (the path PGTFormer.forward takes) and the exhaustive
-// fp64 nearest-codebook L2 argmin (the tcgen05 kernel of the TDCRQVAE3.forward / get_codes path is in
+// fp64 nearest-codebook L2 argmin (the wgmma kernel of the TDCRQVAE3.forward / get_codes path is in
 // l2_argmin_tc.cu; this one serves the tokens it cannot certify and the shapes it does not cover).  Index results are
 // exact: argmax is a pure fp32 compare; argmin is an fp64 argmin of ||z-e||^2 with lowest index on ties, which is
 // stricter than the reference's own fp32 addmm.
@@ -70,7 +70,7 @@ argmax_gather_kernel(const float* __restrict__ logits, int T, int K, const float
 // (an fp32 shortlist is not: with ||z|| >> ||e|| all 1024 distances agree to ~1e-6 relative, below fp32 resolution).
 // 64 tokens x 64 codes per tile, 4 x 4 fp64 accumulators per thread, two fp64 instructions per term (~3 ms at
 // T = 49152, K = 1024, E = 512 on the 64-lane fp64 pipe).  Runs on all T tokens (list == nullptr) for shapes the
-// tcgen05 kernel does not cover, or on the tokens list[0 .. *count) it could not certify — normally none.
+// wgmma kernel does not cover, or on the tokens list[0 .. *count) it could not certify — normally none.
 constexpr int AM_TT = 64;      // tokens per CTA
 constexpr int AM_TC = 64;      // codes per tile
 constexpr int AM_KC = 32;      // feature chunk
@@ -176,7 +176,7 @@ l2_argmin_kernel(const float* __restrict__ z, int T, int E, const float* __restr
   }
 }
 
-// The same fp64 argmin for a SHORT token list (the normal case of the tcgen05 kernel's leftovers: none, or a handful):
+// The same fp64 argmin for a SHORT token list (the normal case of the wgmma kernel's leftovers: none, or a handful):
 // one warp per token, the codebook streamed from L2, so a few tokens spread over the whole chip instead of queueing on
 // one CTA of the tiled kernel.  Does nothing when *count > max_count (the tiled kernel takes over).
 __global__ void __launch_bounds__(256)

@@ -1,4 +1,4 @@
-// decoder.norm_out -> SiLU -> conv_out (3x3, 64 -> 3 channels, fp32 NCHW result) as ONE tcgen05 kernel
+// decoder.norm_out -> SiLU -> conv_out (3x3, 64 -> 3 channels, fp32 NCHW result) as ONE wgmma kernel
 // (`archs/pgtformer_arch.py:707-710`, `archs/tdcrqvae3_arch.py:700-706`: GroupNorm(32, eps 1e-6), swish, Conv2d).
 //
 // Why its own kernel: with Cout = 3 the generic halo conv computes a 64-wide tile for 3 useful columns and stores
@@ -7,11 +7,10 @@
 //   * 8 builder warps read the RAW conv input once (128-bit loads, a pixel's 64 channels = one 128-byte row), apply
 //     y = silu(x * a[f,c] + b[f,c]) (GroupNorm folded into per-(frame, channel) affine terms) and write the bf16
 //     (16+2) x (8+2)-pixel halo slab straight into the 128B-swizzled layout — the normalised tensor never exists in HBM;
-//   * one elected lane issues, per 16x8-pixel tile, 9 taps x 4 k-steps of tcgen05.mma 128x16x16: tap (dy,dx) is the
-//     same slab viewed from row dy*10+dx (SBO = slab pitch, as in the halo conv of gemm_tc.cu), the 9 x 16 x 64 weight
-//     tile is resident in shared memory;
-//   * 4 epilogue warps read the 128 x 16 accumulator from TMEM, add the bias and store the 3 planes (fp32 NCHW).
-// The tile is bound by the tensor core's shared-memory operand reads (4.5 KB per MMA), ~3.5x faster than before.
+//   * one warpgroup issues, per 16x8-pixel tile, 9 taps x 4 k-steps x 2 row halves of wgmma 64x16x16: tap (dy,dx) is
+//     the same slab viewed from row dy*10+dx (SBO = slab pitch, as in the halo conv of gemm_tc.cu), the 9 x 16 x 64
+//     weight tile is resident in shared memory; the same warpgroup adds the bias to the register accumulators and
+//     stores the 3 planes (fp32 NCHW) straight from them.
 #include <cstdio>
 
 #include "common.cuh"
@@ -24,30 +23,11 @@ constexpr int CO_TW = 8, CO_TH = 16;                         // output tile: 16 
 constexpr int CO_SW = CO_TW + 2, CO_SH = CO_TH + 2;          // halo slab
 constexpr int CO_PITCH = CO_SW * 128;                        // bytes between slab image rows
 constexpr int CO_SLAB = ((CO_SH * CO_PITCH + 1023) / 1024) * 1024;   // 23552
-constexpr int CO_NB = 16;                                    // padded Cout (UMMA N)
+constexpr int CO_NB = 16;                                    // padded Cout (wgmma N)
 constexpr int CO_WBYTES = 9 * CO_NB * 128;                   // 18 KB: [tap][16 rows][64 ch] bf16, K-major SW128
 constexpr int CO_BUILDERS = 256;
-constexpr int CO_THREADS = 32 + CO_BUILDERS + 128;
+constexpr int CO_THREADS = CO_BUILDERS + 128;                // builder warps 0..7, MMA / epilogue warpgroup 8..11
 constexpr int CO_SMEM = 2 * CO_SLAB + CO_WBYTES + 2 * 128 * 4 /*ab of the tile's frame, double buffered*/ + 256 + 1024;
-
-__device__ __forceinline__ uint64_t co_desc_sbo(uint32_t saddr, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-__device__ __forceinline__ void tmem_ld_32x16b(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
 
 // silu(v) = v * sigmoid(v) = h + h * tanh(h), h = v / 2: one MUFU (tanh.approx, rel. error 2^-11, below the bf16 rounding
 // of the result) instead of the ex2 + rcp pair — the builders are MUFU-bound
@@ -77,25 +57,16 @@ conv_out_gn_kernel(const ConvOutParams p) {
   uint8_t* sW = smem + 2 * CO_SLAB;                             // [9][16 x 128 B]
   float* sAB = reinterpret_cast<float*>(sW + CO_WBYTES);        // [2][2][64]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sAB + 2 * 128);
-  uint64_t* slab_full = bars;                                   // [2]
-  uint64_t* slab_empty = bars + 2;                              // [2]
-  uint64_t* acc_full = bars + 4;                                // [2]
-  uint64_t* acc_empty = bars + 6;                               // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* slab_full = bars;                                   // [2] builders -> MMA warpgroup
+  uint64_t* slab_empty = bars + 2;                              // [2] MMA warpgroup (one arrive per warp) -> builders
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&slab_full[i], CO_BUILDERS);
-        mbar_init(&slab_empty[i], 1);
-        mbar_init(&acc_full[i], 1);
-        mbar_init(&acc_empty[i], 128);
-      }
-      fence_barrier_init();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&slab_full[i], CO_BUILDERS);
+      mbar_init(&slab_empty[i], 4);
     }
-    tmem_alloc<32>(tmem_ptr);
-    tc_fence_before();
+    fence_barrier_init();
   }
   // weights -> swizzled K-major tiles (rows >= cout are zero)
   for (int i = threadIdx.x; i < 9 * CO_NB * 8; i += CO_THREADS) {
@@ -106,37 +77,11 @@ conv_out_gn_kernel(const ConvOutParams p) {
   }
   fence_proxy_async();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int per_frame = p.tiles_x * p.tiles_y;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc_bf16(128, CO_NB);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it & 1;
-      const uint32_t ph = (it >> 1) & 1;
-      mbar_wait(&slab_full[buf], ph);
-      mbar_wait(&acc_empty[buf], ph ^ 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = smem_u32(slab + buf * CO_SLAB);
-#pragma unroll
-        for (int tap = 0; tap < 9; ++tap) {
-          const uint64_t da = co_desc_sbo(sa + ((tap / 3) * CO_SW + (tap % 3)) * 128, CO_PITCH);
-          const uint64_t db = umma_desc_k_sw128(smem_u32(sW + tap * (CO_NB * 128)));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16_ss(tmem_base + buf * CO_NB, da + 2 * k, db + 2 * k, idesc, (tap | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&slab_empty[buf]);
-        umma_commit(&acc_full[buf]);
-      }
-      __syncwarp();
-    }
-  } else if (warp <= 8) {
+  if (warp < CO_BUILDERS / 32) {
     // ------------------------------------------------------------------ slab builders (GroupNorm + SiLU on the way in)
-    const int bt = threadIdx.x - 32;                             // 0..255
+    const int bt = threadIdx.x;                                  // 0..255
     const int chunk = bt & 7;                                    // 8 channels = one 16-byte chunk
     int it = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
@@ -190,38 +135,53 @@ conv_out_gn_kernel(const ConvOutParams p) {
       mbar_arrive(&slab_full[buf]);
     }
   } else {
-    // ------------------------------------------------------------------ epilogue: TMEM -> + bias -> fp32 NCHW planes
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;                            // GEMM row = pixel (ty = row / 8, tx = row % 8)
-    const uint32_t tacc = tmem_base + (uint32_t(quad * 32) << 16);
+    // ------------------------------------------------------------------ MMA warpgroup: wgmma -> + bias -> fp32 NCHW planes
+    // Accumulator fragment (m64n16): lane holds columns 2 (lane % 4) + {0, 1} of rows 16 w + lane / 4 (+ 8) of each
+    // 64-row half; the lanes with lane % 4 < 2 hold the (at most) three real output channels.
+    const int w = warp & 3;
+    const int t4 = lane & 3;
     float bias[3] = {0.f, 0.f, 0.f};
     for (int c = 0; c < p.cout && c < 3; ++c) bias[c] = p.bias ? __ldg(p.bias + c) : 0.f;
     const size_t plane = (size_t)p.H * p.W;
+    const uint32_t sw = smem_u32(sW);
     int it = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
       const int buf = it & 1;
       const uint32_t ph = (it >> 1) & 1;
       const int f = tile / per_frame, r = tile - f * per_frame;
-      const int y = (r / p.tiles_x) * CO_TH + (row >> 3), x = (r % p.tiles_x) * CO_TW + (row & 7);
-      mbar_wait(&acc_full[buf], ph);
-      tc_fence_after();
-      uint32_t v[16];
-      tmem_ld_32x16b(tacc + buf * CO_NB, v);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&acc_empty[buf]);
-      float* o = p.out + (size_t)f * p.cout * plane + (size_t)y * p.W + x;
+      mbar_wait(&slab_full[buf], ph);
+      const uint32_t sa = smem_u32(slab + buf * CO_SLAB);
+      float acc[2][CO_NB / 2];                                  // tile rows [0, 64) = image rows 0..7, [64, 128) = 8..15
+      wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < 3; ++c)
-        if (c < p.cout) o[c * plane] = __uint_as_float(v[c]) + bias[c];
+      for (int tap = 0; tap < 9; ++tap) {
+        const uint32_t ta = sa + ((tap / 3) * CO_SW + (tap % 3)) * 128;
+        const uint64_t da0 = wgmma_desc_k_sw128(ta, CO_PITCH), da1 = wgmma_desc_k_sw128(ta + 8 * CO_PITCH, CO_PITCH);
+        const uint64_t db = wgmma_desc_k_sw128(sw + tap * (CO_NB * 128));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_bf16<CO_NB>(acc[0], da0 + 2 * k, db + 2 * k, (tap | k) != 0 ? 1u : 0u);
+          wgmma_bf16<CO_NB>(acc[1], da1 + 2 * k, db + 2 * k, (tap | k) != 0 ? 1u : 0u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&slab_empty[buf]);
+      if (t4 < 2) {
+        float* o = p.out + (size_t)f * p.cout * plane;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int row = 64 * h + 16 * w + (lane >> 2) + 8 * (e >> 1);   // GEMM row = pixel (ty = row / 8, tx = row % 8)
+            const int c = 2 * t4 + (e & 1);
+            const int y = (r / p.tiles_x) * CO_TH + (row >> 3), x = (r % p.tiles_x) * CO_TW + (row & 7);
+            if (c < p.cout) o[c * plane + (size_t)y * p.W + x] = acc[h][e] + bias[c < 3 ? c : 0];
+          }
+        }
+      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<32>(tmem_base);
   }
 }
 
@@ -243,7 +203,7 @@ extern "C" int pgt_conv_out_gn(const void* x, int F, int H, int W, int Cin, int 
   p.tiles_x = W / CO_TW; p.tiles_y = H / CO_TH; p.num_tiles = F * p.tiles_x * p.tiles_y;
   static PerDeviceOnce once;
   PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(conv_out_gn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CO_SMEM); }));
-  const int grid = p.num_tiles < 2 * num_sms() ? p.num_tiles : 2 * num_sms();   // 2 CTAs per SM (66 KB smem, 32 TMEM columns each)
+  const int grid = p.num_tiles < 2 * num_sms() ? p.num_tiles : 2 * num_sms();   // 2 CTAs per SM (66 KB smem each)
   char desc[64];
   snprintf(desc, sizeof(desc), "conv_out_gn F%d H%d W%d N%d", F, H, W, Cout);
   ProfScope ps(PGT_PROF_GEMM, 2.0 * F * (double)H * W * Cout * 9 * Cin, st, desc);

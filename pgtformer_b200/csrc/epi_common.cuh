@@ -1,4 +1,4 @@
-// Device helpers shared by the tcgen05 kernels' epilogues.
+// Device helpers shared by the wgmma kernels' epilogues.
 #pragma once
 #include "common.cuh"
 

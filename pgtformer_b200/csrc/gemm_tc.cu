@@ -1,23 +1,21 @@
-// tcgen05 GEMM / implicit-GEMM convolution for sm_100a.
+// wgmma GEMM / implicit-GEMM convolution for sm_90a.
 //
-//   out[rows, N] = epilogue( A[rows, K] * W[N, K]^T )          bf16 operands, fp32 accumulate in TMEM
+//   out[rows, N] = epilogue( A[rows, K] * W[N, K]^T )          bf16 operands, fp32 accumulate in registers
 //
-// Persistent, warp-specialised kernels (352 threads; + 128 in the GroupNorm-fused halo variant):
-//   warp 0      TMA producer: A tile (128 rows x 64 K) and W tile (BN rows x 64 K) per k-block, 128B swizzle
-//   warp 1      TMEM allocator; ONE elected lane walks the whole k loop of a tile (barrier waits included) and issues
-//               tcgen05.mma 128 x BN x 16 — cta_group::2 (M = 256 over a CTA pair, each CTA holding half of every
-//               weight tile) in the PAIR / halo2 kernels
-//   warps 2..9  epilogue, two warps per TMEM lane quadrant (each half-group of 4 warps owns half of the tile's
-//               column panels): tcgen05.ld -> +bias -> activation -> +residual / SFT from the staging slot ->
-//               optional GroupNorm partial statistics -> bf16/fp32 pack into a 128B-swizzled smem staging panel
-//   warp 10     epilogue DMA: TMA-loads the residual (/ SFT scale) panel INTO the staging slot ahead of time and
+// Persistent, warp-specialised kernels (320 threads; + 128 in the GroupNorm-fused halo variant):
+//   warps 0..7  two consumer warpgroups: warpgroup h issues wgmma 64 x BN x 16 for rows [64h, 64h + 64) of the
+//               128-row tile over the whole k loop, then runs the epilogue: the accumulators go through a 128 x 64
+//               fp32 shared-memory exchange (one row per thread, 32 columns per chunk) -> +bias -> activation ->
+//               +residual / SFT from the staging slot -> optional GroupNorm partial statistics -> bf16/fp32 pack into
+//               a 128B-swizzled smem staging panel
+//   warp 8      TMA producer: A tile (128 rows x 64 K) and W tile (BN rows x 64 K) per k-block, 128B swizzle
+//   warp 9      epilogue DMA: TMA-loads the residual (/ SFT scale) panel INTO the staging slot ahead of time and
 //               TMA-stores the finished panel, so both are full-line bulk copies and no CTA barrier sits on the path
-// Pipelines: smem full/empty ring (TMA <-> MMA), a 2-deep TMEM accumulator ring (MMA <-> epilogue) and a 4-slot
-// staging ring (epilogue <-> DMA warp), so the epilogue of tile i overlaps the main loop of tile i+1.
+// Pipelines: smem full/empty ring (TMA <-> wgmma) and a 4-slot staging ring (epilogue <-> DMA warp); the producer
+// runs ahead into the next tile while the consumers finish the epilogue of the current one.
 //
-// Kernels in this file: gemm_tc_kernel<BN, PAIR> (linear / generic implicit-GEMM conv), conv_halo_kernel<BN, GN>
-// (3x3 and upsample-phase convs with Cout <= 128: one halo slab serves every tap), conv_halo2_kernel<BN> (the same on
-// CTA pairs).
+// Kernels in this file: gemm_tc_kernel<BN> (linear / generic implicit-GEMM conv), conv_halo_kernel<BN, GN>
+// (3x3 and upsample-phase convs with Cout <= 128: one halo slab serves every tap).
 //
 // The A operand is produced by TMA in three addressing modes:
 //   LINEAR   2-D map [K, rows]
@@ -38,8 +36,13 @@ namespace pgt {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int EPI_WARPS = 8;
-constexpr int GEMM_THREADS = 64 + EPI_WARPS * 32 + 32;     // TMA producer, MMA issuer, 8 epilogue warps, epilogue-DMA warp
+constexpr int EPI_WARPS = 8;                     // the two consumer warpgroups (wgmma + epilogue)
+constexpr int GEMM_THREADS = EPI_WARPS * 32 + 64;          // consumer warpgroups, TMA producer, epilogue-DMA warp
+constexpr int PRODUCER_WARP = EPI_WARPS;
+constexpr int DMA_WARP = EPI_WARPS + 1;
+constexpr int XCH_LD = 68;                       // accumulator exchange: 128 rows x 64 fp32 (+4 pad: conflict-free reads)
+constexpr int XCH_BYTES = BM * XCH_LD * 4;
+constexpr int EPI_BAR = 1;                       // named barrier of the 256 consumer threads
 constexpr int A_STAGE_BYTES = BM * BK * 2;
 constexpr int PANEL_BYTES = BM * 128;            // one staging panel: 128 rows x 128 B
 constexpr int NUM_SLOTS = 4;                     // staging slots (two per epilogue half-group)
@@ -51,7 +54,6 @@ struct GemmParams {
   int mode;
   int M, N, K;
   int num_kb, m_tiles, n_tiles;
-  int pair_map;          // CTA-pair kernels: tiles 2q, 2q+1 are the two M halves of pair q (same n block)
   // conv geometry in OUTPUT space
   int F, H, W;
   int tw, th, tn, tiles_x, tiles_y;
@@ -82,28 +84,23 @@ struct GemmParams {
   double flops;      // algorithmic 2*M*N*K with the un-padded K (host-side accounting only)
 };
 
-template <int BN, bool PAIR = false>
+template <int BN>
 struct GemmCfg {
-  static constexpr int B_STAGE_BYTES = (PAIR ? BN / 2 : BN) * BK * 2;     // a CTA pair splits every weight tile
+  static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int STAGING_BYTES = NUM_SLOTS * PANEL_BYTES;
-  static constexpr int BUDGET = 232448 - 1024 /*align*/ - STAGING_BYTES - 2 * BN * 4 /*bias*/ - 1024 /*gn*/ - 256 /*barriers*/;
+  static constexpr int BUDGET = 232448 - 1024 /*align*/ - STAGING_BYTES - XCH_BYTES - 256 /*barriers*/;
   static constexpr int STAGES = (BUDGET / STAGE_BYTES) > 6 ? 6 : (BUDGET / STAGE_BYTES);
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 2 * BN * 4 + 1024 + 256 + 1024;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + XCH_BYTES + 256 + 1024;
+  static_assert(SMEM_BYTES <= 232448, "gemm smem budget");
 };
 
 // persistent-loop tile index -> (m block, n block)
 __device__ __forceinline__ void tile_mn(const GemmParams& p, int tile, int& m_blk, int& n_blk) {
-  if (p.pair_map) {
-    const int q = tile >> 1;
-    n_blk = q % p.n_tiles;
-    m_blk = 2 * (q / p.n_tiles) + (tile & 1);
-  } else {
-    n_blk = tile % p.n_tiles;
-    m_blk = tile / p.n_tiles;
-  }
+  n_blk = tile % p.n_tiles;
+  m_blk = tile / p.n_tiles;
 }
+
 
 __device__ __forceinline__ void decode_conv_tile(const GemmParams& p, int m_blk, int& n0, int& y0, int& x0) {
   const int tx = m_blk % p.tiles_x;
@@ -142,15 +139,12 @@ __device__ __forceinline__ void act_chunk(float (&f)[32], int act) {
 }
 
 // ------------------------------------------------------------------------------------------- epilogue
-// Shared by the GEMM/conv kernel and the halo-reuse conv kernel.  Runs on warps 2..9 (256 threads).
+// Shared by the GEMM/conv kernel and the halo-reuse conv kernel.  Runs on warps 0..7 (256 threads).
 struct EpiCtx {
   uint8_t* staging;        // NUM_SLOTS x PANEL_BYTES, 1024-aligned
-  uint64_t* tmem_full;     // [2]
-  uint64_t* tmem_empty;    // [2]
+  float* xch;              // BM x XCH_LD fp32 accumulator exchange
   uint64_t* res_bar;       // [NUM_SLOTS] staging slot prepared (free, residual landed)   DMA warp -> epilogue
   uint64_t* slot_ready;    // [NUM_SLOTS] staging slot holds the finished panel           epilogue -> DMA warp
-  uint32_t tmem_base;
-  uint32_t tmem_empty_cluster;   // != 0: shared::cluster address of the pair leader's tmem_empty[0] (2-CTA kernels)
 };
 
 // One 32-column chunk of a staging panel, accumulators already in registers (v): +bias -> act -> (+residual | SFT)
@@ -281,8 +275,8 @@ __device__ __forceinline__ void epi_finish(const GemmParams& p, const uint32_t (
 
 // Epilogue work is a stream of ITEMS = (tile, 128-byte-wide column panel) flowing through a ring of staging slots.
 // Two roles:
-//   * 8 epilogue warps (two per TMEM lane quadrant, splitting a panel's 32-column chunks): wait until the slot is
-//     prepared, TMEM -> bias / activation / residual / SFT -> swizzled smem, signal `slot_ready`.  No CTA-level
+//   * 8 epilogue warps (two per 32-row quadrant, splitting a panel's 32-column chunks): wait until the slot is
+//     prepared, accumulators -> bias / activation / residual / SFT -> swizzled smem, signal `slot_ready`.  No CTA-level
 //     barrier and no serial bookkeeping sits on this path.
 //   * one DMA warp (epilogue_dma_loop): prepares slots ahead of time (waits for the previous TMA store out of the
 //     slot to drain, TMA-loads the residual / SFT-scale panel into it) and TMA-stores finished panels.
@@ -373,112 +367,115 @@ __device__ __forceinline__ void epilogue_dma_loop(const GemmParams& p, const Epi
   if (lane == 0) bulk_wait0();                           // all output bytes written before the CTA retires
 }
 
+// The epilogue of one tile, on the two consumer warpgroups right after their k loop.  Per 64-column group: both
+// warpgroups write their accumulator rows into the exchange, then thread (quad, half) reads row quad * 32 + lane,
+// columns [32 half, 32 half + 32) (bf16 panels: one chunk each) or the whole panel of parity half (fp32 panels).
+// `k` counts staging items across tiles.
 template <int BN>
-__device__ __forceinline__ void epilogue_loop(const GemmParams& p, const EpiCtx& ctx, int warp, int lane, int num_tiles) {
-  uint64_t* tmem_full = ctx.tmem_full;
-  uint64_t* tmem_empty = ctx.tmem_empty;
-  const uint32_t tmem_base = ctx.tmem_base;
-  const int ew = warp - 2;                   // 0..7
-  const int quad = warp & 3;                 // TMEM lane quadrant this warp may read
-  const int half = ew >> 2;                  // which of the quadrant's two warps
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx& ctx, int warp, int lane, int tile, int& k,
+                                              const float (&acc)[BN / 2]) {
+  const int quad = warp & 3;                 // rows [32 quad, 32 quad + 32) of the tile
+  const int half = warp >> 2;                // which 32-column chunk of a group / parity of an fp32 panel
   const int r = quad * 32 + lane;            // row of the 128-row tile
   const int esize = (p.out_dtype == PGT_BF16) ? 2 : 4;
-  const ItemStream<BN> is(p, num_tiles);
+  const ItemStream<BN> is(p, 0);
   const int PW = is.PW;
   const int nsub = PW / 32;
   const bool sft = (p.epi_mode == PGT_EPI_SFT);
   const bool bias_vec = p.bias != nullptr && (p.N % 32) == 0;   // whole chunks inside N: 128-bit bias reads
+  const float* xrow = ctx.xch + r * XCH_LD;
 
-  int k = 0;                                 // item counter
-  int it = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-    const int acc = it & 1;
-    const uint32_t acc_phase = (it >> 1) & 1;
-    int n_blk, m_blk;
-    tile_mn(p, tile, m_blk, n_blk);
-    const int col_base = n_blk * BN;
-    int n0 = 0, y0 = 0, x0 = 0;
-    if (p.mode != MODE_LINEAR && !p.fast_epi) decode_conv_tile(p, m_blk, n0, y0, x0);
-    const uint32_t t_row = tmem_base + (uint32_t(quad * 32) << 16) + acc * BN;
-    mbar_wait(&tmem_full[acc], acc_phase);
-    tc_fence_after();
+  int n_blk, m_blk;
+  tile_mn(p, tile, m_blk, n_blk);
+  const int col_base = n_blk * BN;
+  const int npan = p.fast_epi ? is.panels_in_tile(tile) : 0;
+  const uint32_t stg = smem_u32(ctx.staging) + r * 128;
+  auto gn_ptr = [&](int col0) -> float* {
+    if (p.gn_stats == nullptr) return nullptr;
+    const size_t chunk = p.gn_tpf > 0 ? (size_t)(m_blk / p.gn_tpf) * p.gn_fstride + (m_blk % p.gn_tpf) * 4 + quad
+                                      : (size_t)m_blk * 4 + quad;
+    return p.gn_stats + (chunk * 32 + col0 / p.gn_cpg) * 2;
+  };
+  // direct path (NCHW fp32 output, unaligned views, mixed residual dtype): this thread's output row
+  bool valid = false;
+  long long orow = 0;
+  int pn = 0, py = 0, px = 0;
+  if (!p.fast_epi) {
+    if (p.mode == MODE_LINEAR) {
+      orow = (long long)m_blk * BM + r;
+      valid = orow < p.M;
+    } else {
+      int n0, y0, x0;
+      decode_conv_tile(p, m_blk, n0, y0, x0);
+      const int ix = r % p.tw;
+      const int t2 = r / p.tw;
+      const int iy = t2 % p.th;
+      const int in = t2 / p.th;
+      pn = n0 + in; py = y0 + iy; px = x0 + ix;
+      valid = (pn < p.F) && (py < p.H) && (px < p.W);
+      orow = ((long long)pn * p.H + py) * p.W + px;
+    }
+  }
+
+  static_for<0, BN / 64>([&](auto gc) {
+    constexpr int g = decltype(gc)::value;
+    if (col_base + g * 64 >= p.N) return;    // uniform over the consumer threads
+    named_bar_sync(EPI_BAR, EPI_WARPS * 32);  // the previous group's rows have been read
+    acc_to_smem<g * 64, 64>(acc, ctx.xch + half * 64 * XCH_LD, XCH_LD, quad, lane);
+    named_bar_sync(EPI_BAR, EPI_WARPS * 32);
 
     if (p.fast_epi) {
-      const int npan = is.panels_in_tile(tile);
-      const uint32_t stg = smem_u32(ctx.staging) + r * 128;
-      auto gn_ptr = [&](int col0) -> float* {
-        if (p.gn_stats == nullptr) return nullptr;
-        const size_t chunk = p.gn_tpf > 0 ? (size_t)(m_blk / p.gn_tpf) * p.gn_fstride + (m_blk % p.gn_tpf) * 4 + quad
-                                          : (size_t)m_blk * 4 + quad;
-        return p.gn_stats + (chunk * 32 + col0 / p.gn_cpg) * 2;
-      };
       if (sft) {
-        // SFT items take two slots (residual / out + scale): ring of 2, one item at a time
-        for (int pnl = 0; pnl < npan; ++pnl, ++k) {
+        // SFT items (bf16, one panel per group) take two slots (residual / out + scale): ring of 2, one item at a time
+        const int pnl = g;
+        if (pnl < npan) {
           const int pos = k & 1;
           mbar_wait(&ctx.res_bar[pos], (k >> 1) & 1);     // slot free, residual and scale panels landed
           const int col0 = col_base + pnl * PW + half * 32;
           uint32_t v[32];
-          tmem_ld_32x32(t_row + pnl * PW + half * 32, v);
-          tmem_ld_wait();
+          smem_row_32(xrow + half * 32, v);
           float4 nb[8];
           epi_finish<true>(p, v, bias_vec ? p.bias + col0 : nullptr, stg + pos * 2 * PANEL_BYTES, r, half, esize, true,
                            gn_ptr(col0), col0, nb, false);
           fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA engine
           mbar_arrive(&ctx.slot_ready[pos]);
+          ++k;
         }
       } else {
-        // One item (panel) at a time; bf16 (two 32-column chunks per panel): the quadrant's two warps take one chunk each,
-        // fp32 (one chunk per panel): they take alternate panels.  The bias chunk is fetched BEFORE the slot wait and the
-        // TMEM read: under a shared-memory / L1 data pipe saturated by MMA operand reads and TMA fills an L1-hit load
-        // takes several hundred cycles, which those waits then cover.
-        for (int pnl = 0; pnl < npan; ++pnl, ++k) {
+        // One item (panel) at a time; bf16 (two 32-column chunks per panel): the two warpgroups' warps of a quadrant
+        // take one chunk each, fp32 (one chunk per panel): they take alternate panels.  The bias chunk is fetched
+        // BEFORE the slot wait.
+        for (int pp = 0; pp < 64 / PW; ++pp) {
+          const int pnl = g * (64 / PW) + pp;
+          if (pnl >= npan) break;
           const int pos = k & 3;
           const bool mine = (nsub == 2) || ((pnl & 1) == half);
           const int sb = (nsub == 2) ? half : 0;
           const int col0 = col_base + pnl * PW + sb * 32;
           float4 b[8];
           if (mine && bias_vec) {
-            const float4* g = reinterpret_cast<const float4*>(p.bias + col0);
+            const float4* gb = reinterpret_cast<const float4*>(p.bias + col0);
 #pragma unroll
-            for (int q = 0; q < 8; ++q) b[q] = __ldg(g + q);
+            for (int q = 0; q < 8; ++q) b[q] = __ldg(gb + q);
           }
           mbar_wait(&ctx.res_bar[pos], (k >> 2) & 1);      // slot free (and residual panel landed)
           if (mine) {
             uint32_t v[32];
-            tmem_ld_32x32(t_row + pnl * PW + sb * 32, v);
-            tmem_ld_wait();
+            smem_row_32(xrow + pnl * PW + sb * 32 - g * 64, v);
             epi_finish<false>(p, v, nullptr, stg + pos * PANEL_BYTES, r, sb, esize, p.has_res_map != 0, gn_ptr(col0), col0, b, bias_vec);
           }
           fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA engine
           mbar_arrive(&ctx.slot_ready[pos]);
+          ++k;
         }
       }
     } else {
-      // ---------------- direct path (NCHW fp32 output, unaligned views, mixed residual dtype): per-thread global I/O
-      bool valid;
-      long long orow;
-      int pn = 0, py = 0, px = 0;
-      if (p.mode == MODE_LINEAR) {
-        orow = (long long)m_blk * BM + r;
-        valid = orow < p.M;
-      } else {
-        const int ix = r % p.tw;
-        const int t2 = r / p.tw;
-        const int iy = t2 % p.th;
-        const int in = t2 / p.th;
-        pn = n0 + in; py = y0 + iy; px = x0 + ix;
-        valid = (pn < p.F) && (py < p.H) && (px < p.W);
-        orow = ((long long)pn * p.H + py) * p.W + px;
-      }
-      const int c_lo = half * (BN / 2), c_hi = c_lo + BN / 2;
-#pragma unroll 1
-      for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
-        if (col_base + c0 >= p.N) break;       // warp-uniform
-        uint32_t v[32];
-        tmem_ld_32x32(t_row + c0, v);
-        tmem_ld_wait();
+      // ---------------- direct path: per-thread global I/O of chunk `half` of the group
+      const int c0 = g * 64 + half * 32;
+      if (col_base + c0 < p.N) {
         if (valid) {
+          uint32_t v[32];
+          smem_row_32(xrow + half * 32, v);
           const int col0 = col_base + c0;
           const int ncol = min(32, p.N - col0);
           float f[32];
@@ -539,48 +536,42 @@ __device__ __forceinline__ void epilogue_loop(const GemmParams& p, const EpiCtx&
               if (j < ncol) op[j] = f[j];
           }
         }
-        __syncwarp();
       }
+      __syncwarp();
     }
-    tc_fence_before();
-    if (ctx.tmem_empty_cluster != 0) {
-      __syncwarp();                                   // one cluster-scope arrive per warp, not per thread
-      if (lane == 0) mbar_arrive_cluster(ctx.tmem_empty_cluster + acc * 8);
-    } else {
-      mbar_arrive(&tmem_empty[acc]);
-    }
-  }
+  });
 }
 
-// PAIR: launched as clusters of two CTAs on cta_group::2 (see conv_halo2_kernel): the pair computes a 256-row tile,
-// each CTA loads its own 128 A rows and HALF of every weight tile; both CTAs' loads complete on the leader's full
-// barriers, the leader's lane issues the M = 256 MMAs and multicasts its commits.
-template <int BN, bool PAIR>
+// Consumer side of a stage ring: one arrive per consumer warp once the warpgroup's wgmmas reading the stage retired.
+__device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
+  __syncwarp();
+  if (lane == 0) mbar_arrive(bar);
+}
+
+template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
                const __grid_constant__ CUtensorMap tmX, const GemmParams p) {
-  using Cfg = GemmCfg<BN, PAIR>;
+  using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
   uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;                 // 1024-aligned (all stage sizes are)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
+  float* xch = reinterpret_cast<float*>(staging + Cfg::STAGING_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES + XCH_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;
-  uint64_t* tmem_empty = bars + 2 * STAGES + 2;
-  uint64_t* res_bar = bars + 2 * STAGES + 4;                           // [NUM_SLOTS]
-  uint64_t* slot_ready = bars + 2 * STAGES + 8;                        // [NUM_SLOTS]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 12);
+  uint64_t* res_bar = bars + 2 * STAGES;                               // [NUM_SLOTS]
+  uint64_t* slot_ready = bars + 2 * STAGES + 4;                        // [NUM_SLOTS]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = p.m_tiles * p.n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (p.fast_epi) tma_prefetch_desc(&tmO);
@@ -588,144 +579,93 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (p.fast_epi && p.epi_mode == PGT_EPI_SFT) tma_prefetch_desc(&tmX);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], EPI_WARPS);       // one arrive per consumer warp
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], PAIR ? 2 * EPI_WARPS : EPI_WARPS * 32);   // pair: one cluster-scope arrive per warp
-      mbar_init(&res_bar[2 * i], 1);             // res_bar / slot_ready [NUM_SLOTS]: one per staging ring position
-      mbar_init(&res_bar[2 * i + 1], 1);
-      mbar_init(&slot_ready[2 * i], EPI_WARPS * 32);
-      mbar_init(&slot_ready[2 * i + 1], EPI_WARPS * 32);
+    for (int i = 0; i < NUM_SLOTS; ++i) {
+      mbar_init(&res_bar[i], 1);                 // res_bar / slot_ready: one per staging ring position
+      mbar_init(&slot_ready[i], EPI_WARPS * 32);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if constexpr (PAIR) tmem_alloc_2cta<Cfg::TMEM_COLS>(tmem_ptr);
-    else tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-    tc_fence_before();
-  }
   __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();              // the peer's barriers exist before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer
     // (whole warp runs the loop and the waits; the copies are issued under elect.sync so that ptxas sees a
     //  single-lane region and emits the uniform-datapath UTMALDG directly)
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int n_blk, m_blk;
-        tile_mn(p, tile, m_blk, n_blk);
-        int n0 = 0, y0 = 0, x0 = 0;
-        if (p.mode != MODE_LINEAR) decode_conv_tile(p, m_blk, n0, y0, x0);
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (elect_one()) {
-            void* dst_a = smem_a + stage * A_STAGE_BYTES;
-            void* dst_b = smem_b + stage * Cfg::B_STAGE_BYTES;
-            int cb = 0, ax = 0, ay = 0, a5 = 0;            // conv: channel coordinate, x, y (, parity) of this k-block's tap
-            if (p.mode != MODE_LINEAR) {
-              const int tap = kb / p.cin_blocks;
-              cb = kb - tap * p.cin_blocks;
-              const int dy = tap / p.ksize;
-              const int dx = tap - dy * p.ksize;
-              if (p.mode == MODE_CONV_S1) {
-                ax = x0 + dx - p.pad_x; ay = y0 + dy - p.pad_y;
-              } else {
-                const int oy = dy - p.pad_lo, ox = dx - p.pad_lo;
-                const int qy = (oy < 0) ? -((1 - oy) >> 1) : (oy >> 1);
-                const int qx = (ox < 0) ? -((1 - ox) >> 1) : (ox >> 1);
-                const int py = oy - 2 * qy, px = ox - 2 * qx;
-                cb = px * p.cin_ld + cb * BK;               // parity-split map: channel coordinate carries the x parity
-                ax = x0 + qx; ay = y0 + qy; a5 = py;
-              }
-            }
-            if constexpr (PAIR) {
-              const uint32_t fb = mapa_u32(smem_u32(&full_bar[stage]), 0);
-              if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-              if (p.mode == MODE_LINEAR) tma_load_2d_2sm(dst_a, &tmA, fb, kb * BK, m_blk * BM);
-              else if (p.mode == MODE_CONV_S1) tma_load_4d_2sm(dst_a, &tmA, fb, cb * BK, ax, ay, n0);
-              else tma_load_5d_2sm(dst_a, &tmA, fb, cb, ax, a5, ay, n0);
-              tma_load_2d_2sm(dst_b, &tmB, fb, kb * BK, n_blk * BN + (int)rank * (BN / 2));
-            } else {
-              mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-              if (p.mode == MODE_LINEAR) tma_load_2d(dst_a, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
-              else if (p.mode == MODE_CONV_S1) tma_load_4d(dst_a, &tmA, &full_bar[stage], cb * BK, ax, ay, n0);
-              else tma_load_5d(dst_a, &tmA, &full_bar[stage], cb, ax, a5, ay, n0);
-              tma_load_2d(dst_b, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (one elected lane issues)
-    if (!PAIR || rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(PAIR ? 2 * BM : BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        // one elected lane walks the whole k loop of the tile (waits included): a per-k-block elect region costs
-        // ~70 issue slots of descriptor / uniform-register setup, more than the MMAs of a narrow tile take
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int n_blk, m_blk;
+      tile_mn(p, tile, m_blk, n_blk);
+      int n0 = 0, y0 = 0, x0 = 0;
+      if (p.mode != MODE_LINEAR) decode_conv_tile(p, m_blk, n0, y0, x0);
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
         if (elect_one()) {
-          int s = stage;
-          uint32_t ph = phase;
-          const uint64_t da0 = umma_desc_k_sw128(smem_u32(smem_a));
-          const uint64_t db0 = umma_desc_k_sw128(smem_u32(smem_b));
-          for (int kb = 0; kb < p.num_kb; ++kb) {
-            mbar_wait(&full_bar[s], ph);
-            tc_fence_after();
-            const uint64_t da = da0 + (uint64_t)(s * (A_STAGE_BYTES >> 4));
-            const uint64_t db = db0 + (uint64_t)(s * (Cfg::B_STAGE_BYTES >> 4));
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              // +32 bytes (2 x 16 B units) per UMMA_K=16 step inside the 128 B swizzle row
-              if constexpr (PAIR) umma_bf16_ss_2cta(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-              else umma_bf16_ss(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
+          void* dst_a = smem_a + stage * A_STAGE_BYTES;
+          void* dst_b = smem_b + stage * Cfg::B_STAGE_BYTES;
+          int cb = 0, ax = 0, ay = 0, a5 = 0;            // conv: channel coordinate, x, y (, parity) of this k-block's tap
+          if (p.mode != MODE_LINEAR) {
+            const int tap = kb / p.cin_blocks;
+            cb = kb - tap * p.cin_blocks;
+            const int dy = tap / p.ksize;
+            const int dx = tap - dy * p.ksize;
+            if (p.mode == MODE_CONV_S1) {
+              ax = x0 + dx - p.pad_x; ay = y0 + dy - p.pad_y;
+            } else {
+              const int oy = dy - p.pad_lo, ox = dx - p.pad_lo;
+              const int qy = (oy < 0) ? -((1 - oy) >> 1) : (oy >> 1);
+              const int qx = (ox < 0) ? -((1 - ox) >> 1) : (ox >> 1);
+              const int py = oy - 2 * qy, px = ox - 2 * qx;
+              cb = px * p.cin_ld + cb * BK;               // parity-split map: channel coordinate carries the x parity
+              ax = x0 + qx; ay = y0 + qy; a5 = py;
             }
-            if constexpr (PAIR) umma_commit_2cta(&empty_bar[s]);   // frees the stage in both CTAs when the MMAs retire
-            else umma_commit(&empty_bar[s]);
-            if (++s == STAGES) { s = 0; ph ^= 1; }
           }
-          if constexpr (PAIR) umma_commit_2cta(&tmem_full[acc]);
-          else umma_commit(&tmem_full[acc]);
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+          if (p.mode == MODE_LINEAR) tma_load_2d(dst_a, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
+          else if (p.mode == MODE_CONV_S1) tma_load_4d(dst_a, &tmA, &full_bar[stage], cb * BK, ax, ay, n0);
+          else tma_load_5d(dst_a, &tmA, &full_bar[stage], cb, ax, a5, ay, n0);
+          tma_load_2d(dst_b, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
         }
         __syncwarp();
-        const int ns = stage + p.num_kb;
-        phase ^= (ns / STAGES) & 1;
-        stage = ns % STAGES;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp < 2 + EPI_WARPS) {
-    // ------------------------------------------------------------------ epilogue (warps 2..9)
-    EpiCtx ctx{staging, tmem_full, tmem_empty, res_bar, slot_ready, tmem_base, PAIR ? mapa_u32(smem_u32(tmem_empty), 0) : 0u};
-    epilogue_loop<BN>(p, ctx, warp, lane, num_tiles);
-  } else {
+  } else if (warp < EPI_WARPS) {
+    // ------------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
+    const EpiCtx ctx{staging, xch, res_bar, slot_ready};
+    const int wg = warp >> 2;
+    const uint32_t a_rows = smem_u32(smem_a) + wg * 64 * 128;        // this warpgroup's 64 rows of every A stage
+    const uint32_t b_base = smem_u32(smem_b);
+    int stage = 0;
+    uint32_t phase = 0;
+    int k = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      float acc[BN / 2];
+      int prev = -1;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t da = wgmma_desc_k_sw128(a_rows + stage * A_STAGE_BYTES);
+        const uint64_t db = wgmma_desc_k_sw128(b_base + stage * Cfg::B_STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk)           // +32 bytes (2 x 16 B units) per K = 16 step inside the 128 B row
+          wgmma_bf16<BN>(acc, da + 2 * kk, db + 2 * kk, (kb | kk) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();                               // the previous k-block's MMAs have retired: free its stage
+        if (prev >= 0) release_stage(&empty_bar[prev], lane);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      release_stage(&empty_bar[prev], lane);
+      epilogue_tile<BN>(p, ctx, warp, lane, tile, k, acc);
+    }
+  } else if (warp == DMA_WARP) {
     // ------------------------------------------------------------------ epilogue DMA warp
-    EpiCtx ctx{staging, tmem_full, tmem_empty, res_bar, slot_ready, tmem_base};
+    const EpiCtx ctx{staging, xch, res_bar, slot_ready};
     epilogue_dma_loop<BN>(p, ctx, tmO, tmR, tmX, lane, num_tiles);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (PAIR) cluster_sync_all();              // neither CTA retires while the peer may still signal it
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_2cta<Cfg::TMEM_COLS>(tmem_base);
-    else tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -734,10 +674,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // 3x3 stride-1 convolution for narrow outputs (Cout <= 128), where the plain implicit GEMM is bound by
 // L2 -> SM traffic (every tap re-reads its 128x64 A tile: 9x input traffic).  Here the 128-pixel tile is a
 // 16-row x 8-pixel patch and ONE (16+2) x (8+2) halo slab per 64-channel block serves all nine taps: tap (dy,dx)
-// is the same slab viewed from row offset dy*10+dx.  This relies on a property of the sm_100 UMMA shared-memory
-// descriptor measured with tools/probe/umma_shift_probe.cu: with SWIZZLE_128B the XOR phase is taken from the
-// absolute smem address, so a K-major operand may start at ANY 128-byte row of a TMA-written slab (base_offset 0)
-// and its 8-row groups may be any constant stride apart (SBO = slab pitch 1280 B, one image row of 10 pixels).
+// is the same slab viewed from row offset dy*10+dx.  The wgmma descriptor takes the SWIZZLE_128B XOR phase from the
+// absolute smem address, as TMA does when it writes the slab, so a K-major operand may start at ANY 128-byte row of
+// the slab and its 8-row groups may be any constant stride apart (SBO = slab pitch 1280 B, one image row of 10 pixels).
 // A traffic drops from 9 to 1.4 tile-loads per channel block; weights stream through their own ring, or stay
 // resident for the whole CTA when all nine taps fit (Cin = 64, Cout <= 64).
 constexpr int HALO_TW = 8, HALO_TH = 16;
@@ -745,23 +684,13 @@ constexpr int HALO_PITCH = (HALO_TW + 2) * 128;                     // bytes bet
 constexpr int HALO_A_BYTES = (HALO_TH + 2) * HALO_PITCH;            // 23040
 constexpr int HALO_A_STRIDE = ((HALO_A_BYTES + 1023) / 1024) * 1024; // 23552: keep every slab 1024-aligned
 
-__device__ __forceinline__ uint64_t umma_desc_k_sw128_sbo(uint32_t saddr, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
 template <int BN>
 struct HaloCfg {
   static constexpr int B_BYTES = BN * 128;
-  static constexpr int A_STAGES = (BN == 64) ? 3 : 2;
-  static constexpr int B_STAGES = (BN == 64) ? 9 : 6;
+  static constexpr int A_STAGES = 2;
+  static constexpr int B_STAGES = (BN == 64) ? 9 : 5;
   static constexpr int STAGING_BYTES = NUM_SLOTS * PANEL_BYTES;
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : 256;
-  static constexpr int SMEM_BYTES = A_STAGES * HALO_A_STRIDE + B_STAGES * B_BYTES + STAGING_BYTES + 2 * BN * 4 + 1024 + 512 + 1024;
+  static constexpr int SMEM_BYTES = A_STAGES * HALO_A_STRIDE + B_STAGES * B_BYTES + STAGING_BYTES + XCH_BYTES + 512 + 1024;
   static_assert(SMEM_BYTES <= 232448, "halo conv smem budget");
 };
 
@@ -779,50 +708,38 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + AS * HALO_A_STRIDE;
   uint8_t* staging = smem_b + BS * Cfg::B_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
+  float* xch = reinterpret_cast<float*>(staging + Cfg::STAGING_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES + XCH_BYTES);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + AS;
   uint64_t* b_full = bars + 2 * AS;
   uint64_t* b_empty = bars + 2 * AS + BS;
-  uint64_t* tmem_full = bars + 2 * AS + 2 * BS;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint64_t* res_bar = tmem_full + 4;                                   // [NUM_SLOTS]
-  uint64_t* slot_ready = tmem_full + 8;                                // [NUM_SLOTS]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 12);
-  uint64_t* a_ready = tmem_full + 14;                                  // [AS] GN variant: slab normalised in place
+  uint64_t* res_bar = bars + 2 * AS + 2 * BS;                          // [NUM_SLOTS]
+  uint64_t* slot_ready = res_bar + NUM_SLOTS;                          // [NUM_SLOTS]
+  uint64_t* a_ready = slot_ready + NUM_SLOTS;                          // [AS] GN variant: slab normalised in place
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = p.m_tiles * p.n_tiles;
   const int cin_pad = p.cin_blocks * BK;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER_WARP && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (p.fast_epi) tma_prefetch_desc(&tmO);
     if (p.has_res_map) tma_prefetch_desc(&tmR);
     if (p.fast_epi && p.epi_mode == PGT_EPI_SFT) tma_prefetch_desc(&tmX);
-    for (int i = 0; i < AS; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); mbar_init(&a_ready[i], HALO_GN_THREADS); }
-    for (int i = 0; i < BS; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], EPI_WARPS * 32);
-      mbar_init(&res_bar[2 * i], 1);
-      mbar_init(&res_bar[2 * i + 1], 1);
-      mbar_init(&slot_ready[2 * i], EPI_WARPS * 32);
-      mbar_init(&slot_ready[2 * i + 1], EPI_WARPS * 32);
+    for (int i = 0; i < AS; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], EPI_WARPS); mbar_init(&a_ready[i], HALO_GN_THREADS); }
+    for (int i = 0; i < BS; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], EPI_WARPS); }
+    for (int i = 0; i < NUM_SLOTS; ++i) {
+      mbar_init(&res_bar[i], 1);
+      mbar_init(&slot_ready[i], EPI_WARPS * 32);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-    tc_fence_before();
-  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ------------------------------------------------------------------ TMA producer
     int as = 0, bs = 0;
     uint32_t aph = 0, bph = 0;
@@ -832,10 +749,9 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       int n0, y0, x0;
       decode_conv_tile(p, m_blk, n0, y0, x0);
       {
-        // pull the slab (and residual panels) of the tile PREFETCH_TILES rounds ahead into L2: three slabs in flight per
-        // SM do not cover the HBM latency of the 512^2 / 256^2 layers
+        // pull the slab (and residual panels) of the tile PREFETCH_TILES rounds ahead into L2
         const int pt = tile + PREFETCH_TILES * (int)gridDim.x;
-        if (BN == 64 && pt < num_tiles && elect_one()) {      // measured: helps the 64-wide layers only
+        if (BN == 64 && pt < num_tiles && elect_one()) {
           int pn0, py0, px0;
           decode_conv_tile(p, pt / p.n_tiles, pn0, py0, px0);
           for (int cb = 0; cb < p.cin_blocks; ++cb) tma_prefetch_4d(&tmA, cb * BK, px0 - 1, py0 - 1, pn0);
@@ -870,97 +786,66 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc_bf16(BM, BN);
+  } else if (warp < EPI_WARPS) {
+    // ------------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
+    // Warpgroup h multiplies tile rows [64h, 64h + 64) = image rows [8h, 8h + 8) of the patch: its view of a tap starts
+    // 8 slab rows further down.
+    const EpiCtx ctx{staging, xch, res_bar, slot_ready};
+    const int wg = warp >> 2;
+    const uint32_t a_view = smem_u32(smem_a) + wg * 8 * HALO_PITCH;
+    const uint32_t b_base = smem_u32(smem_b);
     int as = 0, bs = 0;
     uint32_t aph = 0, bph = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      // one elected lane issues the whole tile (nine taps x four k-steps per channel block, tap offsets are
-      // compile-time constants): per-tap elect regions cost more issue slots than the MMAs of a 64-wide tile take
-      if (elect_one()) {
-        int a = as, b = bs;
-        uint32_t ap = aph, bp = bph;
-        const uint64_t da_base = umma_desc_k_sw128_sbo(smem_u32(smem_a), HALO_PITCH);
-        const uint64_t db_base = umma_desc_k_sw128(smem_u32(smem_b));
-        for (int cb = 0; cb < p.cin_blocks; ++cb) {
-          mbar_wait(GN ? &a_ready[a] : &a_full[a], ap);
-          const uint64_t da0 = da_base + (uint64_t)(a * (HALO_A_STRIDE >> 4));
-          if (p.b_resident) {
-            if (it == 0) {
-              for (int t = 0; t < p.ntaps; ++t) mbar_wait(&b_full[cb * p.ntaps + t], 0);
-            }
-            tc_fence_after();
-            if (p.ntaps == 9) {
-#pragma unroll
-              for (int t = 0; t < 9; ++t) {
-                const uint64_t da = da0 + (uint64_t)(((t / 3) * (HALO_TW + 2) + (t % 3)) * 8);
-                const uint64_t db = db_base + (uint64_t)((cb * 9 + t) * (Cfg::B_BYTES >> 4));
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) umma_bf16_ss(d_tmem, da + 2 * k, db + 2 * k, idesc, (cb | t | k) != 0 ? 1u : 0u);
-              }
-            } else {
-              for (int t = 0; t < p.ntaps; ++t) {
-                const int dy = t / p.tap_kw, dx = t - dy * p.tap_kw;
-                const uint64_t da = da0 + (uint64_t)(((dy + p.tap_oy) * (HALO_TW + 2) + dx + p.tap_ox) * 8);
-                const uint64_t db = db_base + (uint64_t)((cb * p.ntaps + t) * (Cfg::B_BYTES >> 4));
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) umma_bf16_ss(d_tmem, da + 2 * k, db + 2 * k, idesc, (cb | t | k) != 0 ? 1u : 0u);
-              }
-            }
-          } else if (p.ntaps == 9) {
-#pragma unroll
-            for (int t = 0; t < 9; ++t) {
-              mbar_wait(&b_full[b], bp);
-              tc_fence_after();
-              const uint64_t da = da0 + (uint64_t)(((t / 3) * (HALO_TW + 2) + (t % 3)) * 8);
-              const uint64_t db = db_base + (uint64_t)(b * (Cfg::B_BYTES >> 4));
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) umma_bf16_ss(d_tmem, da + 2 * k, db + 2 * k, idesc, (cb | t | k) != 0 ? 1u : 0u);
-              umma_commit(&b_empty[b]);
-              if (++b == BS) { b = 0; bp ^= 1; }
-            }
-          } else {
-            for (int t = 0; t < p.ntaps; ++t) {
-              mbar_wait(&b_full[b], bp);
-              tc_fence_after();
-              const int dy = t / p.tap_kw, dx = t - dy * p.tap_kw;
-              const uint64_t da = da0 + (uint64_t)(((dy + p.tap_oy) * (HALO_TW + 2) + dx + p.tap_ox) * 8);
-              const uint64_t db = db_base + (uint64_t)(b * (Cfg::B_BYTES >> 4));
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) umma_bf16_ss(d_tmem, da + 2 * k, db + 2 * k, idesc, (cb | t | k) != 0 ? 1u : 0u);
-              umma_commit(&b_empty[b]);
-              if (++b == BS) { b = 0; bp ^= 1; }
-            }
+    int k = 0;
+    bool first = true;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      float acc[BN / 2];
+      for (int cb = 0; cb < p.cin_blocks; ++cb) {
+        mbar_wait(GN ? &a_ready[as] : &a_full[as], aph);
+        const uint64_t da0 = wgmma_desc_k_sw128(a_view + as * HALO_A_STRIDE, HALO_PITCH);
+        auto tap_desc = [&](int t) -> uint64_t {       // slab row offset of tap t, in 16-byte descriptor units
+          const int dy = t / p.tap_kw, dx = t - dy * p.tap_kw;
+          return da0 + (uint64_t)(((dy + p.tap_oy) * (HALO_TW + 2) + dx + p.tap_ox) * 8);
+        };
+        if (p.b_resident) {
+          if (first) {
+            for (int t = 0; t < p.ntaps * p.cin_blocks; ++t) mbar_wait(&b_full[t], 0);
+            first = false;
           }
-          umma_commit(&a_empty[a]);
-          if (++a == AS) { a = 0; ap ^= 1; }
+          wgmma_fence();
+          for (int t = 0; t < p.ntaps; ++t) {
+            const uint64_t da = tap_desc(t);
+            const uint64_t db = wgmma_desc_k_sw128(b_base + (cb * p.ntaps + t) * Cfg::B_BYTES);
+#pragma unroll
+            for (int kk = 0; kk < BK / 16; ++kk) wgmma_bf16<BN>(acc, da + 2 * kk, db + 2 * kk, (cb | t | kk) != 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+        } else {
+          int prev = -1;
+          for (int t = 0; t < p.ntaps; ++t) {
+            mbar_wait(&b_full[bs], bph);
+            const uint64_t da = tap_desc(t);
+            const uint64_t db = wgmma_desc_k_sw128(b_base + bs * Cfg::B_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < BK / 16; ++kk) wgmma_bf16<BN>(acc, da + 2 * kk, db + 2 * kk, (cb | t | kk) != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();                             // the previous tap's weight stage is free
+            if (prev >= 0) release_stage(&b_empty[prev], lane);
+            prev = bs;
+            if (++bs == BS) { bs = 0; bph ^= 1; }
+          }
+          wgmma_wait<0>();
+          release_stage(&b_empty[prev], lane);
         }
-        umma_commit(&tmem_full[acc]);
+        release_stage(&a_empty[as], lane);
+        if (++as == AS) { as = 0; aph ^= 1; }
       }
-      __syncwarp();
-      {
-        const int na = as + p.cin_blocks;
-        aph ^= (na / AS) & 1;
-        as = na % AS;
-        if (!p.b_resident) {
-          const int nb = bs + p.ntaps * p.cin_blocks;
-          bph ^= (nb / BS) & 1;
-          bs = nb % BS;
-        }
-      }
+      epilogue_tile<BN>(p, ctx, warp, lane, tile, k, acc);
     }
-  } else if (warp < 2 + EPI_WARPS) {
-    EpiCtx ctx{staging, tmem_full, tmem_empty, res_bar, slot_ready, tmem_base};
-    epilogue_loop<BN>(p, ctx, warp, lane, num_tiles);
-  } else if (warp == 2 + EPI_WARPS) {
-    EpiCtx ctx{staging, tmem_full, tmem_empty, res_bar, slot_ready, tmem_base};
+  } else if (warp == DMA_WARP) {
+    const EpiCtx ctx{staging, xch, res_bar, slot_ready};
     epilogue_dma_loop<BN>(p, ctx, tmO, tmR, tmX, lane, num_tiles);
   } else if (GN) {
     // ------------------------------------------------------------------ GroupNorm + SiLU of the input, in the slab
@@ -1018,227 +903,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (++as == AS) { as = 0; aph ^= 1; }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-}
-
-// ------------------------------------------------------------------------------------------- halo conv on CTA pairs
-// The narrow halo convs are bound by shared-memory bandwidth, not by the tensor pipe: with N <= 128 every UMMA reads as
-// many operand bytes from smem as it has cycles to compute, and the streamed weight tiles are written there as well.
-// cta_group::2 halves the weight side: the two CTAs of a cluster take two neighbouring 128-pixel tiles (M = 256), each
-// loads and holds only HALF of every weight tile (N/2 rows), and the leader's single thread issues MMAs that read A
-// from both SMs and the two weight halves; each CTA's TMEM receives its own 128 x N accumulator and its epilogue runs
-// unchanged.  Both CTAs' TMA loads complete on the LEADER's full barriers; the leader's tcgen05.commit multicasts the
-// empty / accumulator-ready arrivals to both CTAs; the peer's epilogue releases the accumulator with remote arrives.
-template <int BN>
-struct Halo2Cfg {
-  static constexpr int B_BYTES = (BN / 2) * 128;                        // this CTA's half of one tap's weight tile
-  static constexpr int A_STAGES = 4;
-  static constexpr int B_STAGES = (BN == 64) ? 9 : 8;
-  static constexpr int STAGING_BYTES = NUM_SLOTS * PANEL_BYTES;
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : 256;
-  static constexpr int SMEM_BYTES = A_STAGES * HALO_A_STRIDE + B_STAGES * B_BYTES + STAGING_BYTES + 2 * BN * 4 + 1024 + 512;
-  static_assert(SMEM_BYTES <= 232448, "halo2 conv smem budget");
-};
-
-template <int BN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-conv_halo2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
-                  const __grid_constant__ CUtensorMap tmX, const GemmParams p) {
-  using Cfg = Halo2Cfg<BN>;
-  constexpr int AS = Cfg::A_STAGES, BS = Cfg::B_STAGES;
-  extern __shared__ __align__(1024) uint8_t smem[];
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + AS * HALO_A_STRIDE;
-  uint8_t* staging = smem_b + BS * Cfg::B_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
-  uint64_t* a_full = bars;                   // leader's are the live ones (both CTAs' loads land there)
-  uint64_t* a_empty = bars + AS;             // per CTA, fed by the leader's multicast commit
-  uint64_t* b_full = bars + 2 * AS;
-  uint64_t* b_empty = bars + 2 * AS + BS;
-  uint64_t* tmem_full = bars + 2 * AS + 2 * BS;        // per CTA (multicast commit)
-  uint64_t* tmem_empty = tmem_full + 2;                // leader's: 2 x 256 epilogue threads
-  uint64_t* res_bar = tmem_full + 4;
-  uint64_t* slot_ready = tmem_full + 8;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 12);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int num_tiles = p.m_tiles;                     // n_tiles == 1, m_tiles even (host checks)
-  const int cin_pad = p.cin_blocks * BK;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    if (p.fast_epi) tma_prefetch_desc(&tmO);
-    if (p.has_res_map) tma_prefetch_desc(&tmR);
-    if (p.fast_epi && p.epi_mode == PGT_EPI_SFT) tma_prefetch_desc(&tmX);
-    for (int i = 0; i < AS; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < BS; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 2 * EPI_WARPS);            // one arrive per epilogue warp of either CTA
-      mbar_init(&res_bar[2 * i], 1);
-      mbar_init(&res_bar[2 * i + 1], 1);
-      mbar_init(&slot_ready[2 * i], EPI_WARPS * 32);
-      mbar_init(&slot_ready[2 * i + 1], EPI_WARPS * 32);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc_2cta<Cfg::TMEM_COLS>(tmem_ptr);
-    tc_fence_before();
-  }
-  __syncthreads();
-  cluster_sync_all();                                  // the peer's barriers exist before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (both CTAs; leader arms the barriers)
-    int as = 0, bs = 0;
-    uint32_t aph = 0, bph = 0;
-    const uint32_t a_full0 = mapa_u32(smem_u32(a_full), 0), b_full0 = mapa_u32(smem_u32(b_full), 0);
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int n0, y0, x0;
-      decode_conv_tile(p, tile, n0, y0, x0);
-      {
-        const int pt = tile + PREFETCH_TILES * (int)gridDim.x;
-        if (BN == 64 && pt < num_tiles && elect_one()) {
-          int pn0, py0, px0;
-          decode_conv_tile(p, pt, pn0, py0, px0);
-          for (int cb = 0; cb < p.cin_blocks; ++cb) tma_prefetch_4d(&tmA, cb * BK, px0 - 1, py0 - 1, pn0);
-          if (p.has_res_map) {
-            const int rw = p.out_dtype == PGT_BF16 ? 64 : 32;
-            for (int c = 0; c < BN && c < p.N; c += rw) {
-              tma_prefetch_4d(&tmR, c, px0, py0, pn0);
-              if (p.epi_mode == PGT_EPI_SFT) tma_prefetch_4d(&tmX, c, px0, py0, pn0);
-            }
-          }
-        }
-        __syncwarp();
-      }
-      for (int cb = 0; cb < p.cin_blocks; ++cb) {
-        mbar_wait(&a_empty[as], aph ^ 1);
-        if (elect_one()) {
-          if (rank == 0) mbar_arrive_expect_tx(&a_full[as], 2 * HALO_A_BYTES);
-          tma_load_4d_2sm(smem_a + as * HALO_A_STRIDE, &tmA, a_full0 + as * 8, cb * BK, x0 - 1, y0 - 1, n0);
-        }
-        __syncwarp();
-        if (++as == AS) { as = 0; aph ^= 1; }
-        if (p.b_resident && tile != (int)blockIdx.x) continue;   // this CTA's weight halves stay resident in the ring
-        for (int t = 0; t < p.ntaps; ++t) {
-          mbar_wait(&b_empty[bs], bph ^ 1);
-          if (elect_one()) {
-            if (rank == 0) mbar_arrive_expect_tx(&b_full[bs], 2 * Cfg::B_BYTES);
-            tma_load_2d_2sm(smem_b + bs * Cfg::B_BYTES, &tmB, b_full0 + bs * 8, t * cin_pad + cb * BK, (int)rank * (BN / 2));
-          }
-          __syncwarp();
-          if (++bs == BS) { bs = 0; bph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer: the pair leader's elected lane only
-    if (rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(2 * BM, BN);
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        if (elect_one()) {
-          int a = as, b = bs;
-          uint32_t ap = aph, bp = bph;
-          const uint64_t da_base = umma_desc_k_sw128_sbo(smem_u32(smem_a), HALO_PITCH);
-          const uint64_t db_base = umma_desc_k_sw128(smem_u32(smem_b));
-          for (int cb = 0; cb < p.cin_blocks; ++cb) {
-            mbar_wait(&a_full[a], ap);
-            const uint64_t da0 = da_base + (uint64_t)(a * (HALO_A_STRIDE >> 4));
-            if (p.ntaps == 9) {
-#pragma unroll
-              for (int t = 0; t < 9; ++t) {
-                int slot = b;
-                if (p.b_resident) {
-                  slot = cb * 9 + t;
-                  if (it == 0) mbar_wait(&b_full[slot], 0);
-                } else {
-                  mbar_wait(&b_full[b], bp);
-                }
-                tc_fence_after();
-                const uint64_t da = da0 + (uint64_t)(((t / 3) * (HALO_TW + 2) + (t % 3)) * 8);
-                const uint64_t db = db_base + (uint64_t)(slot * (Cfg::B_BYTES >> 4));
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) umma_bf16_ss_2cta(d_tmem, da + 2 * k, db + 2 * k, idesc, (cb | t | k) != 0 ? 1u : 0u);
-                if (!p.b_resident) {
-                  umma_commit_2cta(&b_empty[b]);
-                  if (++b == BS) { b = 0; bp ^= 1; }
-                }
-              }
-            } else {
-              for (int t = 0; t < p.ntaps; ++t) {
-                int slot = b;
-                if (p.b_resident) {
-                  slot = cb * p.ntaps + t;
-                  if (it == 0) mbar_wait(&b_full[slot], 0);
-                } else {
-                  mbar_wait(&b_full[b], bp);
-                }
-                tc_fence_after();
-                const int dy = t / p.tap_kw, dx = t - dy * p.tap_kw;
-                const uint64_t da = da0 + (uint64_t)(((dy + p.tap_oy) * (HALO_TW + 2) + dx + p.tap_ox) * 8);
-                const uint64_t db = db_base + (uint64_t)(slot * (Cfg::B_BYTES >> 4));
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) umma_bf16_ss_2cta(d_tmem, da + 2 * k, db + 2 * k, idesc, (cb | t | k) != 0 ? 1u : 0u);
-                if (!p.b_resident) {
-                  umma_commit_2cta(&b_empty[b]);
-                  if (++b == BS) { b = 0; bp ^= 1; }
-                }
-              }
-            }
-            umma_commit_2cta(&a_empty[a]);
-            if (++a == AS) { a = 0; ap ^= 1; }
-          }
-          umma_commit_2cta(&tmem_full[acc]);
-        }
-        __syncwarp();
-        const int na = as + p.cin_blocks;
-        aph ^= (na / AS) & 1;
-        as = na % AS;
-        if (!p.b_resident) {
-          const int nb = bs + p.ntaps * p.cin_blocks;
-          bph ^= (nb / BS) & 1;
-          bs = nb % BS;
-        }
-      }
-    }
-  } else if (warp < 2 + EPI_WARPS) {
-    EpiCtx ctx{staging, tmem_full, tmem_empty, res_bar, slot_ready, tmem_base, mapa_u32(smem_u32(tmem_empty), 0)};
-    epilogue_loop<BN>(p, ctx, warp, lane, num_tiles);
-  } else {
-    EpiCtx ctx{staging, tmem_full, tmem_empty, res_bar, slot_ready, tmem_base, 0};
-    epilogue_dma_loop<BN>(p, ctx, tmO, tmR, tmX, lane, num_tiles);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                  // neither CTA retires while the peer may still signal it
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2cta<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -1318,40 +982,28 @@ static int encode_weight_map(CUtensorMap* tmB, const void* W, int ldw, int K, in
   return encode_map(tmB, W, 2, dims, str, box);
 }
 
-template <int BN, bool PAIR>
+template <int BN>
 static int launch_gemm(const CUtensorMap& tmA, const void* W, int ldw, GemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, PAIR>;
+  using Cfg = GemmCfg<BN>;
   static_assert(Cfg::STAGES >= 3, "pipeline too shallow");
   CUtensorMap tmB, tmO, tmR, tmX;
-  int rc = encode_weight_map(&tmB, W, ldw, p.K, p.N, PAIR ? BN / 2 : BN);
+  int rc = encode_weight_map(&tmB, W, ldw, p.K, p.N, BN);
   if (rc != PGT_OK) return rc;
   rc = setup_epilogue_maps(p, tmA, tmO, tmR, tmX);
   if (rc != PGT_OK) return rc;
   p.n_tiles = ceil_div(p.N, BN);
-  p.pair_map = PAIR ? 1 : 0;
   static PerDeviceOnce once;
-  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(gemm_tc_kernel<BN, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); }));
+  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); }));
   const int tiles = p.m_tiles * p.n_tiles;
-  int grid = tiles < num_sms() ? tiles : num_sms();
-  if (PAIR) grid &= ~1;
+  const int grid = tiles < num_sms() ? tiles : num_sms();
   {
     char desc[96];
     if (prof_enabled()) {
-      if (p.mode == MODE_LINEAR) snprintf(desc, sizeof(desc), "linear%s M%d N%d K%d BN%d e%d", PAIR ? " x2cta" : "", p.M, p.N, p.K, BN, p.fast_epi);
-      else snprintf(desc, sizeof(desc), "conv%d%s s%d F%d H%d W%d K%d N%d BN%d t%dx%dx%d e%d", p.ksize, PAIR ? " x2cta" : "", p.mode, p.F, p.H, p.W, p.K, p.N, BN, p.tn, p.th, p.tw, p.fast_epi);
+      if (p.mode == MODE_LINEAR) snprintf(desc, sizeof(desc), "linear M%d N%d K%d BN%d e%d", p.M, p.N, p.K, BN, p.fast_epi);
+      else snprintf(desc, sizeof(desc), "conv%d s%d F%d H%d W%d K%d N%d BN%d t%dx%dx%d e%d", p.ksize, p.mode, p.F, p.H, p.W, p.K, p.N, BN, p.tn, p.th, p.tw, p.fast_epi);
     }
     ProfScope ps(PGT_PROF_GEMM, p.flops, stream, desc);
-    if (PAIR) {
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(grid); cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES; cfg.stream = stream;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr; cfg.numAttrs = 1;
-      PGT_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, PAIR>, tmA, tmB, tmO, tmR, tmX, p));
-    } else {
-      gemm_tc_kernel<BN, PAIR><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
-    }
+    gemm_tc_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
   }
   PGT_LAUNCH_OK();
   return PGT_OK;
@@ -1384,53 +1036,11 @@ static int launch_halo(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
   return PGT_OK;
 }
 
-template <int BN>
-static int launch_halo2(const CUtensorMap& tmA, const void* W, int ldw, GemmParams& p, cudaStream_t stream) {
-  using Cfg = Halo2Cfg<BN>;
-  CUtensorMap tmB, tmO, tmR, tmX;
-  int rc = encode_weight_map(&tmB, W, ldw, p.K, p.N, BN / 2);            // each CTA loads half of the N rows
-  if (rc != PGT_OK) return rc;
-  rc = setup_epilogue_maps(p, tmA, tmO, tmR, tmX);
-  if (rc != PGT_OK) return rc;
-  p.n_tiles = 1;
-  p.b_resident = (p.ntaps * p.cin_blocks <= Cfg::B_STAGES) ? 1 : 0;
-  static PerDeviceOnce once;
-  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(conv_halo2_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); }));
-  int grid = p.m_tiles < num_sms() ? p.m_tiles : num_sms();
-  grid &= ~1;                                                            // whole CTA pairs
-  {
-    char desc[96];
-    if (prof_enabled())
-      snprintf(desc, sizeof(desc), "halo%d x2cta F%d H%d W%d K%d N%d BN%d e%d r%d", p.tap_kw, p.F, p.H, p.W, p.K, p.N, BN,
-               p.fast_epi, p.b_resident);
-    ProfScope ps(PGT_PROF_GEMM, p.flops, stream, desc);
-    conv_halo2_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
-  }
-  PGT_LAUNCH_OK();
-  return PGT_OK;
-}
-
-static int pick_bn(int N, int m_tiles) {
-  if (N <= 64) return 64;
-  if (N <= 128) return 128;
-  // wide N: prefer 256-wide tiles when they still fill the machine
-  const int t256 = m_tiles * ceil_div(N, 256);
-  return (t256 >= num_sms()) ? 256 : 128;
-}
-
+// Tiles are at most 128 wide: a warpgroup then holds 64 fp32 accumulators per thread, and a 64 x 128 x 16 wgmma
+// reads 96 operand bytes per cycle of tensor work, inside the shared-memory bandwidth.
 static int dispatch_gemm(const CUtensorMap& tmA, const void* W, int ldw, GemmParams& p, cudaStream_t stream) {
-  static const bool no_pair = getenv("PGT_NO_2CTA") != nullptr;
-  switch (pick_bn(p.N, p.m_tiles)) {
-    case 64: return launch_gemm<64, false>(tmA, W, ldw, p, stream);
-    case 128: return launch_gemm<128, false>(tmA, W, ldw, p, stream);
-    default:
-      // 256-wide conv tiles on CTA pairs: each SM then reads half of every weight tile (UMMA operand traffic 8 instead
-      // of 12 KB per instruction).  Measured: +3 % on the K >= 1024 convs; the short-K linears lose 10 % to the pair's
-      // lock-step and stay on single CTAs.
-      if (!no_pair && p.mode != MODE_LINEAR && p.num_kb >= 16 && (p.m_tiles % 2) == 0 && p.m_tiles >= 2)
-        return launch_gemm<256, true>(tmA, W, ldw, p, stream);
-      return launch_gemm<256, false>(tmA, W, ldw, p, stream);
-  }
+  if (p.N <= 64) return launch_gemm<64>(tmA, W, ldw, p, stream);
+  return launch_gemm<128>(tmA, W, ldw, p, stream);
 }
 
 static int fill_epilogue(GemmParams& p, const pgt_epilogue* ep) {
@@ -1567,13 +1177,6 @@ static int conv_impl(const void* x, int F, int Hin, int Win, int Cin, int ldx, c
         p.gn_c = Cin;
         return Cout <= 64 ? launch_halo<64, true>(tmA, Wp, ldw, p, st) : launch_halo<128, true>(tmA, Wp, ldw, p, st);
       }
-      static const bool no_pair = getenv("PGT_NO_2CTA") != nullptr;
-      // CTA pairs (whole pairs of tiles only).  Measured at 16 clips of 512^2: 128-wide 3x3 layers gain 5-8 % (their
-      // streamed weight tiles stop competing with the A views for smem bandwidth); 64-wide layers are bound by the A
-      // operand reads, which pairing does not reduce, and lose to the pair's lock-step — they stay on single CTAs.
-      static const bool pair64 = getenv("PGT_2CTA_N64") != nullptr;
-      if (!no_pair && (p.m_tiles % 2) == 0 && p.m_tiles >= 2 && p.out_layout == PGT_OUT_NHWC && (pair64 || (Cout > 64 && up_phase < 0)))
-        return Cout <= 64 ? launch_halo2<64>(tmA, Wp, ldw, p, st) : launch_halo2<128>(tmA, Wp, ldw, p, st);
       return Cout <= 64 ? launch_halo<64, false>(tmA, Wp, ldw, p, st) : launch_halo<128, false>(tmA, Wp, ldw, p, st);
     }
   } else {

@@ -1,26 +1,22 @@
 // Nearest-codebook L2 argmin (VQEmbedding.compute_distances + find_nearest_embedding, archs/tdcrqvae3_arch.py:99-126)
-// on tcgen05, exact by construction.
+// on wgmma, exact by construction.
 //
 //   argmin_k ||z - e_k||^2  =  argmin_k ( ||e_k||^2 - 2 z.e_k )        (||z||^2 is constant per token)
 //
 // Pass 0 (z_pack_kernel, HBM-bound): the fp32 z rows are read ONCE with 128-bit streaming loads and written back as bf16
 //   rows z~ together with (||z||^2, ||z - z~||^2) per token (needed for the certificate below).
-// Pass 1 (l2_argmin_pair_kernel, tensor cores): the scores  s~ = z~ . e~_k  of the bf16-rounded operands for all K codes on
-//   CTA PAIRS — M = 256 tokens per tcgen05.mma.cta_group::2, N-tile = 256 codes, k-block = 64:
-//   * each CTA keeps its 128 tokens' A tile (128 x E bf16) resident in shared memory and loads HALF of every codebook
-//     tile through its TMA ring, so one pass over the bf16 codebook (K x E x 2 B = 1 MB) serves 256 tokens: 4 KB of
-//     L2 -> SM traffic per token (a single-CTA sweep pulls 8 KB per token — 384 MB at T = 49 152 — and is bound by it);
-//   * persistent: a pair walks over its 256-token tiles; the A k-blocks of the next tile are loaded by their own producer
-//     warp (per-k-block barriers) as soon as the last N-tile of the current one has consumed them, and the codebook ring
-//     never drains;
-//   * two scan warpgroups alternate over the double-buffered 128 x 256 fp32 accumulator in TMEM: thread = token row,
-//     d~_k = ||e_k||^2 - 2 s~ for 32 codes at a time, BRANCH-FREE chunk minimum, and ONE test per chunk
-//     (chunk min <= running min + W); only then the chunk's codes within W of the (updated) running minimum are appended,
-//     with predicated stores, to the row's candidate list in shared memory.  The list is emptied whenever the minimum drops
-//     by more than W, so it is a superset of the final window {k : d~_k <= min d~ + W}.  (A test-and-branch per code costs
-//     ~46 clk of dependent latency each: measured 23-28 us per tile against 8.6 us of MMAs.)
-//   * merge (all 256 scan threads: each filters its own list against the row's global minimum) and exact resolution
-//     (below) of tile i run while the tensor pipe already works on tile i + 1.
+// Pass 1 (l2_argmin_tc_kernel, tensor cores): the scores  s~ = z~ . e~_k  of the bf16-rounded operands for all K codes,
+//   128 tokens per CTA, N-tile = 128 codes, k-block = 64:
+//   * the CTA keeps its 128 tokens' A tile (128 x E bf16) resident in shared memory and streams the codebook tiles
+//     through a TMA ring; persistent over 128-token tiles, the A k-blocks of the next tile are loaded by their own
+//     producer warp (per-k-block barriers) as soon as the last N-tile of the current one has consumed them;
+//   * two warpgroups, warpgroup h owning token rows [64h, 64h + 64): wgmma 64 x 128 x 16 into registers, then 32 codes at
+//     a time through a shared-memory exchange to two threads per token row (16 codes each): d~_k = ||e_k||^2 - 2 s~,
+//     BRANCH-FREE chunk minimum, and ONE test per chunk (chunk min <= running min + W); only then the chunk's codes within
+//     W of the (updated) running minimum are appended, with predicated stores, to the thread's candidate list in shared
+//     memory.  The list is emptied whenever the minimum drops by more than W, so it is a superset of the final window
+//     {k : d~_k <= min d~ + W}.  (A test-and-branch per code costs tens of cycles of dependent latency each.)
+//   * merge (all 256 threads: each filters its own list against the row's global minimum) and exact resolution (below).
 // Certificate: |d~_k - d_k| <= D := 2 (||z - z~|| max||e~|| + ||z|| max||e - e~||) + slack (Cauchy-Schwarz on the two
 //   rounding-error dot products + fp32 accumulation slack), hence the true argmin lies in {k : d~_k <= min d~ + 2D},
 //   W = 2D.  The window's members (usually ONE) are re-evaluated exactly — fp32 direct sums, whose relative error is
@@ -36,19 +32,23 @@
 
 namespace pgt {
 
-constexpr int LT_BM = 128;                       // tokens per CTA (256 per pair)
-constexpr int LT_BN = 256;                       // codes per N-tile
+constexpr int LT_BM = 128;                       // tokens per CTA
+constexpr int LT_BN = 128;                       // codes per N-tile
 constexpr int LT_BK = 64;                        // k-block (one 128-byte swizzled row)
 constexpr int LT_EMAX = 512;                     // A tile resident: 128 x 512 bf16 = 128 KB
 constexpr int LT_A_KB_BYTES = LT_BM * 128;       // 16 KB per k-block of A
 constexpr int LT_KBMAX = LT_EMAX / LT_BK;        // 8
-constexpr int LT_BST = (LT_BN / 2) * 128;        // codebook stage per CTA: 128 codes x 64 k = 16 KB
-constexpr int LT_NST = 3;                        // codebook ring depth
-constexpr int LT_THREADS = 11 * 32;              // warps: 0 codebook producer, 1 MMA issuer, 2..9 scan / resolve, 10 A producer
+constexpr int LT_BST = LT_BN * 128;              // codebook stage: 128 codes x 64 k = 16 KB
+constexpr int LT_NST = 2;                        // codebook ring depth
+constexpr int LT_THREADS = 10 * 32;              // warps: 0..7 MMA / scan / resolve, 8 codebook producer, 9 A producer
+constexpr int LT_SCH = 16;                       // codes per thread per exchange round
+constexpr int LT_XLD = 36;                       // exchange pitch (fp32): [2 warpgroups][64 rows][32 codes + pad]
 constexpr int LT_TOP = 16;                       // window members resolved in-kernel (more -> exhaustive kernel)
 constexpr int LT_LIST = 16;                      // candidate-list capacity per (token, warpgroup)
 constexpr int LT_XCH = 2 * LT_BM * LT_LIST * 8 /*lists*/ + 2 * LT_BM * 4 /*xmin*/ + LT_BM * LT_TOP * 4 /*mi*/ + 2 * LT_BM * 4 /*ncand, ovf*/;
-constexpr int LT_SMEM = LT_BM * LT_EMAX * 2 + LT_NST * LT_BST + LT_XCH + 512 /*barriers*/ + 1024 /*align*/;
+constexpr int LT_XACC = LT_BM * LT_XLD * 4;
+constexpr int LT_SMEM = LT_BM * LT_EMAX * 2 + LT_NST * LT_BST + LT_XCH + LT_XACC + 512 /*barriers*/ + 1024 /*align*/;
+static_assert(LT_SMEM <= 232448, "l2_argmin smem budget");
 
 __device__ __forceinline__ float4 ld_nc_f4(const float4* p) {       // streaming 128-bit load (read once, keep out of L1)
   float4 v;
@@ -142,54 +142,46 @@ z_pack_kernel(const float* __restrict__ z, int T, int E, __nv_bfloat16* __restri
 }
 
 // ------------------------------------------------------------------------------ scan / merge / exact resolution
-// Scan of one 128 x 256 accumulator buffer, thread = token row (see the header comment).  lst: this thread's candidate
-// list in shared memory (lst_s: its shared-window address), entry j 2 * LT_BM entries further (entry-major: the lanes of
-// a warp hit distinct banks).
-__device__ __forceinline__ void argmin_scan_ntile(uint32_t tacc, const float* __restrict__ norm_nt, int code0, float W,
-                                                  uint32_t lst_s, float& runmin, float& thr, int& cnt) {
+// Scan of LT_SCH consecutive scores s~ of this thread's token row (see the header comment).  lst_s: the shared-window
+// address of this thread's candidate list, entry j 2 * LT_BM entries further (entry-major: the lanes of a warp hit
+// distinct banks).
+__device__ __forceinline__ void argmin_scan_chunk(const uint32_t (&v)[LT_SCH], const float* __restrict__ norm_c, int cbase,
+                                                  float W, uint32_t lst_s, float& runmin, float& thr, int& cnt) {
   uint32_t laddr = lst_s + (uint32_t)cnt * (2 * LT_BM * 8);   // shared-window address of the next list entry
-#pragma unroll 1
-  for (int c = 0; c < LT_BN; c += 32) {
-    uint32_t v[32];
-    tmem_ld_32x32(tacc + c, v);
-    const float4* np = reinterpret_cast<const float4*>(norm_nt + c);
-    float d[32];
+  const float4* np = reinterpret_cast<const float4*>(norm_c);
+  float d[LT_SCH];
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const float4 n4 = __ldg(np + q);                       // same address in every lane: one broadcast transaction
-      d[4 * q] = n4.x; d[4 * q + 1] = n4.y; d[4 * q + 2] = n4.z; d[4 * q + 3] = n4.w;
+  for (int q = 0; q < LT_SCH / 4; ++q) {
+    const float4 n4 = __ldg(np + q);
+    d[4 * q] = n4.x; d[4 * q + 1] = n4.y; d[4 * q + 2] = n4.z; d[4 * q + 3] = n4.w;
+  }
+  float m0 = FLT_MAX, m1 = FLT_MAX, m2 = FLT_MAX, m3 = FLT_MAX;
+#pragma unroll
+  for (int i = 0; i < LT_SCH; i += 4) {
+    d[i] = fmaf(-2.f, __uint_as_float(v[i]), d[i]);             m0 = fminf(m0, d[i]);
+    d[i + 1] = fmaf(-2.f, __uint_as_float(v[i + 1]), d[i + 1]); m1 = fminf(m1, d[i + 1]);
+    d[i + 2] = fmaf(-2.f, __uint_as_float(v[i + 2]), d[i + 2]); m2 = fminf(m2, d[i + 2]);
+    d[i + 3] = fmaf(-2.f, __uint_as_float(v[i + 3]), d[i + 3]); m3 = fminf(m3, d[i + 3]);
+  }
+  const float cm = fminf(fminf(m0, m1), fminf(m2, m3));
+  if (cm <= thr) {                                         // the only branch of the chunk (dead rows: thr = -FLT_MAX)
+    if (cm < runmin) {
+      if (cm + W < runmin) { cnt = 0; laddr = lst_s; }     // every earlier entry is now outside any final window
+      runmin = cm; thr = cm + W;
     }
-    tmem_ld_wait();
-    float m0 = FLT_MAX, m1 = FLT_MAX, m2 = FLT_MAX, m3 = FLT_MAX;
+    // predicated append of every code of the chunk within W of the running minimum — no branch per code
 #pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-      d[i] = fmaf(-2.f, __uint_as_float(v[i]), d[i]);             m0 = fminf(m0, d[i]);
-      d[i + 1] = fmaf(-2.f, __uint_as_float(v[i + 1]), d[i + 1]); m1 = fminf(m1, d[i + 1]);
-      d[i + 2] = fmaf(-2.f, __uint_as_float(v[i + 2]), d[i + 2]); m2 = fminf(m2, d[i + 2]);
-      d[i + 3] = fmaf(-2.f, __uint_as_float(v[i + 3]), d[i + 3]); m3 = fminf(m3, d[i + 3]);
-    }
-    const float cm = fminf(fminf(m0, m1), fminf(m2, m3));
-    if (cm <= thr) {                                         // the only branch of the chunk (dead rows: thr = -FLT_MAX)
-      if (cm < runmin) {
-        if (cm + W < runmin) { cnt = 0; laddr = lst_s; }     // every earlier entry is now outside any final window
-        runmin = cm; thr = cm + W;
-      }
-      // predicated append of every code of the chunk within W of the running minimum — no branch per code: a
-      // test-and-branch costs ~46 clk of dependent latency each (measured), five predicated instructions do not
-      const int cbase = code0 + c;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        asm volatile(
-            "{\n\t.reg .pred h, p;\n\t"
-            "setp.le.f32 h, %2, %3;\n\t"
-            "setp.lt.and.s32 p, %0, %5, h;\n\t"
-            "@p st.shared.v2.b32 [%1], {%6, %4};\n\t"
-            "@h add.s32 %0, %0, 1;\n\t"
-            "@h add.u32 %1, %1, %7;\n\t}"
-            : "+r"(cnt), "+r"(laddr)
-            : "f"(d[i]), "f"(thr), "r"(cbase + i), "n"(LT_LIST), "r"(__float_as_uint(d[i])), "n"(2 * LT_BM * 8)
-            : "memory");
-      }
+    for (int i = 0; i < LT_SCH; ++i) {
+      asm volatile(
+          "{\n\t.reg .pred h, p;\n\t"
+          "setp.le.f32 h, %2, %3;\n\t"
+          "setp.lt.and.s32 p, %0, %5, h;\n\t"
+          "@p st.shared.v2.b32 [%1], {%6, %4};\n\t"
+          "@h add.s32 %0, %0, 1;\n\t"
+          "@h add.u32 %1, %1, %7;\n\t}"
+          : "+r"(cnt), "+r"(laddr)
+          : "f"(d[i]), "f"(thr), "r"(cbase + i), "n"(LT_LIST), "r"(__float_as_uint(d[i])), "n"(2 * LT_BM * 8)
+          : "memory");
     }
   }
 }
@@ -260,131 +252,91 @@ __device__ __forceinline__ int argmin_resolve_exact(const float* __restrict__ z,
   return best;
 }
 
-// ------------------------------------------------------------------------------ the pair sweep
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(LT_THREADS, 1)
-l2_argmin_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const float* __restrict__ z, const float2* __restrict__ zn2, int T, int E,
-                      const float* __restrict__ cb, const float* __restrict__ norm, int K, int64_t* __restrict__ idx,
-                      float* __restrict__ quant, int* __restrict__ fb_count, int* __restrict__ fb_list) {
+// ------------------------------------------------------------------------------ the sweep
+__global__ void __launch_bounds__(LT_THREADS, 1)
+l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const float* __restrict__ z, const float2* __restrict__ zn2, int T, int E,
+                    const float* __restrict__ cb, const float* __restrict__ norm, int K, int64_t* __restrict__ idx,
+                    float* __restrict__ quant, int* __restrict__ fb_count, int* __restrict__ fb_list) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                                          // [E/64][128 rows][128 B]: this CTA's 128 tokens
-  uint8_t* sB = sA + LT_BM * LT_EMAX * 2;                      // [NST][128 rows][128 B]: this CTA's half of a codebook tile
+  uint8_t* sB = sA + LT_BM * LT_EMAX * 2;                      // [NST][128 codes][128 B]
   uint8_t* tail = sB + LT_NST * LT_BST;
-  float2* lists = reinterpret_cast<float2*>(tail);             // [LT_LIST][2 groups][128 rows] (d~, code)
-  float* xmin = reinterpret_cast<float*>(lists + LT_LIST * 2 * LT_BM);   // [2][128] running minima of the two warpgroups
+  float2* lists = reinterpret_cast<float2*>(tail);             // [LT_LIST][2 owners][128 rows] (d~, code)
+  float* xmin = reinterpret_cast<float*>(lists + LT_LIST * 2 * LT_BM);   // [2][128] running minima of the two owners
   int* mi = reinterpret_cast<int*>(xmin + 2 * LT_BM);          // [128][LT_TOP] window members
   int* ncand = mi + LT_BM * LT_TOP;                            // [128] members found (zero between tiles)
   int* ovf = ncand + LT_BM;                                    // [128] a list overflowed
-  uint64_t* b_full = reinterpret_cast<uint64_t*>(tail + LT_XCH);       // [NST]   (used in the leader)
+  float* xacc = reinterpret_cast<float*>(tail + LT_XCH);       // accumulator exchange
+  uint64_t* b_full = reinterpret_cast<uint64_t*>(tail + LT_XCH + LT_XACC);   // [NST]
   uint64_t* b_empty = b_full + LT_NST;                         // [NST]
-  uint64_t* a_full = b_empty + LT_NST;                         // [8]     (leader)
+  uint64_t* a_full = b_empty + LT_NST;                         // [8]
   uint64_t* a_empty = a_full + LT_KBMAX;                       // [8]
-  uint64_t* t_full = a_empty + LT_KBMAX;                       // [2]
-  uint64_t* t_empty = t_full + 2;                              // [2]     (leader)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(t_empty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int KB = E / LT_BK;                                    // k-blocks
   const int NT = K / LT_BN;                                    // N-tiles
-  const int n_pt = (T + 2 * LT_BM - 1) / (2 * LT_BM);          // 256-token pair tiles
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
+  const int n_t = (T + LT_BM - 1) / LT_BM;                     // 128-token tiles
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < LT_NST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < LT_KBMAX; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&t_full[i], 1); mbar_init(&t_empty[i], 8); }   // 4 scan warps in each CTA
+    for (int i = 0; i < LT_NST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 8); }
+    for (int i = 0; i < LT_KBMAX; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 8); }
     fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc_2cta<512>(tmem_ptr);
-    tc_fence_before();
   }
   if (threadIdx.x < LT_BM) { ncand[threadIdx.x] = 0; ovf[threadIdx.x] = 0; }
   __syncthreads();
-  cluster_sync_all();                                          // the peer's barriers exist before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t rank = cluster_ctarank();
 
-  if (warp == 0) {
-    // ---------------------------------------------------------------- codebook producer: this CTA's half of every tile
+  if (warp == 8) {
+    // ---------------------------------------------------------------- codebook producer
     int st = 0;
     uint32_t ph = 0;
-    for (int pt = pair; pt < n_pt; pt += npairs) {
+    for (int tt = blockIdx.x; tt < n_t; tt += gridDim.x) {
       for (int nt = 0; nt < NT; ++nt) {
         for (int kb = 0; kb < KB; ++kb) {
           mbar_wait(&b_empty[st], ph ^ 1);
           if (elect_one()) {
-            const uint32_t fb = mapa_u32(smem_u32(&b_full[st]), 0);
-            if (rank == 0) mbar_arrive_expect_tx(&b_full[st], 2 * LT_BST);
-            tma_load_2d_2sm(sB + st * LT_BST, &tmB, fb, kb * LT_BK, nt * LT_BN + (int)rank * (LT_BN / 2));
+            mbar_arrive_expect_tx(&b_full[st], LT_BST);
+            tma_load_2d(sB + st * LT_BST, &tmB, &b_full[st], kb * LT_BK, nt * LT_BN);
           }
           __syncwarp();
           if (++st == LT_NST) { st = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 10) {
+  } else if (warp == 9) {
     // ---------------------------------------------------------------- A producer: the bf16 z rows of this CTA's 128 tokens
     int it = 0;
-    for (int pt = pair; pt < n_pt; pt += npairs, ++it) {
-      const int t0 = pt * 2 * LT_BM + (int)rank * LT_BM;
+    for (int tt = blockIdx.x; tt < n_t; tt += gridDim.x, ++it) {
+      const int t0 = tt * LT_BM;
       for (int kb = 0; kb < KB; ++kb) {
         if (it > 0) mbar_wait(&a_empty[kb], (it - 1) & 1);       // the previous tile's last N-tile has read this k-block
         if (elect_one()) {
-          const uint32_t fa = mapa_u32(smem_u32(&a_full[kb]), 0);
-          if (rank == 0) mbar_arrive_expect_tx(&a_full[kb], 2 * LT_A_KB_BYTES);
-          tma_load_2d_2sm(sA + kb * LT_A_KB_BYTES, &tmA, fa, kb * LT_BK, t0);       // rows >= T: zero fill
+          mbar_arrive_expect_tx(&a_full[kb], LT_A_KB_BYTES);
+          tma_load_2d(sA + kb * LT_A_KB_BYTES, &tmA, &a_full[kb], kb * LT_BK, t0);       // rows >= T: zero fill
         }
         __syncwarp();
       }
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer (pair leader; one elected lane)
-    if (rank == 0 && elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(2 * LT_BM, LT_BN);
-      const uint64_t da0 = umma_desc_k_sw128(smem_u32(sA));
-      const uint64_t db0 = umma_desc_k_sw128(smem_u32(sB));
-      int st = 0, it = 0, gc = 0;                              // gc: N-tiles issued so far (accumulator buffer = gc & 1)
-      uint32_t ph = 0;
-      for (int pt = pair; pt < n_pt; pt += npairs, ++it) {
-        for (int nt = 0; nt < NT; ++nt, ++gc) {
-          const int buf = gc & 1, use = gc >> 1;
-          if (use > 0) { mbar_wait(&t_empty[buf], (use - 1) & 1); tc_fence_after(); }
-          for (int kb = 0; kb < KB; ++kb) {
-            if (nt == 0) mbar_wait(&a_full[kb], it & 1);
-            mbar_wait(&b_full[st], ph);
-            tc_fence_after();
-            const uint64_t da = da0 + (uint64_t)(kb * (LT_A_KB_BYTES >> 4));
-            const uint64_t db = db0 + (uint64_t)(st * (LT_BST >> 4));
-#pragma unroll
-            for (int k = 0; k < LT_BK / 16; ++k)
-              umma_bf16_ss_2cta(tmem_base + buf * LT_BN, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            umma_commit_2cta(&b_empty[st]);                    // frees the stage in both CTAs
-            if (nt == NT - 1) umma_commit_2cta(&a_empty[kb]);  // the tile is done with this A k-block
-            if (kb == KB - 1) umma_commit_2cta(&t_full[buf]);
-            if (++st == LT_NST) { st = 0; ph ^= 1; }
-          }
-        }
-      }
-    }
-    __syncwarp();
   } else {
-    // ---------------------------------------------------------------- 8 worker warps: scan, merge, exact resolution
-    const int w8 = warp - 2;                                   // 0..7
-    const int g = w8 >> 2;                                     // warpgroup g scans the N-tiles with (global count & 1) == g
-    const int quad = warp & 3;                                 // TMEM lane quadrant this warp may read
-    const int r = quad * 32 + lane;
-    const uint32_t tacc = tmem_base + (uint32_t(quad * 32) << 16) + g * LT_BN;
-    const uint32_t te = mapa_u32(smem_u32(&t_empty[g]), 0);
+    // ---------------------------------------------------------------- 8 worker warps: MMA, scan, merge, exact resolution
+    const int w8 = warp;                                       // 0..7
+    const int wg = warp >> 2, w = warp & 3;
+    const int g = w >> 1;                                      // list owner: which 16 codes of every 32 this thread scans
+    const int rl = (w & 1) * 32 + lane;
+    const int r = wg * 64 + rl;                                // token row of the tile
+    const int bar_id = 2 + wg;                                 // named barrier of this warpgroup's exchange
+    float* xw = xacc + wg * 64 * LT_XLD;
+    const uint32_t a_rows = smem_u32(sA) + wg * 64 * 128;
     const float emax = sqrtf(__ldg(norm + K)), demax = sqrtf(__ldg(norm + K + 1));
     float2* lst = lists + g * LT_BM + r;
-    int it = 0, use = 0;
-    for (int pt = pair; pt < n_pt; pt += npairs, ++it) {
-      const int t0 = pt * 2 * LT_BM + (int)rank * LT_BM;
+    int st = 0;
+    uint32_t ph = 0;
+    int it = 0;
+    for (int tt = blockIdx.x; tt < n_t; tt += gridDim.x, ++it) {
+      const int t0 = tt * LT_BM;
       const bool live = t0 + r < T;
       float W;
       {
@@ -396,16 +348,47 @@ l2_argmin_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       float runmin = live ? FLT_MAX : -FLT_MAX, thr = runmin;  // rows past T never pass the chunk test
       int cnt = 0;
       for (int nt = 0; nt < NT; ++nt) {
-        if (((it * NT + nt) & 1) != g) continue;
-        mbar_wait(&t_full[g], use & 1);
-        ++use;
-        tc_fence_after();
-        argmin_scan_ntile(tacc, norm + nt * LT_BN, nt * LT_BN, W, smem_u32(lst), runmin, thr, cnt);
-        tc_fence_before();
+        float acc[LT_BN / 2];
+        int prev = -1;
+        for (int kb = 0; kb < KB; ++kb) {
+          if (nt == 0) mbar_wait(&a_full[kb], it & 1);
+          mbar_wait(&b_full[st], ph);
+          const uint64_t da = wgmma_desc_k_sw128(a_rows + kb * LT_A_KB_BYTES);
+          const uint64_t db = wgmma_desc_k_sw128(smem_u32(sB) + st * LT_BST);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < LT_BK / 16; ++k) wgmma_bf16<LT_BN>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&b_empty[prev]); }
+          prev = st;
+          if (++st == LT_NST) { st = 0; ph ^= 1; }
+        }
+        wgmma_wait<0>();
         __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(te);                // one cluster-scope arrive per warp
+        if (lane == 0) {
+          mbar_arrive(&b_empty[prev]);
+          if (nt == NT - 1)
+            for (int kb = 0; kb < KB; ++kb) mbar_arrive(&a_empty[kb]);   // the tile is done with its A k-blocks
+        }
+        static_for<0, LT_BN / 32>([&](auto rc) {
+          constexpr int R = decltype(rc)::value;
+          named_bar_sync(bar_id, 128);
+          acc_to_smem<32 * R, 32>(acc, xw, LT_XLD, w, lane);
+          named_bar_sync(bar_id, 128);
+          uint32_t v[LT_SCH];
+          const float* src = xw + rl * LT_XLD + g * LT_SCH;
+#pragma unroll
+          for (int q = 0; q < LT_SCH / 4; ++q) {
+            const float4 f = reinterpret_cast<const float4*>(src)[q];
+            v[4 * q] = __float_as_uint(f.x); v[4 * q + 1] = __float_as_uint(f.y);
+            v[4 * q + 2] = __float_as_uint(f.z); v[4 * q + 3] = __float_as_uint(f.w);
+          }
+          const int c = nt * LT_BN + 32 * R + g * LT_SCH;
+          argmin_scan_chunk(v, norm + c, c, W, smem_u32(lst), runmin, thr, cnt);
+        });
       }
-      // merge: every thread filters its own list against the row's minimum over both warpgroups
+      // merge: every thread filters its own list against the row's minimum over both owners
       xmin[g * LT_BM + r] = runmin;
       named_bar_sync(1, 256);
       {
@@ -461,13 +444,6 @@ l2_argmin_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                          // neither CTA retires while the peer may still signal it
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2cta<512>(tmem_base);
-  }
 }
 
 int l2_argmin_list_launch(const float* z, int T, int E, const float* codebook, int K, int64_t* idx, float* quant,
@@ -512,13 +488,13 @@ extern "C" int pgt_l2_argmin_tc(const float* z, int T, int E, const float* codeb
   __nv_bfloat16* zb = reinterpret_cast<__nv_bfloat16*>(workspace + ws_off_zb(T));
   CUtensorMap tmA, tmB;
   int rc = tmap_rows_bf16(&tmA, zb, E, T, E, LT_BM);
-  if (rc == PGT_OK) rc = tmap_rows_bf16(&tmB, cb_bf16, E, K, E, LT_BN / 2);      // each CTA of a pair loads half a tile
+  if (rc == PGT_OK) rc = tmap_rows_bf16(&tmB, cb_bf16, E, K, E, LT_BN);
   if (rc != PGT_OK) return rc;
   static PerDeviceOnce once;
-  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(l2_argmin_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM); }));
+  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(l2_argmin_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM); }));
   PGT_CUDA_OK(cudaMemsetAsync(workspace, 0, sizeof(int32_t), st));
-  const int n_pt = ceil_div(T, 2 * LT_BM);
-  const int npairs = n_pt < num_sms() / 2 ? n_pt : num_sms() / 2;
+  const int n_t = ceil_div(T, LT_BM);
+  const int grid = n_t < num_sms() ? n_t : num_sms();
   {
     ProfScope ps(PGT_PROF_ARGMIN, 2.0 * T * (double)K * E, st, "l2_argmin_tc");
     // pack grid: warps take 4 rows per step; pick the CTA count in [SMs, 2 SMs] that leaves the smallest ragged last step
@@ -533,8 +509,8 @@ extern "C" int pgt_l2_argmin_tc(const float* z, int T, int E, const float* codeb
       }
     }
     z_pack_kernel<<<pack_ctas, 256, 0, st>>>(z, T, E, zb, zn2);
-    l2_argmin_pair_kernel<<<2 * npairs, LT_THREADS, LT_SMEM, st>>>(tmA, tmB, z, zn2, T, E, codebook, cb_norm, K, idx, quant,
-                                                                   fb_count, fb_list);
+    l2_argmin_tc_kernel<<<grid, LT_THREADS, LT_SMEM, st>>>(tmA, tmB, z, zn2, T, E, codebook, cb_norm, K, idx, quant,
+                                                           fb_count, fb_list);
     PGT_LAUNCH_OK();
   }
   // tokens whose certificate window did not fit the shortlist (degenerate codebooks): exhaustive exact kernel

@@ -3,14 +3,14 @@
 // [3C, C] weight at load): the normalised token matrix is never written to HBM — x is read once, LN happens in shared
 // memory in place, and the same tile is the A operand of all N / 256 column blocks.
 //
-// Per CTA, persistent over 128-token tiles (352 threads):
-//   warp 0      TMA producer of the weight k-blocks ([256 x 64] each, 2-deep ring; N/256 x 4 per tile)
-//   warp 1      tcgen05.mma issuer: column block j accumulates in TMEM columns [256 (j & 1), +256) — the epilogue of
-//               block j overlaps the MMAs of block j + 1
-//   warps 2..9  epilogue of the column blocks: acc + bias -> bf16 -> swizzled 64-column staging panel
-//   warp 10     DMA: TMA load of x tiles into the buffer the MMAs of two tiles ago have released, TMA store of each
+// Per CTA, persistent over 128-token tiles (448 threads):
+//   warps 0..7  two consumer warpgroups: warpgroup h multiplies rows [64h, 64h + 64) of the tile with one 128-column
+//               weight block at a time (wgmma 64 x 128 x 16, fp32 accumulators in registers), then adds the bias and
+//               writes bf16 pairs straight from the accumulator fragments into the swizzled 64-column staging panels
+//   warp 8      TMA producer of the weight k-blocks ([128 x 64] each, 4-deep ring; N/128 x 4 per tile)
+//   warp 9      DMA: TMA load of x tiles into the buffer the MMAs of two tiles ago have released, TMA store of each
 //               finished [128 x 64] panel
-//   warps 11..14 LayerNorm of the NEXT x tile in place, one thread per row (no cross-thread exchange), concurrent with
+//   warps 10..13 LayerNorm of the NEXT x tile in place, one thread per row (no cross-thread exchange), concurrent with
 //               the epilogues and MMAs of the current tile
 //
 // Two x buffers (round 2, second pass).  A device timeline of the single-buffer version (clock64 stamps, T = 786432):
@@ -32,9 +32,10 @@ namespace pgt {
 constexpr int LL_C = 256;
 constexpr int LL_BM = 128;
 constexpr int LL_SUB = LL_BM * 128;            // one [128 x 64] bf16 sub-tile: 16 KB
-constexpr int LL_WST = 2;                      // weight ring depth
-constexpr int LL_WBYTES = LL_C * 128;          // one [256 x 64] weight k-block: 32 KB
-constexpr int LL_THREADS = 480;
+constexpr int LL_BN = 128;                     // weight block (columns) per wgmma pass
+constexpr int LL_WST = 4;                      // weight ring depth
+constexpr int LL_WBYTES = LL_BN * 128;         // one [128 x 64] weight k-block: 16 KB
+constexpr int LL_THREADS = 448;
 constexpr int LL_SMEM = 8 * LL_SUB /*two x / A tiles*/ + 2 * LL_SUB /*staging panels*/ + LL_WST * LL_WBYTES + 256;
 static_assert(LL_SMEM <= 232448, "ln_linear smem budget");
 
@@ -56,139 +57,106 @@ ln_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   uint8_t* sW = sO + 2 * LL_SUB;                // weight ring
   uint64_t* bars = reinterpret_cast<uint64_t*>(sW + LL_WST * LL_WBYTES);
   uint64_t* x_full = bars;           // [2] DMA -> LayerNorm warps
-  uint64_t* sx_free = bars + 2;      // [2] MMA commit (last column block of the tile in that buffer) -> DMA
-  uint64_t* y_ready = bars + 4;      // [2] LayerNorm warps (128) -> MMA
-  uint64_t* acc_full = bars + 6;     // [2] MMA commit -> compute
-  uint64_t* acc_free = bars + 8;     // [2] compute (256) -> MMA
-  uint64_t* so_free = bars + 10;     // [2] DMA (store has read staging panel s) -> compute
-  uint64_t* out_ready = bars + 12;   // [2] compute (256) -> DMA
-  uint64_t* w_full = bars + 14;      // [LL_WST]
+  uint64_t* sx_free = bars + 2;      // [2] consumers (one arrive per warp, after the tile's last MMAs) -> DMA
+  uint64_t* y_ready = bars + 4;      // [2] LayerNorm warps (128) -> consumers
+  uint64_t* so_free = bars + 6;      // [2] DMA (store has read staging panel s) -> consumers
+  uint64_t* out_ready = bars + 8;    // [2] consumers (256) -> DMA
+  uint64_t* w_full = bars + 10;      // [LL_WST]
   uint64_t* w_empty = w_full + LL_WST;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(w_empty + LL_WST);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmX); tma_prefetch_desc(&tmO); tma_prefetch_desc(&tmW);
     for (int i = 0; i < 2; ++i) {
-      mbar_init(&x_full[i], 1); mbar_init(&sx_free[i], 1); mbar_init(&y_ready[i], 128);
-      mbar_init(&acc_full[i], 1); mbar_init(&acc_free[i], 256);
+      mbar_init(&x_full[i], 1); mbar_init(&sx_free[i], 8); mbar_init(&y_ready[i], 128);
       mbar_init(&so_free[i], 1); mbar_init(&out_ready[i], 256);
     }
-    for (int i = 0; i < LL_WST; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 1); }
+    for (int i = 0; i < LL_WST; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc<512>(tmem_ptr);
-    tc_fence_before();
-  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int NB = p.nb;
+  const int NB2 = NB * (LL_C / LL_BN);
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ weight producer
     int st = 0;
     uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x) {
-      for (int j = 0; j < NB; ++j) {
+      for (int j = 0; j < NB2; ++j) {
         for (int kb = 0; kb < 4; ++kb) {
           mbar_wait(&w_empty[st], ph ^ 1);
           if (elect_one()) {
             mbar_arrive_expect_tx(&w_full[st], LL_WBYTES);
-            tma_load_2d(sW + st * LL_WBYTES, &tmW, &w_full[st], kb * 64, j * LL_C);
+            tma_load_2d(sW + st * LL_WBYTES, &tmW, &w_full[st], kb * 64, j * LL_BN);
           }
           __syncwarp();
           if (++st == LL_WST) { st = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc_bf16(LL_BM, LL_C);
+  } else if (warp < 8) {
+    // ------------------------------------------------------------------ consumer warpgroups
+    const int wg = warp >> 2, w = warp & 3;
+    const int t4 = lane & 3;
+    const uint32_t so = smem_u32(sO);
     int st = 0;
     uint32_t ph = 0;
     int it = 0;
+    int n = 0;                                           // running panel number: staging buffer n & 1, its (n >> 1)-th use
     for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x, ++it) {
       const int xb = it & 1;
       mbar_wait(&y_ready[xb], (it >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        int s = st;
-        uint32_t sp = ph;
-        const uint64_t da0 = umma_desc_k_sw128(smem_u32(sX + xb * 4 * LL_SUB));
-        const uint64_t db0 = umma_desc_k_sw128(smem_u32(sW));
-        for (int j = 0; j < NB; ++j) {
-          const int g = it * NB + j;
-          mbar_wait(&acc_free[g & 1], ((g >> 1) & 1) ^ 1);
-          tc_fence_after();
-          for (int kb = 0; kb < 4; ++kb) {
-            mbar_wait(&w_full[s], sp);
-            tc_fence_after();
-            const uint64_t da = da0 + (uint64_t)(kb * (LL_SUB >> 4));
-            const uint64_t db = db0 + (uint64_t)(s * (LL_WBYTES >> 4));
+      const uint32_t a_rows = smem_u32(sX + xb * 4 * LL_SUB) + wg * 64 * 128;
+      for (int j = 0; j < NB2; ++j) {
+        float acc[LL_BN / 2];
+        int prev = -1;
+        for (int kb = 0; kb < 4; ++kb) {
+          mbar_wait(&w_full[st], ph);
+          const uint64_t da = wgmma_desc_k_sw128(a_rows + kb * LL_SUB);
+          const uint64_t db = wgmma_desc_k_sw128(smem_u32(sW) + st * LL_WBYTES);
+          wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < 4; ++k) umma_bf16_ss(tmem_base + (g & 1) * LL_C, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            umma_commit(&w_empty[s]);
-            if (++s == LL_WST) { s = 0; sp ^= 1; }
-          }
-          umma_commit(&acc_full[g & 1]);
+          for (int k = 0; k < 4; ++k) wgmma_bf16<LL_BN>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&w_empty[prev]); }
+          prev = st;
+          if (++st == LL_WST) { st = 0; ph ^= 1; }
         }
-        umma_commit(&sx_free[xb]);                  // every MMA that reads this x buffer has retired
-      }
-      __syncwarp();
-      const int ns = st + 4 * NB;
-      ph ^= (ns / LL_WST) & 1;
-      st = ns % LL_WST;
-    }
-  } else if (warp < 10) {
-    // ------------------------------------------------------------------ compute warps
-    const int quad = warp & 3;
-    const int half = (warp - 2) >> 2;                    // which 32-column chunk of a 64-column panel
-    const int r = quad * 32 + lane;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x, ++it) {
-      // ---- per column block: acc + bias -> bf16 -> 64-column staging panels (ping-pong)
-      for (int j = 0; j < NB; ++j) {
-        const int g = it * NB + j;
-        const uint32_t t_row = tmem_base + (uint32_t(quad * 32) << 16) + (g & 1) * LL_C;
-        mbar_wait(&acc_full[g & 1], (g >> 1) & 1);
-        tc_fence_after();
-#pragma unroll 1
-        for (int pp = 0; pp < 4; ++pp) {
-          const int n = g * 4 + pp;                    // running panel number: staging buffer n & 1, its (n >> 1)-th use
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&w_empty[prev]);
+          if (j == NB2 - 1) mbar_arrive(&sx_free[xb]);   // every MMA that reads this x buffer has retired
+        }
+        // ---- acc + bias -> bf16 -> two 64-column staging panels: fragment column pair (2 t4, 2 t4 + 1) of 8-column
+        // chunk jj is one 4-byte word of the swizzled row
+#pragma unroll
+        for (int pp = 0; pp < LL_BN / 64; ++pp, ++n) {
           const int sb = n & 1;
-          const int c0 = pp * 64 + half * 32;
-          const float4* b4 = reinterpret_cast<const float4*>(p.bias + j * LL_C + c0);
-          float4 bv[8];                                // requested before the waits: L1-hit loads are slow under MMA load
+          const float* bias = p.bias + j * LL_BN + pp * 64 + 2 * t4;
+          float2 bv[8];                                // requested before the wait
 #pragma unroll
-          for (int i = 0; i < 8; ++i) bv[i] = __ldg(b4 + i);
+          for (int jj = 0; jj < 8; ++jj) bv[jj] = __ldg(reinterpret_cast<const float2*>(bias + 8 * jj));
           mbar_wait(&so_free[sb], ((n >> 1) & 1) ^ 1);   // the store that last used this panel has read it
-          uint32_t v[32];
-          tmem_ld_32x32(t_row + c0, v);
-          tmem_ld_wait();
-          if (pp == 3) {                               // last TMEM read of this thread: the accumulator may be reused
-            tc_fence_before();
-            mbar_arrive(&acc_free[g & 1]);
-          }
-          const uint32_t dst = smem_u32(sO) + sb * LL_SUB + r * 128;
-          const int ch0 = half * 4;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 ba = bv[2 * i], bb = bv[2 * i + 1];
-            const uint32_t ox = pack_bf16x2(__uint_as_float(v[8 * i + 0]) + ba.x, __uint_as_float(v[8 * i + 1]) + ba.y);
-            const uint32_t oy = pack_bf16x2(__uint_as_float(v[8 * i + 2]) + ba.z, __uint_as_float(v[8 * i + 3]) + ba.w);
-            const uint32_t oz = pack_bf16x2(__uint_as_float(v[8 * i + 4]) + bb.x, __uint_as_float(v[8 * i + 5]) + bb.y);
-            const uint32_t ow = pack_bf16x2(__uint_as_float(v[8 * i + 6]) + bb.z, __uint_as_float(v[8 * i + 7]) + bb.w);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst + (((ch0 + i) ^ (r & 7)) << 4)), "r"(ox), "r"(oy),
-                         "r"(oz), "r"(ow) : "memory");
+          for (int hr = 0; hr < 2; ++hr) {
+            const int r = wg * 64 + w * 16 + (lane >> 2) + 8 * hr;
+            const uint32_t dst = so + sb * LL_SUB + r * 128 + t4 * 4;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int f = 4 * (pp * 8 + jj) + 2 * hr;
+              const uint32_t o = pack_bf16x2(acc[f] + bv[jj].x, acc[f + 1] + bv[jj].y);
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst + ((jj ^ (r & 7)) << 4)), "r"(o) : "memory");
+            }
           }
           fence_proxy_async();
           mbar_arrive(&out_ready[sb]);
         }
       }
     }
-  } else if (warp == 10) {
+  } else if (warp == 9) {
     // ------------------------------------------------------------------ DMA warp
     int it = 0;
     int pending = -1;                                  // staging panel of the newest committed store (not yet released)
@@ -206,19 +174,21 @@ ln_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
       const int xb = it & 1;
       for (int j = 0; j < NB; ++j) {
         const int g = it * NB + j;
-        if (j == NB - 1) {
-          // this tile's x buffer is free once its last column block's MMAs have retired: fetch the tile after next
-          const int nt = tile + 2 * gridDim.x;
-          if (nt < p.m_tiles) {
-            mbar_wait(&sx_free[xb], (it >> 1) & 1);
-            if (lane == 0) {
-              mbar_arrive_expect_tx(&x_full[xb], 4 * LL_SUB);
-              for (int kb = 0; kb < 4; ++kb) tma_load_2d(sX + (xb * 4 + kb) * LL_SUB, &tmX, &x_full[xb], kb * 64, nt * LL_BM);
-            }
-            __syncwarp();
-          }
-        }
         for (int pp = 0; pp < 4; ++pp) {
+          if (j == NB - 1 && pp == 4 - LL_BN / 64) {
+            // this tile's x buffer is free once the MMAs of its last 128-column block have retired: fetch the tile after
+            // next.  The consumers release it before they write that block's panels, and only after the panels before
+            // them have been stored (their staging slots are needed), so the wait sits exactly here.
+            const int nt = tile + 2 * gridDim.x;
+            if (nt < p.m_tiles) {
+              mbar_wait(&sx_free[xb], (it >> 1) & 1);
+              if (lane == 0) {
+                mbar_arrive_expect_tx(&x_full[xb], 4 * LL_SUB);
+                for (int kb = 0; kb < 4; ++kb) tma_load_2d(sX + (xb * 4 + kb) * LL_SUB, &tmX, &x_full[xb], kb * 64, nt * LL_BM);
+              }
+              __syncwarp();
+            }
+          }
           const int n = g * 4 + pp;
           const int sb = n & 1;
           mbar_wait(&out_ready[sb], (n >> 1) & 1);
@@ -237,8 +207,8 @@ ln_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     }
     if (lane == 0) bulk_wait0();
   } else {
-    // ------------------------------------------------------------------ LayerNorm warps (11..14): thread = row
-    const int r = (warp - 11) * 32 + lane;
+    // ------------------------------------------------------------------ LayerNorm warps (10..13): thread = row
+    const int r = (warp - 10) * 32 + lane;
     const bool affine = p.ln_g != nullptr;             // nullptr: gamma / beta folded into W / bias by the caller
     int t = 0;
     for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x, ++t) {
@@ -291,13 +261,6 @@ ln_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
       mbar_arrive(&y_ready[t & 1]);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
 }
 
 static int ll_enc2d(CUtensorMap* map, const void* base, int ld, long long rows, int cols, int box_rows) {
@@ -317,7 +280,7 @@ extern "C" int pgt_ln_linear_bf16(const void* x, int ldx, int T, int C, const fl
   CUtensorMap tx, to, tw;
   int rc = ll_enc2d(&tx, x, ldx, T, C, LL_BM);
   if (rc == PGT_OK) rc = ll_enc2d(&to, out, ldo, T, N, LL_BM);
-  if (rc == PGT_OK) rc = ll_enc2d(&tw, W, ldw, N, C, LL_C);
+  if (rc == PGT_OK) rc = ll_enc2d(&tw, W, ldw, N, C, LL_BN);
   if (rc != PGT_OK) return rc;
   static PerDeviceOnce once;
   PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(ln_linear_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LL_SMEM); }));

@@ -1,17 +1,14 @@
-// Global multi-head attention forward on tcgen05 (flash-attention, d = 64, no mask), sm_100a.
+// Global multi-head attention forward on wgmma (flash-attention, d = 64, no mask), sm_90a.
 //
-// One CTA = one (clip, head) and TWO 128-query tiles (ping-pong groups G0/G1) that share the K/V stream:
-//   warp 0      TMA producer: Q tiles once, then K_j / V_j tiles (128 keys x 64, 128B swizzle) through a 3-deep ring
-//   warp 1      single-thread tcgen05.mma issuer:  S_g = Q_g K_j^T (128x128x64, fp32 in TMEM),
-//               [O_g | L_g] += P_g [V_j | 1] (128x80x128; P_g bf16 in swizzled smem, V_j consumed MN-major straight from
-//               its TMA tile, a second MN atom of ones appended through the descriptor's LBO): the softmax
-//               denominator comes off the tensor pipe, summed over exactly the bf16 P that the numerator uses
-//   warps 2..5  softmax group 0, warps 6..9 softmax group 1 (thread = query row): ONE pass over S per key tile —
-//               p = 2^(s*c - m_ref) against a reference exponent m_ref that is the row maximum of the first tile and is
-//               only raised (by a whole power of two, so the rescale of O and L in TMEM is exact) when a later tile
-//               produces p > 2^8; O and L stay in TMEM for the whole key loop and are read once at the end.
-// While group g runs its exponentials the tensor pipe works for the other group.
-// TMEM: S0 [0,128) S1 [128,256) O0' [256,336) O1' [336,416), O' = [O (64) | L (16)].
+// One CTA = one (clip, head) and one 128-query tile, two warpgroups of 64 queries that share the K/V stream:
+//   warp 8      TMA producer: the Q tile once, then K_j / V_j tiles (128 keys x 64, 128B swizzle) through a 3-deep ring
+//   warps 0..7  warpgroup h owns query rows [64h, 64h + 64): S = Q K_j^T (wgmma 64 x 128 x 16, fp32 in registers),
+//               one pass over S per key tile — p = 2^(s*c - m_ref) against a reference exponent m_ref that is the row
+//               maximum of the first tile and is only raised (by a whole power of two, so the rescale of O and L is
+//               exact) when a later tile produces p > 2^8 —, P packed to bf16 in registers as the A operand of
+//               O += P V_j (wgmma 64 x 64 x 16, V consumed MN-major straight from its TMA tile), and the denominator L
+//               summed over exactly the bf16 P that the numerator uses.  Each row's 128 scores of a tile live in the
+//               four lanes of a quad; row maxima and sums combine by shuffles.
 #include <cudaTypedefs.h>
 
 #include "common.cuh"
@@ -21,117 +18,46 @@
 namespace pgt {
 
 constexpr int FT_D = 64;
-constexpr int FT_BM = 128;                 // queries per group
+constexpr int FT_BM = 128;                 // queries per CTA (64 per warpgroup)
 constexpr int FT_BN = 128;                 // keys per tile
 constexpr int FT_NST = 3;                  // K/V ring depth
 constexpr int FT_TILE = FT_BN * FT_D * 2;  // 16 KB: one 128 x 64 bf16 tile
-constexpr int FT_THREADS = 64 + 256;
-constexpr int FT_SMEM = 2 * FT_TILE /*Q*/ + FT_NST * 2 * FT_TILE /*K,V*/ + 2 * 2 * FT_TILE /*P*/ + FT_TILE /*ones*/ + 256 + 1024;
+constexpr int FT_THREADS = 256 + 32;
+constexpr int FT_SMEM = FT_TILE /*Q*/ + FT_NST * 2 * FT_TILE /*K,V*/ + 256 + 1024;
 constexpr float FT_TAU = 256.f;              // p above this raises the reference exponent for the following tiles
-
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-        "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-        "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16_ft(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16_ft(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void st_shared_v4(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(smem_u32(p)), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ float fast_exp2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// MN-major (the N x K operand is stored K-rows x N-contiguous), 128B swizzle: 8 K-rows per 1024 B atom.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes = 16384) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;   // LBO: byte distance to the next 64-element MN atom
-  d |= static_cast<uint64_t>((1024 >> 4) & 0x3FFF) << 32;     // SBO: stride between 8-row K groups
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
 
 __global__ void __launch_bounds__(FT_THREADS, 1)
 mha_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
               const __grid_constant__ CUtensorMap tmV, int L, __nv_bfloat16* __restrict__ out, int ldo) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                                   // [2][16 KB]
-  uint8_t* sK = sQ + 2 * FT_TILE;                       // [NST][16 KB]
+  uint8_t* sQ = smem;                                   // [16 KB]
+  uint8_t* sK = sQ + FT_TILE;                           // [NST][16 KB]
   uint8_t* sV = sK + FT_NST * FT_TILE;                  // [NST][16 KB]
-  uint8_t* sP = sV + FT_NST * FT_TILE;                  // [2 groups][2 key halves][16 KB]
-  uint8_t* sOnes = sP + 4 * FT_TILE;                    // 16 KB of bf16 1.0 (the B operand of the row-sum MMA)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sOnes + FT_TILE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + FT_NST * FT_TILE);
   uint64_t* q_full = bars;                              // [1]
   uint64_t* kv_full = bars + 1;                         // [NST]
-  uint64_t* kv_empty = kv_full + FT_NST;                // [NST]
-  uint64_t* s_full = kv_empty + FT_NST;                 // [2]
-  uint64_t* p_full = s_full + 2;                        // [2]
-  uint64_t* o_full = p_full + 2;                        // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(o_full + 2);
+  uint64_t* kv_empty = kv_full + FT_NST;                // [NST] one arrive per consumer warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int h = blockIdx.y, clip = blockIdx.z;
-  const int q0 = clip * L + blockIdx.x * 2 * FT_BM;     // first query row (global token index) of this CTA
+  const int q0 = clip * L + blockIdx.x * FT_BM;         // first query row (global token index) of this CTA
   const int kv0 = clip * L;
   const int NT = L / FT_BN;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
-    for (int i = 0; i < FT_NST; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(&s_full[g], 1);
-      mbar_init(&p_full[g], 128);
-      mbar_init(&o_full[g], 1);
-    }
+    for (int i = 0; i < FT_NST; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 8); }
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < FT_TILE / 16; i += FT_THREADS)
-    reinterpret_cast<uint4*>(sOnes)[i] = make_uint4(0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
-  fence_proxy_async();
-  if (warp == 1) {
-    tmem_alloc<512>(tmem_ptr);
-    tc_fence_before();
-  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer
     if (elect_one()) {
-      mbar_arrive_expect_tx(q_full, 2 * FT_TILE);
+      mbar_arrive_expect_tx(q_full, FT_TILE);
       tma_load_2d(sQ, &tmQ, q_full, h * FT_D, q0);
-      tma_load_2d(sQ + FT_TILE, &tmQ, q_full, h * FT_D, q0 + FT_BM);
     }
     __syncwarp();
     int st = 0;
@@ -146,176 +72,110 @@ mha_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ C
       __syncwarp();
       if (++st == FT_NST) { st = 0; ph ^= 1; }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc_s = umma_idesc_bf16(FT_BM, FT_BN);                   // S: A,B K-major
-    constexpr uint32_t idesc_o = umma_idesc_bf16(FT_BM, FT_D) | (1u << 16);       // O: B (= V) MN-major
-    auto issue_s = [&](int g, int st) {
-      const uint64_t da = umma_desc_k_sw128(smem_u32(sQ + g * FT_TILE));
-      const uint64_t db = umma_desc_k_sw128(smem_u32(sK + st * FT_TILE));
+  } else {
+    // ------------------------------------------------------------------ attention warpgroups
+    const int wg = warp >> 2, w = warp & 3;
+    const int t4 = lane & 3;
+    const float sl2 = 0.125f * 1.4426950408889634f;     // d^-1/2 * log2(e)
+    const uint64_t dq = wgmma_desc_k_sw128(smem_u32(sQ) + wg * 64 * 128);
+    float o[FT_D / 2];                                   // O: rows (g, g + 8) of the warp's 16, 64 columns
+    float mb[2] = {0.f, 0.f};                            // reference exponent per row (log2 domain)
+    float lsum[2] = {0.f, 0.f};                          // this lane's share of the row sums of the bf16 P
+    int pending[2] = {0, 0};                             // raise the reference by 2^pending before the next tile
 #pragma unroll
-      for (int k = 0; k < FT_D / 16; ++k) umma_bf16_ss(tmem_base + g * FT_BN, da + 2 * k, db + 2 * k, idesc_s, k != 0 ? 1u : 0u);
-      umma_commit(&s_full[g]);
-    };
-    // O' = P [V | 1]: the B operand is the MN-major V tile (64 columns) followed, LBO bytes further, by an atom of
-    // ones (16 of its columns used), so columns 64..79 of the accumulator collect the row sums of P
-    constexpr uint32_t idesc_o80 = umma_idesc_bf16(FT_BM, FT_D + 16) | (1u << 16);
-    auto issue_o = [&](int g, int st, uint32_t acc) {
-#pragma unroll
-      for (int kt = 0; kt < 2; ++kt) {
-        const uint64_t da = umma_desc_k_sw128(smem_u32(sP + (g * 2 + kt) * FT_TILE));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          // 16 keys per step: +32 B inside P's swizzled row (K-major), +16 key rows = 2048 B in the V tile (MN-major)
-          const uint32_t vaddr = smem_u32(sV + st * FT_TILE + (kt * 64 + k * 16) * 128);
-          const uint64_t db = umma_desc_mn_sw128(vaddr, smem_u32(sOnes) - vaddr);
-          umma_bf16_ss(tmem_base + 256 + g * (FT_D + 16), da + 2 * k, db, idesc_o80, (acc | kt | k) != 0 ? 1u : 0u);
-        }
-      }
-      umma_commit(&o_full[g]);
-    };
+    for (int i = 0; i < FT_D / 2; ++i) o[i] = 0.f;
     mbar_wait(q_full, 0);
-    mbar_wait(&kv_full[0], 0);
-    tc_fence_after();
-    if (elect_one()) { issue_s(0, 0); issue_s(1, 0); }
-    __syncwarp();
     int st = 0;
     uint32_t ph = 0;
     for (int j = 0; j < NT; ++j) {
-      const uint32_t par = j & 1;
-      int nst = st + 1;
-      uint32_t nph = ph;
-      if (nst == FT_NST) { nst = 0; nph ^= 1; }
-      for (int g = 0; g < 2; ++g) {
-        mbar_wait(&p_full[g], par);                    // P_g(j) is in smem, S_g has been read out, O_g / L_g rescaled if due
-        if (g == 0 && j + 1 < NT) mbar_wait(&kv_full[nst], nph);
-        tc_fence_after();
-        if (elect_one()) {
-          // S of the next tile first: the softmax group starts on it while P V of this tile (needed only before the
-          // next P is written) runs behind it
-          if (j + 1 < NT) issue_s(g, nst);
-          issue_o(g, st, j > 0 ? 1u : 0u);
-          if (g == 1) umma_commit(&kv_empty[st]);      // every MMA reading K_j / V_j has been issued
-        }
-        __syncwarp();
+      mbar_wait(&kv_full[st], ph);
+      float s[FT_BN / 2];
+      {
+        const uint64_t dk = wgmma_desc_k_sw128(smem_u32(sK + st * FT_TILE));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < FT_D / 16; ++k) wgmma_bf16<FT_BN>(s, dq + 2 * k, dk + 2 * k, k != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
       }
-      st = nst; ph = nph;
-    }
-  } else {
-    // ------------------------------------------------------------------ softmax groups
-    const int g = (warp - 2) >> 2;
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;                      // query row inside the group's tile
-    const uint32_t lane_base = uint32_t(quad * 32) << 16;
-    const uint32_t tS = tmem_base + lane_base + g * FT_BN;
-    const uint32_t tO = tmem_base + lane_base + 256 + g * (FT_D + 16);
-    const uint32_t tL = tO + FT_D;                       // row sums: columns 64..79 of the O' accumulator
-    uint8_t* prow = sP + g * 2 * FT_TILE + r * 128;
-    const float sl2 = 0.125f * 1.4426950408889634f;     // d^-1/2 * log2(e)
-    float mb = 0.f;                                      // reference exponent (log2 domain)
-    int pending = 0;                                     // raise the reference by 2^pending before the next tile
-    for (int j = 0; j < NT; ++j) {
-      const uint32_t par = j & 1;
-      mbar_wait(&s_full[g], par);
-      tc_fence_after();
       if (j == 0) {
         // the only second pass: the row maximum of the first tile anchors the reference exponent
-        float mx = -1e30f;
-#pragma unroll 1
-        for (int c = 0; c < FT_BN; c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32(tS + c, v);
-          tmem_ld_wait();
 #pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-        }
-        mb = mx * sl2;
-      }
-      const float scale_due = __int_as_float((127 - pending) << 23);     // 2^-pending (1.0 when nothing is due)
-      mb += (float)pending;
-      // one pass: p = 2^(s * sl2 - mb) -> packed bf16, running maximum of p on the packed values
-      uint32_t pk[FT_BN / 2];
-      __nv_bfloat162 pmax = __floats2bfloat162_rn(0.f, 0.f);
+        for (int e = 0; e < 2; ++e) {
+          float mx = -1e30f;
 #pragma unroll
-      for (int c = 0; c < FT_BN; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tS + c, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float p0 = fast_exp2(fmaf(__uint_as_float(v[i]), sl2, -mb));
-          const float p1 = fast_exp2(fmaf(__uint_as_float(v[i + 1]), sl2, -mb));
-          const __nv_bfloat162 pp = __floats2bfloat162_rn(p0, p1);
-          pmax = __hmax2(pmax, pp);
-          pk[(c + i) >> 1] = *reinterpret_cast<const uint32_t*>(&pp);
+          for (int c = 0; c < FT_BN / 8; ++c) mx = fmaxf(mx, fmaxf(s[4 * c + 2 * e], s[4 * c + 2 * e + 1]));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          mb[e] = mx * sl2;
         }
       }
-      // P V (and P 1) of the previous tile must have finished reading the P tile; it also orders the rescale below
-      if (j > 0) {
-        mbar_wait(&o_full[g], par ^ 1);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, pending != 0)) {
-          // exact power-of-two rescale of this row's O and L in TMEM (lanes with nothing due multiply by 1)
+      float scale_due[2];
 #pragma unroll
-          for (int c = 0; c < FT_D; c += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32(tO + c, v);
-            tmem_ld_wait();
+      for (int e = 0; e < 2; ++e) {
+        scale_due[e] = __int_as_float((127 - pending[e]) << 23);     // 2^-pending (1.0 when nothing is due)
+        mb[e] += (float)pending[e];
+      }
+      // one pass: p = 2^(s * sl2 - mb) -> packed bf16 (the A fragments of P V), running maximum of the packed values
+      uint32_t pa[FT_BN / 16][4];
+      float pm[2] = {0.f, 0.f};
+      float ts[2] = {0.f, 0.f};
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * scale_due);
-            tmem_st_32x32(tO + c, v);
-          }
-          uint32_t lv[16];
-          tmem_ld_32x16_ft(tL, lv);
-          tmem_ld_wait();
+      for (int c = 0; c < FT_BN / 8; ++c) {
 #pragma unroll
-          for (int i = 0; i < 16; ++i) lv[i] = __float_as_uint(__uint_as_float(lv[i]) * scale_due);
-          tmem_st_32x16_ft(tL, lv);
-          tmem_st_wait();
+        for (int e = 0; e < 2; ++e) {
+          const float p0 = ex2_approx(fmaf(s[4 * c + 2 * e], sl2, -mb[e]));
+          const float p1 = ex2_approx(fmaf(s[4 * c + 2 * e + 1], sl2, -mb[e]));
+          const uint32_t pp = pack_bf16x2(p0, p1);
+          const float2 pr = unpack_bf16x2(pp);
+          pm[e] = fmaxf(pm[e], fmaxf(pr.x, pr.y));
+          ts[e] += pr.x + pr.y;
+          pa[c >> 1][(c & 1) * 2 + e] = pp;
         }
       }
+      // exact power-of-two rescale of this row's O and L (rows with nothing due multiply by 1)
 #pragma unroll
-      for (int q = 0; q < FT_BN / 8; ++q) {
-        uint8_t* dst = prow + (q >> 3) * FT_TILE;            // key half (64 keys = one 128 B row of the sub-tile)
-        st_shared_v4(dst + (((q & 7) ^ (r & 7)) << 4), pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
+      for (int e = 0; e < 2; ++e) {
+        lsum[e] = fmaf(lsum[e], scale_due[e], ts[e]);
+#pragma unroll
+        for (int c = 0; c < FT_D / 8; ++c) {
+          o[4 * c + 2 * e] *= scale_due[e];
+          o[4 * c + 2 * e + 1] *= scale_due[e];
+        }
       }
-      tc_fence_before();
-      fence_proxy_async();                                   // P (generic writes) -> visible to the tensor core's smem reads
-      mbar_arrive(&p_full[g]);
+      {
+        const uint32_t v0 = smem_u32(sV + st * FT_TILE);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < FT_BN / 16; ++k)           // 16 keys per step: +16 key rows = 2048 B in the V tile (MN-major)
+          wgmma_m64n64k16_rs_tb(o, pa[k], wgmma_desc_mn_sw128(v0 + k * 16 * 128), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&kv_empty[st]);       // every MMA reading K_j / V_j has completed
+      if (++st == FT_NST) { st = 0; ph ^= 1; }
       // did this tile outgrow the reference?  (p <= 2^8 keeps bf16 / fp32 comfortably in range)
-      const float pm = fmaxf(__low2float(pmax), __high2float(pmax));
-      pending = pm > FT_TAU ? (int)((__float_as_uint(pm) >> 23) & 0xff) - 127 : 0;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float m = fmaxf(pm[e], __shfl_xor_sync(0xffffffffu, pm[e], 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        pending[e] = m > FT_TAU ? (int)((__float_as_uint(m) >> 23) & 0xff) - 127 : 0;
+      }
     }
     // O / L
-    mbar_wait(&o_full[g], (NT - 1) & 1);
-    tc_fence_after();
-    uint32_t lv[16];
-    tmem_ld_32x16_ft(tL, lv);
-    tmem_ld_wait();
-    const float inv = 1.f / __uint_as_float(lv[0]);
-    __nv_bfloat16* orow = out + (size_t)(q0 + g * FT_BM + r) * ldo + h * FT_D;
 #pragma unroll
-    for (int c = 0; c < FT_D; c += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32(tO + c, v);
-      tmem_ld_wait();
+    for (int e = 0; e < 2; ++e) {
+      float l = lsum[e];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const float inv = 1.f / l;
+      const int r = wg * 64 + 16 * w + (lane >> 2) + 8 * e;
+      __nv_bfloat16* orow = out + (size_t)(q0 + r) * ldo + h * FT_D + 2 * t4;
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        uint4 u;
-        u.x = pack_bf16x2(__uint_as_float(v[8 * q + 0]) * inv, __uint_as_float(v[8 * q + 1]) * inv);
-        u.y = pack_bf16x2(__uint_as_float(v[8 * q + 2]) * inv, __uint_as_float(v[8 * q + 3]) * inv);
-        u.z = pack_bf16x2(__uint_as_float(v[8 * q + 4]) * inv, __uint_as_float(v[8 * q + 5]) * inv);
-        u.w = pack_bf16x2(__uint_as_float(v[8 * q + 6]) * inv, __uint_as_float(v[8 * q + 7]) * inv);
-        reinterpret_cast<uint4*>(orow)[(c >> 3) + q] = u;
-      }
+      for (int c = 0; c < FT_D / 8; ++c)
+        *reinterpret_cast<uint32_t*>(orow + 8 * c) = pack_bf16x2(o[4 * c + 2 * e] * inv, o[4 * c + 2 * e + 1] * inv);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -326,7 +186,7 @@ static int encode_rows_map(CUtensorMap* map, const void* base, int ld, long long
 // Returns PGT_ERR_UNSUPPORTED when the shape is not covered (caller falls back to the mma.sync kernel).
 int mha_tc_launch(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, int clips, int L, int heads,
                   int d, void* out, int ldo, cudaStream_t stream) {
-  if (d != FT_D || L % (2 * FT_BM) != 0) return PGT_ERR_UNSUPPORTED;
+  if (d != FT_D || L % FT_BM != 0) return PGT_ERR_UNSUPPORTED;
   auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   if (!al(q) || !al(k) || !al(v) || !al(out) || ldq % 8 || ldk % 8 || ldv % 8 || ldo % 8) return PGT_ERR_UNSUPPORTED;
   CUtensorMap tq, tk, tv;
@@ -337,7 +197,7 @@ int mha_tc_launch(const void* q, int ldq, const void* k, int ldk, const void* v,
   if (rc != PGT_OK) return rc;
   static PerDeviceOnce once;
   PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(mha_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FT_SMEM); }));
-  dim3 grid(L / (2 * FT_BM), heads, clips);
+  dim3 grid(L / FT_BM, heads, clips);
   mha_tc_kernel<<<grid, FT_THREADS, FT_SMEM, stream>>>(tq, tk, tv, L, reinterpret_cast<__nv_bfloat16*>(out), ldo);
   PGT_LAUNCH_OK();
   return PGT_OK;

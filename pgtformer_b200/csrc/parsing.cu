@@ -1,7 +1,7 @@
 // Kernels specific to the face-parsing branch (BiSeNet / ResNet18, archs/pgtformer_arch.py:34-397 in the
 // reference): 3x3 stride-2 max-pool, global average pool, per-(frame,channel)
 // attention re-weighting, and the bilinear(align_corners) assembly of the three 19-class heads into the
-// 57(+7 pad)-channel conditioning map.  Every convolution of the branch (the 7x7 stem included) runs on the tcgen05
+// 57(+7 pad)-channel conditioning map.  Every convolution of the branch (the 7x7 stem included) runs on the wgmma
 // kernels with BatchNorm folded into weights / bias.
 #include <float.h>
 

@@ -1,9 +1,11 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA/TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
 // Everything here is device-only and header-only.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 namespace pgt {
 
@@ -127,142 +129,136 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ---------------------------------------------------------------- CTA pairs (cluster of 2, cta_group::2)
-// Mechanics validated by tools/probe/umma_2cta_probe.cu.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same smem location in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-// TMA loads whose complete_tx lands on a barrier given as a shared::cluster address (the pair leader's)
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1,
-                                                int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
-          "r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// A warpgroup (four consecutive warps 4k..4k+3) issues D[64 x N] (+)= A[64 x 16] * B[N x 16]^T with both operands read
+// from shared memory through matrix descriptors and the fp32 accumulator D in registers: d[4j + e] of warp w, lane l
+// holds row 16w + l/4 + 8 (e >> 1), column 8j + 2 (l % 4) + (e & 1).
 
-__device__ __forceinline__ void tma_load_5d_2sm(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1,
-                                                int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::
-          "r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {     // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* dst_smem) {   // one whole warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile: rows of 128 B, 8-row atoms 1024 B apart (SBO), LBO unused.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t saddr) {
+// K-major, 128-byte-swizzled operand: rows of 128 B as TMA SWIZZLE_128B writes them, 8-row groups `sbo` bytes apart
+// (1024 for a dense tile); LBO is unused for this layout.  Advancing the start address by 32 B steps K by 16.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t saddr, uint32_t sbo = 1024) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);          // start address  [0,14)
-  d |= static_cast<uint64_t>(0) << 16;                        // leading byte offset (ignored for SW128 K-major)
-  d |= static_cast<uint64_t>((1024 >> 4) & 0x3FFF) << 32;     // stride byte offset [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                        // descriptor version = 1 (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                        // layout type SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 16;                        // leading byte offset (unused)
+  d |= static_cast<uint64_t>((sbo >> 4) & 0x3FFF) << 32;      // stride byte offset [32,46)
+  d |= static_cast<uint64_t>(1) << 62;                        // layout type SWIZZLE_128B
   return d;
 }
 
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, dense.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// accumulator operand lists of the wrappers below: "+f"(d[i]) .. "+f"(d[i + n - 1])
+#define PGT_D4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define PGT_D8(i) PGT_D4(i), PGT_D4(i + 4)
+#define PGT_D24(i) PGT_D8(i), PGT_D8(i + 8), PGT_D8(i + 16)
+#define PGT_D32(i) PGT_D8(i), PGT_D8(i + 8), PGT_D8(i + 16), PGT_D8(i + 24)
+#define PGT_D64(i) PGT_D32(i), PGT_D32(i + 32)
+#define PGT_D128(i) PGT_D64(i), PGT_D64(i + 64)
+// m64nNk16, bf16 x bf16 -> fp32, both operands K-major from shared memory; acc == 0 overwrites D.
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : PGT_D8(0)
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_m64n48k16(float (&d)[24], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+      : PGT_D24(0)
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : PGT_D32(0)
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : PGT_D64(0)
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : PGT_D128(0)
+      : "l"(da), "l"(db), "r"(acc));
+}
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
+  if constexpr (N == 16) wgmma_m64n16k16(d, da, db, acc);
+  else if constexpr (N == 48) wgmma_m64n48k16(d, da, db, acc);
+  else if constexpr (N == 64) wgmma_m64n64k16(d, da, db, acc);
+  else if constexpr (N == 128) wgmma_m64n128k16(d, da, db, acc);
+  else { static_assert(N == 256, "wgmma N"); wgmma_m64n256k16(d, da, db, acc); }
 }
 
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
+// m64n64k16 with A from registers and B MN-major (transposed) from shared memory.  a[0..3] = bf16 pairs (row g, k 2t..),
+// (row g + 8, k 2t..), (row g, k 2t + 8..), (row g + 8, k 2t + 8..) with g = lane / 4, t = lane % 4 inside the warp's
+// 16 rows — the layout of columns [16 i, 16 i + 16) of an fp32 accumulator fragment, so a softmax result feeds the next
+// MMA without shared memory.
+__device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrives on `bar` once every previously issued tcgen05.mma of this thread has completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+      : PGT_D32(0)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
 }
 
-// M = 256 across a CTA pair: each CTA supplies its 128 rows of A and N/2 rows of B (same smem offsets in both),
-// each CTA's TMEM receives its 128 x N accumulator half.  Issued by the leader CTA only.
-__device__ __forceinline__ void umma_bf16_ss_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrives on the barrier at this smem offset in BOTH CTAs once the pair's MMAs issued so far have completed.
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
+// MN-major SW128 operand (rows = K, 64 MN-contiguous elements per 128-byte row; 8-row groups 1024 B apart): the B view
+// of a row-major [keys x d] tile such as V.
+__device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
+  d |= static_cast<uint64_t>(1) << 16;                        // LBO: next 64-element atom along MN (unused: N <= 64)
+  d |= static_cast<uint64_t>((1024 >> 4) & 0x3FFF) << 32;     // SBO: next 8 rows along K
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
 }
 
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <-> TMEM lane base+i).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+// Columns [C0, C0 + C) of a warpgroup's m64 accumulator -> fp32 rows of `scratch` (pitch `ld` floats, column C0 stored
+// at column 0, fragment row i at scratch row i).  The usual second half of a row-per-thread epilogue: after a barrier
+// over the warpgroups that share the scratch, thread t reads row t.
+template <int C0, int C, int R>
+__device__ __forceinline__ void acc_to_smem(const float (&d)[R], float* scratch, int ld, int warp_in_wg, int lane) {
+  static_assert(C0 % 8 == 0 && C % 8 == 0 && C0 + C <= 2 * R, "whole 8-column fragments inside D");
+  const int row = 16 * warp_in_wg + (lane >> 2);
+  float* p0 = scratch + row * ld + 2 * (lane & 3);
+  float* p1 = p0 + 8 * ld;
+#pragma unroll
+  for (int j = 0; j < C / 8; ++j) {
+    constexpr int f0 = C0 / 8;
+    const int f = f0 + j;
+    *reinterpret_cast<float2*>(p0 + 8 * j) = make_float2(d[4 * f + 0], d[4 * f + 1]);
+    *reinterpret_cast<float2*>(p1 + 8 * j) = make_float2(d[4 * f + 2], d[4 * f + 3]);
+  }
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+// compile-time loop (accumulator registers are only addressable with constant indices)
+template <int I, int N, typename F>
+__device__ __forceinline__ void static_for(F&& f) {
+  if constexpr (I < N) {
+    f(std::integral_constant<int, I>{});
+    static_for<I + 1, N>(f);
+  }
+}
+
+// 32 consecutive fp32 of one scratch row -> registers (the shape the epilogues consume)
+__device__ __forceinline__ void smem_row_32(const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float4 f = reinterpret_cast<const float4*>(src)[q];
+    v[4 * q + 0] = __float_as_uint(f.x); v[4 * q + 1] = __float_as_uint(f.y);
+    v[4 * q + 2] = __float_as_uint(f.z); v[4 * q + 3] = __float_as_uint(f.w);
+  }
+}
 
 }  // namespace pgt

@@ -1,4 +1,4 @@
-// The two Cin = 3 convolutions on tcgen05: Encoder.conv_in (3x3 / 1, archs/tdcrqvae3_arch.py:500-504) and the BiSeNet
+// The two Cin = 3 convolutions on wgmma: Encoder.conv_in (3x3 / 1, archs/tdcrqvae3_arch.py:500-504) and the BiSeNet
 // stem Resnet18.conv1 + bn1 + relu (7x7 / 2, archs/pgtformer_arch.py:95-99,110-112) read the fp32 NCHW image directly.
 // K = 27 / 147 is far too small for a TMA-fed implicit GEMM (no 16-byte channel vectors to tile), and a patch matrix
 // in HBM costs more than the conv, so the im2col happens inside the kernel:
@@ -6,13 +6,13 @@
 //   builders     (4 warps for 3x3, 8 for 7x7: two threads share a pixel, each gathers half of its K range): thread = one
 //                output pixel; gathers its 3 k^2 inputs (coalesced across the warp: lanes are neighbouring pixels),
 //                optional (x - mean) / std, bf16, and writes the row of the 128 x K A tile straight into the
-//                128B-swizzled K-major layout the UMMA descriptor expects (double buffered)
-//   next 4 warps epilogue: TMEM -> bias (+ReLU) -> optional GroupNorm(32) partial statistics -> bf16 -> swizzled
-//                staging tile -> one TMA store per tile
-//   last warp    tcgen05.mma issuer: K/16 instructions per tile against the weight tile resident in smem, accumulator
-//                [128 x 64] fp32 in TMEM (double buffered)
-// The 3x3 kernel runs two CTAs per SM (74 KB of shared memory, 128 TMEM columns each): a tile's chain
-// gather -> MMA -> epilogue -> store is latency-bound, a second CTA fills the gaps.
+//                128B-swizzled K-major layout the wgmma descriptor expects (double buffered)
+//   last 4 warps one warpgroup: 2 x K/16 wgmma 64 x 64 x 16 per tile (both 64-row halves) against the weight tile
+//                resident in smem, [128 x 64] fp32 accumulator in registers -> shared-memory exchange (thread = row)
+//                -> bias (+ReLU) -> optional GroupNorm(32) partial statistics -> bf16 -> swizzled staging tile -> one
+//                TMA store per tile
+// The 3x3 kernel runs two CTAs per SM (109 KB of shared memory each): a tile's chain gather -> MMA -> epilogue -> store
+// is latency-bound, a second CTA fills the gaps.
 #include <cudaTypedefs.h>
 
 #include "common.cuh"
@@ -25,6 +25,8 @@ namespace pgt {
 constexpr int RC_N = 64;                 // output channels (both layers)
 constexpr int RC_SUB = 128 * 128;        // [128 rows x 64 k] bf16 A sub-tile
 constexpr int RC_BSUB = RC_N * 128;      // [64 rows x 64 k] bf16 weight sub-tile
+constexpr int RC_XLD = RC_N + 4;         // accumulator exchange pitch (fp32)
+constexpr int RC_XCH = 128 * RC_XLD * 4;
 
 struct RgbConvParams {
   const float* x;                        // [F, 3, H, W] fp32
@@ -45,10 +47,10 @@ struct RgbCfg {
   static constexpr int NCH = KSTEPS * 2;                        // 16-byte chunks written per row
   static constexpr int A_BYTES = NSUB * RC_SUB;
   static constexpr int B_BYTES = NSUB * RC_BSUB;
-  static constexpr int SMEM = 2 * A_BYTES + B_BYTES + 2 * RC_SUB /*staging*/ + 256;
+  static constexpr int SMEM = 2 * A_BYTES + B_BYTES + 2 * RC_SUB /*staging*/ + RC_XCH + 256;
   static constexpr int BW = KS == 3 ? 4 : 8;                    // builder warps
   static constexpr int PARTS = BW / 4;                          // threads per output pixel
-  static constexpr int THREADS = (BW + 5) * 32;
+  static constexpr int THREADS = (BW + 4) * 32;
   static constexpr int PER_SM = KS == 3 ? 2 : 1;                // resident CTAs per SM
 };
 
@@ -88,34 +90,26 @@ rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
   uint8_t* sA = smem;                                   // [2][NSUB] sub-tiles
   uint8_t* sB = sA + 2 * Cfg::A_BYTES;                  // [NSUB] weight sub-tiles
   uint8_t* sO = sB + Cfg::B_BYTES;                      // [2] staging tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sO + 2 * RC_SUB);
-  uint64_t* a_full = bars;           // [2] builders (128) -> MMA
-  uint64_t* a_free = bars + 2;       // [2] MMA commit -> builders
-  uint64_t* acc_full = bars + 4;     // [2] MMA commit -> epilogue
-  uint64_t* acc_free = bars + 6;     // [2] epilogue (128) -> MMA
-  uint64_t* b_full = bars + 8;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 9);
+  float* xch = reinterpret_cast<float*>(sO + 2 * RC_SUB);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sO + 2 * RC_SUB + RC_XCH);
+  uint64_t* a_full = bars;           // [2] builders -> MMA warpgroup
+  uint64_t* a_free = bars + 2;       // [2] MMA warpgroup (one arrive per warp) -> builders
+  uint64_t* b_full = bars + 4;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int BW = Cfg::BW;
-  if (warp == BW + 4) {
+  if (warp == BW) {
     if (lane == 0) {
       tma_prefetch_desc(&tmW); tma_prefetch_desc(&tmO);
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&a_full[i], BW * 32); mbar_init(&a_free[i], 1); mbar_init(&acc_full[i], 1); mbar_init(&acc_free[i], 128);
-      }
+      for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], BW * 32); mbar_init(&a_free[i], 4); }
       mbar_init(b_full, 1);
       fence_barrier_init();
       mbar_arrive_expect_tx(b_full, Cfg::B_BYTES);
       for (int s = 0; s < Cfg::NSUB; ++s) tma_load_2d(sB + s * RC_BSUB, &tmW, b_full, s * 64, 0);
     }
     __syncwarp();
-    tmem_alloc<128>(tmem_ptr);
-    tc_fence_before();
   }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < BW) {
     // ------------------------------------------------------------------ builders
@@ -141,30 +135,41 @@ rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       fence_proxy_async();
       mbar_arrive(&a_full[buf]);
     }
-  } else if (warp < BW + 4) {
-    // ------------------------------------------------------------------ epilogue
+  } else {
+    // ------------------------------------------------------------------ MMA + epilogue warpgroup
     const int quad = warp & 3;
     const int r = quad * 32 + lane;
     const int et = threadIdx.x - BW * 32;
+    const float* xrow = xch + r * RC_XLD;
+    mbar_wait(b_full, 0);
     int it = 0;
     for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x, ++it) {
       const int buf = it & 1;
-      mbar_wait(&acc_full[buf], (it >> 1) & 1);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (uint32_t(quad * 32) << 16) + buf * RC_N;
-      // staging[buf] was last read by the store two tiles back
+      mbar_wait(&a_full[buf], (it >> 1) & 1);
+      float acc0[RC_N / 2], acc1[RC_N / 2];               // rows [0, 64) and [64, 128) of the tile
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < Cfg::KSTEPS; ++ks) {
+        const uint32_t a = smem_u32(sA + buf * Cfg::A_BYTES + (ks >> 2) * RC_SUB);
+        const uint64_t db = wgmma_desc_k_sw128(smem_u32(sB + (ks >> 2) * RC_BSUB)) + 2 * (ks & 3);
+        wgmma_bf16<RC_N>(acc0, wgmma_desc_k_sw128(a) + 2 * (ks & 3), db, ks != 0 ? 1u : 0u);
+        wgmma_bf16<RC_N>(acc1, wgmma_desc_k_sw128(a + 64 * 128) + 2 * (ks & 3), db, ks != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&a_free[buf]);
+      // staging[buf] was last read by the store two tiles back; the exchange by the previous tile's epilogue
       if (et == 0) bulk_wait_read<1>();
+      named_bar_sync(1, 128);
+      acc_to_smem<0, RC_N>(acc0, xch, RC_XLD, quad, lane);
+      acc_to_smem<0, RC_N>(acc1, xch + 64 * RC_XLD, RC_XLD, quad, lane);
       named_bar_sync(1, 128);
       uint8_t* srow = sO + buf * RC_SUB + r * 128;
 #pragma unroll
       for (int hb = 0; hb < 2; ++hb) {
         uint32_t v[32];
-        tmem_ld_32x32(t_row + hb * 32, v);
-        tmem_ld_wait();
-        if (hb == 1) {
-          tc_fence_before();
-          mbar_arrive(&acc_free[buf]);
-        }
+        smem_row_32(xrow + hb * 32, v);
         float f[32];
         const float4* b4 = reinterpret_cast<const float4*>(p.bias + hb * 32);
 #pragma unroll
@@ -197,36 +202,6 @@ rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       }
     }
     if (et == 0) bulk_wait0();
-  } else {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc_bf16(128, RC_N);
-    mbar_wait(b_full, 0);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x, ++it) {
-      const int buf = it & 1;
-      const uint32_t par = (it >> 1) & 1;
-      mbar_wait(&acc_free[buf], par ^ 1);
-      mbar_wait(&a_full[buf], par);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < Cfg::KSTEPS; ++ks) {
-          const uint64_t da = umma_desc_k_sw128(smem_u32(sA + buf * Cfg::A_BYTES + (ks >> 2) * RC_SUB)) + 2 * (ks & 3);
-          const uint64_t db = umma_desc_k_sw128(smem_u32(sB + (ks >> 2) * RC_BSUB)) + 2 * (ks & 3);
-          umma_bf16_ss(tmem_base + buf * RC_N, da, db, idesc, ks != 0 ? 1u : 0u);
-        }
-        umma_commit(&a_free[buf]);
-        umma_commit(&acc_full[buf]);
-      }
-      __syncwarp();
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == BW + 4) {
-    tc_fence_after();
-    tmem_dealloc<128>(tmem_base);
   }
 }
 
@@ -241,7 +216,7 @@ static int launch_rgb(const CUtensorMap& tw, const CUtensorMap& to, const RgbCon
   PGT_CUDA_OK(once.run([] {
     cudaError_t e = cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     if (e != cudaSuccess) return e;
-    // the resident-CTA count is fixed by the kernel's own budget (__launch_bounds__, shared memory, 128 TMEM columns), not
+    // the resident-CTA count is fixed by the kernel's own budget (__launch_bounds__, shared memory), not
     // asked of the occupancy calculator: it answered 1 for the 3x3 kernel and left half of every SM idle
     return cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                 cudaSharedmemCarveoutMaxShared);

@@ -1,22 +1,18 @@
-// Fused Swin MLP half-block on tcgen05 (C = 256):   out = x + W2 * GELU(W1 * LN(x) + b1) + b2
+// Fused Swin MLP half-block on wgmma (C = 256):   out = x + W2 * GELU(W1 * LN(x) + b1) + b2
 // Replaces LayerNorm(norm2) + Mlp(fc1, exact GELU, fc2) + residual of VSTSREncoderTransformerBlock
 // (modules/rstt_layers.py:116-132,335-336): five HBM passes over the token matrix (LN r/w, fc1 r/w, fc2 r+r/w)
 // become two (read x, write out); the 128 x 256 hidden tile never leaves the SM.
 //
-// The per-tile chain  load -> LN -> GEMM1 -> GELU -> GEMM2 -> +x -> store  is strictly serial, and its ALU phases
-// (LN, GELU, residual) cost several times the two MMAs, so each CTA runs TWO tile pipelines ("groups") side by side:
-// while one group's warps wait for a TMA load or an MMA, the other group's warps own the issue slots.
-//
-// Per CTA, persistent over 128-token tiles (640 threads):
-//   warp 0        TMA producer of the weight k-blocks (W1 / W2, 256 x 64 each, 3-deep ring shared by both groups)
-//   warp 1        tcgen05.mma issuer for both groups in the fixed order  G2(b') G1(a) G2(a) G1(b)  (b half a tile behind
-//                 a);  group g accumulates
-//                 in TMEM columns [256 g, 256 g + 256) — GEMM2 reuses GEMM1's columns once the GELU pass has read them
-//   warp 2+g      DMA of group g: TMA load of the x tile, re-fetch of x (an L2 hit) for the residual once GEMM2 has
-//                 consumed the buffer, TMA store of the finished tile
-//   warps 4..19   compute, 8 per group: LayerNorm of the tile in place, GELU epilogue written back in place as the
-//                 A operand of GEMM2, final epilogue acc + b2 + x in place.  One 64 KB buffer per group carries
-//                 x -> LN(x) -> hidden -> x (again) -> out.
+// Per CTA, persistent over 128-token tiles (320 threads):
+//   warps 0..7    two consumer warpgroups; warpgroup h owns rows [64h, 64h + 64) of the tile through the whole chain
+//                 LN -> GEMM1 -> GELU -> GEMM2 -> +b2 +x, so the in-place rewrites of the tile buffer only ever wait for
+//                 the warpgroup's own MMAs: LayerNorm of its rows in place (two threads per row), wgmma 64 x 256 x 16
+//                 (fp32 accumulators in registers), GELU epilogue written back in place as the A operand of GEMM2, final
+//                 epilogue acc + b2 + x in place.  Accumulators reach the row-per-thread epilogues through a 64 x 64
+//                 fp32 exchange per warpgroup.  One 64 KB buffer carries x -> LN(x) -> hidden -> x (again) -> out.
+//   warp 8        TMA producer of the weight k-blocks (W1 / W2, 256 x 64 each, 3-deep ring)
+//   warp 9        DMA: TMA load of the x tile, re-fetch of x (an L2 hit) for the residual once GEMM2 has consumed the
+//                 buffer, TMA store of the finished tile
 #include <cudaTypedefs.h>
 
 #include "common.cuh"
@@ -31,8 +27,11 @@ constexpr int SM_BM = 128;
 constexpr int SM_SUB = SM_BM * 128;            // one [128 x 64] bf16 sub-tile: 16 KB
 constexpr int SM_WST = 3;                      // weight ring depth
 constexpr int SM_WBYTES = SM_C * 128;          // one [256 x 64] weight k-block: 32 KB
-constexpr int SM_THREADS = 640;
-constexpr int SM_SMEM = 2 * 4 * SM_SUB /*tiles*/ + SM_WST * SM_WBYTES + 2 * 128 * 8 /*xch*/ + 256;
+constexpr int SM_THREADS = 320;
+constexpr int SM_XLD = 68;                     // accumulator exchange pitch (fp32)
+constexpr int SM_XCH = SM_BM * SM_XLD * 4;
+constexpr int SM_SMEM = 4 * SM_SUB /*tile*/ + SM_WST * SM_WBYTES + SM_XCH + 128 * 8 /*LN pair exchange*/ + 256;
+static_assert(SM_SMEM <= 232448, "swin_mlp smem budget");
 
 struct SwinMlpParams {
   int T, m_tiles;
@@ -44,21 +43,59 @@ struct SwinMlpParams {
   float* gn_stats;      // optional [m_tiles][4][32][2]
 };
 
-struct SmGroupBars {
-  uint64_t x_full, res_full, y_ready, acc1_full, h_ready, acc2_full, out_ready;
+struct SmBars {
+  uint64_t x_full, res_full, acc2_done, out_ready;
 };
 
-// compute warps of one group
-__device__ __forceinline__ void swin_mlp_compute(const SwinMlpParams& p, uint8_t* sX, float2* xch, SmGroupBars* gb,
-                                                 uint32_t t_acc, int g, int n_it, int quad, int half, int lane) {
-  const int r = quad * 32 + lane;
-  const uint32_t t_row = t_acc + (uint32_t(quad * 32) << 16);
-  const int c_lo = half * 128;
-  for (int it = 0; it < n_it; ++it) {
-    const int tile = blockIdx.x + (2 * it + g) * gridDim.x;
-    const uint32_t par = it & 1;
+// consumer warpgroups: warp 0..7 of the CTA, warpgroup wg owns rows [64 wg, 64 wg + 64) of every tile
+__device__ __forceinline__ void swin_mlp_compute(const SwinMlpParams& p, uint8_t* sX, uint8_t* sW, float* xacc, float2* xln,
+                                                 SmBars* bar, uint64_t* w_full, uint64_t* w_empty, int warp, int lane) {
+  const int wg = warp >> 2, w = warp & 3;
+  const int half = w >> 1;                            // which 32 columns of a 64-column group this thread takes
+  const int rl = (w & 1) * 32 + lane;                 // row inside the warpgroup's 64
+  const int r = wg * 64 + rl;                         // row of the tile
+  const int quad = r >> 5;
+  const int bar_id = 1 + wg;                          // named barrier of this warpgroup
+  float* xw = xacc + wg * 64 * SM_XLD;                // this warpgroup's exchange rows
+  const float* xrow = xw + rl * SM_XLD;
+  const uint32_t a_rows = smem_u32(sX) + wg * 64 * 128;
+  int st = 0;
+  uint32_t ph = 0;
+  uint32_t par = 0;
+  float acc[SM_C / 2];
+
+  // one GEMM over the four k-blocks of the ring (W1 or W2), A = this warpgroup's rows of the tile buffer
+  auto gemm = [&]() {
+    int prev = -1;
+    for (int kb = 0; kb < 4; ++kb) {
+      mbar_wait(&w_full[st], ph);
+      const uint64_t da = wgmma_desc_k_sw128(a_rows + kb * SM_SUB);
+      const uint64_t db = wgmma_desc_k_sw128(smem_u32(sW) + st * SM_WBYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_bf16<SM_C>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&w_empty[prev]); }
+      prev = st;
+      if (++st == SM_WST) { st = 0; ph ^= 1; }
+    }
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&w_empty[prev]);
+  };
+  // columns [64 G, 64 G + 64) of the accumulators -> exchange; then this thread's 32 of them for row r
+  auto exchange = [&](auto gc, uint32_t (&v)[32]) {
+    constexpr int G = decltype(gc)::value;
+    named_bar_sync(bar_id, 128);
+    acc_to_smem<64 * G, 64>(acc, xw, SM_XLD, w, lane);
+    named_bar_sync(bar_id, 128);
+    smem_row_32(xrow + half * 32, v);
+  };
+
+  for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x, par ^= 1) {
     // ---- LayerNorm(x) in place -> A operand of GEMM1 (two threads per row; the halves meet through smem)
-    mbar_wait(&gb->x_full, par);
+    mbar_wait(&bar->x_full, par);
     float s = 0.f, q = 0.f;
 #pragma unroll
     for (int sub = 0; sub < 2; ++sub) {
@@ -71,16 +108,16 @@ __device__ __forceinline__ void swin_mlp_compute(const SwinMlpParams& p, uint8_t
         q += a.x * a.x + a.y * a.y + b.x * b.x + b.y * b.y + cc.x * cc.x + cc.y * cc.y + d.x * d.x + d.y * d.y;
       }
     }
-    if (half == 0) xch[r] = make_float2(s, q);
-    named_bar_sync(5 + g, 256);
+    if (half == 0) xln[r] = make_float2(s, q);
+    named_bar_sync(bar_id, 128);
     if (half == 1) {
-      const float2 o = xch[r];
+      const float2 o = xln[r];
       s += o.x; q += o.y;
-      xch[r] = make_float2(s, q);
+      xln[r] = make_float2(s, q);
     }
-    named_bar_sync(5 + g, 256);
+    named_bar_sync(bar_id, 128);
     if (half == 0) {
-      const float2 o = xch[r];
+      const float2 o = xln[r];
       s = o.x; q = o.y;
     }
     const float mean = s * (1.f / SM_C);
@@ -117,18 +154,17 @@ __device__ __forceinline__ void swin_mlp_compute(const SwinMlpParams& p, uint8_t
       }
     }
     fence_proxy_async();
-    mbar_arrive(&gb->y_ready);
-    // ---- hidden = GELU(acc + b1) -> A operand of GEMM2 (in place: GEMM1 has finished reading the buffer)
-    mbar_wait(&gb->acc1_full, par);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c0 = c_lo; c0 < c_lo + 128; c0 += 32) {
+    named_bar_sync(bar_id, 128);
+    gemm();                                            // GEMM1
+    // ---- hidden = GELU(acc + b1) -> A operand of GEMM2 (in place: this warpgroup's GEMM1 has finished reading its rows)
+    static_for<0, SM_C / 64>([&](auto gc) {
+      constexpr int G = decltype(gc)::value;
       uint32_t v[32];
-      tmem_ld_32x32(t_row + c0, v);
-      tmem_ld_wait();
+      exchange(gc, v);
+      const int c0 = G * 64 + half * 32;
       const float4* b4 = reinterpret_cast<const float4*>(p.b1 + c0);
-      uint8_t* dst = sX + (c0 >> 6) * SM_SUB + r * 128;
-      const int ch0 = (c0 & 63) >> 3;
+      uint8_t* dst = sX + G * SM_SUB + r * 128;
+      const int ch0 = half * 4;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float4 ba = __ldg(b4 + 2 * i), bb = __ldg(b4 + 2 * i + 1);
@@ -139,23 +175,23 @@ __device__ __forceinline__ void swin_mlp_compute(const SwinMlpParams& p, uint8_t
         o.w = pack_bf16x2(gelu_erf(__uint_as_float(v[8 * i + 6]) + bb.z), gelu_erf(__uint_as_float(v[8 * i + 7]) + bb.w));
         *reinterpret_cast<uint4*>(dst + (((ch0 + i) ^ (r & 7)) << 4)) = o;
       }
-    }
-    tc_fence_before();
+    });
     fence_proxy_async();
-    mbar_arrive(&gb->h_ready);
-    // ---- out = acc + b2 + x in place over the re-fetched x tile (then TMA-stored by the group's DMA warp)
-    mbar_wait(&gb->acc2_full, par);
-    tc_fence_after();
-    mbar_wait(&gb->res_full, par);
-#pragma unroll 1
-    for (int c0 = c_lo; c0 < c_lo + 128; c0 += 32) {
+    named_bar_sync(bar_id, 128);
+    gemm();                                            // GEMM2
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bar->acc2_done);
+    // ---- out = acc + b2 + x in place over the re-fetched x tile (then TMA-stored by the DMA warp)
+    mbar_wait(&bar->res_full, par);
+    static_for<0, SM_C / 64>([&](auto gc) {
+      constexpr int G = decltype(gc)::value;
       uint32_t v[32];
-      tmem_ld_32x32(t_row + c0, v);
-      tmem_ld_wait();
+      exchange(gc, v);
+      const int c0 = G * 64 + half * 32;
       float f[32];
       const float4* b4 = reinterpret_cast<const float4*>(p.b2 + c0);
-      uint8_t* row = sX + (c0 >> 6) * SM_SUB + r * 128;
-      const int ch0 = (c0 & 63) >> 3;
+      uint8_t* row = sX + G * SM_SUB + r * 128;
+      const int ch0 = half * 4;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float4 ba = __ldg(b4 + 2 * i), bb = __ldg(b4 + 2 * i + 1);
@@ -173,10 +209,9 @@ __device__ __forceinline__ void swin_mlp_compute(const SwinMlpParams& p, uint8_t
       }
       if (p.gn_stats != nullptr)
         gn_chunk_stats<8>(f, p.gn_stats + (((size_t)tile * 4 + quad) * 32 + c0 / 8) * 2, 0, lane);
-    }
-    tc_fence_before();
+    });
     fence_proxy_async();
-    mbar_arrive(&gb->out_ready);
+    mbar_arrive(&bar->out_ready);
   }
 }
 
@@ -186,111 +221,57 @@ swin_mlp_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
                 const SwinMlpParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];     // no static smem in this kernel: the window starts 1024-aligned
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* sW = smem + 2 * 4 * SM_SUB;                  // weight ring behind the two tile buffers
-  float2* xch = reinterpret_cast<float2*>(sW + SM_WST * SM_WBYTES);     // [2 groups][128 rows] (sum, sumsq)
-  SmGroupBars* gbar = reinterpret_cast<SmGroupBars*>(xch + 256);         // [2]
-  uint64_t* w_full = reinterpret_cast<uint64_t*>(gbar + 2);              // [SM_WST]
+  uint8_t* sX = smem;                                   // the tile buffer: 4 sub-tiles of [128 x 64]
+  uint8_t* sW = smem + 4 * SM_SUB;                      // weight ring
+  float* xacc = reinterpret_cast<float*>(sW + SM_WST * SM_WBYTES);        // [128 rows][SM_XLD]
+  float2* xln = reinterpret_cast<float2*>(sW + SM_WST * SM_WBYTES + SM_XCH);   // [128 rows] (sum, sumsq)
+  SmBars* bar = reinterpret_cast<SmBars*>(xln + 128);
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(bar + 1);               // [SM_WST]
   uint64_t* w_empty = w_full + SM_WST;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(w_empty + SM_WST);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmX); tma_prefetch_desc(&tmO); tma_prefetch_desc(&tmW1); tma_prefetch_desc(&tmW2);
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(&gbar[g].x_full, 1); mbar_init(&gbar[g].res_full, 1);
-      mbar_init(&gbar[g].y_ready, 256); mbar_init(&gbar[g].acc1_full, 1);
-      mbar_init(&gbar[g].h_ready, 256); mbar_init(&gbar[g].acc2_full, 1);
-      mbar_init(&gbar[g].out_ready, 256);
-    }
-    for (int i = 0; i < SM_WST; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 1); }
+    mbar_init(&bar->x_full, 1); mbar_init(&bar->res_full, 1);
+    mbar_init(&bar->acc2_done, 8); mbar_init(&bar->out_ready, 256);
+    for (int i = 0; i < SM_WST; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc<512>(tmem_ptr);
-    tc_fence_before();
-  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  // this CTA's tiles: blockIdx.x + j * gridDim.x; group g owns the j = 2 i + g
-  const int n_loc = (int)blockIdx.x < p.m_tiles ? (p.m_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  const int n_grp[2] = {(n_loc + 1) >> 1, n_loc >> 1};
-
-  // GEMM order of the CTA (weight producer and MMA issuer walk the same list).  Group b runs half a tile behind group a:
-  //   ... G2(b, i-1)  G1(a, i)  G2(a, i)  G1(b, i)  G2(b, i) ...
-  // so that one group's TMA load / LayerNorm / store phases fall into the other's GEMM + GELU phases.  With the two groups
-  // in phase (G1a G1b G2a G2b) every CTA of the grid loaded, normalised and stored at the same moments, and each x load
-  // queued behind 19 MB of simultaneous requests.
-  auto for_each_gemm = [&](auto&& fn) {
-    for (int it = 0; it < n_grp[0]; ++it) {
-      if (it >= 1 && it - 1 < n_grp[1]) fn(1, 1, it - 1);
-      fn(0, 0, it);
-      fn(1, 0, it);
-      if (it < n_grp[1]) fn(0, 1, it);
+  if (warp == 8) {
+    // ------------------------------------------------------------------ weight producer: W1 then W2 per tile
+    int st = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x) {
+      for (int gemm = 0; gemm < 2; ++gemm) {
+        for (int kb = 0; kb < 4; ++kb) {
+          mbar_wait(&w_empty[st], ph ^ 1);
+          if (elect_one()) {
+            mbar_arrive_expect_tx(&w_full[st], SM_WBYTES);
+            tma_load_2d(sW + st * SM_WBYTES, gemm == 0 ? &tmW1 : &tmW2, &w_full[st], kb * 64, 0);
+          }
+          __syncwarp();
+          if (++st == SM_WST) { st = 0; ph ^= 1; }
+        }
+      }
     }
-    if (n_grp[1] >= 1 && n_grp[1] == n_grp[0]) fn(1, 1, n_grp[1] - 1);
-  };
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ weight producer (same order as the MMA warp)
-    int st = 0;
-    uint32_t ph = 0;
-    for_each_gemm([&](int gemm, int /*g*/, int /*it*/) {
-      for (int kb = 0; kb < 4; ++kb) {
-        mbar_wait(&w_empty[st], ph ^ 1);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&w_full[st], SM_WBYTES);
-          tma_load_2d(sW + st * SM_WBYTES, gemm == 0 ? &tmW1 : &tmW2, &w_full[st], kb * 64, 0);
-        }
-        __syncwarp();
-        if (++st == SM_WST) { st = 0; ph ^= 1; }
-      }
-    });
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = umma_idesc_bf16(SM_BM, SM_C);
-    int st = 0;
-    uint32_t ph = 0;
-    for_each_gemm([&](int gemm, int g, int it) {
-      const uint32_t par = it & 1;
-      uint8_t* sX = smem + g * 4 * SM_SUB;
-      mbar_wait(gemm == 0 ? &gbar[g].y_ready : &gbar[g].h_ready, par);
-      tc_fence_after();
-      for (int kb = 0; kb < 4; ++kb) {
-        mbar_wait(&w_full[st], ph);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t da = umma_desc_k_sw128(smem_u32(sX + kb * SM_SUB));
-          const uint64_t db = umma_desc_k_sw128(smem_u32(sW + st * SM_WBYTES));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16_ss(tmem_base + g * SM_C, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          umma_commit(&w_empty[st]);
-          if (kb == 3) umma_commit(gemm == 0 ? &gbar[g].acc1_full : &gbar[g].acc2_full);
-        }
-        __syncwarp();
-        if (++st == SM_WST) { st = 0; ph ^= 1; }
-      }
-    });
-  } else if (warp < 4) {
-    // ------------------------------------------------------------------ DMA warp of group g
-    const int g = warp - 2;
-    uint8_t* sX = smem + g * 4 * SM_SUB;
-    for (int it = 0; it < n_grp[g]; ++it) {
-      const int tile = blockIdx.x + (2 * it + g) * gridDim.x;
-      const uint32_t par = it & 1;
+  } else if (warp == 9) {
+    // ------------------------------------------------------------------ DMA warp
+    uint32_t par = 0;
+    for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x, par ^= 1) {
       if (lane == 0) {
-        mbar_arrive_expect_tx(&gbar[g].x_full, 4 * SM_SUB);
-        for (int kb = 0; kb < 4; ++kb) tma_load_2d(sX + kb * SM_SUB, &tmX, &gbar[g].x_full, kb * 64, tile * SM_BM);
+        mbar_arrive_expect_tx(&bar->x_full, 4 * SM_SUB);
+        for (int kb = 0; kb < 4; ++kb) tma_load_2d(sX + kb * SM_SUB, &tmX, &bar->x_full, kb * 64, tile * SM_BM);
       }
       __syncwarp();
-      mbar_wait(&gbar[g].acc2_full, par);        // GEMM2 has consumed the buffer: bring x back for the residual
+      mbar_wait(&bar->acc2_done, par);          // GEMM2 has consumed the buffer: bring x back for the residual
       if (lane == 0) {
-        mbar_arrive_expect_tx(&gbar[g].res_full, 4 * SM_SUB);
-        for (int kb = 0; kb < 4; ++kb) tma_load_2d(sX + kb * SM_SUB, &tmX, &gbar[g].res_full, kb * 64, tile * SM_BM);
+        mbar_arrive_expect_tx(&bar->res_full, 4 * SM_SUB);
+        for (int kb = 0; kb < 4; ++kb) tma_load_2d(sX + kb * SM_SUB, &tmX, &bar->res_full, kb * 64, tile * SM_BM);
       }
       __syncwarp();
-      mbar_wait(&gbar[g].out_ready, par);
+      mbar_wait(&bar->out_ready, par);
       if (lane == 0) {
         for (int kb = 0; kb < 4; ++kb) tma_store_2d(&tmO, sX + kb * SM_SUB, kb * 64, tile * SM_BM);
         bulk_commit();
@@ -300,17 +281,8 @@ swin_mlp_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__
     }
     if (lane == 0) bulk_wait0();
   } else {
-    // ------------------------------------------------------------------ compute warps
-    const int g = (warp - 4) >> 3;
-    swin_mlp_compute(p, smem + g * 4 * SM_SUB, xch + g * 128, &gbar[g], tmem_base + g * SM_C, g, n_grp[g], warp & 3,
-                     ((warp - 4) & 7) >> 2, lane);
-  }
+    swin_mlp_compute(p, sX, sW, xacc, xln, bar, w_full, w_empty, warp, lane);
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 

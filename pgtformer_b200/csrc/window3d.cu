@@ -7,8 +7,8 @@
 // This is the widening row SURVEY 8(f) #4, not the hot path: TDRQVAE runs two such layers on the 32x32 latent grid
 // only.  One CTA per (window, head); q / k / v rows of the head are gathered into shared memory (padded tokens take the
 // projection of a zero row, i.e. the qkv bias or zero), a warp owns 16 query rows: S = q k^T and O = P v on
-// mma.sync.m16n8k16 with fp32 softmax in registers.  The tcgen05 kernel of window_attn_tc.cu is specialised to the
-// 3x4x4 windows of the PGTFormer path (N = 48 fills TMA boxes and UMMA tiles exactly); N = 75 with padding does not.
+// mma.sync.m16n8k16 with fp32 softmax in registers.  The wgmma kernel of window_attn_tc.cu is specialised to the
+// 3x4x4 windows of the PGTFormer path (N = 48 fills TMA boxes and wgmma tiles exactly); N = 75 with padding does not.
 #include "common.cuh"
 #include "tmap.cuh"
 

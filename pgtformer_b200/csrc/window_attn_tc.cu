@@ -1,23 +1,22 @@
 // Shifted-window spatio-temporal attention core (WindowAttention3D, modules/rstt_layers.py:195-234, with the roll /
 // window_partition / window_reverse / shift mask of VSTSREncoderTransformerBlock :301-329 and EncoderLayer :552-568)
-// on TMA + tcgen05, sm_100a.
+// on TMA + wgmma, sm_90a.
 //
 // Work unit: a PAIR of 3x4x4 windows (2 x 48 tokens) and one 64-column chunk of the heads (2 heads of d = 32, or one of
 // d = 64).  Persistent CTAs, warp-specialised:
-//   warp 0     TMA producer.  A window's q / k / v rows of one chunk are ONE 5-D box [64 ch, 4 x, 4 y, 3 frames, clip] of
+//   warp 8     TMA producer.  A window's q / k / v rows of one chunk are ONE 5-D box [64 ch, 4 x, 4 y, 3 frames, clip] of
 //              the [T, 3C] qkv matrix (128B swizzle) — the roll by -shift is a coordinate offset, window_partition is the
 //              box shape.  Windows in the last window row / column of a shifted block wrap around the frame: they are 2
 //              (or 4) half (quarter) boxes, landing one after the other, so their rows sit in a permuted order; attention
 //              does not care as long as bias and mask are permuted alike, which the host does once per layer (below).
 //              4-deep ring of (k | v | q) chunk tiles.
-//   warp 1     tcgen05.mma issuer.  Per head and pair:  S = Q K^T as two 128x48xd MMAs (window 0 from tile row 0, window
-//              1 through a view that starts 16 rows before the tile, so that its rows land on TMEM lanes 64..111 and every
-//              warp of a softmax group sees ONE window), then O = P V as two 128 x d x 48 MMAs (V consumed MN-major
-//              straight from its TMA tile).  For d = 32 the scores are double-buffered in TMEM and S runs two heads ahead.
-//   warps 2-5 / 6-9   two softmax groups that alternate chunks: thread = query row, tcgen05.ld of its 48 scores,
-//              t = s * scale*log2e + table, exp2, row sum — overlapping the P V of the previous head —, then that head's
-//              O * (1/sum) from TMEM -> bf16 -> 64 (128) contiguous bytes of the token's output row in HBM
-//              (window_reverse + roll back are index math), then bf16 P into the swizzled A tile.
+//   warps 0-3 / 4-7   two warpgroups that alternate chunks.  Per head and window: S = Q K^T as one wgmma 64 x 48 x d
+//              (window 0 from tile row 0, window 1 through a view that starts 16 rows before it, so that its 48 rows are
+//              rows 16..63 of the MMA), softmax on the register fragments (t = s * scale*log2e + table, exp2, row max and
+//              sum across the four lanes of a row), P converted in registers into the A operand of O = P V (wgmma
+//              64 x 64 x 16 with A from registers, V read MN-major straight from its TMA tile; for d = 32 the N = 64
+//              view spans both heads of the chunk and the other head's half is ignored), then O * (1/sum) -> bf16 -> the
+//              token's output row in HBM (window_reverse + roll back are index math).
 // Bias / mask table (built at load time by the engine, fp16, already multiplied by log2 e):
 //   tab[type][head][j = key/8][row][8]   type 0 interior, 1 x-wrapped (right edge), 2 y-wrapped (bottom edge), 3 corner;
 //   entry = relative_position_bias[pi_t(row)][pi_t(key)] + (-100 where the reference's shift mask separates the two
@@ -34,11 +33,10 @@ constexpr int WT_N = 48;                          // tokens per window
 constexpr int WT_TILE = 2 * WT_N * 128;           // 12 KB: one operand chunk of a window pair (96 rows x 128 B)
 constexpr int WT_STAGE = 3 * WT_TILE;             // k | v | q
 constexpr int WT_NST = 4;
-constexpr int WT_PTILE = 128 * 128;               // 16 KB: P tile in TMEM-lane space
-constexpr int WT_THREADS = 64 + 256;
+constexpr int WT_THREADS = 256 + 32;
 constexpr int WT_HEADS = 8;
 constexpr int WT_TAB_BYTES = WT_HEADS * 6 * WT_N * 16;            // 36 KB: one type of the fp16 table
-constexpr int WT_SMEM = 2048 /*pad*/ + WT_NST * WT_STAGE + 2 * WT_PTILE + WT_TAB_BYTES + 512 /*barriers*/ + 1024 /*align*/;
+constexpr int WT_SMEM = 2048 /*pad*/ + WT_NST * WT_STAGE + WT_TAB_BYTES + 512 /*barriers*/ + 1024 /*align*/;
 
 struct WinParams {
   int clips, H, W, C, heads, d, shift;
@@ -48,27 +46,6 @@ struct WinParams {
   float sl2;                                         // d^-1/2 * log2(e)
   const uint4* tab;                                  // [4][heads][6][48] x 16 B
 };
-
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// MN-major SW128 operand (V: key rows x d contiguous): 8 key rows per 1024-byte atom.
-__device__ __forceinline__ uint64_t wt_desc_mn_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>((16384 >> 4) & 0x3FFF) << 16;    // LBO: next 64-column atom (never used: N <= 64)
-  d |= static_cast<uint64_t>((1024 >> 4) & 0x3FFF) << 32;     // SBO: next 8 key rows
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
 
 struct WinCoord {
   int clip, x0, y0, xs, ys;        // xs / ys: 1 when the window wraps in x / y
@@ -106,52 +83,31 @@ window_attn_tc_kernel(const __grid_constant__ CUtensorMap tmI0, const __grid_con
                       const __grid_constant__ CUtensorMap tmI2, const __grid_constant__ CUtensorMap tmI3,
                       const WinParams p) {
   constexpr int HPC = 64 / D;                                   // heads per 64-column chunk
-  constexpr int NSB = D == 32 ? 2 : 1;                          // score buffers per group in TMEM
-  constexpr int TM_O = NSB * 96;                                // group-relative TMEM column of O (2 windows x D)
-  static_assert(TM_O + 2 * D <= 256, "TMEM budget per group");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* ring = smem + 2048;                                  // [NST][k | v | q]
-  uint8_t* sP = ring + WT_NST * WT_STAGE;                       // [2 groups][128 rows x 128 B]
-  uint8_t* sTab = sP + 2 * WT_PTILE;                            // type-0 table
+  uint8_t* ring = smem + 2048;                                  // [NST][k | v | q] (the window-1 Q view reaches 2 KB back)
+  uint8_t* sTab = ring + WT_NST * WT_STAGE;                     // type-0 table
   uint64_t* bars = reinterpret_cast<uint64_t*>(sTab + WT_TAB_BYTES);
   uint64_t* st_full = bars;                                     // [NST]
-  uint64_t* st_empty = st_full + WT_NST;                        // [NST]
-  uint64_t* s_full = st_empty + WT_NST;                         // [2 groups][2 buffers]
-  uint64_t* p_full = s_full + 4;                                // [2]
-  uint64_t* o_full = p_full + 2;                                // [2]
-  uint64_t* o_empty = o_full + 2;                               // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(o_empty + 2);
+  uint64_t* st_empty = st_full + WT_NST;                        // [NST] one arrive per warp of the consuming warpgroup
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const CUtensorMap* tmI[4] = {&tmI0, &tmI1, &tmI2, &tmI3};
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(tmI[i]);
-    for (int i = 0; i < WT_NST; ++i) { mbar_init(&st_full[i], 1); mbar_init(&st_empty[i], 1); }
-    for (int i = 0; i < 4; ++i) mbar_init(&s_full[i], 1);
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(&p_full[g], 128);
-      mbar_init(&o_full[g], 1);
-      mbar_init(&o_empty[g], 128);
-    }
+    for (int i = 0; i < WT_NST; ++i) { mbar_init(&st_full[i], 1); mbar_init(&st_empty[i], 4); }
     fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc<512>(tmem_ptr);
-    tc_fence_before();
   }
   // type-0 table -> shared memory (all threads)
   for (int i = threadIdx.x; i < WT_TAB_BYTES / 16; i += WT_THREADS) reinterpret_cast<uint4*>(sTab)[i] = __ldg(p.tab + i);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   const int my_pairs = (p.n_pairs - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // pairs blockIdx.x, +gridDim.x, ..
   const int NCH = p.n_chunks;
-  const int items = my_pairs * (NCH / 2) * HPC;                 // per group: (pair, chunk = g mod 2, head in chunk)
+  const int items = my_pairs * (NCH / 2) * HPC;                 // per warpgroup: (pair, chunk = g mod 2, head in chunk)
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer
     int st = 0;
     uint32_t ph = 0;
@@ -189,207 +145,129 @@ window_attn_tc_kernel(const __grid_constant__ CUtensorMap tmI0, const __grid_con
         if (++st == WT_NST) { st = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc_s = umma_idesc_bf16(128, WT_N);
-    constexpr uint32_t idesc_o = umma_idesc_bf16(128, D) | (1u << 16);
-    auto stage_of = [&](int g, int n, int& st, uint32_t& ph) {    // global chunk index of item n of group g
-      const int q = (n / HPC) * 2 + g;
-      st = q % WT_NST; ph = (q / WT_NST) & 1;
-    };
-    auto issue_s = [&](int g, int n) {                         // caller has checked that the stage is full
-      int st; uint32_t ph;
-      stage_of(g, n, st, ph);
-      const int hh = n % HPC;
-      tc_fence_after();
-      if (elect_one()) {
-        uint8_t* sK = ring + st * WT_STAGE;
-        uint8_t* sQ = sK + 2 * WT_TILE;
-        const uint32_t tS = tmem_base + g * 256 + (n % NSB) * 96;
-        const uint32_t koff = hh * 64;                           // second head of a d = 32 chunk: +64 B inside the row
-#pragma unroll
-        for (int wi = 0; wi < 2; ++wi) {
-          // window 1 through the view that starts 16 rows before the tile: its rows land on lanes 64..111
-          const uint64_t da = umma_desc_k_sw128(smem_u32(sQ) + koff - (wi ? 16 * 128 : 0));
-          const uint64_t db = umma_desc_k_sw128(smem_u32(sK) + koff + wi * WT_N * 128);
-#pragma unroll
-          for (int k = 0; k < D / 16; ++k) umma_bf16_ss(tS + wi * WT_N, da + 2 * k, db + 2 * k, idesc_s, k != 0 ? 1u : 0u);
-        }
-        umma_commit(&s_full[g * 2 + (n % NSB)]);
-      }
-      __syncwarp();
-    };
-    auto issue_o = [&](int g, int n) {
-      int st; uint32_t ph;
-      stage_of(g, n, st, ph);
-      const int hh = n % HPC;
-      tc_fence_after();
-      if (elect_one()) {
-        uint8_t* sV = ring + st * WT_STAGE + WT_TILE;
-        const uint32_t tO = tmem_base + g * 256 + TM_O;
-        const uint32_t voff = hh * 64;                           // d = 32: half-atom view of the MN-major V tile
-        const uint64_t da = umma_desc_k_sw128(smem_u32(sP + g * WT_PTILE));
-#pragma unroll
-        for (int wi = 0; wi < 2; ++wi) {
-#pragma unroll
-          for (int k = 0; k < WT_N / 16; ++k) {
-            const uint64_t db = wt_desc_mn_sw128(smem_u32(sV) + voff + (wi * WT_N + k * 16) * 128);
-            umma_bf16_ss(tO + wi * D, da + 2 * k, db, idesc_o, k != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit(&o_full[g]);
-        if (hh == HPC - 1) umma_commit(&st_empty[st]);           // every MMA reading this stage has been issued
-      }
-      __syncwarp();
-    };
-    // Event loop: per group, P V of item no[g] as soon as its P is in shared memory (and O drained), S of item
-    // ns[g] (at most NSB ahead of the P V) as soon as its stage has landed — whichever is ready first, so neither a
-    // slow group nor a late TMA box holds the other group's MMAs back.
-    int ns[2] = {0, 0}, no[2] = {0, 0};
-    uint32_t idle = 0;
-    while (no[0] < items || no[1] < items) {
-      bool progressed = false;
-#pragma unroll
-      for (int g = 0; g < 2; ++g) {
-        if (no[g] < items && no[g] < ns[g]) {
-          const int n = no[g];
-          const bool ready = mbar_test_wait(&p_full[g], n & 1) && (n == 0 || mbar_test_wait(&o_empty[g], (n - 1) & 1));
-          if (__all_sync(0xffffffffu, ready)) {                // warp-uniform decision
-            issue_o(g, n);
-            no[g] = n + 1;
-            progressed = true;
-          }
-        }
-        if (ns[g] < items && ns[g] < no[g] + NSB) {
-          const int n = ns[g];
-          int st; uint32_t ph;
-          stage_of(g, n, st, ph);
-          const bool ready = n % HPC != 0 || mbar_test_wait(&st_full[st], ph);
-          if (__all_sync(0xffffffffu, ready)) {
-            issue_s(g, n);
-            ns[g] = n + 1;
-            progressed = true;
-          }
-        }
-      }
-      if (progressed) idle = 0;
-      else if (++idle > (1u << 28)) __trap();                    // protocol bug: fail the launch instead of hanging
-    }
-  } else {
-    // ------------------------------------------------------------------ softmax / output groups
-    const int g = (warp - 2) >> 2;
-    const int quad = warp & 3;
-    const int L = quad * 32 + lane;                              // TMEM lane = row of the P tile
-    const int wi = quad >> 1;                                    // window of the pair this warp sees
-    const int rw_raw = L - wi * 64;                              // row inside the window (valid < 48)
-    const bool valid_row = rw_raw < WT_N;
-    const int rw = valid_row ? rw_raw : WT_N - 1;
-    const uint32_t lane_base = uint32_t(quad * 32) << 16;
-    const uint32_t tG = tmem_base + lane_base + g * 256;
-    const uint32_t tO = tG + TM_O + wi * D;
-    uint8_t* prow = sP + g * WT_PTILE + L * 128;
-    // state carried from item n to its deferred output step
-    float inv_prev = 0.f;
-    __nv_bfloat16* dst_prev = nullptr;
-    bool store_prev = false;
-    int cur_pair = -1, type = 0;
-    __nv_bfloat16* orow = nullptr;                               // output row of this thread's token (current pair)
-    bool win_ok = false;
-
-    auto finish_prev = [&](int n_prev) {                         // O(n_prev) * 1/sum -> bf16 -> HBM
-      mbar_wait(&o_full[g], n_prev & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int half = 0; half < D / 32; ++half) {
-        uint32_t v[32];
-        tmem_ld_32x32(tO + half * 32, v);
-        tmem_ld_wait();
-        if (half == D / 32 - 1) { tc_fence_before(); mbar_arrive(&o_empty[g]); }
-        if (store_prev) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 u;
-            u.x = pack_bf16x2(__uint_as_float(v[8 * q + 0]) * inv_prev, __uint_as_float(v[8 * q + 1]) * inv_prev);
-            u.y = pack_bf16x2(__uint_as_float(v[8 * q + 2]) * inv_prev, __uint_as_float(v[8 * q + 3]) * inv_prev);
-            u.z = pack_bf16x2(__uint_as_float(v[8 * q + 4]) * inv_prev, __uint_as_float(v[8 * q + 5]) * inv_prev);
-            u.w = pack_bf16x2(__uint_as_float(v[8 * q + 6]) * inv_prev, __uint_as_float(v[8 * q + 7]) * inv_prev);
-            reinterpret_cast<uint4*>(dst_prev)[half * 4 + q] = u;
-          }
-        }
-      }
-    };
+  } else if (warp < 8) {
+    // ------------------------------------------------------------------ attention warpgroups
+    const int g = warp >> 2;
+    const int w = warp & 3;
+    const int t4 = lane & 3;
+    const int mr = 16 * w + (lane >> 2);                         // MMA rows mr and mr + 8 of this thread (0..63)
+    int cur_pair = -1;
+    int type[2] = {0, 0};
+    __nv_bfloat16* orow[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // [window][row half]
+    bool ok[2][2] = {{false, false}, {false, false}};
+    int rwin[2][2] = {{0, 0}, {0, 0}};                           // window row of [window][row half] (clamped)
 
     for (int n = 0; n < items; ++n) {
       const int hh = n % HPC;
-      const int cidx = n / HPC;                                  // this group's chunk counter
+      const int cidx = n / HPC;                                  // this warpgroup's chunk counter
       const int pair = blockIdx.x + (cidx / (NCH / 2)) * gridDim.x;
       const int chunk = (cidx % (NCH / 2)) * 2 + g;
       const int head = chunk * HPC + hh;
+      const int q = 2 * cidx + g;                                // position of the chunk in the producer's sequence
+      const int st = q % WT_NST;
+      const uint32_t ph = (q / WT_NST) & 1;
       if (pair != cur_pair) {
         cur_pair = pair;
-        const int w = 2 * pair + wi;
-        win_ok = w < p.n_windows;
-        const WinCoord wc = win_coord(p, win_ok ? w : 2 * pair);
-        type = wc.ys * 2 + wc.xs;
-        orow = p.out + (size_t)win_token(p, wc, rw) * p.ldo;
-      }
-      // bias / mask row of this thread: type 0 from shared memory, wrapped types from L2 (generic pointer)
-      const uint4* trow = (type == 0 ? reinterpret_cast<const uint4*>(sTab) : p.tab + (size_t)type * (WT_TAB_BYTES / 16)) +
-                          (size_t)head * 6 * WT_N + rw;
-      uint4 bq[6];
 #pragma unroll
-      for (int j = 0; j < 6; ++j) bq[j] = trow[j * WT_N];
-      mbar_wait(&s_full[g * 2 + (n % NSB)], (n / NSB) & 1);
-      tc_fence_after();
-      uint32_t s0[32], s1[16];
-      const uint32_t tS = tG + (n % NSB) * 96 + wi * WT_N;
-      tmem_ld_32x32(tS, s0);
-      tmem_ld_32x16(tS + 32, s1);
-      tmem_ld_wait();
-      float t[WT_N];
-      float mx = -1e30f;
+        for (int wi = 0; wi < 2; ++wi) {
+          const int wn = 2 * pair + wi;
+          const bool win_ok = wn < p.n_windows;
+          const WinCoord wc = win_coord(p, win_ok ? wn : 2 * pair);
+          type[wi] = wc.ys * 2 + wc.xs;
 #pragma unroll
-      for (int j = 0; j < 6; ++j) {
-        const uint32_t u[4] = {bq[j].x, bq[j].y, bq[j].z, bq[j].w};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float2 b2 = __half22float2(*reinterpret_cast<const __half2*>(&u[e]));
-          const int c = j * 8 + 2 * e;
-          const float sa = __uint_as_float(c < 32 ? s0[c] : s1[c - 32]);
-          const float sb = __uint_as_float(c + 1 < 32 ? s0[c + 1] : s1[c + 1 - 32]);
-          t[c] = fmaf(sa, p.sl2, b2.x);
-          t[c + 1] = fmaf(sb, p.sl2, b2.y);
-          mx = fmaxf(mx, fmaxf(t[c], t[c + 1]));
+          for (int e = 0; e < 2; ++e) {
+            const int rw = mr + 8 * e - (wi ? 16 : 0);           // window 1 occupies MMA rows 16..63
+            ok[wi][e] = win_ok && rw >= 0 && rw < WT_N;
+            rwin[wi][e] = rw < 0 ? 0 : (rw >= WT_N ? WT_N - 1 : rw);
+            orow[wi][e] = p.out + (size_t)win_token(p, wc, rwin[wi][e]) * p.ldo;
+          }
         }
       }
-      float sum = 0.f;
-      uint32_t pk[WT_N / 2];
+      if (hh == 0) mbar_wait(&st_full[st], ph);
+      const uint32_t sK = smem_u32(ring + st * WT_STAGE);
+      const uint32_t sV = sK + WT_TILE;
+      const uint32_t sQ = sV + WT_TILE;
+      const uint32_t koff = hh * D * 2;                          // second head of a d = 32 chunk: +64 B inside the row
 #pragma unroll
-      for (int c = 0; c < WT_N; c += 2) {
-        const float e0 = ex2_approx(t[c] - mx), e1 = ex2_approx(t[c + 1] - mx);
-        sum += e0 + e1;
-        pk[c >> 1] = pack_bf16x2(e0, e1);
+      for (int wi = 0; wi < 2; ++wi) {
+        // ---- S = Q K^T for window wi
+        float s[WT_N / 2];
+        const uint64_t da = wgmma_desc_k_sw128(sQ + koff + (wi ? (WT_N - 16) * 128 : 0));
+        const uint64_t db = wgmma_desc_k_sw128(sK + koff + wi * WT_N * 128);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < D / 16; ++k) wgmma_bf16<WT_N>(s, da + 2 * k, db + 2 * k, k != 0 ? 1u : 0u);
+        wgmma_commit();
+        // bias / mask of this thread's two rows (type 0 from shared memory, wrapped types from L2) while the MMA runs
+        const uint32_t* tb = reinterpret_cast<const uint32_t*>(type[wi] == 0 ? reinterpret_cast<const uint4*>(sTab)
+                                                                             : p.tab + (size_t)type[wi] * (WT_TAB_BYTES / 16));
+        uint32_t bw[2][6];
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+          for (int j = 0; j < 6; ++j) bw[e][j] = tb[(((size_t)head * 6 + j) * WT_N + rwin[wi][e]) * 4 + t4];
+        wgmma_wait<0>();
+        // ---- softmax over the 48 keys of each row: 12 per lane, the row's four lanes combine by shuffles
+        float mx[2] = {-1e30f, -1e30f};
+#pragma unroll
+        for (int j = 0; j < 6; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float2 b2 = __half22float2(*reinterpret_cast<const __half2*>(&bw[e][j]));
+            s[4 * j + 2 * e] = fmaf(s[4 * j + 2 * e], p.sl2, b2.x);
+            s[4 * j + 2 * e + 1] = fmaf(s[4 * j + 2 * e + 1], p.sl2, b2.y);
+            mx[e] = fmaxf(mx[e], fmaxf(s[4 * j + 2 * e], s[4 * j + 2 * e + 1]));
+          }
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 1));
+          mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 2));
+        }
+        float sum[2] = {0.f, 0.f};
+        uint32_t pa[3][4];                                       // P as the A operand, one k16 step per entry
+#pragma unroll
+        for (int j = 0; j < 6; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float e0 = ex2_approx(s[4 * j + 2 * e] - mx[e]), e1 = ex2_approx(s[4 * j + 2 * e + 1] - mx[e]);
+            sum[e] += e0 + e1;
+            pa[j >> 1][(j & 1) * 2 + e] = pack_bf16x2(e0, e1);
+          }
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 1);
+          sum[e] += __shfl_xor_sync(0xffffffffu, sum[e], 2);
+        }
+        // ---- O = P V (N = 64: the chunk's 64 V columns; d = 32 uses the half of head hh)
+        float o[32];
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < WT_N / 16; ++k)
+          wgmma_m64n64k16_rs_tb(o, pa[k], wgmma_desc_mn_sw128(sV + (wi * WT_N + k * 16) * 128), k != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (wi == 1 && hh == HPC - 1) {                          // every MMA reading this stage has completed
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&st_empty[st]);
+        }
+        // ---- O * (1/sum) -> bf16 -> the token's output row
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          if (!ok[wi][e]) continue;
+          const float inv = 1.f / sum[e];
+          __nv_bfloat16* dst = orow[wi][e] + chunk * 64 + hh * D + 2 * t4;
+#pragma unroll
+          for (int j = 0; j < D / 8; ++j) {
+            float v0, v1;                                      // columns hh * D + 8 j + 2 t4 (+1)
+            if (HPC == 1 || hh == 0) { v0 = o[(j * 4) + 2 * e]; v1 = o[(j * 4) + 2 * e + 1]; }
+            else { v0 = o[((D / 8) + j) * 4 + 2 * e]; v1 = o[((D / 8) + j) * 4 + 2 * e + 1]; }
+            *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(v0 * inv, v1 * inv);
+          }
+        }
       }
-      // the previous head's P V has had the whole softmax above to complete: drain it, which also frees the P tile
-      if (n > 0) finish_prev(n - 1);
-#pragma unroll
-      for (int j = 0; j < 6; ++j)
-        *reinterpret_cast<uint4*>(prow + ((j ^ (L & 7)) << 4)) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-      tc_fence_before();
-      fence_proxy_async();                                       // P (generic writes) -> visible to the tensor core
-      mbar_arrive(&p_full[g]);
-      inv_prev = 1.f / sum;
-      dst_prev = orow + chunk * 64 + hh * D;
-      store_prev = valid_row && win_ok;
     }
-    if (items > 0) finish_prev(items - 1);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 

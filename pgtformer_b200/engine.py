@@ -1,4 +1,4 @@
-"""B200 forward engine for PGTFormer: one-time weight repack into kernel layouts + the launch
+"""H100 forward engine for PGTFormer: one-time weight repack into kernel layouts + the launch
 sequence of `PGTFormer.forward` / `TDCRQVAE3.forward` over libpgt_b200.so.
 
 Data layout in HBM (DESIGN.md §3): every activation is channels-last bf16 — feature maps
@@ -93,7 +93,7 @@ class Engine:
         self.arch = Arch(network_g)
         self.dev = torch.device(device)
         if self.dev.type != 'cuda':
-            raise RuntimeError('pgtformer_b200 has no CPU path: the engine needs a CUDA (sm_100a) device')
+            raise RuntimeError('pgtformer_b200 has no CPU path: the engine needs a CUDA (sm_90a) device')
         self.w = {}
         with torch.cuda.device(self.dev):
             self._sd = {k: v.detach().to(self.dev) for k, v in state_dict.items()}
@@ -129,7 +129,7 @@ class Engine:
                 heads = sd[name].shape[1]
                 idx = sd[p + '.relative_position_index'].view(-1).long()
                 w[p + '.bias_tab'] = sd[name].float()[idx].view(48, 48, heads).permute(2, 0, 1).contiguous()
-                w[p + '.tab16'] = ops.window_tables(w[p + '.bias_tab'])     # tcgen05 window kernel: bias + mask, 4 box layouts
+                w[p + '.tab16'] = ops.window_tables(w[p + '.bias_tab'])     # wgmma window kernel: bias + mask, 4 box layouts
                 w[p + '.qkv.weight'] = _pack_lin(torch.cat([sd[p + '.q.weight'], sd[p + '.kv.weight']], 0).float())
                 w[p + '.qkv.bias'] = torch.cat([sd[p + '.q.bias'], sd[p + '.kv.bias']], 0).float().contiguous()
                 blk = p[:-len('.attn')]
@@ -165,7 +165,7 @@ class Engine:
     fuse_cat_in_place = True  # SFT concat: encoder / decoder level outputs written straight into the concat buffer
     _fusing = False           # set per forward: SFT fusion active (w > 0)
     fuse_conv_out = True      # decoder norm_out + SiLU + conv_out (64 -> 3) as one kernel (conv_out.cu)
-    window_tc = True          # window attention core on TMA + tcgen05 (window_attn_tc.cu)
+    window_tc = True          # window attention core on TMA + wgmma (window_attn_tc.cu)
     fuse_ln_qkv = True        # norm1 + q/kv projection of the C=256 Swin blocks as one kernel
     fuse_swin_mlp = True      # LN + fc1 + GELU + fc2 + residual of the C=256 Swin blocks as one kernel
     # GroupNorm+SiLU applied inside the consuming 3x3 conv (pgt_conv_gn_bf16, bit-identical).  Off by default: the
@@ -203,7 +203,7 @@ class Engine:
         if gn_out and self.fuse_gn_stats and cout % 32 == 0 and cout // 32 in (2, 4, 8, 16, 32) and out.is_contiguous():
             tpf = ops.conv_tiles_per_frame(H, W, cout, kw.get('ksize', 3), stride, kw.get('pad_lo', 1))
             if tpf > 0:
-                stats = self._new(Fr * tpf * 4 * 64, dtype=torch.float32)      # [tile][TMEM quadrant][32 groups][2]
+                stats = self._new(Fr * tpf * 4 * 64, dtype=torch.float32)      # [tile][32-row quadrant][32 groups][2]
                 out._pgt_gn = (stats, tpf * 4)
         if fused_ab is not None:
             kw.pop('ksize', None); kw.pop('stride', None); kw.pop('pad_lo', None)
@@ -666,7 +666,7 @@ class Engine:
         z_e = self._lin(h.view(T, -1), 'quant_conv', a.embed_dim, out_dtype=torch.float32)
         codes = torch.empty(T, dtype=torch.int64, device=self.dev)
         z_q = self._new(T, a.embed_dim, dtype=torch.float32)
-        if 'codebook.pack' not in self.w:                  # bf16 copy + norms for the tcgen05 argmin, once per load
+        if 'codebook.pack' not in self.w:                  # bf16 copy + norms for the wgmma argmin, once per load
             self.w['codebook.pack'] = ops.codebook_pack(self.w['codebook'], a.n_embed)
         ops.l2_argmin_tc(z_e, self.w['codebook'], self.w['codebook.pack'], a.n_embed, codes, z_q)
         loss = (z_e - z_q).pow(2).mean()

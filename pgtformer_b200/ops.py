@@ -295,7 +295,7 @@ WINDOW_MODE_N64 = 0          # d = 32 heads: 0 = P V with a half-atom N = 32 vie
 
 
 def window_attention_tc(qkv, clips, H, W, C, heads, shift, tab16, out, mode_n64=None):
-    """TMA + tcgen05 window attention core; returns None when the shape is not covered (caller uses window_attention)."""
+    """TMA + wgmma window attention core; returns None when the shape is not covered (caller uses window_attention)."""
     lib = L.load()
     assert qkv.dtype == torch.bfloat16 and tab16.dtype == torch.float16 and tab16.is_contiguous()
     rc = lib.pgt_window_attention_tc(_p(qkv), _rows(qkv)[2], clips, H, W, C, heads, shift, _p(tab16), _p(out),
@@ -363,7 +363,7 @@ def last_l2_argmin_fallbacks():
 
 
 def l2_argmin_tc(z, codebook, pack, K, idx_out, quant=None):
-    """tcgen05 nearest-codebook argmin (exact, see l2_argmin_tc.cu); falls back to the exhaustive kernel for shapes the
+    """wgmma nearest-codebook argmin (exact, see l2_argmin_tc.cu); falls back to the exhaustive kernel for shapes the
     tensor-core kernel does not cover (K % 256, E % 128, E > 512)."""
     lib = L.load()
     T, E = z.shape

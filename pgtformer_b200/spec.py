@@ -147,9 +147,9 @@ class Arch:
         if any(y % x != 0 for x, y in zip(self.code_shape[:2], self.latent_shape[:2])):
             raise ValueError('incompatible code shape or latent shape')      # tdcrqvae3_arch.py:234
         if self.tf != 3 or self.num_frames != 3 or any(w != (4, 4) for w in self.window_sizes):
-            raise ValueError('B200 path is built for 3-frame clips and 4x4x3 windows')
+            raise ValueError('the CUDA path is built for 3-frame clips and 4x4x3 windows')
         if self.code_shape[2] != 1:
-            raise ValueError('B200 path is built for quantiser depth 1')
+            raise ValueError('the CUDA path is built for quantiser depth 1')
         # levels that carry a window-attention layer (curr_res walk of tdcrqvae3_arch.py:482-510)
         self.level_has_attn = tuple((self.resolution >> i) in self.attn_resolutions
                                     for i in range(self.num_levels))

@@ -1,4 +1,4 @@
-"""Video-Swin `BasicLayer` (SURVEY 8(f) #4, second half) on the B200 kernels: depth x SwinTransformerBlock3D
+"""Video-Swin `BasicLayer` (SURVEY 8(f) #4, second half) on the H100 kernels: depth x SwinTransformerBlock3D
 (`modules/swin.py:170-271` of the reference) = LayerNorm -> qkv projection -> 3-D shifted-window attention with zero
 padding to window multiples (pgt_window3d_attention) -> proj + residual -> LayerNorm -> Mlp (ratio 4, exact GELU) +
 residual.  Activations are channels-last bf16 token rows [B*D*H*W, C]; every op is a call into libpgt_b200.so."""
@@ -87,7 +87,7 @@ class BasicLayer(nn.Module):
         """x: [B, C, D, H, W] on a CUDA device -> same shape and dtype (`modules/swin.py:380-405`)."""
         from . import ops
         if not x.is_cuda:
-            raise RuntimeError('pgtformer_b200 has no CPU path: BasicLayer needs a CUDA (sm_100a) device')
+            raise RuntimeError('pgtformer_b200 has no CPU path: BasicLayer needs a CUDA (sm_90a) device')
         B, C, D, H, W = x.shape
         heads = self.num_heads
         T = B * D * H * W

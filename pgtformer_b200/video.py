@@ -1,4 +1,4 @@
-"""Streaming video restoration around the model — the B200 counterpart of the reference's frame loop
+"""Streaming video restoration around the model — the GPU counterpart of the reference's frame loop
 (`inference.py:21-82` `process_video_ffmpeg` + `apply_net_to_frames :12-19` + `rgbnp2tensor :6-10`).
 
 The reference restores frame i from the window (f[i-1], f[i], f[i+1]) — the first and the last frame are duplicated

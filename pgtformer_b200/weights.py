@@ -2,8 +2,8 @@
 
 No trained weights are reachable offline (SURVEY F10), so every test / bench uses a synthetic
 state dict that is a pure function of (name, shape, kind, seed): independent of module
-construction order, hence reproducible on the GPU box (where the reference does not exist) and
-loadable into the reference here with `load_state_dict(strict=True)` to mint golden vectors.
+construction order, hence reproducible wherever the tests run (without the reference) and
+loadable into the reference with `load_state_dict(strict=True)` to mint golden vectors.
 Scales follow PyTorch's default init (U(+-1/sqrt(fan_in))) so activations stay O(1); biases,
 norm affine terms and the relative-position tables are deliberately non-trivial so that index /
 bias mistakes are visible in parity tests.

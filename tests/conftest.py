@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100: run with -m gpu)')
 
 
 def pytest_collection_modifyitems(config, items):
@@ -48,3 +48,10 @@ def synth_sd(arch_spec):
 def load_golden(name):
     import torch
     return torch.load(os.path.join(ROOT, 'tests', 'golden', name), map_location='cpu')
+
+
+def golden_sample(t, g, key):
+    """The elements of t that golden record g keeps for `key` (oracle/make_golden.py: a strided flat sample of the
+    reference tensor, whose full shape t must have)."""
+    assert tuple(t.shape) == tuple(g[key + '_shape']), (tuple(t.shape), g[key + '_shape'])
+    return t.float().cpu().reshape(-1)[::g[key + '_stride']]

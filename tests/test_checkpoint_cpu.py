@@ -1,6 +1,5 @@
 """Checkpoint formats of the drop-in class (SURVEY 8f #3): HF `config.json + model.safetensors` directories
-(`PGTFormer.from_pretrained`, inference.py:118) and BasicSR `.pth` files with `params_ema` (inference_cn.py:124-126),
-including a directory written by the REFERENCE class itself when /root/reference is present."""
+(`PGTFormer.from_pretrained`, inference.py:118) and BasicSR `.pth` files with `params_ema` (inference_cn.py:124-126)."""
 import os
 
 import pytest
@@ -52,20 +51,6 @@ def test_basicsr_params_ema_pth(network_g, tmp_path):
     assert not missing.missing_keys and not missing.unexpected_keys
     for k, v in m2.state_dict().items():
         assert torch.equal(v, want[k]), k
-
-
-@pytest.mark.skipif(not os.path.isdir('/root/reference/archs'), reason='reference tree not mounted')
-def test_directory_written_by_the_reference_class_loads(network_g, tmp_path):
-    """What `PGTFormer.from_pretrained("kepeng/pgtformer-base")` downloads is a directory the reference class wrote."""
-    from archs.pgtformer_arch import PGTFormer
-    from oracle import reference_loader as RL
-    ref = RL.build_reference_model(network_g)
-    ref.save_pretrained(str(tmp_path))
-    ours = PGTFormer.from_pretrained(str(tmp_path))
-    rsd, osd = ref.state_dict(), ours.state_dict()
-    assert set(rsd) == set(osd) and len(osd) == 961        # registration order differs, names do not
-    for k in rsd:
-        assert torch.equal(rsd[k], osd[k]), k
 
 
 def test_submodule_load_and_refresh_drop_the_packed_engine(network_g):

@@ -495,7 +495,7 @@ def test_conv_up2x_groupnorm_stats(Fr, H, W, C):
 @pytest.mark.parametrize('ks,stride,pad,norm,Fr,H,W', [(3, 1, 1, False, 3, 32, 48), (7, 2, 3, True, 3, 32, 48),
                                                        (3, 1, 1, False, 2, 20, 36), (7, 2, 3, True, 5, 64, 64)])
 def test_conv_rgb_tensor_core(ks, stride, pad, norm, Fr, H, W):
-    """Cin = 3 convs (encoder conv_in, BiSeNet stem) with the im2col done inside the tcgen05 kernel; ragged last tile,
+    """Cin = 3 convs (encoder conv_in, BiSeNet stem) with the im2col done inside the wgmma kernel; ragged last tile,
     normalisation before the zero padding, fused GroupNorm statistics."""
     from pgtformer_b200.engine import _pack_rgb
     o = ops()

@@ -12,7 +12,7 @@ F9); the full-forward checks therefore (a) bound lq_feat / logits, (b) report co
 import pytest
 import torch
 
-from conftest import load_golden
+from conftest import golden_sample, load_golden
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -23,6 +23,13 @@ def relerr(got, ref):
     assert got.shape == ref.shape, (got.shape, ref.shape)
     assert torch.isfinite(got).all()
     return ((got - ref).abs().max() / ref.abs().max().clamp_min(1e-12)).item()
+
+
+def sampled_relerr(got, g, key):
+    """relerr against a golden tensor kept as a strided sample: max |got - ref| over the sample / max |ref| overall."""
+    s = golden_sample(got, g, key)
+    assert torch.isfinite(got).all()
+    return ((s - g[key].float()).abs().max() / max(g[key + '_absmax'], 1e-12)).item()
 
 
 def psnr(got, ref):
@@ -152,19 +159,19 @@ def test_forward_against_reference_golden(model, fixture):
     g = load_golden(fixture)
     x = golden_input(g['seed'], g['b'], g['H']).to(DEV)
     out, logits, lq = model(x, w=1, adain=True)
-    assert out.shape == g['out'].shape and logits.shape == g['logits'].shape and lq.shape == g['lq_feat'].shape
     assert out.dtype == logits.dtype == lq.dtype == torch.float32
-    assert relerr(lq, g['lq_feat']) < 2.5e-2
-    assert relerr(logits, g['logits']) < 2.5e-2
-    gcodes = g['logits'].argmax(-1)
+    # the fixture keeps a strided sample of each reference tensor (golden_sample checks the full shape) and max|ref|
+    assert sampled_relerr(lq, g, 'lq_feat') < 2.5e-2
+    assert sampled_relerr(logits, g, 'logits') < 2.5e-2
+    gcodes = g['codes']
     agree = (logits.argmax(-1).cpu() == gcodes).float().mean().item()
     print('code agreement vs reference: %.4f' % agree)
     assert agree > 0.90
     # teacher-forced reference codes -> decoder output comparable with the reference's `out`
     out_tf, _, _ = model(x, w=1, adain=True, force_codes=gcodes)
-    p = psnr(out_tf, g['out'])
+    p = psnr(golden_sample(out_tf, g, 'out'), g['out'])
     print('teacher-forced PSNR vs reference out: %.2f dB' % p)
-    assert p > 35.0 and relerr(out_tf, g['out']) < 8e-2
+    assert p > 35.0 and sampled_relerr(out_tf, g, 'out') < 8e-2
     # code_only contract (stage II) returns (logits, lq_feat)
     lo, lq2 = model(x, w=1, adain=True, code_only=True)
     assert torch.equal(lo, logits) and torch.equal(lq2, lq)
@@ -183,7 +190,7 @@ def test_vq_path_codes_against_reference_golden(model):
     print('L2-argmin code agreement vs reference: %.4f' % agree)
     assert agree > 0.9
     out, _, codes2 = model.forward_vq(x)
-    assert torch.equal(codes, codes2) and out.shape == g['vq_out'].shape
+    assert torch.equal(codes, codes2) and tuple(out.shape) == tuple(g['vq_out_shape'])
 
 
 def test_batch_equals_per_clip(model):
@@ -223,16 +230,8 @@ def test_cuda_graph_replay_matches_eager(model):
 
 
 def _record(name, res):
-    """Keeps the measured parity numbers with the run (gpurun_out/ travels back from the GPU box)."""
+    """Prints the measured parity numbers with the test output."""
     import json
-    import os
-    d = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'gpurun_out')
-    try:
-        os.makedirs(d, exist_ok=True)
-        with open(os.path.join(d, 'parity_%s.json' % name), 'w') as f:
-            json.dump(res, f, indent=1)
-    except OSError:
-        pass
     print('parity[%s] %s' % (name, json.dumps(res)))
 
 
@@ -261,8 +260,9 @@ def test_forward_against_reference_golden_full_size(model, size):
 
 
 def test_demo_video_psnr_against_reference(model):
-    """First 8 frames of the reference's assets/inputdemovideo.mp4 through the streaming pipeline vs the reference's
-    own `inference.py` loop on the same frames (fixture: oracle/make_golden.py --video), same synthetic checkpoint."""
+    """First 8 frames of the reference's assets/inputdemovideo.mp4 (downscaled to 128^2) through the streaming pipeline
+    vs the reference's own `inference.py` loop on the same frames (fixture: oracle/make_golden.py --video), same
+    synthetic checkpoint."""
     import sys
     import os
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tools'))

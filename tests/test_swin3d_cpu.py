@@ -1,5 +1,5 @@
-"""Video-Swin BasicLayer (SURVEY 8(f) #4): the oracle restatement against fixtures minted from the reference's own
-`modules/swin.py` (oracle/make_golden.py --swin), and against the live reference module when /root/reference is present."""
+"""Video-Swin BasicLayer (SURVEY 8(f) #4): the oracle restatement and the drop-in's state dict against fixtures minted
+from the reference's own `modules/swin.py` (oracle/make_golden.py --swin)."""
 import os
 
 import pytest
@@ -28,20 +28,12 @@ def test_oracle_matches_reference_golden(case):
 
 
 def test_dropin_state_dict_is_reference_compatible():
-    """Same parameter / buffer names and shapes as the reference's BasicLayer (checked against the live module when the
-    reference tree is present, against the recorded count otherwise)."""
+    """Same parameter / buffer names, shapes and dtypes as the reference's BasicLayer, and the same relative position
+    index (fixture: the reference module's state dict spec, oracle/make_golden.py --swin)."""
     from modules.swin import BasicLayer
     ours = BasicLayer(256, 4, 8, (5, 5, 5)).state_dict()
     assert len(ours) == 52 and ours['blocks.1.attn.relative_position_bias_table'].shape == (729, 8)
-    from oracle.reference_loader import REFERENCE_ROOT, _ensure_paths, reference_available
-    if not reference_available():
-        pytest.skip('reference tree not present')
-    import importlib.util
-    _ensure_paths()
-    spec = importlib.util.spec_from_file_location('_pgt_reference.modules.swin', os.path.join(REFERENCE_ROOT, 'modules', 'swin.py'))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    ref = mod.BasicLayer(256, 4, 8, (5, 5, 5)).state_dict()
-    assert set(ours) == set(ref)
-    assert all(ours[k].shape == ref[k].shape and ours[k].dtype == ref[k].dtype for k in ref)
-    assert torch.equal(ours['blocks.0.attn.relative_position_index'], ref['blocks.0.attn.relative_position_index'])
+    ref = load_golden('swin3d_state_dict_spec.pt')
+    assert set(ours) == set(ref['spec'])
+    assert all(tuple(ours[k].shape) == shape and str(ours[k].dtype) == dtype for k, (shape, dtype) in ref['spec'].items())
+    assert torch.equal(ours['blocks.0.attn.relative_position_index'], ref['relative_position_index'].long())

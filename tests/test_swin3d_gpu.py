@@ -1,4 +1,4 @@
-"""Video-Swin BasicLayer on the B200 kernels (SURVEY 8(f) #4) through the C ABI: the generic 3-D window attention core
+"""Video-Swin BasicLayer on the H100 kernels (SURVEY 8(f) #4) through the C ABI: the generic 3-D window attention core
 vs the oracle restatement of `modules/swin.py` (padding, 3-D shift, clipped windows), and the whole drop-in layer vs the
 fixtures minted from the reference's own module."""
 import pytest

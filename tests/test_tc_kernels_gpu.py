@@ -1,5 +1,5 @@
-"""GPU parity of the round-2 tcgen05 kernels THROUGH THE C ABI against the CPU oracle:
-  * pgt_window_attention_tc (TMA + tcgen05 shifted-window attention core) vs the oracle's roll / window_partition /
+"""GPU parity of the round-2 wgmma kernels THROUGH THE C ABI against the CPU oracle:
+  * pgt_window_attention_tc (TMA + wgmma shifted-window attention core) vs the oracle's roll / window_partition /
     attention / window_reverse, every box layout (interior, x-wrapped, y-wrapped, corner), both P V operand modes;
   * pgt_l2_argmin_tc (tensor-core scores + certified window + exact re-evaluation) vs an fp64 argmin — bit-exact in the
     four SURVEY section-7 regimes, at small T (direct fp64 differences) and at the BASELINE sizes T = 49152 / 98304.
@@ -61,7 +61,7 @@ def test_window_attention_tc(C, H, W, clips, shifted, mode_n64):
     tab16 = o.window_tables(bias_tab.to(DEV))
     out = torch.full((T, C), float('nan'), dtype=torch.bfloat16, device=DEV)
     r = o.window_attention_tc(qkv.to(DEV), clips, H, W, C, heads, 2 if shifted else 0, tab16, out, mode_n64=mode_n64)
-    assert r is not None, 'shape not covered by the tcgen05 kernel'
+    assert r is not None, 'shape not covered by the wgmma kernel'
     torch.cuda.synchronize()
     ref = window_reference(qkv, clips, H, W, C, heads, bias_tab, shifted)
     got = out.float().cpu()
@@ -72,7 +72,7 @@ def test_window_attention_tc(C, H, W, clips, shifted, mode_n64):
 
 
 def test_window_attention_tc_matches_mma_sync_kernel():
-    """The round-1 mma.sync kernel and the tcgen05 kernel agree to bf16 rounding on a batch large enough that every
+    """The round-1 mma.sync kernel and the wgmma kernel agree to bf16 rounding on a batch large enough that every
     CTA of the persistent grid processes several window pairs."""
     from pgtformer_b200.weights import relative_position_index
     o = ops()
@@ -191,7 +191,7 @@ def test_l2_argmin_tc_bit_exact_baseline_sizes(synth_sd, regime, T):
 @pytest.mark.parametrize('K,E,T', [(768, 512, 40000), (512, 256, 33333), (256, 128, 700), (1024, 384, 20001)])
 def test_l2_argmin_tc_other_codebook_shapes(synth_sd, K, E, T):
     """Pair sweep with an odd number of N-tiles (the accumulator buffers alternate across tiles), fewer k-blocks, several
-    256-token tiles per CTA pair and a ragged last tile (one CTA of the last pair entirely past T)."""
+    several 128-token tiles per CTA and a ragged last tile."""
     o = ops()
     cb = synth_sd['quantizer.codebooks.0.weight'][:K, :E].contiguous()
     z = rnd((T, E), 31 + K)

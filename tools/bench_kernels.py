@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Micro-benchmarks of the north_star kernels through the C ABI (CUDA events, warm-up, inputs larger than L2 or an L2
-flush between iterations): window attention (mma.sync round-1 kernel vs TMA + tcgen05), L2 argmin (FFMA vs tcgen05),
+flush between iterations): window attention (mma.sync round-1 kernel vs TMA + wgmma), L2 argmin (FFMA vs wgmma),
 row argmax + gather.  Prints one JSON line per case: achieved GB/s and TFLOP/s against MEASURED_PEAKS.json.
     python tools/bench_kernels.py [--quick]
 """
@@ -65,9 +65,9 @@ def bench_window(C, H, clips, shift, pk, out):
     bytes_ = T * 4 * C * 2                                        # read q,k,v + write o (SURVEY 8d)
     flops = 4.0 * 48 * 48 * C * (T // 48)
     cases = [('mma_sync', lambda: ops.window_attention(qkv, clips, H, H, C, heads, shift, bias, o)),
-             ('tcgen05', lambda: ops.window_attention_tc(qkv, clips, H, H, C, heads, shift, tab16, o, mode_n64=0))]
+             ('wgmma', lambda: ops.window_attention_tc(qkv, clips, H, H, C, heads, shift, tab16, o, mode_n64=0))]
     if C // heads == 32:
-        cases.append(('tcgen05_n64', lambda: ops.window_attention_tc(qkv, clips, H, H, C, heads, shift, tab16, o, mode_n64=1)))
+        cases.append(('wgmma_n64', lambda: ops.window_attention_tc(qkv, clips, H, H, C, heads, shift, tab16, o, mode_n64=1)))
     for name, fn in cases:
         ms = timed(fn)
         out({'kernel': 'window_attention', 'impl': name, 'C': C, 'H': H, 'clips': clips, 'shift': shift, 'ms': ms,
@@ -88,8 +88,8 @@ def bench_argmin(T, regime, pk, out, with_ffma=True):
     pack = ops.codebook_pack(cb, 1024)
     flops = 2.0 * T * 1024 * 512
     bytes_ = T * 512 * 4 + 1024 * 512 * 4 + T * 8                 # SURVEY 8(d): z fp32 + codebook + indices
-    cases = [('tcgen05', lambda: ops.l2_argmin_tc(z, cb, pack, 1024, idx, None)),
-             ('tcgen05+quant', lambda: ops.l2_argmin_tc(z, cb, pack, 1024, idx, quant))]
+    cases = [('wgmma', lambda: ops.l2_argmin_tc(z, cb, pack, 1024, idx, None)),
+             ('wgmma+quant', lambda: ops.l2_argmin_tc(z, cb, pack, 1024, idx, quant))]
     if with_ffma:
         cases.append(('fp64_exhaustive', lambda: ops.l2_argmin(z, cb, 1024, idx, None)))
     for name, fn in cases:

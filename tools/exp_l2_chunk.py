@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Experiment: depth-first (frame-chunked) execution of an attention-free level.  GroupNorm statistics are per frame, so
-a chain conv -> GN apply -> conv -> ... can run on a few frames at a time; with a chunk whose tensors fit the 126 MB L2
+a chain conv -> GN apply -> conv -> ... can run on a few frames at a time; with a chunk whose tensors fit the 50 MB L2
 the intermediate tensors are re-read from L2 instead of HBM.  Times the decoder's 512^2 and 256^2 res-block chains for
 several chunk sizes (CUDA events, whole chain, 48 frames).
     python tools/exp_l2_chunk.py

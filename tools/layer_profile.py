@@ -1,9 +1,11 @@
 """Per-launch device times of one forward (CUDA events around every launch of the profiled
-classes): writes gpurun_out/layers_b{clips}.csv and prints the GEMM layers sorted by time."""
+classes): writes layers_b{clips}_{size}.csv into the directory given as the third argument (default: a temporary
+directory) and prints the GEMM layers sorted by time."""
 import collections
 import csv
 import os
 import sys
+import tempfile
 
 import torch
 
@@ -23,8 +25,9 @@ x = torch.rand(clips * 3, 3, size, size).cuda()
 for _ in range(2):
     m(x, w=1, adain=True)
 torch.cuda.synchronize()
-os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
-path = os.path.join(ROOT, 'gpurun_out', 'layers_b%d_%d.csv' % (clips, size))
+out_dir = sys.argv[3] if len(sys.argv) > 3 else tempfile.mkdtemp(prefix='pgt_layers_')
+os.makedirs(out_dir, exist_ok=True)
+path = os.path.join(out_dir, 'layers_b%d_%d.csv' % (clips, size))
 ops.profile_begin()
 m(x, w=1, adain=True)
 prof = ops.profile_end(path)

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Per-kernel SASS opcode census of libpgt_b200.so (cuobjdump -sass): what proves a Blackwell-native kernel
-(B200_PROFILING.md): UTC*MMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st, UTMALDG/UTMASTG = TMA, HMMA = legacy mma.sync.
-    python tools/sass_opcodes.py > profiles/r2_sass_opcodes.txt
+"""Per-kernel SASS opcode census of libpgt_b200.so (cuobjdump -sass): which instructions each kernel really runs on
+sm_90a.  HGMMA = wgmma, UTMALDG / UTMASTG / UTMAPF = TMA loads / stores / prefetches, SYNCS = mbarrier operations,
+HMMA = warp-level mma.sync.
+    python tools/sass_opcodes.py
 """
 import collections
 import os
@@ -11,7 +12,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, 'pgtformer_b200', 'lib', 'libpgt_b200.so')
-OPS = ['UTCHMMA', 'UTCQMMA', 'UTCBAR', 'LDTM', 'STTM', 'UTMALDG', 'UTMASTG', 'UTMAPF', 'UBLKCP', 'HMMA', 'LDGSTS', 'MUFU', 'DFMA', 'FFMA']
+OPS = ['HGMMA', 'UTMALDG', 'UTMASTG', 'UTMAPF', 'UBLKCP', 'SYNCS', 'HMMA', 'LDGSTS', 'MUFU', 'DFMA', 'FFMA']
 
 
 def main():
@@ -33,7 +34,7 @@ def main():
             for o in OPS:
                 if op.startswith(o):
                     cur[o] += 1
-    print('# SASS opcode counts per kernel of %s (cuobjdump -sass, sm_100a)' % os.path.relpath(LIB, ROOT))
+    print('# SASS opcode counts per kernel of %s (cuobjdump -sass, sm_90a)' % os.path.relpath(LIB, ROOT))
     print('%-58s' % 'kernel' + ''.join('%9s' % o for o in OPS))
     for k, c in counts.items():
         print('%-58s' % k[:57] + ''.join('%9d' % c[o] for o in OPS))
