@@ -15,6 +15,7 @@ pgtformer_b200.engine.Engine; kernel-layout weight copies are derived caches reb
 load_state_dict() / .to().  Inference only (the reference's training loop is not in its repo,
 SURVEY F12); there is no CPU path.
 """
+import math
 import os
 
 import torch
@@ -29,6 +30,10 @@ try:
 except Exception:                                       # pragma: no cover
     class PyTorchModelHubMixin:                         # type: ignore
         pass
+
+
+def _shape(x):
+    return tuple(x.shape) if torch.is_tensor(x) else type(x).__name__
 
 
 class _Node(nn.Module):
@@ -122,8 +127,9 @@ class _B200Model(nn.Module):
 
 @ARCH_REGISTRY.register()
 class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
-    """Registered stage-I autoencoder (`archs/tdcrqvae3_arch.py:710-792`): forward / get_codes
-    run the encoder, the nearest-codebook L2 argmin kernel and the decoder."""
+    """Registered stage-I autoencoder (`archs/tdcrqvae3_arch.py:710-872`): forward / get_codes run the encoder, the
+    nearest-codebook L2 argmin kernel and the decoder; encode / decode / decode_code / get_soft_codes and the partial-
+    code methods expose the codec's parts (PGTFormer inherits them, as in the reference)."""
 
     def __init__(self, *, embed_dim=64, n_embed=512, decay=0.99, loss_type='mse', latent_loss_weight=0.25,
                  bottleneck_type='rq', ddconfig=None, checkpointing=False, tf=3, **kwargs):
@@ -141,6 +147,99 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
     @torch.no_grad()
     def get_codes(self, input):
         return self.engine().forward_vq(input, code_only=True)[2]
+
+    # ---- the rest of the stage-I codec surface (`archs/tdcrqvae3_arch.py:774-872`), depth-1 quantiser.  Arguments are
+    # checked on the host before any launch: bad shapes raise ValueError, codes outside [0, n_embed] IndexError (index
+    # n_embed is the codebook's padding row, which nn.Embedding accepts).
+    def _frames(self, x):
+        """[b, t, 3, H, W] (the reference's form) or [b*t, 3, H, W] -> [b*t, 3, H, W]."""
+        if not torch.is_tensor(x) or x.dim() not in (4, 5):
+            raise ValueError('expected frames [b, t, 3, H, W] or [b*t, 3, H, W], got %s' % (_shape(x),))
+        if x.dim() == 5:
+            x = x.reshape(-1, *x.shape[2:])
+        Fr, C, H, W = x.shape
+        if C != 3 or Fr == 0 or Fr % self.t != 0 or H % 64 != 0 or W % 64 != 0 or H == 0 or W == 0:
+            raise ValueError('expected %d-frame clips of 3 x H x W with H, W multiples of 64, got %s'
+                             % (self.t, tuple(x.shape)))
+        return x
+
+    def _check_latent(self, Fr, h, w):
+        if Fr == 0 or Fr % self.t != 0 or h == 0 or w == 0 or h % 4 != 0 or w % 4 != 0:
+            raise ValueError('expected %d-frame clips with a latent map of multiples of 4 (frames multiples of 64), '
+                             'got [%d, %d, %d]' % (self.t, Fr, h, w))
+
+    def _check_code(self, code):
+        if not torch.is_tensor(code) or code.dim() != 4 or code.shape[-1] != self.code_shape[-1] or \
+                code.dtype.is_floating_point or code.dtype.is_complex or code.dtype == torch.bool:
+            raise ValueError('expected integer codes [F, h, w, %d], got %s %s'
+                             % (self.code_shape[-1], _shape(code), getattr(code, 'dtype', '')))
+        if code.numel() > 0:
+            lo, hi = torch.aminmax(code)
+            n = self.arch.n_embed
+            if int(lo) < 0 or int(hi) > n:
+                raise IndexError('code out of range [0, %d]: min %d, max %d' % (n, int(lo), int(hi)))
+
+    @torch.no_grad()
+    def encode(self, x):
+        """z_e = quant_conv(Encoder(x)) as NHWC fp32 [b*t, H/16, W/16, embed_dim]."""
+        x = self._frames(x)
+        return self.engine().encode(x)
+
+    @torch.no_grad()
+    def decode(self, z_q):
+        """post_quant_conv + Decoder.forward (no SFT fusion) of NHWC z_q [F, h, w, embed_dim] -> fp32 [F, 3, 16h, 16w]."""
+        if not torch.is_tensor(z_q) or z_q.dim() != 4 or z_q.shape[-1] != self.arch.embed_dim or \
+                not z_q.dtype.is_floating_point:
+            raise ValueError('expected z_q [F, h, w, %d] floating point, got %s' % (self.arch.embed_dim, _shape(z_q)))
+        self._check_latent(*z_q.shape[:3])
+        return self.engine().decode(z_q)
+
+    @torch.no_grad()
+    def decode_code(self, code):
+        """Codebook rows of the int codes [F, h, w, 1] (any h, w the decoder takes), decoded to frames."""
+        self._check_code(code)
+        self._check_latent(*code.shape[:3])
+        eng = self.engine()
+        Fr, h, w, _ = code.shape
+        return eng.decode(eng.embed_code(code).view(Fr, h, w, self.arch.embed_dim))
+
+    @torch.no_grad()
+    def get_code_emb_with_depth(self, code):
+        """(codebook rows [F, h, w, 1, embed_dim] fp32, None), as RQBottleneck.embed_code_with_depth returns them."""
+        self._check_code(code)
+        Fr, h, w, d = code.shape
+        return self.engine().embed_code(code).view(Fr, h, w, d, self.arch.embed_dim), None
+
+    @torch.no_grad()
+    def decode_partial_code(self, code, code_idx, decode_type='select'):
+        """Decodes with codebooks [0 .. code_idx]; with one codebook 'select' and 'add' are both decode_code."""
+        self._check_code(code)
+        assert code_idx < code.shape[-1]
+        if decode_type not in ('select', 'add'):
+            raise NotImplementedError(f"{decode_type} is not implemented in partial decoding")
+        return self.decode_code(code)
+
+    @torch.no_grad()
+    def forward_partial_code(self, xs, code_idx, decode_type='select'):
+        code = self.get_codes(self._frames(xs))
+        return self.decode_partial_code(code, code_idx, decode_type)
+
+    @torch.no_grad()
+    def get_soft_codes(self, xs, temp=1.0, stochastic=False):
+        """(soft_code [F, h, w, 1, n_embed] fp32 = softmax(-||z_e - e_k||^2 / temp), code [F, h, w, 1] int64): the
+        exact nearest code (== get_codes), or with stochastic=True one draw per token from its soft_code row."""
+        try:
+            t = float(temp)
+        except (TypeError, ValueError):
+            raise ValueError('temp must be a finite number > 0, got %r' % (temp,)) from None
+        if not math.isfinite(t) or t <= 0.0:
+            raise ValueError('temp must be a finite number > 0, got %r' % (temp,))
+        x = self._frames(xs)
+        eng = self.engine()
+        z_e = eng.encode(x)
+        Fr, h, w, E = z_e.shape
+        p, code = eng.soft_codes(z_e.view(-1, E), t, stochastic=bool(stochastic))
+        return p.view(Fr, h, w, 1, -1), code.view(Fr, h, w, 1)
 
 
 @ARCH_REGISTRY.register()

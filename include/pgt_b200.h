@@ -256,6 +256,18 @@ int64_t pgt_l2_argmin_ws_ints(int T);
 int pgt_l2_argmin_tc(const float* z, int T, int E, const float* codebook, const void* cb_bf16, const float* cb_norm,
                      int K, int64_t* idx, float* quant, int32_t* workspace, void* stream);
 
+/* ---- soft codes (RQBottleneck.get_soft_codes, archs/tdcrqvae3_arch.py:429-457, depth 1).
+ * pgt_soft_codes: out[t, k] = softmax_k((2 z[t].e_k - ||e_k||^2) / temp) = softmax_k(-||z[t] - e_k||^2 / temp) over the
+ *   first K codebook rows; z fp32 [T, E]; codebook fp32 [K(+1), E]; cb_norm fp32 [>= K] = ||e_k||^2 (the norms
+ *   pgt_codebook_pack writes); out fp32 [T, K].  3xTF32 tensor-core dot products (soft_codes.cu), fp32 softmax.
+ *   temp must be finite and > 0.  Returns PGT_ERR_UNSUPPORTED unless K % 128 == 0 and E % 32 == 0.
+ * pgt_sample_codes: idx[t] = one draw from row t of p fp32 [T, K] (non-negative, any positive sum), Philox keyed by the
+ *   DEVICE int64 seed[2]; a zero-probability index is never drawn; a row with no positive entry yields -1.  Replaces
+ *   torch.multinomial(soft_code, 1) (:441-444). */
+int pgt_soft_codes(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
+                   float* out, void* stream);
+int pgt_sample_codes(const float* p, int T, int K, const int64_t* seed, int64_t* idx, void* stream);
+
 /* ---- AdaIN: y = (q - mean_q)/std_q * std_l + mean_l per (frame, channel) over HW, unbiased
  * variance + eps.  q: bf16/fp32 [F, HW, ldq]; l (style) bf16 [F, HW, ldl]; y bf16.
  * Replaces adaptive_instance_normalization (archs/codeformer_arch.py:15-46). */

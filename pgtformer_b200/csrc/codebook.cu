@@ -2,7 +2,8 @@
 // fp64 nearest-codebook L2 argmin (the wgmma kernel of the TDCRQVAE3.forward / get_codes path is in
 // l2_argmin_tc.cu; this one serves the tokens it cannot certify and the shapes it does not cover).  Index results are
 // exact: argmax is a pure fp32 compare; argmin is an fp64 argmin of ||z-e||^2 with lowest index on ties, which is
-// stricter than the reference's own fp32 addmm.
+// stricter than the reference's own fp32 addmm.  Also the multinomial sampler of the soft codes (soft_codes.cu).
+#include <curand_kernel.h>
 #include <float.h>
 
 #include "common.cuh"
@@ -214,6 +215,66 @@ l2_argmin_short_list_kernel(const float* __restrict__ z, int E, const float* __r
 
 constexpr int AM_SHORT_LIST = 2048;
 
+// ------------------------------------------------------------------------------ multinomial sampling of soft codes
+// torch.multinomial(p, 1) of RQBottleneck.get_soft_codes (archs/tdcrqvae3_arch.py:441-444), one warp per row of K
+// probabilities (lane l owns the contiguous slice [l * per, (l + 1) * per)).  u in [0, 1) from Philox (key seed[0],
+// subsequence = row, offset seed[1]); the code is the first index whose running sum exceeds u * total.  The lane prefix
+// is a serial chain (monotone, and unchanged across a lane whose slice is all zeros), and inside the chosen lane a
+// zero-probability code never raises the running sum, so such a code is never returned; when rounding leaves no index
+// above the threshold the last code with p > 0 is taken.  A row without any positive entry yields -1.  The seed is read
+// on the device: no host synchronisation, and a CUDA graph replays fresh draws when seed is refilled before replay.
+__global__ void __launch_bounds__(256)
+sample_codes_kernel(const float* __restrict__ p, int T, int K, const int64_t* __restrict__ seed, int64_t* __restrict__ idx) {
+  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (row >= T) return;
+  const int per = (K + 31) / 32;
+  const int c0 = min(K, lane * per), c1 = min(K, c0 + per);
+  const float* pr = p + (size_t)row * K;
+  float tot = 0.f;
+  int lastnz = -1;
+  for (int c = c0; c < c1; ++c) {
+    const float v = __ldg(pr + c);
+    tot += v;
+    if (v > 0.f) lastnz = c;
+  }
+  float incl = 0.f;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float v = __shfl_sync(0xffffffffu, tot, j);
+    if (j <= lane) incl += v;
+  }
+  float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane == 0) excl = 0.f;
+  const float total = __shfl_sync(0xffffffffu, incl, 31);
+  float u = 0.f;
+  if (lane == 0) {
+    curandStatePhilox4_32_10_t st;
+    curand_init((unsigned long long)seed[0], (unsigned long long)row, (unsigned long long)seed[1], &st);
+    u = 1.f - curand_uniform(&st);                               // (0, 1] -> [0, 1)
+  }
+  const float x = __shfl_sync(0xffffffffu, u, 0) * total;
+  const unsigned above = __ballot_sync(0xffffffffu, incl > x);
+  int code = -1;
+  if (above != 0) {
+    const int sel = __ffs(above) - 1;
+    if (lane == sel) {
+      float c = excl;
+      for (int k = c0; k < c1; ++k) {
+        const float v = __ldg(pr + k);
+        c += v;
+        if (c > x && v > 0.f) { code = k; break; }
+      }
+      if (code < 0) code = lastnz;                               // incl > excl: this slice has a positive entry
+    }
+    code = __shfl_sync(0xffffffffu, code, sel);
+  } else {
+    const unsigned nz = __ballot_sync(0xffffffffu, lastnz >= 0);
+    if (nz != 0) code = __shfl_sync(0xffffffffu, lastnz, 31 - __clz(nz));
+  }
+  if (lane == 0) idx[row] = code;
+}
+
 int l2_argmin_list_launch(const float* z, int T, int E, const float* codebook, int K, int64_t* idx, float* quant,
                           const int* list, const int* count, int grid, cudaStream_t st) {
   if (E % AM_KC != 0 || E % 4 != 0) return PGT_ERR_UNSUPPORTED;
@@ -241,6 +302,14 @@ extern "C" int pgt_argmax_gather(const float* logits, int T, int K, const float*
                static_cast<cudaStream_t>(stream));
   argmax_gather_kernel<<<ceil_div(T, warps), warps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       logits, T, K, codebook, E, idx_in, idx, quant, ldq, quant_dtype);
+  PGT_LAUNCH_OK();
+  return PGT_OK;
+}
+
+extern "C" int pgt_sample_codes(const float* p, int T, int K, const int64_t* seed, int64_t* idx, void* stream) {
+  PGT_CHECK_ARG(p && seed && idx && T > 0 && K > 0);
+  ProfScope ps(PGT_PROF_ARGMAX, (double)T * K * 4 + (double)T * 8, static_cast<cudaStream_t>(stream), "sample_codes");
+  sample_codes_kernel<<<ceil_div(T, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(p, T, K, seed, idx);
   PGT_LAUNCH_OK();
   return PGT_OK;
 }

@@ -79,6 +79,26 @@ void l2_argmin(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor
   check(rc, "l2_argmin");
 }
 
+void soft_codes(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor& norm, int64_t K, double temp,
+                at::Tensor out) {
+  TORCH_CHECK(z.is_cuda() && z.scalar_type() == at::kFloat && z.is_contiguous() && codebook.scalar_type() == at::kFloat &&
+              codebook.is_contiguous() && norm.scalar_type() == at::kFloat && out.scalar_type() == at::kFloat &&
+              out.is_contiguous() && out.size(0) == z.size(0) && out.size(1) == K,
+              "soft_codes: fp32 contiguous z [T, E], codebook, norm, out [T, K]");
+  c10::cuda::CUDAGuard guard(z.device());
+  check(pgt_soft_codes(z.data_ptr<float>(), (int)z.size(0), (int)z.size(1), codebook.data_ptr<float>(), norm.data_ptr<float>(),
+                       (int)K, (float)temp, out.data_ptr<float>(), stream_of(z)), "soft_codes");
+}
+
+void sample_codes(const at::Tensor& p, const at::Tensor& seed, at::Tensor idx) {
+  TORCH_CHECK(p.is_cuda() && p.scalar_type() == at::kFloat && p.is_contiguous() && seed.scalar_type() == at::kLong &&
+              seed.numel() == 2 && seed.device() == p.device() && idx.scalar_type() == at::kLong && idx.numel() == p.size(0),
+              "sample_codes: fp32 contiguous p [T, K], device int64 seed [2], int64 idx [T]");
+  c10::cuda::CUDAGuard guard(p.device());
+  check(pgt_sample_codes(p.data_ptr<float>(), (int)p.size(0), (int)p.size(1), seed.data_ptr<int64_t>(), idx.data_ptr<int64_t>(),
+                         stream_of(p)), "sample_codes");
+}
+
 void linear(const at::Tensor& a, const at::Tensor& w, const c10::optional<at::Tensor>& bias, int64_t act,
             const c10::optional<at::Tensor>& residual, at::Tensor out) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && w.stride(1) == 1,
@@ -112,6 +132,8 @@ TORCH_LIBRARY(pgt, m) {
   m.def("codebook_pack(Tensor codebook, int K) -> (Tensor, Tensor)");
   m.def("l2_argmin(Tensor z, Tensor codebook, Tensor cb16, Tensor norm, int K, Tensor(a!) idx, Tensor(b!)? quant) -> ()");
   m.def("linear(Tensor a, Tensor w, Tensor? bias, int act, Tensor? residual, Tensor(a!) out) -> ()");
+  m.def("soft_codes(Tensor z, Tensor codebook, Tensor norm, int K, float temp, Tensor(a!) out) -> ()");
+  m.def("sample_codes(Tensor p, Tensor seed, Tensor(a!) idx) -> ()");
 }
 
 TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
@@ -121,4 +143,6 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("codebook_pack", codebook_pack);
   m.impl("l2_argmin", l2_argmin);
   m.impl("linear", linear);
+  m.impl("soft_codes", soft_codes);
+  m.impl("sample_codes", sample_codes);
 }

@@ -652,26 +652,83 @@ class Engine:
         graph.replay()
         return outs
 
+    # ------------------------------------------------------------------ stage-I codec (TDCRQVAE3 methods)
+    def _codebook_pack(self):
+        """bf16 copy + fp32 norms of the codebook (l2_argmin_tc, soft_codes), once per load."""
+        if 'codebook.pack' not in self.w:
+            self.w['codebook.pack'] = ops.codebook_pack(self.w['codebook'], self.arch.n_embed)
+        return self.w['codebook.pack']
+
+    @_on_device
+    @torch.no_grad()
+    def encode(self, x):
+        """TDCRQVAE3.encode (`archs/tdcrqvae3_arch.py:774-777`): x fp32 [F,3,H,W] -> z_e fp32 NHWC [F,H/16,W/16,E]."""
+        a = self.arch
+        x = x.to(self.dev, torch.float32).contiguous()
+        Fr, _, H, W = x.shape
+        self._fusing = False                                   # the plain autoencoder has no SFT fusion
+        h, _ = self.encoder(x)
+        z_e = self._lin(h.view(Fr * (H // 16) * (W // 16), -1), 'quant_conv', a.embed_dim, out_dtype=torch.float32)
+        return z_e.view(Fr, H // 16, W // 16, a.embed_dim)
+
+    @_on_device
+    @torch.no_grad()
+    def decode(self, z_q):
+        """TDCRQVAE3.decode (`:779-783`): z_q NHWC [F,h,w,E] -> post_quant_conv -> Decoder.forward (no SFT fusion)
+        -> fp32 NCHW [F,3,16h,16w]."""
+        a = self.arch
+        Fr, hh, ww, E = z_q.shape
+        self._fusing = False
+        z = self._lin(z_q.to(self.dev, BF).reshape(Fr * hh * ww, E), 'post_quant_conv', a.z_channels)
+        return self.decoder(z.view(Fr, hh, ww, a.z_channels))
+
+    @_on_device
+    @torch.no_grad()
+    def embed_code(self, codes):
+        """RQBottleneck.embed_code, depth 1 (`:355-368`): int64 codes [T] (each in [0, n_embed], the last row being
+        the padding row; the gather does no range check) -> fp32 [T, E] codebook rows."""
+        self._fusing = False
+        codes = codes.to(self.dev, torch.int64).reshape(-1).contiguous()
+        quant = self._new(codes.numel(), self.arch.embed_dim, dtype=torch.float32)
+        ops.argmax_gather(None, self.w['codebook'], None, quant, idx_in=codes)
+        return quant
+
+    @_on_device
+    @torch.no_grad()
+    def soft_codes(self, z_e, temp, stochastic=False):
+        """RQBottleneck.get_soft_codes, depth 1 (`:429-457`): z_e fp32 [T, E] -> (p fp32 [T, K], codes int64 [T]).
+        Codes are the exact L2 argmin (== forward_vq's) or, stochastic, one draw per row from p with a seed taken on
+        the device from the default CUDA generator (reproducible under torch.manual_seed, no host sync)."""
+        a = self.arch
+        self._fusing = False
+        z = z_e.to(self.dev, torch.float32).reshape(-1, a.embed_dim).contiguous()
+        T = z.shape[0]
+        pack = self._codebook_pack()
+        p = self._new(T, a.n_embed, dtype=torch.float32)
+        ops.soft_codes(z, self.w['codebook'], pack[1], a.n_embed, temp, p)
+        codes = torch.empty(T, dtype=torch.int64, device=self.dev)
+        if stochastic:
+            seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (2,), dtype=torch.int64, device=self.dev)
+            ops.sample_codes(p, seed, codes)
+        else:
+            ops.l2_argmin_tc(z, self.w['codebook'], pack, a.n_embed, codes)
+        return p, codes
+
     @_on_device
     @torch.no_grad()
     def forward_vq(self, x, code_only=False):
         """TDCRQVAE3.forward (`archs/tdcrqvae3_arch.py:760-783`): encode -> L2 argmin -> embed -> decode."""
         a = self.arch
-        x = x.to(self.dev, torch.float32).contiguous()
-        Fr, _, H, W = x.shape
-        hh, ww = H // 16, W // 16
+        z_e = self.encode(x)
+        Fr, hh, ww, _ = z_e.shape
         T = Fr * hh * ww
-        self._fusing = False                                   # the plain autoencoder has no SFT fusion
-        h, _ = self.encoder(x)
-        z_e = self._lin(h.view(T, -1), 'quant_conv', a.embed_dim, out_dtype=torch.float32)
+        z_e = z_e.view(T, a.embed_dim)
         codes = torch.empty(T, dtype=torch.int64, device=self.dev)
         z_q = self._new(T, a.embed_dim, dtype=torch.float32)
-        if 'codebook.pack' not in self.w:                  # bf16 copy + norms for the wgmma argmin, once per load
-            self.w['codebook.pack'] = ops.codebook_pack(self.w['codebook'], a.n_embed)
-        ops.l2_argmin_tc(z_e, self.w['codebook'], self.w['codebook.pack'], a.n_embed, codes, z_q)
+        ops.l2_argmin_tc(z_e, self.w['codebook'], self._codebook_pack(), a.n_embed, codes, z_q)
         loss = (z_e - z_q).pow(2).mean()
         codes = codes.view(Fr, hh, ww, 1)
+        z_q = z_q.view(Fr, hh, ww, -1)
         if code_only:
-            return z_q.view(Fr, hh, ww, -1), loss, codes
-        z = self._lin(z_q.to(BF), 'post_quant_conv', a.z_channels)
-        return self.decoder(z.view(Fr, hh, ww, a.z_channels)), loss, codes
+            return z_q, loss, codes
+        return self.decode(z_q), loss, codes

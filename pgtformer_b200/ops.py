@@ -324,10 +324,17 @@ def mha(q, k, v, clips, L_, heads, d, out):
 
 
 def argmax_gather(logits, codebook, idx_out, quant, idx_in=None):
+    """Row argmax of logits + codebook gather; with idx_in (int64, every entry a valid codebook row: the kernel does no
+    range check) logits may be None and only the gather runs."""
     lib = L.load()
-    T, K = logits.shape
-    assert logits.dtype == torch.float32 and logits.is_contiguous() and codebook.dtype == torch.float32
-    assert idx_out.dtype == torch.int64
+    if logits is None:
+        assert idx_in is not None and idx_in.dtype == torch.int64 and idx_in.is_contiguous()
+        T, K = idx_in.numel(), 4                       # K is not read when the codes are given
+    else:
+        T, K = logits.shape
+        assert logits.dtype == torch.float32 and logits.is_contiguous()
+    assert codebook.dtype == torch.float32
+    assert idx_out is None or idx_out.dtype == torch.int64
     L.check(lib.pgt_argmax_gather(_p(logits), T, K, _p(codebook), codebook.shape[1], _p(idx_in), _p(idx_out),
                                   _p(quant), _rows(quant)[2] if quant is not None else 0,
                                   _dt(quant) if quant is not None else 0, _stream()))
@@ -377,6 +384,29 @@ def l2_argmin_tc(z, codebook, pack, K, idx_out, quant=None):
         return l2_argmin(z, codebook, K, idx_out, quant)
     L.check(rc)
     return idx_out, quant
+
+
+def soft_codes(z, codebook, norm, K, temp, out):
+    """out[T, K] = softmax_k(-||z - e_k||^2 / temp) over the first K codebook rows (soft_codes.cu); norm: the fp32
+    ||e_k||^2 of codebook_pack."""
+    lib = L.load()
+    T, E = z.shape
+    assert z.dtype == torch.float32 and z.is_contiguous() and codebook.dtype == torch.float32 and codebook.is_contiguous()
+    assert codebook.shape[1] == E and codebook.shape[0] >= K and norm.dtype == torch.float32 and norm.numel() >= K
+    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (T, K)
+    L.check(lib.pgt_soft_codes(_p(z), T, E, _p(codebook), _p(norm), K, float(temp), _p(out), _stream(z)))
+    return out
+
+
+def sample_codes(p, seed, idx_out):
+    """idx_out[t] = one draw from the distribution in row t of p (codebook.cu sample_codes_kernel); seed: device int64
+    [2] (Philox key and offset), read on the device."""
+    lib = L.load()
+    T, K = p.shape
+    assert p.dtype == torch.float32 and p.is_contiguous() and idx_out.dtype == torch.int64 and idx_out.numel() == T
+    assert seed.dtype == torch.int64 and seed.numel() == 2 and seed.device == p.device and idx_out.device == p.device
+    L.check(lib.pgt_sample_codes(_p(p), T, K, _p(seed), _p(idx_out), _stream(p)))
+    return idx_out
 
 
 def adain(q, style, out, eps=1e-5):
