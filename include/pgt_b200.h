@@ -226,7 +226,9 @@ int pgt_window3d_attention(const void* qkv, int ldqkv, const void* pad_qkv, int 
  * q,k,v: bf16 [clips*L, ld*] with head h at columns [h*d, (h+1)*d); out bf16 [clips*L, ldo].
  * Replaces the nn.MultiheadAttention core (archs/codeformer_arch.py:105,129-130); the
  * head-averaged attention weights the reference materialises (need_weights=True) are never
- * consumed (`[0]` at :130) and are not produced. */
+ * consumed (`[0]` at :130) and are not produced.  Head widths 64, 256 and 512; d = 256 / 512 (any L >= 1) is the core
+ * of TDRQVAE's dense AttnBlock (archs/tdrqvae_arch.py:151-203: clips = frames, heads = 1, d = C) and needs 16-byte
+ * aligned q / k / v / out, else PGT_ERR_UNSUPPORTED. */
 int pgt_mha_fwd(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, int clips, int L,
                 int heads, int d, void* out, int ldo, void* stream);
 

@@ -299,6 +299,8 @@ mha_fwd_kernel(const __nv_bfloat16* __restrict__ q, int ldq, const __nv_bfloat16
 
 int mha_tc_launch(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, int clips, int L, int heads,
                   int d, void* out, int ldo, cudaStream_t stream);      // mha_tc.cu (wgmma path)
+int attn_wide_launch(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, int clips, int L, int heads,
+                     int d, void* out, int ldo, cudaStream_t stream);   // attn_wide_tc.cu (d = 256 / 512)
 
 }  // namespace pgt
 
@@ -342,6 +344,10 @@ extern "C" int pgt_mha_fwd(const void* q, int ldq, const void* k, int ldk, const
                            int heads, int d, void* out, int ldo, void* stream) {
   PGT_CHECK_ARG(q && k && v && out && clips > 0 && L > 0 && heads > 0);
   PGT_CHECK_ARG(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0);
+  if (d == 256 || d == 512) {                        // wide heads: the wgmma kernel is the only path
+    ProfScope pst(PGT_PROF_MHA, 4.0 * (double)L * L * d * heads * clips, static_cast<cudaStream_t>(stream), "mha_wide");
+    return attn_wide_launch(q, ldq, k, ldk, v, ldv, clips, L, heads, d, out, ldo, static_cast<cudaStream_t>(stream));
+  }
   if (d != 64) return PGT_ERR_UNSUPPORTED;
   static const bool no_tc = getenv("PGT_MHA_NO_TC") != nullptr;
   if (!no_tc) {

@@ -70,6 +70,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (++spins > (1u << 26)) __trap();
   }
 }
+// Unbounded wait, for warpgroups raised with setmaxnreg.inc: a trap path reachable from such a region makes ptxas hold
+// the whole kernel to the launch-bound register count.  Pair it with a bounded wait on the other side of the pipeline.
+__device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
+  }
+}
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -164,6 +170,13 @@ __device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t da, uint
       : PGT_D8(0)
       : "l"(da), "l"(db), "r"(acc));
 }
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : PGT_D8(0), PGT_D8(8)
+      : "l"(da), "l"(db), "r"(acc));
+}
 __device__ __forceinline__ void wgmma_m64n48k16(float (&d)[24], uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
@@ -195,6 +208,7 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t da, u
 template <int N>
 __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
   if constexpr (N == 16) wgmma_m64n16k16(d, da, db, acc);
+  else if constexpr (N == 32) wgmma_m64n32k16(d, da, db, acc);
   else if constexpr (N == 48) wgmma_m64n48k16(d, da, db, acc);
   else if constexpr (N == 64) wgmma_m64n64k16(d, da, db, acc);
   else if constexpr (N == 128) wgmma_m64n128k16(d, da, db, acc);
@@ -212,13 +226,28 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint
       : PGT_D32(0)
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
 }
+// The same with N = 256 (B spans four 64-element MN atoms, `lbo` bytes apart: see wgmma_desc_mn_sw128).
+__device__ __forceinline__ void wgmma_m64n256k16_rs_tb(float (&d)[128], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, {%128, %129, %130, %131}, %132, p, 1, 1, 1;\n\t}"
+      : PGT_D128(0)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+}
+
+// Register budget of a warpgroup (all four warps execute it): producers give registers back, consumers take them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // MN-major SW128 operand (rows = K, 64 MN-contiguous elements per 128-byte row; 8-row groups 1024 B apart): the B view
-// of a row-major [keys x d] tile such as V.
-__device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t saddr) {
+// of a row-major [keys x d] tile such as V.  An operand wider than 64 along MN is a row of such atoms `lbo` bytes apart
+// (for TMA column chunks of [rows x 64], the chunk size).
+__device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(uint32_t saddr, uint32_t lbo = 16) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>(1) << 16;                        // LBO: next 64-element atom along MN (unused: N <= 64)
+  d |= static_cast<uint64_t>((lbo >> 4) & 0x3FFF) << 16;     // LBO: next 64-element atom along MN (unused: N <= 64)
   d |= static_cast<uint64_t>((1024 >> 4) & 0x3FFF) << 32;     // SBO: next 8 rows along K
   d |= static_cast<uint64_t>(1) << 62;
   return d;
