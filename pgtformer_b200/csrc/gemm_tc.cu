@@ -2,20 +2,25 @@
 //
 //   out[rows, N] = epilogue( A[rows, K] * W[N, K]^T )          bf16 operands, fp32 accumulate in registers
 //
-// Persistent, warp-specialised kernels (320 threads; + 128 in the GroupNorm-fused halo variant):
-//   warps 0..7  two consumer warpgroups: warpgroup h issues wgmma 64 x BN x 16 for rows [64h, 64h + 64) of the
-//               128-row tile over the whole k loop, then runs the epilogue: the accumulators go through a 128 x 64
-//               fp32 shared-memory exchange (one row per thread, 32 columns per chunk) -> +bias -> activation ->
-//               +residual / SFT from the staging slot -> optional GroupNorm partial statistics -> bf16/fp32 pack into
-//               a 128B-swizzled smem staging panel
-//   warp 8      TMA producer: A tile (128 rows x 64 K) and W tile (BN rows x 64 K) per k-block, 128B swizzle
-//   warp 9      epilogue DMA: TMA-loads the residual (/ SFT scale) panel INTO the staging slot ahead of time and
+// Persistent, warp-specialised kernels (384 threads = three warpgroups; the GroupNorm-fused halo variant keeps 320 + 128):
+//   warps 0..7  two consumer warpgroups, raised to CONSUMER_REGS registers with setmaxnreg: warpgroup h issues wgmma
+//               64 x BN x 16 for rows [64h, 64h + 64) of the 128-row tile over the whole k loop, then runs the epilogue:
+//               the accumulators go through a 128 x 64 fp32 shared-memory exchange (one row per thread, 32 columns per
+//               chunk) -> +bias -> activation -> +residual / SFT from the staging slot -> optional GroupNorm partial
+//               statistics -> bf16/fp32 pack into a 128B-swizzled smem staging panel
+//   warps 8..11 warpgroup 2, lowered to PRODUCER_REGS registers:
+//     warp 8    TMA producer: A tile (128 rows x 64 K) and W tile (BN rows x 64 K) per k-block, 128B swizzle
+//     warp 9    epilogue DMA: TMA-loads the residual (/ SFT scale) panel INTO the staging slot ahead of time and
 //               TMA-stores the finished panel, so both are full-line bulk copies and no CTA barrier sits on the path
-// Pipelines: smem full/empty ring (TMA <-> wgmma) and a 4-slot staging ring (epilogue <-> DMA warp); the producer
-// runs ahead into the next tile while the consumers finish the epilogue of the current one.
+//     warps 10, 11 idle (setmaxnreg acts on whole warpgroups)
+// Pipelines: smem full/empty ring (TMA <-> wgmma) and a staging ring of 4 slots (2 at BN = 256) (epilogue <-> DMA warp);
+// the producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
+// Consumer waits do not time out (a reachable trap would hold ptxas to the launch-bound register count); the producer
+// and the DMA warp wait with a bound, and the producer ends by waiting until every stage it filled has been released,
+// so a transaction that never completes traps the launch instead of hanging it.
 //
-// Kernels in this file: gemm_tc_kernel<BN> (linear / generic implicit-GEMM conv), conv_halo_kernel<BN, GN>
-// (3x3 and upsample-phase convs with Cout <= 128: one halo slab serves every tap).
+// Kernels in this file: gemm_tc_kernel<BN> (linear / generic implicit-GEMM conv; BN = 64, 128 or 256),
+// conv_halo_kernel<BN, GN> (3x3 and upsample-phase convs with Cout <= 128: one halo slab serves every tap).
 //
 // The A operand is produced by TMA in three addressing modes:
 //   LINEAR   2-D map [K, rows]
@@ -37,15 +42,21 @@ namespace pgt {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int EPI_WARPS = 8;                     // the two consumer warpgroups (wgmma + epilogue)
-constexpr int GEMM_THREADS = EPI_WARPS * 32 + 64;          // consumer warpgroups, TMA producer, epilogue-DMA warp
+constexpr int GEMM_THREADS = EPI_WARPS * 32 + 128;         // consumer warpgroups + the producer / DMA warpgroup
 constexpr int PRODUCER_WARP = EPI_WARPS;
 constexpr int DMA_WARP = EPI_WARPS + 1;
+// setmaxnreg budgets: 2 x 128 x 232 + 128 x 40 = 64512 = 384 x 168, the pool the launch bound gives the CTA
+constexpr int CONSUMER_REGS = 232;
+constexpr int PRODUCER_REGS = 40;
+static_assert(2 * 128 * CONSUMER_REGS + 128 * PRODUCER_REGS <= 65536, "register file");
 constexpr int XCH_LD = 68;                       // accumulator exchange: 128 rows x 64 fp32 (+4 pad: conflict-free reads)
 constexpr int XCH_BYTES = BM * XCH_LD * 4;
 constexpr int EPI_BAR = 1;                       // named barrier of the 256 consumer threads
 constexpr int A_STAGE_BYTES = BM * BK * 2;
 constexpr int PANEL_BYTES = BM * 128;            // one staging panel: 128 rows x 128 B
-constexpr int NUM_SLOTS = 4;                     // staging slots (two per epilogue half-group)
+// staging slots: 4 (two per epilogue half-group); at BN = 256 a 48 KB stage leaves room for 3 stages and 2 slots
+template <int BN>
+constexpr int staging_slots() { return BN == 256 ? 2 : 4; }
 constexpr int PREFETCH_TILES = 2;                // L2 prefetch distance of the TMA producers, in rounds of gridDim tiles
 
 enum { MODE_LINEAR = 0, MODE_CONV_S1 = 1, MODE_CONV_S2 = 2 };
@@ -88,7 +99,8 @@ template <int BN>
 struct GemmCfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGING_BYTES = NUM_SLOTS * PANEL_BYTES;
+  static constexpr int SLOTS = staging_slots<BN>();
+  static constexpr int STAGING_BYTES = SLOTS * PANEL_BYTES;
   static constexpr int BUDGET = 232448 - 1024 /*align*/ - STAGING_BYTES - XCH_BYTES - 256 /*barriers*/;
   static constexpr int STAGES = (BUDGET / STAGE_BYTES) > 6 ? 6 : (BUDGET / STAGE_BYTES);
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + XCH_BYTES + 256 + 1024;
@@ -112,27 +124,28 @@ __device__ __forceinline__ void decode_conv_tile(const GemmParams& p, int m_blk,
   n0 = tf * p.tn;
 }
 
-__device__ __forceinline__ void act_chunk(float (&f)[32], int act) {
+template <int N>
+__device__ __forceinline__ void act_chunk(float (&f)[N], int act) {
   switch (act) {                                  // hoisted: one switch per 32-value chunk
     case PGT_ACT_GELU:
 #pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = gelu_erf(f[j]);
+      for (int j = 0; j < N; ++j) f[j] = gelu_erf(f[j]);
       break;
     case PGT_ACT_SILU:
 #pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = apply_act(f[j], PGT_ACT_SILU);
+      for (int j = 0; j < N; ++j) f[j] = apply_act(f[j], PGT_ACT_SILU);
       break;
     case PGT_ACT_LRELU02:
 #pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.2f * f[j]);
+      for (int j = 0; j < N; ++j) f[j] = fmaxf(f[j], 0.2f * f[j]);
       break;
     case PGT_ACT_RELU:
 #pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.f);
+      for (int j = 0; j < N; ++j) f[j] = fmaxf(f[j], 0.f);
       break;
     case PGT_ACT_SIGMOID:
 #pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = apply_act(f[j], PGT_ACT_SIGMOID);
+      for (int j = 0; j < N; ++j) f[j] = apply_act(f[j], PGT_ACT_SIGMOID);
       break;
     default: break;
   }
@@ -141,10 +154,10 @@ __device__ __forceinline__ void act_chunk(float (&f)[32], int act) {
 // ------------------------------------------------------------------------------------------- epilogue
 // Shared by the GEMM/conv kernel and the halo-reuse conv kernel.  Runs on warps 0..7 (256 threads).
 struct EpiCtx {
-  uint8_t* staging;        // NUM_SLOTS x PANEL_BYTES, 1024-aligned
+  uint8_t* staging;        // staging_slots<BN>() x PANEL_BYTES, 1024-aligned
   float* xch;              // BM x XCH_LD fp32 accumulator exchange
-  uint64_t* res_bar;       // [NUM_SLOTS] staging slot prepared (free, residual landed)   DMA warp -> epilogue
-  uint64_t* slot_ready;    // [NUM_SLOTS] staging slot holds the finished panel           epilogue -> DMA warp
+  uint64_t* res_bar;       // [slots] staging slot prepared (free, residual landed)   DMA warp -> epilogue
+  uint64_t* slot_ready;    // [slots] staging slot holds the finished panel           epilogue -> DMA warp
 };
 
 // One 32-column chunk of a staging panel, accumulators already in registers (v): +bias -> act -> (+residual | SFT)
@@ -238,7 +251,7 @@ __device__ __forceinline__ void epi_finish(const GemmParams& p, const uint32_t (
       sts128(off[q], o);
     }
     if (gq != nullptr) {                       // fused GroupNorm statistics of the (pre-rounding) output values
-      const int lane = r & 31;
+      const int lane = lane_id();              // re-read, not kept live across the k loop (BN = 256 has no spare registers)
       switch (p.gn_cpg) {
         case 2: gn_chunk_stats<2>(f, gq, 0, lane); break;
         case 4: gn_chunk_stats<4>(f, gq, 0, lane); break;
@@ -310,9 +323,11 @@ __device__ __forceinline__ void epilogue_dma_loop(const GemmParams& p, const Epi
                                                   const CUtensorMap& tmR, const CUtensorMap& tmX, int lane, int num_tiles) {
   if (!p.fast_epi) return;
   const ItemStream<BN> is(p, num_tiles);
-  const bool sft = (p.epi_mode == PGT_EPI_SFT);
+  constexpr int SLOTS = staging_slots<BN>();
+  static_assert(SLOTS == 4 || SLOTS == 2, "ring positions are computed with shifts");
+  const bool sft = SLOTS == 4 && p.epi_mode == PGT_EPI_SFT;   // dispatch_gemm keeps SFT off the 2-slot ring
   const int S = sft ? 2 : 1;                 // staging slots per item (SFT: residual/out + scale)
-  const int R = NUM_SLOTS / S;               // ring length in items
+  const int R = SLOTS / S;                   // ring length in items: 4, or 2 (SFT, or BN = 256)
   auto coords = [&](const ItemCursor& c, int& col, int& m_blk, int& n0, int& y0, int& x0) {
     int nb;
     tile_mn(p, c.tile, m_blk, nb);
@@ -341,8 +356,7 @@ __device__ __forceinline__ void epilogue_dma_loop(const GemmParams& p, const Epi
     for (int i = 0; i < R && is.valid(cp); ++i) { prepare(cp, i); is.next(cp); }
   }
   __syncwarp();
-  static_assert(NUM_SLOTS == 4, "ring positions are computed with shifts");
-  const int rshift = sft ? 1 : 2;                        // R = 4, or 2 with SFT: no runtime division on this path
+  const int rshift = R == 4 ? 2 : 1;                     // no runtime division on this path
   for (int k = 0; is.valid(cs); ++k, is.next(cs)) {
     const int pos = k & (R - 1);
     mbar_wait(&ctx.slot_ready[pos], (k >> rshift) & 1);  // the 8 epilogue warps have written item k
@@ -381,7 +395,9 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
   const ItemStream<BN> is(p, 0);
   const int PW = is.PW;
   const int nsub = PW / 32;
-  const bool sft = (p.epi_mode == PGT_EPI_SFT);
+  constexpr int SLOTS = staging_slots<BN>();
+  constexpr int SLOT_SHIFT = SLOTS == 4 ? 2 : 1;
+  const bool sft = SLOTS == 4 && p.epi_mode == PGT_EPI_SFT;
   const bool bias_vec = p.bias != nullptr && (p.N % 32) == 0;   // whole chunks inside N: 128-bit bias reads
   const float* xrow = ctx.xch + r * XCH_LD;
 
@@ -430,7 +446,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
         const int pnl = g;
         if (pnl < npan) {
           const int pos = k & 1;
-          mbar_wait(&ctx.res_bar[pos], (k >> 1) & 1);     // slot free, residual and scale panels landed
+          mbar_wait_spin(&ctx.res_bar[pos], (k >> 1) & 1);   // slot free, residual and scale panels landed
           const int col0 = col_base + pnl * PW + half * 32;
           uint32_t v[32];
           smem_row_32(xrow + half * 32, v);
@@ -448,21 +464,23 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
         for (int pp = 0; pp < 64 / PW; ++pp) {
           const int pnl = g * (64 / PW) + pp;
           if (pnl >= npan) break;
-          const int pos = k & 3;
+          const int pos = k & (SLOTS - 1);
           const bool mine = (nsub == 2) || ((pnl & 1) == half);
           const int sb = (nsub == 2) ? half : 0;
           const int col0 = col_base + pnl * PW + sb * 32;
           float4 b[8];
-          if (mine && bias_vec) {
+          const bool pre = BN < 256 && bias_vec;         // BN = 256: no registers to spare, read the bias in epi_finish
+          if (mine && pre) {
             const float4* gb = reinterpret_cast<const float4*>(p.bias + col0);
 #pragma unroll
             for (int q = 0; q < 8; ++q) b[q] = __ldg(gb + q);
           }
-          mbar_wait(&ctx.res_bar[pos], (k >> 2) & 1);      // slot free (and residual panel landed)
+          mbar_wait_spin(&ctx.res_bar[pos], (k >> SLOT_SHIFT) & 1);   // slot free (and residual panel landed)
           if (mine) {
             uint32_t v[32];
             smem_row_32(xrow + pnl * PW + sb * 32 - g * 64, v);
-            epi_finish<false>(p, v, nullptr, stg + pos * PANEL_BYTES, r, sb, esize, p.has_res_map != 0, gn_ptr(col0), col0, b, bias_vec);
+            epi_finish<false>(p, v, bias_vec && !pre ? p.bias + col0 : nullptr, stg + pos * PANEL_BYTES, r, sb, esize,
+                              p.has_res_map != 0, gn_ptr(col0), col0, b, pre);
           }
           fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA engine
           mbar_arrive(&ctx.slot_ready[pos]);
@@ -470,39 +488,41 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
         }
       }
     } else {
-      // ---------------- direct path: per-thread global I/O of chunk `half` of the group
+      // ---------------- direct path: per-thread global I/O of chunk `half` of the group, 16 columns at a time (the
+      // accumulators of the later groups are still live: a 32-wide chunk of guarded loads would not fit beside them)
       const int c0 = g * 64 + half * 32;
-      if (col_base + c0 < p.N) {
-        if (valid) {
-          uint32_t v[32];
-          smem_row_32(xrow + half * 32, v);
-          const int col0 = col_base + c0;
-          const int ncol = min(32, p.N - col0);
-          float f[32];
+      if (valid) {
+#pragma unroll 1
+        for (int sc16 = 0; sc16 < 32; sc16 += 16) {
+          const int col0 = col_base + c0 + sc16;
+          if (col0 >= p.N) break;
+          const int ncol = min(16, p.N - col0);
+          const float* xs = xrow + half * 32 + sc16;
+          float f[16];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]) + ((p.bias != nullptr && j < ncol) ? __ldg(p.bias + col0 + j) : 0.f);
+          for (int j = 0; j < 16; ++j) f[j] = xs[j] + ((p.bias != nullptr && j < ncol) ? __ldg(p.bias + col0 + j) : 0.f);
           if (p.act != PGT_ACT_NONE && !p.relu_after_res) act_chunk(f, p.act);
           if (p.residual != nullptr) {
             if (p.res_dtype == PGT_BF16) {
               const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.residual) + orow * p.ldr + col0;
-              float rr[32];
+              float rr[16];
 #pragma unroll
-              for (int j = 0; j < 32; ++j) rr[j] = (j < ncol) ? __bfloat162float(rp[j]) : 0.f;
+              for (int j = 0; j < 16; ++j) rr[j] = (j < ncol) ? __bfloat162float(rp[j]) : 0.f;
               if (p.epi_mode == PGT_EPI_SFT) {
                 const __nv_bfloat16* ap = reinterpret_cast<const __nv_bfloat16*>(p.aux) + orow * p.ldaux + col0;
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
+                for (int j = 0; j < 16; ++j) {
                   const float sc = (j < ncol) ? __bfloat162float(ap[j]) : 0.f;
                   f[j] = rr[j] + p.sft_w * (rr[j] * sc + f[j]);
                 }
               } else {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) f[j] += rr[j];
+                for (int j = 0; j < 16; ++j) f[j] += rr[j];
               }
             } else {
               const float* rp = reinterpret_cast<const float*>(p.residual) + orow * p.ldr + col0;
 #pragma unroll
-              for (int j = 0; j < 32; ++j)
+              for (int j = 0; j < 16; ++j)
                 if (j < ncol) f[j] += __ldg(rp + j);
             }
           }
@@ -510,13 +530,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
           if (p.out_layout == PGT_OUT_NCHW) {
             float* op = reinterpret_cast<float*>(p.out);
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
+            for (int j = 0; j < 16; ++j)
               if (j < ncol) op[(((long long)pn * p.N + (col0 + j)) * p.H + py) * p.W + px] = f[j];
           } else if (p.out_dtype == PGT_BF16) {
             __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + orow * p.ldo + col0;
-            if (ncol == 32 && ((p.ldo & 7) == 0)) {
+            if (ncol == 16 && ((p.ldo & 7) == 0)) {
 #pragma unroll
-              for (int q = 0; q < 4; ++q) {
+              for (int q = 0; q < 2; ++q) {
                 uint4 u;
                 u.x = pack_bf16x2(f[q * 8 + 0], f[q * 8 + 1]);
                 u.y = pack_bf16x2(f[q * 8 + 2], f[q * 8 + 3]);
@@ -526,13 +546,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
               }
             } else {
 #pragma unroll
-              for (int j = 0; j < 32; ++j)
+              for (int j = 0; j < 16; ++j)
                 if (j < ncol) op[j] = __float2bfloat16_rn(f[j]);
             }
           } else {
             float* op = reinterpret_cast<float*>(p.out) + orow * p.ldo + col0;
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
+            for (int j = 0; j < 16; ++j)
               if (j < ncol) op[j] = f[j];
           }
         }
@@ -564,8 +584,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES + XCH_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* res_bar = bars + 2 * STAGES;                               // [NUM_SLOTS]
-  uint64_t* slot_ready = bars + 2 * STAGES + 4;                        // [NUM_SLOTS]
+  uint64_t* res_bar = bars + 2 * STAGES;                               // [Cfg::SLOTS]
+  uint64_t* slot_ready = res_bar + Cfg::SLOTS;                         // [Cfg::SLOTS]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -581,7 +601,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], EPI_WARPS);       // one arrive per consumer warp
     }
-    for (int i = 0; i < NUM_SLOTS; ++i) {
+    for (int i = 0; i < Cfg::SLOTS; ++i) {
       mbar_init(&res_bar[i], 1);                 // res_bar / slot_ready: one per staging ring position
       mbar_init(&slot_ready[i], EPI_WARPS * 32);
     }
@@ -589,51 +609,64 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   __syncthreads();
 
-  if (warp == PRODUCER_WARP) {
-    // ------------------------------------------------------------------ TMA producer
-    // (whole warp runs the loop and the waits; the copies are issued under elect.sync so that ptxas sees a
-    //  single-lane region and emits the uniform-datapath UTMALDG directly)
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int n_blk, m_blk;
-      tile_mn(p, tile, m_blk, n_blk);
-      int n0 = 0, y0 = 0, x0 = 0;
-      if (p.mode != MODE_LINEAR) decode_conv_tile(p, m_blk, n0, y0, x0);
-      for (int kb = 0; kb < p.num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        if (elect_one()) {
-          void* dst_a = smem_a + stage * A_STAGE_BYTES;
-          void* dst_b = smem_b + stage * Cfg::B_STAGE_BYTES;
-          int cb = 0, ax = 0, ay = 0, a5 = 0;            // conv: channel coordinate, x, y (, parity) of this k-block's tap
-          if (p.mode != MODE_LINEAR) {
-            const int tap = kb / p.cin_blocks;
-            cb = kb - tap * p.cin_blocks;
-            const int dy = tap / p.ksize;
-            const int dx = tap - dy * p.ksize;
-            if (p.mode == MODE_CONV_S1) {
-              ax = x0 + dx - p.pad_x; ay = y0 + dy - p.pad_y;
-            } else {
-              const int oy = dy - p.pad_lo, ox = dx - p.pad_lo;
-              const int qy = (oy < 0) ? -((1 - oy) >> 1) : (oy >> 1);
-              const int qx = (ox < 0) ? -((1 - ox) >> 1) : (ox >> 1);
-              const int py = oy - 2 * qy, px = ox - 2 * qx;
-              cb = px * p.cin_ld + cb * BK;               // parity-split map: channel coordinate carries the x parity
-              ax = x0 + qx; ay = y0 + qy; a5 = py;
+  if (warp >= EPI_WARPS) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP) {
+      // ---------------------------------------------------------------- TMA producer
+      // (whole warp runs the loop and the waits; the copies are issued under elect.sync so that ptxas sees a
+      //  single-lane region and emits the uniform-datapath UTMALDG directly)
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int n_blk, m_blk;
+        tile_mn(p, tile, m_blk, n_blk);
+        int n0 = 0, y0 = 0, x0 = 0;
+        if (p.mode != MODE_LINEAR) decode_conv_tile(p, m_blk, n0, y0, x0);
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          if (elect_one()) {
+            void* dst_a = smem_a + stage * A_STAGE_BYTES;
+            void* dst_b = smem_b + stage * Cfg::B_STAGE_BYTES;
+            int cb = 0, ax = 0, ay = 0, a5 = 0;            // conv: channel coordinate, x, y (, parity) of this k-block's tap
+            if (p.mode != MODE_LINEAR) {
+              const int tap = kb / p.cin_blocks;
+              cb = kb - tap * p.cin_blocks;
+              const int dy = tap / p.ksize;
+              const int dx = tap - dy * p.ksize;
+              if (p.mode == MODE_CONV_S1) {
+                ax = x0 + dx - p.pad_x; ay = y0 + dy - p.pad_y;
+              } else {
+                const int oy = dy - p.pad_lo, ox = dx - p.pad_lo;
+                const int qy = (oy < 0) ? -((1 - oy) >> 1) : (oy >> 1);
+                const int qx = (ox < 0) ? -((1 - ox) >> 1) : (ox >> 1);
+                const int py = oy - 2 * qy, px = ox - 2 * qx;
+                cb = px * p.cin_ld + cb * BK;               // parity-split map: channel coordinate carries the x parity
+                ax = x0 + qx; ay = y0 + qy; a5 = py;
+              }
             }
+            mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+            if (p.mode == MODE_LINEAR) tma_load_2d(dst_a, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
+            else if (p.mode == MODE_CONV_S1) tma_load_4d(dst_a, &tmA, &full_bar[stage], cb * BK, ax, ay, n0);
+            else tma_load_5d(dst_a, &tmA, &full_bar[stage], cb, ax, a5, ay, n0);
+            tma_load_2d(dst_b, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
           }
-          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          if (p.mode == MODE_LINEAR) tma_load_2d(dst_a, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
-          else if (p.mode == MODE_CONV_S1) tma_load_4d(dst_a, &tmA, &full_bar[stage], cb * BK, ax, ay, n0);
-          else tma_load_5d(dst_a, &tmA, &full_bar[stage], cb, ax, a5, ay, n0);
-          tma_load_2d(dst_b, &tmB, &full_bar[stage], kb * BK, n_blk * BN);
+          __syncwarp();
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        __syncwarp();
+      }
+      // drain: bounded waits until the consumers have released every stage filled above
+      for (int i = 0; i < STAGES; ++i) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+    } else if (warp == DMA_WARP) {
+      // ---------------------------------------------------------------- epilogue DMA warp
+      const EpiCtx ctx{staging, xch, res_bar, slot_ready};
+      epilogue_dma_loop<BN>(p, ctx, tmO, tmR, tmX, lane, num_tiles);
     }
-  } else if (warp < EPI_WARPS) {
+  } else {
     // ------------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
+    setmaxnreg_inc<CONSUMER_REGS>();
     const EpiCtx ctx{staging, xch, res_bar, slot_ready};
     const int wg = warp >> 2;
     const uint32_t a_rows = smem_u32(smem_a) + wg * 64 * 128;        // this warpgroup's 64 rows of every A stage
@@ -645,7 +678,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       float acc[BN / 2];
       int prev = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
+        mbar_wait_spin(&full_bar[stage], phase);
         const uint64_t da = wgmma_desc_k_sw128(a_rows + stage * A_STAGE_BYTES);
         const uint64_t db = wgmma_desc_k_sw128(b_base + stage * Cfg::B_STAGE_BYTES);
         wgmma_fence();
@@ -662,10 +695,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       release_stage(&empty_bar[prev], lane);
       epilogue_tile<BN>(p, ctx, warp, lane, tile, k, acc);
     }
-  } else if (warp == DMA_WARP) {
-    // ------------------------------------------------------------------ epilogue DMA warp
-    const EpiCtx ctx{staging, xch, res_bar, slot_ready};
-    epilogue_dma_loop<BN>(p, ctx, tmO, tmR, tmX, lane, num_tiles);
   }
 }
 
@@ -689,15 +718,20 @@ struct HaloCfg {
   static constexpr int B_BYTES = BN * 128;
   static constexpr int A_STAGES = 2;
   static constexpr int B_STAGES = (BN == 64) ? 9 : 5;
-  static constexpr int STAGING_BYTES = NUM_SLOTS * PANEL_BYTES;
+  static constexpr int SLOTS = staging_slots<BN>();
+  static constexpr int STAGING_BYTES = SLOTS * PANEL_BYTES;
   static constexpr int SMEM_BYTES = A_STAGES * HALO_A_STRIDE + B_STAGES * B_BYTES + STAGING_BYTES + XCH_BYTES + 512 + 1024;
   static_assert(SMEM_BYTES <= 232448, "halo conv smem budget");
 };
 
+// The GroupNorm-fused variant keeps its own layout without setmaxnreg: warps 0..9 as above, then four GroupNorm warps.
 constexpr int HALO_GN_THREADS = 128;             // extra warps of the GroupNorm-fused variant
+constexpr int HALO_GN_FIRST = (DMA_WARP + 1) * 32;
+template <bool GN>
+constexpr int halo_threads() { return GN ? HALO_GN_FIRST + HALO_GN_THREADS : GEMM_THREADS; }
 
 template <int BN, bool GN>
-__global__ void __launch_bounds__(GN ? GEMM_THREADS + HALO_GN_THREADS : GEMM_THREADS, 1)
+__global__ void __launch_bounds__(halo_threads<GN>(), 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
                  const __grid_constant__ CUtensorMap tmX, const GemmParams p) {
@@ -714,9 +748,9 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* a_empty = bars + AS;
   uint64_t* b_full = bars + 2 * AS;
   uint64_t* b_empty = bars + 2 * AS + BS;
-  uint64_t* res_bar = bars + 2 * AS + 2 * BS;                          // [NUM_SLOTS]
-  uint64_t* slot_ready = res_bar + NUM_SLOTS;                          // [NUM_SLOTS]
-  uint64_t* a_ready = slot_ready + NUM_SLOTS;                          // [AS] GN variant: slab normalised in place
+  uint64_t* res_bar = bars + 2 * AS + 2 * BS;                          // [Cfg::SLOTS]
+  uint64_t* slot_ready = res_bar + Cfg::SLOTS;                         // [Cfg::SLOTS]
+  uint64_t* a_ready = slot_ready + Cfg::SLOTS;                         // [AS] GN variant: slab normalised in place
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -731,7 +765,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (p.fast_epi && p.epi_mode == PGT_EPI_SFT) tma_prefetch_desc(&tmX);
     for (int i = 0; i < AS; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], EPI_WARPS); mbar_init(&a_ready[i], HALO_GN_THREADS); }
     for (int i = 0; i < BS; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], EPI_WARPS); }
-    for (int i = 0; i < NUM_SLOTS; ++i) {
+    for (int i = 0; i < Cfg::SLOTS; ++i) {
       mbar_init(&res_bar[i], 1);
       mbar_init(&slot_ready[i], EPI_WARPS * 32);
     }
@@ -739,55 +773,123 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
   __syncthreads();
 
-  if (warp == PRODUCER_WARP) {
-    // ------------------------------------------------------------------ TMA producer
-    int as = 0, bs = 0;
-    uint32_t aph = 0, bph = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int n_blk = tile % p.n_tiles;
-      const int m_blk = tile / p.n_tiles;
-      int n0, y0, x0;
-      decode_conv_tile(p, m_blk, n0, y0, x0);
-      {
-        // pull the slab (and residual panels) of the tile PREFETCH_TILES rounds ahead into L2
-        const int pt = tile + PREFETCH_TILES * (int)gridDim.x;
-        if (BN == 64 && pt < num_tiles && elect_one()) {
-          int pn0, py0, px0;
-          decode_conv_tile(p, pt / p.n_tiles, pn0, py0, px0);
-          for (int cb = 0; cb < p.cin_blocks; ++cb) tma_prefetch_4d(&tmA, cb * BK, px0 - 1, py0 - 1, pn0);
-          if (p.has_res_map) {
-            const int c0 = (pt % p.n_tiles) * BN;
-            const int rw = p.out_dtype == PGT_BF16 ? 64 : 32;
-            for (int c = 0; c < BN && c0 + c < p.N; c += rw) {
-              tma_prefetch_4d(&tmR, c0 + c, px0, py0, pn0);
-              if (p.epi_mode == PGT_EPI_SFT) tma_prefetch_4d(&tmX, c0 + c, px0, py0, pn0);
+  if (warp >= EPI_WARPS) {
+    if constexpr (!GN) setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == PRODUCER_WARP) {
+      // ---------------------------------------------------------------- TMA producer
+      int as = 0, bs = 0;
+      uint32_t aph = 0, bph = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int n_blk = tile % p.n_tiles;
+        const int m_blk = tile / p.n_tiles;
+        int n0, y0, x0;
+        decode_conv_tile(p, m_blk, n0, y0, x0);
+        {
+          // pull the slab (and residual panels) of the tile PREFETCH_TILES rounds ahead into L2
+          const int pt = tile + PREFETCH_TILES * (int)gridDim.x;
+          if (BN == 64 && pt < num_tiles && elect_one()) {
+            int pn0, py0, px0;
+            decode_conv_tile(p, pt / p.n_tiles, pn0, py0, px0);
+            for (int cb = 0; cb < p.cin_blocks; ++cb) tma_prefetch_4d(&tmA, cb * BK, px0 - 1, py0 - 1, pn0);
+            if (p.has_res_map) {
+              const int c0 = (pt % p.n_tiles) * BN;
+              const int rw = p.out_dtype == PGT_BF16 ? 64 : 32;
+              for (int c = 0; c < BN && c0 + c < p.N; c += rw) {
+                tma_prefetch_4d(&tmR, c0 + c, px0, py0, pn0);
+                if (p.epi_mode == PGT_EPI_SFT) tma_prefetch_4d(&tmX, c0 + c, px0, py0, pn0);
+              }
             }
           }
+          __syncwarp();
         }
-        __syncwarp();
-      }
-      for (int cb = 0; cb < p.cin_blocks; ++cb) {
-        mbar_wait(&a_empty[as], aph ^ 1);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&a_full[as], HALO_A_BYTES);
-          tma_load_4d(smem_a + as * HALO_A_STRIDE, &tmA, &a_full[as], cb * BK, x0 - 1, y0 - 1, n0);
-        }
-        __syncwarp();
-        if (++as == AS) { as = 0; aph ^= 1; }
-        if (p.b_resident && tile != (int)blockIdx.x) continue;   // weights already resident in the ring
-        for (int t = 0; t < p.ntaps; ++t) {
-          mbar_wait(&b_empty[bs], bph ^ 1);
+        for (int cb = 0; cb < p.cin_blocks; ++cb) {
+          mbar_wait(&a_empty[as], aph ^ 1);
           if (elect_one()) {
-            mbar_arrive_expect_tx(&b_full[bs], Cfg::B_BYTES);
-            tma_load_2d(smem_b + bs * Cfg::B_BYTES, &tmB, &b_full[bs], t * cin_pad + cb * BK, n_blk * BN);
+            mbar_arrive_expect_tx(&a_full[as], HALO_A_BYTES);
+            tma_load_4d(smem_a + as * HALO_A_STRIDE, &tmA, &a_full[as], cb * BK, x0 - 1, y0 - 1, n0);
           }
           __syncwarp();
-          if (++bs == BS) { bs = 0; bph ^= 1; }
+          if (++as == AS) { as = 0; aph ^= 1; }
+          if (p.b_resident && tile != (int)blockIdx.x) continue;   // weights already resident in the ring
+          for (int t = 0; t < p.ntaps; ++t) {
+            mbar_wait(&b_empty[bs], bph ^ 1);
+            if (elect_one()) {
+              mbar_arrive_expect_tx(&b_full[bs], Cfg::B_BYTES);
+              tma_load_2d(smem_b + bs * Cfg::B_BYTES, &tmB, &b_full[bs], t * cin_pad + cb * BK, n_blk * BN);
+            }
+            __syncwarp();
+            if (++bs == BS) { bs = 0; bph ^= 1; }
+          }
+        }
+      }
+      // drain: bounded waits until the consumers have released every slab loaded above
+      for (int i = 0; i < AS; ++i) {
+        mbar_wait(&a_empty[as], aph ^ 1);
+        if (++as == AS) { as = 0; aph ^= 1; }
+      }
+    } else if (warp == DMA_WARP) {
+      const EpiCtx ctx{staging, xch, res_bar, slot_ready};
+      epilogue_dma_loop<BN>(p, ctx, tmO, tmR, tmX, lane, num_tiles);
+    } else if (GN) {
+      // ------------------------------------------------------------------ GroupNorm + SiLU of the input, in the slab
+      // y = silu(x * a[f,c] + b[f,c]) exactly as gn_apply_kernel computes it, applied to every in-image pixel of the
+      // slab once it has landed (the zero padding TMA wrote for out-of-image pixels must stay zero), then handed to the
+      // MMA lane through a_ready.  Thread = one 16-byte channel chunk column (fixed 8 channels) x every 16th pixel row.
+      const int t = threadIdx.x - HALO_GN_FIRST;
+      const int c = t & 7, rl = t >> 3;
+      int as = 0;
+      uint32_t aph = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int n0, y0, x0;
+        decode_conv_tile(p, tile / p.n_tiles, n0, y0, x0);
+        for (int cb = 0; cb < p.cin_blocks; ++cb) {
+          float ah[8], bh[8];
+          const int ch0 = cb * BK + c * 8;
+          if (ch0 < p.gn_c) {
+            const float4* pa = reinterpret_cast<const float4*>(p.gn_ab + ((size_t)n0 * 2 + 0) * p.gn_c + ch0);
+            const float4* pb = reinterpret_cast<const float4*>(p.gn_ab + ((size_t)n0 * 2 + 1) * p.gn_c + ch0);
+            const float4 a0 = __ldg(pa), a1 = __ldg(pa + 1), b0 = __ldg(pb), b1 = __ldg(pb + 1);
+            ah[0] = a0.x; ah[1] = a0.y; ah[2] = a0.z; ah[3] = a0.w; ah[4] = a1.x; ah[5] = a1.y; ah[6] = a1.z; ah[7] = a1.w;
+            bh[0] = b0.x; bh[1] = b0.y; bh[2] = b0.z; bh[3] = b0.w; bh[4] = b1.x; bh[5] = b1.y; bh[6] = b1.z; bh[7] = b1.w;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { ah[j] *= 0.5f; bh[j] *= 0.5f; }     // silu(v) = h + h tanh(h), h = v / 2
+          } else {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { ah[j] = 0.f; bh[j] = 0.f; }         // channel padding stays zero
+          }
+          mbar_wait(&a_full[as], aph);
+          uint8_t* slab = smem_a + as * HALO_A_STRIDE;
+#pragma unroll 4
+          for (int j = 0; j < 12; ++j) {
+            const int r = rl + 16 * j;
+            if (r >= (HALO_TH + 2) * (HALO_TW + 2)) break;
+            const int sy = r / (HALO_TW + 2), sx = r - sy * (HALO_TW + 2);
+            if ((unsigned)(y0 - 1 + sy) >= (unsigned)p.H || (unsigned)(x0 - 1 + sx) >= (unsigned)p.W) continue;
+            uint4* ptr = reinterpret_cast<uint4*>(slab + r * 128 + ((c ^ (r & 7)) << 4));
+            const uint4 u = *ptr;
+            const float2 q0 = unpack_bf16x2(u.x), q1 = unpack_bf16x2(u.y), q2 = unpack_bf16x2(u.z), q3 = unpack_bf16x2(u.w);
+            float v[8] = {q0.x, q0.y, q1.x, q1.y, q2.x, q2.y, q3.x, q3.y};
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const float h = fmaf(v[e], ah[e], bh[e]);
+              float th;
+              asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(h));
+              v[e] = fmaf(h, th, h);
+            }
+            uint4 o;
+            o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]);
+            o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
+            *ptr = o;
+          }
+          fence_proxy_async();
+          mbar_arrive(&a_ready[as]);
+          if (++as == AS) { as = 0; aph ^= 1; }
         }
       }
     }
-  } else if (warp < EPI_WARPS) {
+  } else {
     // ------------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
+    if constexpr (!GN) setmaxnreg_inc<CONSUMER_REGS>();
     // Warpgroup h multiplies tile rows [64h, 64h + 64) = image rows [8h, 8h + 8) of the patch: its view of a tap starts
     // 8 slab rows further down.
     const EpiCtx ctx{staging, xch, res_bar, slot_ready};
@@ -801,7 +903,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       float acc[BN / 2];
       for (int cb = 0; cb < p.cin_blocks; ++cb) {
-        mbar_wait(GN ? &a_ready[as] : &a_full[as], aph);
+        mbar_wait_spin(GN ? &a_ready[as] : &a_full[as], aph);
         const uint64_t da0 = wgmma_desc_k_sw128(a_view + as * HALO_A_STRIDE, HALO_PITCH);
         auto tap_desc = [&](int t) -> uint64_t {       // slab row offset of tap t, in 16-byte descriptor units
           const int dy = t / p.tap_kw, dx = t - dy * p.tap_kw;
@@ -809,7 +911,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         };
         if (p.b_resident) {
           if (first) {
-            for (int t = 0; t < p.ntaps * p.cin_blocks; ++t) mbar_wait(&b_full[t], 0);
+            for (int t = 0; t < p.ntaps * p.cin_blocks; ++t) mbar_wait_spin(&b_full[t], 0);
             first = false;
           }
           wgmma_fence();
@@ -824,7 +926,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         } else {
           int prev = -1;
           for (int t = 0; t < p.ntaps; ++t) {
-            mbar_wait(&b_full[bs], bph);
+            mbar_wait_spin(&b_full[bs], bph);
             const uint64_t da = tap_desc(t);
             const uint64_t db = wgmma_desc_k_sw128(b_base + bs * Cfg::B_BYTES);
             wgmma_fence();
@@ -843,65 +945,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (++as == AS) { as = 0; aph ^= 1; }
       }
       epilogue_tile<BN>(p, ctx, warp, lane, tile, k, acc);
-    }
-  } else if (warp == DMA_WARP) {
-    const EpiCtx ctx{staging, xch, res_bar, slot_ready};
-    epilogue_dma_loop<BN>(p, ctx, tmO, tmR, tmX, lane, num_tiles);
-  } else if (GN) {
-    // ------------------------------------------------------------------ GroupNorm + SiLU of the input, in the slab
-    // y = silu(x * a[f,c] + b[f,c]) exactly as gn_apply_kernel computes it, applied to every in-image pixel of the
-    // slab once it has landed (the zero padding TMA wrote for out-of-image pixels must stay zero), then handed to the
-    // MMA lane through a_ready.  Thread = one 16-byte channel chunk column (fixed 8 channels) x every 16th pixel row.
-    const int t = threadIdx.x - GEMM_THREADS;
-    const int c = t & 7, rl = t >> 3;
-    int as = 0;
-    uint32_t aph = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      int n0, y0, x0;
-      decode_conv_tile(p, tile / p.n_tiles, n0, y0, x0);
-      for (int cb = 0; cb < p.cin_blocks; ++cb) {
-        float ah[8], bh[8];
-        const int ch0 = cb * BK + c * 8;
-        if (ch0 < p.gn_c) {
-          const float4* pa = reinterpret_cast<const float4*>(p.gn_ab + ((size_t)n0 * 2 + 0) * p.gn_c + ch0);
-          const float4* pb = reinterpret_cast<const float4*>(p.gn_ab + ((size_t)n0 * 2 + 1) * p.gn_c + ch0);
-          const float4 a0 = __ldg(pa), a1 = __ldg(pa + 1), b0 = __ldg(pb), b1 = __ldg(pb + 1);
-          ah[0] = a0.x; ah[1] = a0.y; ah[2] = a0.z; ah[3] = a0.w; ah[4] = a1.x; ah[5] = a1.y; ah[6] = a1.z; ah[7] = a1.w;
-          bh[0] = b0.x; bh[1] = b0.y; bh[2] = b0.z; bh[3] = b0.w; bh[4] = b1.x; bh[5] = b1.y; bh[6] = b1.z; bh[7] = b1.w;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { ah[j] *= 0.5f; bh[j] *= 0.5f; }     // silu(v) = h + h tanh(h), h = v / 2
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { ah[j] = 0.f; bh[j] = 0.f; }         // channel padding stays zero
-        }
-        mbar_wait(&a_full[as], aph);
-        uint8_t* slab = smem_a + as * HALO_A_STRIDE;
-#pragma unroll 4
-        for (int j = 0; j < 12; ++j) {
-          const int r = rl + 16 * j;
-          if (r >= (HALO_TH + 2) * (HALO_TW + 2)) break;
-          const int sy = r / (HALO_TW + 2), sx = r - sy * (HALO_TW + 2);
-          if ((unsigned)(y0 - 1 + sy) >= (unsigned)p.H || (unsigned)(x0 - 1 + sx) >= (unsigned)p.W) continue;
-          uint4* ptr = reinterpret_cast<uint4*>(slab + r * 128 + ((c ^ (r & 7)) << 4));
-          const uint4 u = *ptr;
-          const float2 q0 = unpack_bf16x2(u.x), q1 = unpack_bf16x2(u.y), q2 = unpack_bf16x2(u.z), q3 = unpack_bf16x2(u.w);
-          float v[8] = {q0.x, q0.y, q1.x, q1.y, q2.x, q2.y, q3.x, q3.y};
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float h = fmaf(v[e], ah[e], bh[e]);
-            float th;
-            asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(h));
-            v[e] = fmaf(h, th, h);
-          }
-          uint4 o;
-          o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]);
-          o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
-          *ptr = o;
-        }
-        fence_proxy_async();
-        mbar_arrive(&a_ready[as]);
-        if (++as == AS) { as = 0; aph ^= 1; }
-      }
     }
   }
 }
@@ -1029,17 +1072,28 @@ static int launch_halo(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
       snprintf(desc, sizeof(desc), "halo3%s F%d H%d W%d K%d N%d BN%d e%d r%d", GN ? "+gn" : "", p.F, p.H, p.W, p.K, p.N, BN,
                p.fast_epi, p.b_resident);
     ProfScope ps(PGT_PROF_GEMM, p.flops, stream, desc);
-    conv_halo_kernel<BN, GN><<<grid, GN ? GEMM_THREADS + HALO_GN_THREADS : GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(
+    conv_halo_kernel<BN, GN><<<grid, halo_threads<GN>(), Cfg::SMEM_BYTES, stream>>>(
         tmA, tmB, tmO, tmR, tmX, p);
   }
   PGT_LAUNCH_OK();
   return PGT_OK;
 }
 
-// Tiles are at most 128 wide: a warpgroup then holds 64 fp32 accumulators per thread, and a 64 x 128 x 16 wgmma
-// reads 96 operand bytes per cycle of tensor work, inside the shared-memory bandwidth.
+// Tile width from the shape.  A 128 x 256 tile moves 27 % fewer operand bytes per FLOP than 128 x 128 and reads each
+// A tile (every conv tap's) once instead of once per 128 columns; it is used when N > 128 fills whole 256-column tiles
+// about as well as 128-column ones, the k loop has at least 8 blocks, and there are enough tiles to occupy every SM.
+// Shorter k loops do not amortise the epilogue, which the 2-slot staging ring slows down: on an H100 (400 W) the
+// K = 128 / 256 launches of the flagship workload ran 5-12 % slower at BN = 256, every K >= 512 launch 1.0-1.7x faster.
+// SFT items take two staging slots and so stay on the 4-slot ring of the 128-wide kernel.
+static bool wide_tiles(const GemmParams& p) {
+  if (p.N <= 128 || p.num_kb < 8 || p.epi_mode == PGT_EPI_SFT) return false;
+  if (ceil_div(p.N, 256) * 256 > ceil_div(p.N, 128) * 128) return false;    // ragged: 256-wide would pad 128 more columns
+  return p.m_tiles * ceil_div(p.N, 256) >= num_sms();
+}
+
 static int dispatch_gemm(const CUtensorMap& tmA, const void* W, int ldw, GemmParams& p, cudaStream_t stream) {
   if (p.N <= 64) return launch_gemm<64>(tmA, W, ldw, p, stream);
+  if (wide_tiles(p)) return launch_gemm<256>(tmA, W, ldw, p, stream);
   return launch_gemm<128>(tmA, W, ldw, p, stream);
 }
 

@@ -13,6 +13,13 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
+// %laneid, read where it is used (volatile: the compiler may not keep it in a register from an earlier read)
+__device__ __forceinline__ int lane_id() {
+  int l;
+  asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
+  return l;
+}
+
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
