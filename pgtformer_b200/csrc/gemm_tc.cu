@@ -15,6 +15,8 @@
 //     warps 10, 11 idle (setmaxnreg acts on whole warpgroups)
 // Pipelines: smem full/empty ring (TMA <-> wgmma) and a staging ring of 4 slots (2 at BN = 256) (epilogue <-> DMA warp);
 // the producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
+// conv_halo_kernel<BN, false> runs the consumers PING-PONG instead: each warpgroup owns alternate tiles (all 128 rows)
+// and its epilogue (epilogue_tile_wg) runs under the other warpgroup's MMAs.
 // Consumer waits do not time out (a reachable trap would hold ptxas to the launch-bound register count); the producer
 // and the DMA warp wait with a bound, and the producer ends by waiting until every stage it filled has been released,
 // so a transaction that never completes traps the launch instead of hanging it.
@@ -51,7 +53,13 @@ constexpr int PRODUCER_REGS = 40;
 static_assert(2 * 128 * CONSUMER_REGS + 128 * PRODUCER_REGS <= 65536, "register file");
 constexpr int XCH_LD = 68;                       // accumulator exchange: 128 rows x 64 fp32 (+4 pad: conflict-free reads)
 constexpr int XCH_BYTES = BM * XCH_LD * 4;
+constexpr int XCH_WG_LD = 36;                    // per-warpgroup exchange (ping-pong): 128 rows x 32 fp32 (+4 pad)
+constexpr int XCH_WG_BYTES = BM * XCH_WG_LD * 4;
 constexpr int EPI_BAR = 1;                       // named barrier of the 256 consumer threads
+// ping-pong named barriers, each one per consumer warpgroup h (id + h)
+constexpr int PP_XCH_BAR = 2;                    // the warpgroup's 128 threads around its exchange
+constexpr int PP_MMA_BAR = 4;                    // "the other warpgroup has issued all MMAs of its tile": h may issue
+constexpr int PP_EPI_BAR = 6;                    // "the other warpgroup has finished its epilogue": h may start its own
 constexpr int A_STAGE_BYTES = BM * BK * 2;
 constexpr int PANEL_BYTES = BM * 128;            // one staging panel: 128 rows x 128 B
 // staging slots: 4 (two per epilogue half-group); at BN = 256 a 48 KB stage leaves room for 3 stages and 2 slots
@@ -288,7 +296,8 @@ __device__ __forceinline__ void epi_finish(const GemmParams& p, const uint32_t (
 
 // Epilogue work is a stream of ITEMS = (tile, 128-byte-wide column panel) flowing through a ring of staging slots.
 // Two roles:
-//   * 8 epilogue warps (two per 32-row quadrant, splitting a panel's 32-column chunks): wait until the slot is
+//   * 8 epilogue warps (two per 32-row quadrant, splitting a panel's 32-column chunks; in the ping-pong halo kernel
+//     the 4 warps of the tile's warpgroup, one per quadrant, taking both chunks): wait until the slot is
 //     prepared, accumulators -> bias / activation / residual / SFT -> swizzled smem, signal `slot_ready`.  No CTA-level
 //     barrier and no serial bookkeeping sits on this path.
 //   * one DMA warp (epilogue_dma_loop): prepares slots ahead of time (waits for the previous TMA store out of the
@@ -381,6 +390,103 @@ __device__ __forceinline__ void epilogue_dma_loop(const GemmParams& p, const Epi
   if (lane == 0) bulk_wait0();                           // all output bytes written before the CTA retires
 }
 
+// Direct path (NCHW fp32 output, unaligned views, mixed residual dtype): output row of tile row r.
+struct DirectRow {
+  bool valid;
+  long long orow;
+  int pn, py, px;
+};
+
+__device__ __forceinline__ DirectRow direct_row(const GemmParams& p, int m_blk, int r) {
+  DirectRow d{false, 0, 0, 0, 0};
+  if (p.mode == MODE_LINEAR) {
+    d.orow = (long long)m_blk * BM + r;
+    d.valid = d.orow < p.M;
+  } else {
+    int n0, y0, x0;
+    decode_conv_tile(p, m_blk, n0, y0, x0);
+    const int ix = r % p.tw;
+    const int t2 = r / p.tw;
+    const int iy = t2 % p.th;
+    const int in = t2 / p.th;
+    d.pn = n0 + in; d.py = y0 + iy; d.px = x0 + ix;
+    d.valid = (d.pn < p.F) && (d.py < p.H) && (d.px < p.W);
+    d.orow = ((long long)d.pn * p.H + d.py) * p.W + d.px;
+  }
+  return d;
+}
+
+// Direct path: columns [col0, col0 + 16) of one output row, accumulators at xs (exchange row), guarded loads / stores.
+__device__ __forceinline__ void epi_direct16(const GemmParams& p, const DirectRow& d, const float* xs, int col0) {
+  const int ncol = min(16, p.N - col0);
+  const long long orow = d.orow;
+  float f[16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) f[j] = xs[j] + ((p.bias != nullptr && j < ncol) ? __ldg(p.bias + col0 + j) : 0.f);
+  if (p.act != PGT_ACT_NONE && !p.relu_after_res) act_chunk(f, p.act);
+  if (p.residual != nullptr) {
+    if (p.res_dtype == PGT_BF16) {
+      const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.residual) + orow * p.ldr + col0;
+      float rr[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) rr[j] = (j < ncol) ? __bfloat162float(rp[j]) : 0.f;
+      if (p.epi_mode == PGT_EPI_SFT) {
+        const __nv_bfloat16* ap = reinterpret_cast<const __nv_bfloat16*>(p.aux) + orow * p.ldaux + col0;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float sc = (j < ncol) ? __bfloat162float(ap[j]) : 0.f;
+          f[j] = rr[j] + p.sft_w * (rr[j] * sc + f[j]);
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) f[j] += rr[j];
+      }
+    } else {
+      const float* rp = reinterpret_cast<const float*>(p.residual) + orow * p.ldr + col0;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        if (j < ncol) f[j] += __ldg(rp + j);
+    }
+  }
+  if (p.relu_after_res) act_chunk(f, PGT_ACT_RELU);
+  if (p.out_layout == PGT_OUT_NCHW) {
+    float* op = reinterpret_cast<float*>(p.out);
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+      if (j < ncol) op[(((long long)d.pn * p.N + (col0 + j)) * p.H + d.py) * p.W + d.px] = f[j];
+  } else if (p.out_dtype == PGT_BF16) {
+    __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + orow * p.ldo + col0;
+    if (ncol == 16 && ((p.ldo & 7) == 0)) {
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        uint4 u;
+        u.x = pack_bf16x2(f[q * 8 + 0], f[q * 8 + 1]);
+        u.y = pack_bf16x2(f[q * 8 + 2], f[q * 8 + 3]);
+        u.z = pack_bf16x2(f[q * 8 + 4], f[q * 8 + 5]);
+        u.w = pack_bf16x2(f[q * 8 + 6], f[q * 8 + 7]);
+        reinterpret_cast<uint4*>(op)[q] = u;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        if (j < ncol) op[j] = __float2bfloat16_rn(f[j]);
+    }
+  } else {
+    float* op = reinterpret_cast<float*>(p.out) + orow * p.ldo + col0;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+      if (j < ncol) op[j] = f[j];
+  }
+}
+
+// Fused GroupNorm statistics row of (tile m_blk, 32-row quadrant quad) for the chunk starting at column col0.
+__device__ __forceinline__ float* gn_stats_ptr(const GemmParams& p, int m_blk, int quad, int col0) {
+  if (p.gn_stats == nullptr) return nullptr;
+  const size_t chunk = p.gn_tpf > 0 ? (size_t)(m_blk / p.gn_tpf) * p.gn_fstride + (m_blk % p.gn_tpf) * 4 + quad
+                                    : (size_t)m_blk * 4 + quad;
+  return p.gn_stats + (chunk * 32 + col0 / p.gn_cpg) * 2;
+}
+
 // The epilogue of one tile, on the two consumer warpgroups right after their k loop.  Per 64-column group: both
 // warpgroups write their accumulator rows into the exchange, then thread (quad, half) reads row quad * 32 + lane,
 // columns [32 half, 32 half + 32) (bf16 panels: one chunk each) or the whole panel of parity half (fp32 panels).
@@ -406,32 +512,9 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
   const int col_base = n_blk * BN;
   const int npan = p.fast_epi ? is.panels_in_tile(tile) : 0;
   const uint32_t stg = smem_u32(ctx.staging) + r * 128;
-  auto gn_ptr = [&](int col0) -> float* {
-    if (p.gn_stats == nullptr) return nullptr;
-    const size_t chunk = p.gn_tpf > 0 ? (size_t)(m_blk / p.gn_tpf) * p.gn_fstride + (m_blk % p.gn_tpf) * 4 + quad
-                                      : (size_t)m_blk * 4 + quad;
-    return p.gn_stats + (chunk * 32 + col0 / p.gn_cpg) * 2;
-  };
-  // direct path (NCHW fp32 output, unaligned views, mixed residual dtype): this thread's output row
-  bool valid = false;
-  long long orow = 0;
-  int pn = 0, py = 0, px = 0;
-  if (!p.fast_epi) {
-    if (p.mode == MODE_LINEAR) {
-      orow = (long long)m_blk * BM + r;
-      valid = orow < p.M;
-    } else {
-      int n0, y0, x0;
-      decode_conv_tile(p, m_blk, n0, y0, x0);
-      const int ix = r % p.tw;
-      const int t2 = r / p.tw;
-      const int iy = t2 % p.th;
-      const int in = t2 / p.th;
-      pn = n0 + in; py = y0 + iy; px = x0 + ix;
-      valid = (pn < p.F) && (py < p.H) && (px < p.W);
-      orow = ((long long)pn * p.H + py) * p.W + px;
-    }
-  }
+  auto gn_ptr = [&](int col0) -> float* { return gn_stats_ptr(p, m_blk, quad, col0); };
+  // direct path: this thread's output row
+  const DirectRow drow = p.fast_epi ? DirectRow{false, 0, 0, 0, 0} : direct_row(p, m_blk, r);
 
   static_for<0, BN / 64>([&](auto gc) {
     constexpr int g = decltype(gc)::value;
@@ -491,70 +574,83 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
       // ---------------- direct path: per-thread global I/O of chunk `half` of the group, 16 columns at a time (the
       // accumulators of the later groups are still live: a 32-wide chunk of guarded loads would not fit beside them)
       const int c0 = g * 64 + half * 32;
-      if (valid) {
+      if (drow.valid) {
 #pragma unroll 1
         for (int sc16 = 0; sc16 < 32; sc16 += 16) {
           const int col0 = col_base + c0 + sc16;
           if (col0 >= p.N) break;
-          const int ncol = min(16, p.N - col0);
-          const float* xs = xrow + half * 32 + sc16;
-          float f[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) f[j] = xs[j] + ((p.bias != nullptr && j < ncol) ? __ldg(p.bias + col0 + j) : 0.f);
-          if (p.act != PGT_ACT_NONE && !p.relu_after_res) act_chunk(f, p.act);
-          if (p.residual != nullptr) {
-            if (p.res_dtype == PGT_BF16) {
-              const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.residual) + orow * p.ldr + col0;
-              float rr[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j) rr[j] = (j < ncol) ? __bfloat162float(rp[j]) : 0.f;
-              if (p.epi_mode == PGT_EPI_SFT) {
-                const __nv_bfloat16* ap = reinterpret_cast<const __nv_bfloat16*>(p.aux) + orow * p.ldaux + col0;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                  const float sc = (j < ncol) ? __bfloat162float(ap[j]) : 0.f;
-                  f[j] = rr[j] + p.sft_w * (rr[j] * sc + f[j]);
-                }
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] += rr[j];
-              }
-            } else {
-              const float* rp = reinterpret_cast<const float*>(p.residual) + orow * p.ldr + col0;
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (j < ncol) f[j] += __ldg(rp + j);
-            }
-          }
-          if (p.relu_after_res) act_chunk(f, PGT_ACT_RELU);
-          if (p.out_layout == PGT_OUT_NCHW) {
-            float* op = reinterpret_cast<float*>(p.out);
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (j < ncol) op[(((long long)pn * p.N + (col0 + j)) * p.H + py) * p.W + px] = f[j];
-          } else if (p.out_dtype == PGT_BF16) {
-            __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + orow * p.ldo + col0;
-            if (ncol == 16 && ((p.ldo & 7) == 0)) {
-#pragma unroll
-              for (int q = 0; q < 2; ++q) {
-                uint4 u;
-                u.x = pack_bf16x2(f[q * 8 + 0], f[q * 8 + 1]);
-                u.y = pack_bf16x2(f[q * 8 + 2], f[q * 8 + 3]);
-                u.z = pack_bf16x2(f[q * 8 + 4], f[q * 8 + 5]);
-                u.w = pack_bf16x2(f[q * 8 + 6], f[q * 8 + 7]);
-                reinterpret_cast<uint4*>(op)[q] = u;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (j < ncol) op[j] = __float2bfloat16_rn(f[j]);
-            }
-          } else {
-            float* op = reinterpret_cast<float*>(p.out) + orow * p.ldo + col0;
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              if (j < ncol) op[j] = f[j];
-          }
+          epi_direct16(p, drow, xrow + half * 32 + sc16, col0);
+        }
+      }
+      __syncwarp();
+    }
+  });
+}
+
+// The epilogue of one tile run by ONE consumer warpgroup (ping-pong schedule: the other warpgroup's MMAs run meanwhile).
+// The warpgroup holds all 128 rows as two m64 row blocks, acc[0] = rows [0, 64) and acc[1] = rows [64, 128).  Per
+// 32-column chunk: both blocks go through the warpgroup's own 128 x 32 fp32 exchange (ctx.xch), then thread
+// (wq, lane) reads row r = 32 wq + lane and finishes it with the same epi_finish / gn_chunk_stats arithmetic as
+// epilogue_tile, so outputs and statistics are bit-identical to it.  An item (panel) is signalled to the DMA warp
+// once all its chunks are written (slot_ready counts the warpgroup's 128 threads).  `k` is the ring index of the
+// tile's first item; `bar` is a named barrier of this warpgroup's 128 threads.
+template <int BN>
+__device__ __forceinline__ void epilogue_tile_wg(const GemmParams& p, const EpiCtx& ctx, int wq, int bar, int tile, int k,
+                                                 const float (&acc)[2][BN / 2]) {
+  const int lane = lane_id();                // re-read, not kept live across the k loop (BN = 128 has no spare registers)
+  const int r = wq * 32 + lane;
+  const int esize = (p.out_dtype == PGT_BF16) ? 2 : 4;
+  const ItemStream<BN> is(p, 0);
+  const int nsub = is.PW / 32;               // 32-column chunks per panel: 2 (bf16) or 1 (fp32)
+  constexpr int SLOTS = staging_slots<BN>();
+  constexpr int SLOT_SHIFT = SLOTS == 4 ? 2 : 1;
+  const bool sft = SLOTS == 4 && p.epi_mode == PGT_EPI_SFT;    // bf16 only: one 64-column item in two slots
+  const bool bias_vec = p.bias != nullptr && (p.N % 32) == 0;
+  const float* xrow = ctx.xch + r * XCH_WG_LD;
+
+  int n_blk, m_blk;
+  tile_mn(p, tile, m_blk, n_blk);
+  const int col_base = n_blk * BN;
+  const int npan = p.fast_epi ? is.panels_in_tile(tile) : 0;
+  const uint32_t stg = smem_u32(ctx.staging) + r * 128;
+  const DirectRow drow = p.fast_epi ? DirectRow{false, 0, 0, 0, 0} : direct_row(p, m_blk, r);
+
+  static_for<0, BN / 32>([&](auto cc) {
+    constexpr int c = decltype(cc)::value;
+    const int pnl = c / nsub, sub = c - pnl * nsub;
+    if (p.fast_epi && pnl >= npan) return;   // uniform over the warpgroup
+    const int col0 = col_base + c * 32;
+    if (col0 < p.N) {                        // a chunk wholly past N is clipped by the TMA store: skip its arithmetic
+      named_bar_sync(bar, 128);              // the previous chunk's rows have been read
+      acc_to_smem<c * 32, 32>(acc[0], ctx.xch, XCH_WG_LD, wq, lane);
+      acc_to_smem<c * 32, 32>(acc[1], ctx.xch + 64 * XCH_WG_LD, XCH_WG_LD, wq, lane);
+      named_bar_sync(bar, 128);
+    }
+    if (p.fast_epi) {
+      const int item = k + pnl;
+      const int pos = sft ? (item & 1) : (item & (SLOTS - 1));
+      if (sub == 0) mbar_wait_spin(&ctx.res_bar[pos], sft ? ((item >> 1) & 1) : ((item >> SLOT_SHIFT) & 1));
+      if (col0 < p.N) {
+        uint32_t v[32];
+        smem_row_32(xrow, v);
+        float4 nb[8];
+        if (sft)
+          epi_finish<true>(p, v, bias_vec ? p.bias + col0 : nullptr, stg + pos * 2 * PANEL_BYTES, r, sub, esize, true,
+                           gn_stats_ptr(p, m_blk, wq, col0), col0, nb, false);
+        else
+          epi_finish<false>(p, v, bias_vec ? p.bias + col0 : nullptr, stg + pos * PANEL_BYTES, r, sub, esize,
+                            p.has_res_map != 0, gn_stats_ptr(p, m_blk, wq, col0), col0, nb, false);
+      }
+      if (sub == nsub - 1) {
+        fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA engine
+        mbar_arrive(&ctx.slot_ready[pos]);
+      }
+    } else if (col0 < p.N) {
+      if (drow.valid) {
+#pragma unroll 1
+        for (int sc16 = 0; sc16 < 32; sc16 += 16) {
+          if (col0 + sc16 >= p.N) break;
+          epi_direct16(p, drow, xrow + sc16, col0 + sc16);
         }
       }
       __syncwarp();
@@ -713,16 +809,30 @@ constexpr int HALO_PITCH = (HALO_TW + 2) * 128;                     // bytes bet
 constexpr int HALO_A_BYTES = (HALO_TH + 2) * HALO_PITCH;            // 23040
 constexpr int HALO_A_STRIDE = ((HALO_A_BYTES + 1023) / 1024) * 1024; // 23552: keep every slab 1024-aligned
 
-template <int BN>
+// The ping-pong variant (GN = false) gives each consumer warpgroup its own exchange (2 x 18 KB instead of 34 KB).  At
+// BN = 128 that costs a weight stage: the ring keeps 4 of 16 KB.  A 3x3 tap of BN = 128 is never resident (9 > 5) and
+// the 4-tap upsample phases with Cin <= 64 still are; with the previous schedule, 4 stages timed the same as 5 on every
+// BN = 128 shape of tools/micro_conv.py halo (H100 80GB HBM3, 700 W).  The staging ring keeps its 4 slots, because an
+// SFT item takes two of them.
+template <int BN, bool GN>
 struct HaloCfg {
   static constexpr int B_BYTES = BN * 128;
   static constexpr int A_STAGES = 2;
-  static constexpr int B_STAGES = (BN == 64) ? 9 : 5;
+  static constexpr int B_STAGES = (BN == 64) ? 9 : GN ? 5 : 4;
   static constexpr int SLOTS = staging_slots<BN>();
   static constexpr int STAGING_BYTES = SLOTS * PANEL_BYTES;
-  static constexpr int SMEM_BYTES = A_STAGES * HALO_A_STRIDE + B_STAGES * B_BYTES + STAGING_BYTES + XCH_BYTES + 512 + 1024;
+  static constexpr int XCH = GN ? XCH_BYTES : 2 * XCH_WG_BYTES;
+  static constexpr int SMEM_BYTES = A_STAGES * HALO_A_STRIDE + B_STAGES * B_BYTES + STAGING_BYTES + XCH + 512 + 1024;
   static_assert(SMEM_BYTES <= 232448, "halo conv smem budget");
 };
+
+// ring position after n more stages of a ring of S
+template <int S>
+__device__ __forceinline__ void ring_skip(int& s, uint32_t& ph, int n) {
+  const int t = s + n;
+  ph ^= (uint32_t)(t / S) & 1u;
+  s = t % S;
+}
 
 // The GroupNorm-fused variant keeps its own layout without setmaxnreg: warps 0..9 as above, then four GroupNorm warps.
 constexpr int HALO_GN_THREADS = 128;             // extra warps of the GroupNorm-fused variant
@@ -735,15 +845,16 @@ __global__ void __launch_bounds__(halo_threads<GN>(), 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
                  const __grid_constant__ CUtensorMap tmX, const GemmParams p) {
-  using Cfg = HaloCfg<BN>;
+  using Cfg = HaloCfg<BN, GN>;
   constexpr int AS = Cfg::A_STAGES, BS = Cfg::B_STAGES;
+  constexpr int RELEASERS = GN ? EPI_WARPS : 4;   // warps releasing a ring stage: both warpgroups, or the ping-pong owner
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + AS * HALO_A_STRIDE;
   uint8_t* staging = smem_b + BS * Cfg::B_BYTES;
   float* xch = reinterpret_cast<float*>(staging + Cfg::STAGING_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES + XCH_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES + Cfg::XCH);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + AS;
   uint64_t* b_full = bars + 2 * AS;
@@ -763,11 +874,11 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (p.fast_epi) tma_prefetch_desc(&tmO);
     if (p.has_res_map) tma_prefetch_desc(&tmR);
     if (p.fast_epi && p.epi_mode == PGT_EPI_SFT) tma_prefetch_desc(&tmX);
-    for (int i = 0; i < AS; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], EPI_WARPS); mbar_init(&a_ready[i], HALO_GN_THREADS); }
-    for (int i = 0; i < BS; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], EPI_WARPS); }
+    for (int i = 0; i < AS; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], RELEASERS); mbar_init(&a_ready[i], HALO_GN_THREADS); }
+    for (int i = 0; i < BS; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], RELEASERS); }
     for (int i = 0; i < Cfg::SLOTS; ++i) {
       mbar_init(&res_bar[i], 1);
-      mbar_init(&slot_ready[i], EPI_WARPS * 32);
+      mbar_init(&slot_ready[i], RELEASERS * 32);
     }
     fence_barrier_init();
   }
@@ -887,9 +998,90 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
+  } else if constexpr (!GN) {
+    // ------------------------------------------------------------------ ping-pong consumer warpgroups
+    // The j-th tile of the CTA belongs to warpgroup j & 1, which multiplies all 128 rows (two m64 row blocks on one B
+    // descriptor; block 1 = image rows [8, 16) of the patch, 8 slab rows further down) and runs the whole epilogue.
+    // Two ordered hand-overs keep the rings and the staging items in tile order:
+    //   MMA turn  a warpgroup issues tile j once the other has ISSUED every wgmma of tile j - 1, so the tensor pipe
+    //             holds tile j - 1's tail when tile j arrives, and the slab / weight stages are consumed in tile order;
+    //   epilogue  it starts the epilogue of tile j once the other has finished that of tile j - 1 (the DMA warp takes
+    //             items in order).
+    // So one warpgroup's epilogue runs under the other's MMAs.  Each hand-over is a named barrier of 256 threads: the
+    // waiting warpgroup syncs, the other arrives, and only when the tile it waits for exists, so none is left pending.
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = warp >> 2;
+    const EpiCtx ctx{staging, xch + wg * (XCH_WG_BYTES / 4), res_bar, slot_ready};
+    const uint32_t a_base = smem_u32(smem_a);
+    const uint32_t b_base = smem_u32(smem_b);
+    constexpr uint64_t ROW_BLOCK = 8 * HALO_PITCH / 16;   // descriptor units from row block 0 to row block 1
+    const ItemStream<BN> is(p, num_tiles);
+    const int b_per_tile = p.b_resident ? 0 : p.ntaps * p.cin_blocks;
+    int as = 0, bs = 0;
+    uint32_t aph = 0, bph = 0;
+    int k = 0;
+    bool first = true;
+    for (int tile = blockIdx.x, j = 0; tile < num_tiles; tile += gridDim.x, ++j) {
+      const bool has_next = tile + (int)gridDim.x < num_tiles;
+      const int items = p.fast_epi ? is.panels_in_tile(tile) : 0;
+      if ((j & 1) != wg) {                             // the other warpgroup's tile: step over its stages and items
+        ring_skip<AS>(as, aph, p.cin_blocks);
+        ring_skip<BS>(bs, bph, b_per_tile);
+        k += items;
+        continue;
+      }
+      if (j > 0) named_bar_sync(PP_MMA_BAR + wg, 256);
+      float acc[2][BN / 2];
+      for (int cb = 0; cb < p.cin_blocks; ++cb) {
+        const bool hand_over = has_next && cb == p.cin_blocks - 1;
+        mbar_wait_spin(&a_full[as], aph);
+        const uint64_t da0 = wgmma_desc_k_sw128(a_base + as * HALO_A_STRIDE, HALO_PITCH);
+        auto tap_desc = [&](int t) -> uint64_t {
+          const int dy = t / p.tap_kw, dx = t - dy * p.tap_kw;
+          return da0 + (uint64_t)(((dy + p.tap_oy) * (HALO_TW + 2) + dx + p.tap_ox) * 8);
+        };
+        if (p.b_resident && first) {
+          for (int t = 0; t < p.ntaps * p.cin_blocks; ++t) mbar_wait_spin(&b_full[t], 0);
+          first = false;
+        }
+        // One wgmma site for resident and streamed weights: with two, ptxas serialises every wgmma (C7520).
+        int prev = -1;
+        for (int t = 0; t < p.ntaps; ++t) {
+          int bst = cb * p.ntaps + t;                    // resident: the tap's fixed stage
+          if (!p.b_resident) {
+            mbar_wait_spin(&b_full[bs], bph);
+            bst = bs;
+          }
+          const uint64_t da = tap_desc(t);
+          const uint64_t db = wgmma_desc_k_sw128(b_base + bst * Cfg::B_BYTES);
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < BK / 16; ++kk) {
+            const uint32_t accum = (cb | t | kk) != 0 ? 1u : 0u;
+            wgmma_bf16<BN>(acc[0], da + 2 * kk, db + 2 * kk, accum);
+            wgmma_bf16<BN>(acc[1], da + ROW_BLOCK + 2 * kk, db + 2 * kk, accum);
+          }
+          wgmma_commit();
+          if (hand_over && t == p.ntaps - 1) named_bar_arrive(PP_MMA_BAR + (wg ^ 1), 256);
+          wgmma_wait<1>();                               // the previous tap's weight stage is free
+          if (!p.b_resident) {
+            if (prev >= 0) release_stage(&b_empty[prev], lane);
+            prev = bs;
+            if (++bs == BS) { bs = 0; bph ^= 1; }
+          }
+        }
+        wgmma_wait<0>();
+        if (!p.b_resident) release_stage(&b_empty[prev], lane);
+        release_stage(&a_empty[as], lane);
+        if (++as == AS) { as = 0; aph ^= 1; }
+      }
+      if (j > 0) named_bar_sync(PP_EPI_BAR + wg, 256);
+      epilogue_tile_wg<BN>(p, ctx, warp & 3, PP_XCH_BAR + wg, tile, k, acc);
+      if (has_next) named_bar_arrive(PP_EPI_BAR + (wg ^ 1), 256);
+      k += items;
+    }
   } else {
-    // ------------------------------------------------------------------ consumer warpgroups: wgmma + epilogue
-    if constexpr (!GN) setmaxnreg_inc<CONSUMER_REGS>();
+    // ------------------------------------------------------------------ GroupNorm-fused variant: consumer warpgroups
     // Warpgroup h multiplies tile rows [64h, 64h + 64) = image rows [8h, 8h + 8) of the patch: its view of a tap starts
     // 8 slab rows further down.
     const EpiCtx ctx{staging, xch, res_bar, slot_ready};
@@ -1054,7 +1246,7 @@ static int launch_gemm(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
 
 template <int BN, bool GN>
 static int launch_halo(const CUtensorMap& tmA, const void* W, int ldw, GemmParams& p, cudaStream_t stream) {
-  using Cfg = HaloCfg<BN>;
+  using Cfg = HaloCfg<BN, GN>;
   CUtensorMap tmB, tmO, tmR, tmX;
   int rc = encode_weight_map(&tmB, W, ldw, p.K, p.N, BN);
   if (rc != PGT_OK) return rc;

@@ -141,6 +141,10 @@ __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Signal a named barrier without waiting: the other side of an ordered hand-over waits on it with named_bar_sync.
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // A warpgroup (four consecutive warps 4k..4k+3) issues D[64 x N] (+)= A[64 x 16] * B[N x 16]^T with both operands read

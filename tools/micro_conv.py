@@ -1,7 +1,8 @@
 """Micro-benchmark of single conv shapes (CUDA events, 20 reps).  The wide cases (Cout > 128, the flagship workload's
 own shapes at 16 clips = 48 frames) time the launch dispatch_gemm picks against the same conv launched as 128-channel
 slices, which take the library's Cout <= 128 path (the halo kernel for stride-1 3x3 and upsample-phase convs,
-gemm_tc_kernel<128> otherwise): both in one process, with no switch in the library.  `python tools/micro_conv.py wide`."""
+gemm_tc_kernel<128> otherwise): both in one process, with no switch in the library.  `python tools/micro_conv.py wide`.
+`python tools/micro_conv.py halo` times each Cout <= 128 halo-kernel shape of the flagship workload alone."""
 import os
 import sys
 import torch
@@ -76,6 +77,45 @@ def wide_up2x(F, H, C):
                                            ops.ctypes.byref(ep), ops._stream()))
     wide_case('up2x F%d %d^2->%d^2 %d->%d' % (F, H, 2 * H, C, C), 2.0 * F * 4 * H * H * C * 4 * C, run, C)
 
+
+def halo_case(name, flops, fn):
+    ms = timeit(fn)
+    print('%-40s %8.3f ms %5.0f TF/s' % (name, ms, flops / ms / 1e9))
+
+
+def halo_conv(F, H, Cin, N, residual=False):
+    x = torch.randn(F, H, H, Cin, device=dev).bfloat16()
+    wp = _pack_conv(torch.randn(N, Cin, 3, 3, device=dev) * 0.05)
+    b = torch.zeros(N, device=dev)
+    res = torch.randn(F, H, H, N, device=dev).bfloat16() if residual else None
+    out = torch.empty(F, H, H, N, device=dev, dtype=torch.bfloat16)
+    halo_case('conv F%d %d^2 %d->%d res=%d' % (F, H, Cin, N, residual), 2.0 * F * H * H * N * 9 * Cin,
+              lambda: ops.conv(x, wp, N, out, bias=b, residual=res))
+    del x, res, out
+
+
+def halo_up2x(F, H, C):
+    x = torch.randn(F, H, H, C, device=dev).bfloat16()
+    wp4 = _pack_up2x(torch.randn(C, C, 3, 3, device=dev) * 0.05)
+    b = torch.zeros(C, device=dev)
+    out = torch.empty(F, 2 * H, 2 * H, C, device=dev, dtype=torch.bfloat16)
+    halo_case('up2x F%d %d^2->%d^2 %d->%d' % (F, H, 2 * H, C, C), 2.0 * F * 4 * H * H * C * 4 * C,
+              lambda: ops.conv_up2x(x, wp4, C, out, bias=b))
+    del x, out
+
+
+if len(sys.argv) > 1 and sys.argv[1] == 'halo':
+    # the flagship workload's Cout <= 128 halo shapes at 16 clips = 48 frames (288 channels: the SFT concat buffer)
+    halo_conv(48, 512, 64, 64)
+    halo_conv(48, 512, 64, 64, residual=True)
+    halo_conv(48, 512, 128, 64)
+    halo_conv(48, 256, 64, 128)
+    halo_conv(48, 256, 128, 128, residual=True)
+    halo_conv(48, 256, 288, 128)
+    halo_conv(48, 256, 256, 128)
+    halo_up2x(48, 256, 128)
+    halo_conv(48, 128, 64, 64)
+    sys.exit(0)
 
 if len(sys.argv) > 1 and sys.argv[1] == 'wide':
     wide_conv(48, 128, 256, 256)
