@@ -62,7 +62,8 @@ def _materialise(root, spec, seed):
                 child._pgt_root = rootref
                 node.add_module(part, child)
             node = node._modules[part]
-        t = synth_tensor(name, shape, 'codebook' if kind == 'codebook_ema' else kind, dtype, seed)
+        t = synth_tensor(name, shape, 'codebook' if kind == 'codebook_ema' else kind, dtype, seed,
+                         window=getattr(spec, 'windows', {}).get(name))
         if kind == 'codebook_ema':
             t = t[:-1] if t.shape[0] == shape[0] + 1 else t
         if kind in ('bn_mean', 'bn_var', 'bn_count', 'rpb_index', 'zeros', 'codebook_ema'):
@@ -109,12 +110,45 @@ class _B200Model(nn.Module):
 
     def engine(self):
         if self.__dict__.get('_engine') is None:
-            from pgtformer_b200.engine import Engine
             dev = next(self.parameters()).device
             if dev.type != 'cuda':
                 raise RuntimeError('pgtformer_b200: no CPU path — move the model to a CUDA (sm_90a) device first')
-            self.__dict__['_engine'] = Engine(self._network_g, self.state_dict(), dev)
+            self.__dict__['_engine'] = self._engine_class()(self._network_g, self.state_dict(), dev)
         return self.__dict__['_engine']
+
+    def _engine_class(self):
+        from pgtformer_b200.engine import Engine
+        return Engine
+
+    # ---- depth-1 code helpers shared by the codecs.  Arguments are checked on the host before any launch: bad shapes
+    # raise ValueError, codes outside [0, n_embed] IndexError (index n_embed is the codebook's padding row, which
+    # nn.Embedding accepts).
+    def _check_code(self, code):
+        if not torch.is_tensor(code) or code.dim() != 4 or code.shape[-1] != self.code_shape[-1] or \
+                code.dtype.is_floating_point or code.dtype.is_complex or code.dtype == torch.bool:
+            raise ValueError('expected integer codes [F, h, w, %d], got %s %s'
+                             % (self.code_shape[-1], _shape(code), getattr(code, 'dtype', '')))
+        if code.numel() > 0:
+            lo, hi = torch.aminmax(code)
+            n = self.arch.n_embed
+            if int(lo) < 0 or int(hi) > n:
+                raise IndexError('code out of range [0, %d]: min %d, max %d' % (n, int(lo), int(hi)))
+
+    @torch.no_grad()
+    def get_code_emb_with_depth(self, code):
+        """(codebook rows [F, h, w, 1, embed_dim] fp32, None), as RQBottleneck.embed_code_with_depth returns them."""
+        self._check_code(code)
+        Fr, h, w, d = code.shape
+        return self.engine().embed_code(code).view(Fr, h, w, d, self.arch.embed_dim), None
+
+    @torch.no_grad()
+    def decode_partial_code(self, code, code_idx, decode_type='select'):
+        """Decodes with codebooks [0 .. code_idx]; with one codebook 'select' and 'add' are both decode_code."""
+        self._check_code(code)
+        assert code_idx < code.shape[-1]
+        if decode_type not in ('select', 'add'):
+            raise NotImplementedError(f"{decode_type} is not implemented in partial decoding")
+        return self.decode_code(code)
 
     def train(self, mode=True):
         """The reference's train() forgets `return self` (archs/pgtformer_arch.py:577-581), so
@@ -148,9 +182,8 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
     def get_codes(self, input):
         return self.engine().forward_vq(input, code_only=True)[2]
 
-    # ---- the rest of the stage-I codec surface (`archs/tdcrqvae3_arch.py:774-872`), depth-1 quantiser.  Arguments are
-    # checked on the host before any launch: bad shapes raise ValueError, codes outside [0, n_embed] IndexError (index
-    # n_embed is the codebook's padding row, which nn.Embedding accepts).
+    # ---- the rest of the stage-I codec surface (`archs/tdcrqvae3_arch.py:774-872`), depth-1 quantiser; arguments are
+    # checked on the host before any launch (see _B200Model._check_code).
     def _frames(self, x):
         """[b, t, 3, H, W] (the reference's form) or [b*t, 3, H, W] -> [b*t, 3, H, W]."""
         if not torch.is_tensor(x) or x.dim() not in (4, 5):
@@ -167,17 +200,6 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
         if Fr == 0 or Fr % self.t != 0 or h == 0 or w == 0 or h % 4 != 0 or w % 4 != 0:
             raise ValueError('expected %d-frame clips with a latent map of multiples of 4 (frames multiples of 64), '
                              'got [%d, %d, %d]' % (self.t, Fr, h, w))
-
-    def _check_code(self, code):
-        if not torch.is_tensor(code) or code.dim() != 4 or code.shape[-1] != self.code_shape[-1] or \
-                code.dtype.is_floating_point or code.dtype.is_complex or code.dtype == torch.bool:
-            raise ValueError('expected integer codes [F, h, w, %d], got %s %s'
-                             % (self.code_shape[-1], _shape(code), getattr(code, 'dtype', '')))
-        if code.numel() > 0:
-            lo, hi = torch.aminmax(code)
-            n = self.arch.n_embed
-            if int(lo) < 0 or int(hi) > n:
-                raise IndexError('code out of range [0, %d]: min %d, max %d' % (n, int(lo), int(hi)))
 
     @torch.no_grad()
     def encode(self, x):
@@ -202,22 +224,6 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
         eng = self.engine()
         Fr, h, w, _ = code.shape
         return eng.decode(eng.embed_code(code).view(Fr, h, w, self.arch.embed_dim))
-
-    @torch.no_grad()
-    def get_code_emb_with_depth(self, code):
-        """(codebook rows [F, h, w, 1, embed_dim] fp32, None), as RQBottleneck.embed_code_with_depth returns them."""
-        self._check_code(code)
-        Fr, h, w, d = code.shape
-        return self.engine().embed_code(code).view(Fr, h, w, d, self.arch.embed_dim), None
-
-    @torch.no_grad()
-    def decode_partial_code(self, code, code_idx, decode_type='select'):
-        """Decodes with codebooks [0 .. code_idx]; with one codebook 'select' and 'add' are both decode_code."""
-        self._check_code(code)
-        assert code_idx < code.shape[-1]
-        if decode_type not in ('select', 'add'):
-            raise NotImplementedError(f"{decode_type} is not implemented in partial decoding")
-        return self.decode_code(code)
 
     @torch.no_grad()
     def forward_partial_code(self, xs, code_idx, decode_type='select'):

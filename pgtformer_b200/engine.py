@@ -88,9 +88,11 @@ def _pack_rgb(w):
 
 
 class Engine:
+    arch_class = Arch
+
     def __init__(self, network_g, state_dict, device):
         ops.L.load()                                   # fail loudly if the CUDA library is missing
-        self.arch = Arch(network_g)
+        self.arch = self.arch_class(network_g)
         self.dev = torch.device(device)
         if self.dev.type != 'cuda':
             raise RuntimeError('pgtformer_b200 has no CPU path: the engine needs a CUDA (sm_90a) device')
@@ -421,8 +423,19 @@ class Engine:
         the first one with attention, including the Downsample into it — nothing here looks across frames, so the
         streaming pipeline runs it once per distinct frame.  Returns (h, feats, next level)."""
         a = self.arch
+        h = self.conv_in(x)
+        feats = []
+        lvl = 0
+        while lvl < a.num_levels - 1 and not a.level_has_attn[lvl]:
+            h = self._encoder_level(h, lvl, feats)
+            lvl += 1
+        return h, feats, lvl
+
+    def conv_in(self, x):
+        """encoder.conv_in on the fp32 NCHW frames.  Cin = 3: the kernel builds the patch rows itself; its epilogue also
+        yields block 0's GroupNorm statistics."""
+        a = self.arch
         Fr, _, H, W = x.shape
-        # Cin = 3: the kernel builds the patch rows itself; its epilogue also yields block 0's GroupNorm statistics
         h = self._new(Fr, H, W, a.ch)
         stats = None
         if self.fuse_gn_stats and (H * W) % 128 == 0 and a.ch == 64:
@@ -430,12 +443,7 @@ class Engine:
             stats = self._new(Fr * tpf * 4 * 64, dtype=torch.float32)
             h._pgt_gn = (stats, tpf * 4)
         ops.conv_rgb(x, self.w['encoder.conv_in.weight'], self.w['encoder.conv_in.bias'], h, 3, 1, 1, gn_stats=stats)
-        feats = []
-        lvl = 0
-        while lvl < a.num_levels - 1 and not a.level_has_attn[lvl]:
-            h = self._encoder_level(h, lvl, feats)
-            lvl += 1
-        return h, feats, lvl
+        return h
 
     def _encoder_level(self, h, lvl, feats):
         a = self.arch
@@ -518,15 +526,23 @@ class Engine:
             if fuse:
                 h = self.fuse_sft(feats[lvl], h, a.fuse_level_key[lvl], wgt, gn_next=(lvl == 0))
             if lvl != 0:
-                Fr, H, W, C = h.shape
-                p = 'decoder.up.%d.upsample.conv' % lvl
-                out = self._new(Fr, 2 * H, 2 * W, C)
-                stats = None
-                tpf = ops.conv_tiles_per_frame(H, W, C, 2, 1, 1)
-                if self.fuse_gn_stats and tpf > 0 and C // 32 in (2, 4, 8, 16, 32):
-                    stats = self._new(Fr * 16 * tpf * 64, dtype=torch.float32)     # [frame][phase][tile][quadrant][32][2]
-                    out._pgt_gn = (stats, 16 * tpf)
-                h = ops.conv_up2x(h, self.w[p + '.weight'], C, out, bias=self.w[p + '.bias'], gn_stats=stats)
+                h = self.up2x(h, 'decoder.up.%d.upsample.conv' % lvl)
+        return self.decoder_out(h)
+
+    def up2x(self, h, p):
+        """Upsample (nearest x2 + conv3x3) as four 2x2 phase convs; the epilogue emits the next norm1's statistics."""
+        Fr, H, W, C = h.shape
+        out = self._new(Fr, 2 * H, 2 * W, C)
+        stats = None
+        tpf = ops.conv_tiles_per_frame(H, W, C, 2, 1, 1)
+        if self.fuse_gn_stats and tpf > 0 and C // 32 in (2, 4, 8, 16, 32):
+            stats = self._new(Fr * 16 * tpf * 64, dtype=torch.float32)     # [frame][phase][tile][quadrant][32][2]
+            out._pgt_gn = (stats, 16 * tpf)
+        return ops.conv_up2x(h, self.w[p + '.weight'], C, out, bias=self.w[p + '.bias'], gn_stats=stats)
+
+    def decoder_out(self, h):
+        """decoder.norm_out + SiLU + decoder.conv_out -> fp32 NCHW [F, out_ch, H, W]."""
+        a = self.arch
         Fr, H, W, _ = h.shape
         out = self._new(Fr, a.out_ch, H, W, dtype=torch.float32)
         if self.fuse_conv_out:

@@ -17,6 +17,10 @@ N_WIN_TOK = 48
 
 
 class Spec(OrderedDict):
+    def __init__(self, *a, **k):
+        super().__init__(*a, **k)
+        self.windows = {}         # name of a relative_position_index buffer -> its (D, H, W) window (default: WINDOW)
+
     def add(self, name, shape, kind, dtype='float32'):
         assert name not in self, name
         self[name] = (tuple(int(s) for s in shape), kind, dtype)
@@ -237,4 +241,142 @@ def build_spec(network_g):
         _conv(s, p + '.tconvdec', c, tcc, 1)
         _conv(s, p + '.tfusion0', 2 * t * tcc, tcc * t, 1)
         _conv(s, p + '.tfusion1', tcc, tcc, 1)
+    return a, s
+
+
+# --------------------------------------------------------------------------- TDRQVAE (archs/tdrqvae_arch.py:787-841)
+ATTN_WIDTHS = (64, 256, 512)          # pgt_mha_fwd head widths (the AttnBlock is one head of width C)
+SWIN_HEAD_WIDTHS = (16, 32, 64)       # pgt_window3d_attention head widths
+SWIN_MAX_TOKENS = 128                 # pgt_window3d_attention: tokens per window
+
+
+def _attn_block(s, p, c):
+    """AttnBlock (`archs/tdrqvae_arch.py:151-176`): GroupNorm + four 1x1 convs."""
+    _norm(s, p + '.norm', c)
+    for n in ('q', 'k', 'v', 'proj_out'):
+        _conv(s, '%s.%s' % (p, n), c, c, 1)
+
+
+def _swin3d_layer(s, p, c, depth, heads, window, mlp_ratio=4):
+    """Video-Swin BasicLayer (`modules/swin.py:326-378`): depth x SwinTransformerBlock3D, qkv without bias."""
+    n = window[0] * window[1] * window[2]
+    nrel = (2 * window[0] - 1) * (2 * window[1] - 1) * (2 * window[2] - 1)
+    for i in range(depth):
+        b = '%s.blocks.%d' % (p, i)
+        _norm(s, b + '.norm1', c)
+        s.add(b + '.attn.relative_position_bias_table', (nrel, heads), 'rpb_table')
+        s.add(b + '.attn.relative_position_index', (n, n), 'rpb_index', 'int64')
+        s.windows[b + '.attn.relative_position_index'] = tuple(window)
+        _linear(s, b + '.attn.qkv', c, 3 * c, bias=False)
+        _linear(s, b + '.attn.proj', c, c)
+        _norm(s, b + '.norm2', c)
+        _linear(s, b + '.mlp.fc1', c, mlp_ratio * c)
+        _linear(s, b + '.mlp.fc2', mlp_ratio * c, c)
+
+
+class TDRQVAEArch:
+    """Resolved constants of TDRQVAE: the 2-D RQ-VAE Encoder / Decoder (`archs/tdrqvae_arch.py:587-784`) around a
+    depth-1 RQBottleneck and two Video-Swin BasicLayers.  Raises ValueError for what the reference rejects and for
+    what the CUDA kernels cannot run."""
+
+    def __init__(self, network_g):
+        g = dict(network_g)
+        dd = dict(g['ddconfig'])
+        self.tf = int(g.get('tf', 7))
+        self.embed_dim = int(g.get('embed_dim', 64))
+        self.n_embed = int(g.get('n_embed', 512))
+        if g.get('bottleneck_type', 'rq') != 'rq':
+            raise ValueError("invalid 'bottleneck_type' (must be 'rq')")     # tdrqvae_arch.py:829
+        self.latent_shape = tuple(g['latent_shape'])
+        self.code_shape = tuple(g['code_shape'])
+        if not len(self.code_shape) == len(self.latent_shape) == 3:
+            raise ValueError('incompatible code shape or latent shape')      # tdrqvae_arch.py:357-360
+        if any(y % x != 0 for x, y in zip(self.code_shape[:2], self.latent_shape[:2])):
+            raise ValueError('incompatible code shape or latent shape')
+        if self.code_shape[2] != 1:
+            raise ValueError('the CUDA path is built for quantiser depth 1')
+        self.ch = int(dd['ch'])
+        self.ch_mult = tuple(dd['ch_mult'])
+        self.num_res_blocks = int(dd['num_res_blocks'])
+        self.resolution = int(dd['resolution'])
+        self.attn_resolutions = tuple(dd['attn_resolutions'])
+        self.z_channels = int(dd['z_channels'])
+        self.in_channels = int(dd['in_channels'])
+        self.out_ch = int(dd['out_ch'])
+        self.double_z = bool(dd.get('double_z', True))
+        self.stages_atten = int(dd['stages_atten'])
+        self.num_head = int(dd['num_head'])
+        self.window_size = tuple(int(w) for w in dd['window_size'])
+        self.num_levels = len(self.ch_mult)
+        self.down = 2 ** (self.num_levels - 1)                            # frame size / latent size
+        self.level_ch = tuple(self.ch * m for m in self.ch_mult)
+        # levels with AttnBlocks: the curr_res walk of the constructor (:606-627), fixed by `resolution`
+        self.level_has_attn = tuple((self.resolution >> i) in self.attn_resolutions for i in range(self.num_levels))
+        if self.double_z:
+            raise ValueError('double_z: Encoder.conv_out would give 2 * z_channels, quant_conv reads z_channels')
+        if self.in_channels != 3 or self.ch != 64:
+            raise ValueError('the CUDA path is built for RGB input and ch = 64')
+        if any(c % 32 for c in self.level_ch):
+            raise ValueError('GroupNorm(32): every level width must be a multiple of 32')
+        widths = {c for c, a in zip(self.level_ch, self.level_has_attn) if a} | {self.level_ch[-1]}
+        if not widths <= set(ATTN_WIDTHS):
+            raise ValueError('AttnBlock widths %s: the attention kernel takes %s' % (sorted(widths), ATTN_WIDTHS))
+        if self.stages_atten < 1 or self.num_head < 1 or self.embed_dim % self.num_head or \
+                self.embed_dim // self.num_head not in SWIN_HEAD_WIDTHS:
+            raise ValueError('Video-Swin layers of %d blocks, %d heads over %d channels: head width must be one of %s'
+                             % (self.stages_atten, self.num_head, self.embed_dim, SWIN_HEAD_WIDTHS))
+        if len(self.window_size) != 3 or min(self.window_size) < 1 or \
+                self.window_size[0] * self.window_size[1] * self.window_size[2] > SWIN_MAX_TOKENS:
+            raise ValueError('Video-Swin window %s: at most %d tokens' % (self.window_size, SWIN_MAX_TOKENS))
+
+
+def build_tdrqvae_spec(network_g):
+    a = TDRQVAEArch(network_g)
+    s = Spec()
+    in_mult = (1,) + a.ch_mult
+    # ---- Encoder (tdrqvae_arch.py:587-648)
+    _conv(s, 'encoder.conv_in', a.in_channels, a.ch, 3)
+    for lvl in range(a.num_levels):
+        block_in = a.ch * in_mult[lvl]
+        block_out = a.level_ch[lvl]
+        for b in range(a.num_res_blocks):
+            _td_resblock(s, 'encoder.down.%d.block.%d' % (lvl, b), block_in, block_out)
+            block_in = block_out
+        if a.level_has_attn[lvl]:
+            for b in range(a.num_res_blocks):
+                _attn_block(s, 'encoder.down.%d.attn.%d' % (lvl, b), block_in)
+        if lvl != a.num_levels - 1:
+            _conv(s, 'encoder.down.%d.downsample.conv' % lvl, block_in, block_in, 3)
+    _td_resblock(s, 'encoder.mid.block_1', block_in, block_in)
+    _attn_block(s, 'encoder.mid.attn_1', block_in)
+    _td_resblock(s, 'encoder.mid.block_2', block_in, block_in)
+    _norm(s, 'encoder.norm_out', block_in)
+    _conv(s, 'encoder.conv_out', block_in, a.z_channels, 3)
+    # ---- Decoder (:683-751)
+    block_in = a.level_ch[-1]
+    _conv(s, 'decoder.conv_in', a.z_channels, block_in, 3)
+    _td_resblock(s, 'decoder.mid.block_1', block_in, block_in)
+    _attn_block(s, 'decoder.mid.attn_1', block_in)
+    _td_resblock(s, 'decoder.mid.block_2', block_in, block_in)
+    for lvl in reversed(range(a.num_levels)):
+        block_out = a.level_ch[lvl]
+        for b in range(a.num_res_blocks + 1):
+            _td_resblock(s, 'decoder.up.%d.block.%d' % (lvl, b), block_in, block_out)
+            block_in = block_out
+        if a.level_has_attn[lvl]:
+            for b in range(a.num_res_blocks + 1):
+                _attn_block(s, 'decoder.up.%d.attn.%d' % (lvl, b), block_in)
+        if lvl != 0:
+            _conv(s, 'decoder.up.%d.upsample.conv' % lvl, block_in, block_in, 3)
+    _norm(s, 'decoder.norm_out', block_in)
+    _conv(s, 'decoder.conv_out', block_in, a.out_ch, 3)
+    # ---- quantiser (:206-223, 381-394): one shared codebook of depth 1
+    e = a.embed_dim
+    s.add('quantizer.codebooks.0.weight', (a.n_embed + 1, e), 'codebook')
+    s.add('quantizer.codebooks.0.cluster_size_ema', (a.n_embed,), 'zeros')
+    s.add('quantizer.codebooks.0.embed_ema', (a.n_embed, e), 'codebook_ema')
+    _conv(s, 'quant_conv', a.z_channels, e, 1)
+    _conv(s, 'post_quant_conv', e, a.z_channels, 1)
+    for p in ('tdswin_pre', 'tdswin_post'):
+        _swin3d_layer(s, p, e, a.stages_atten, a.num_head, a.window_size)
     return a, s

@@ -65,27 +65,14 @@ class BasicLayer(nn.Module):
 
     def _pack(self):
         if self._packed is None:
-            w = []
-            for blk in self.blocks:
-                d = {'n1w': blk.norm1.weight.float().contiguous(), 'n1b': blk.norm1.bias.float().contiguous(),
-                     'n2w': blk.norm2.weight.float().contiguous(), 'n2b': blk.norm2.bias.float().contiguous(),
-                     'qkv': blk.attn.qkv.weight.to(BF).contiguous(),
-                     'qkv_b': blk.attn.qkv.bias.float().contiguous() if blk.attn.qkv.bias is not None else None,
-                     'proj': blk.attn.proj.weight.to(BF).contiguous(), 'proj_b': blk.attn.proj.bias.float().contiguous(),
-                     'fc1': blk.mlp.fc1.weight.to(BF).contiguous(), 'fc1_b': blk.mlp.fc1.bias.float().contiguous(),
-                     'fc2': blk.mlp.fc2.weight.to(BF).contiguous(), 'fc2_b': blk.mlp.fc2.bias.float().contiguous(),
-                     'table': blk.attn.relative_position_bias_table.float(), 'index': blk.attn.relative_position_index,
-                     'bias': {}}
-                # a padded token is a zero row after the norm: its projection is the qkv bias (or zero)
-                d['pad'] = d['qkv_b'].to(BF).contiguous() if d['qkv_b'] is not None else None
-                w.append(d)
-            self._packed = w
+            named = dict(self.named_parameters())
+            named.update(self.named_buffers())
+            self._packed = pack_blocks(named.get, self.depth)
         return self._packed
 
     @torch.no_grad()
     def forward(self, x):
         """x: [B, C, D, H, W] on a CUDA device -> same shape and dtype (`modules/swin.py:380-405`)."""
-        from . import ops
         if not x.is_cuda:
             raise RuntimeError('pgtformer_b200 has no CPU path: BasicLayer needs a CUDA (sm_90a) device')
         B, C, D, H, W = x.shape
@@ -93,20 +80,55 @@ class BasicLayer(nn.Module):
         T = B * D * H * W
         with torch.cuda.device(x.device):
             h = x.permute(0, 2, 3, 4, 1).reshape(T, C).to(BF).contiguous()           # 'b c d h w -> b d h w c'
-            ws = tuple(min(s, w) for s, w in zip((D, H, W), self.window_size))        # get_window_size
-            N = ws[0] * ws[1] * ws[2]
-            new = lambda *s, dt=BF: torch.empty(*s, dtype=dt, device=x.device)
-            for i, d in enumerate(self._pack()):
-                if N not in d['bias']:                                                 # relative_position_index[:N, :N]
-                    idx = d['index'][:N, :N].reshape(-1).to(x.device)
-                    d['bias'][N] = d['table'][idx].view(N, N, heads).permute(2, 0, 1).contiguous()
-                shift = (0, 0, 0) if i % 2 == 0 else self.shift_size
-                y = ops.layernorm(h, d['n1w'], d['n1b'], new(T, C))
-                qkv = ops.linear(y, d['qkv'], new(T, 3 * C), bias=d['qkv_b'])
-                a = ops.window3d_attention(qkv, B, D, H, W, C, heads, self.window_size, shift, d['bias'][N], new(T, C),
-                                           pad_qkv=d['pad'])
-                h = ops.linear(a, d['proj'], new(T, C), bias=d['proj_b'], residual=h)
-                y = ops.layernorm(h, d['n2w'], d['n2b'], new(T, C))
-                m = ops.linear(y, d['fc1'], new(T, d['fc1'].shape[0]), bias=d['fc1_b'], act=ops.ACT_GELU)
-                h = ops.linear(m, d['fc2'], new(T, C), bias=d['fc2_b'], residual=h)
+            h = basic_layer_rows(h, B, D, H, W, self._pack(), heads, self.window_size)
             return h.view(B, D, H, W, C).permute(0, 4, 1, 2, 3).to(x.dtype).contiguous()
+
+
+def pack_blocks(get, depth):
+    """Kernel-layout weights of `depth` SwinTransformerBlock3D; get('blocks.<i>.<name>') returns the reference-named
+    tensor on the device (None for a qkv bias the layer does not have).  The expanded relative-position bias is
+    cached per window size N in each block's 'bias' dict by basic_layer_rows."""
+    w = []
+    for i in range(depth):
+        g = lambda n: get('blocks.%d.%s' % (i, n))
+        qkv_b = g('attn.qkv.bias')
+        d = {'n1w': g('norm1.weight').float().contiguous(), 'n1b': g('norm1.bias').float().contiguous(),
+             'n2w': g('norm2.weight').float().contiguous(), 'n2b': g('norm2.bias').float().contiguous(),
+             'qkv': g('attn.qkv.weight').to(BF).contiguous(),
+             'qkv_b': qkv_b.float().contiguous() if qkv_b is not None else None,
+             'proj': g('attn.proj.weight').to(BF).contiguous(), 'proj_b': g('attn.proj.bias').float().contiguous(),
+             'fc1': g('mlp.fc1.weight').to(BF).contiguous(), 'fc1_b': g('mlp.fc1.bias').float().contiguous(),
+             'fc2': g('mlp.fc2.weight').to(BF).contiguous(), 'fc2_b': g('mlp.fc2.bias').float().contiguous(),
+             'table': g('attn.relative_position_bias_table').float(), 'index': g('attn.relative_position_index'),
+             'bias': {}}
+        # a padded token is a zero row after the norm: its projection is the qkv bias (or zero)
+        d['pad'] = d['qkv_b'].to(BF).contiguous() if d['qkv_b'] is not None else None
+        w.append(d)
+    return w
+
+
+def basic_layer_rows(h, B, D, H, W, blocks, heads, window, out=None):
+    """BasicLayer.forward (`modules/swin.py:380-405`) on token rows: h [B*D*H*W, C] bf16 in (b, d, h, w) order (the
+    'b d h w c' layout of the reference), blocks from pack_blocks.  Returns the rows after the last block: a new bf16
+    tensor, or `out` (bf16 or fp32 [T, C]) when given, which the last block's fc2 + residual epilogue writes."""
+    from . import ops
+    T, C = h.shape
+    shift_size = tuple(i // 2 for i in window)
+    ws = tuple(min(s, w) for s, w in zip((D, H, W), window))                  # get_window_size
+    N = ws[0] * ws[1] * ws[2]
+    new = lambda *s, dt=BF: torch.empty(*s, dtype=dt, device=h.device)
+    for i, d in enumerate(blocks):
+        if N not in d['bias']:                                                 # relative_position_index[:N, :N]
+            idx = d['index'][:N, :N].reshape(-1).to(h.device)
+            d['bias'][N] = d['table'][idx].view(N, N, heads).permute(2, 0, 1).contiguous()
+        shift = (0, 0, 0) if i % 2 == 0 else shift_size
+        y = ops.layernorm(h, d['n1w'], d['n1b'], new(T, C))
+        qkv = ops.linear(y, d['qkv'], new(T, 3 * C), bias=d['qkv_b'])
+        a = ops.window3d_attention(qkv, B, D, H, W, C, heads, window, shift, d['bias'][N], new(T, C),
+                                   pad_qkv=d['pad'])
+        h = ops.linear(a, d['proj'], new(T, C), bias=d['proj_b'], residual=h)
+        y = ops.layernorm(h, d['n2w'], d['n2b'], new(T, C))
+        m = ops.linear(y, d['fc1'], new(T, d['fc1'].shape[0]), bias=d['fc1_b'], act=ops.ACT_GELU)
+        last = out is not None and i == len(blocks) - 1
+        h = ops.linear(m, d['fc2'], out if last else new(T, C), bias=d['fc2_b'], residual=h)
+    return h

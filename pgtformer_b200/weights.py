@@ -16,10 +16,12 @@ import torch
 from .spec import WINDOW
 
 
-def relative_position_index():
-    """[48,48] int64 index into the 245-row bias table: offset (dd+2)*49 + (dh+3)*7 + (dw+3)
-    for tokens ordered (d, h, w) over (3,4,4)  (`modules/rstt_layers.py:163-184`)."""
-    D, Wh, Ww = WINDOW
+def relative_position_index(window=WINDOW):
+    """[N,N] int64 index (N = D*Wh*Ww) into the (2D-1)(2Wh-1)(2Ww-1)-row bias table: offset
+    (dd+D-1)*(2Wh-1)*(2Ww-1) + (dh+Wh-1)*(2Ww-1) + (dw+Ww-1) for tokens ordered (d, h, w).  The default (3,4,4) window
+    gives PGTFormer's [48,48] index (`modules/rstt_layers.py:163-184`), (5,5,5) TDRQVAE's Video-Swin [125,125] one
+    (`modules/swin.py:117-130`)."""
+    D, Wh, Ww = window
     d = torch.arange(D).view(D, 1, 1).expand(D, Wh, Ww).reshape(-1)
     h = torch.arange(Wh).view(1, Wh, 1).expand(D, Wh, Ww).reshape(-1)
     w = torch.arange(Ww).view(1, 1, Ww).expand(D, Wh, Ww).reshape(-1)
@@ -36,7 +38,8 @@ def _gen(name, seed):
     return g
 
 
-def synth_tensor(name, shape, kind, dtype, seed=0):
+def synth_tensor(name, shape, kind, dtype, seed=0, window=None):
+    """window: the (D, H, W) attention window of an 'rpb_index' buffer (Spec.windows; default spec.WINDOW)."""
     g = _gen(name, seed)
     if kind in ('conv_w', 'linear_w'):
         fan_in = 1
@@ -59,7 +62,9 @@ def synth_tensor(name, shape, kind, dtype, seed=0):
     if kind == 'rpb_table':
         return 0.5 * torch.randn(shape, generator=g)
     if kind == 'rpb_index':
-        return relative_position_index()
+        idx = relative_position_index(WINDOW if window is None else tuple(window))
+        assert tuple(idx.shape) == tuple(shape), (name, shape, window)
+        return idx
     if kind == 'codebook':                       # nn.Embedding init N(0,1); padding row = 0
         w = torch.randn(shape, generator=g)
         w[-1].zero_()
@@ -74,7 +79,7 @@ def synth_state_dict(spec, seed=0):
     for name, (shape, kind, dtype) in spec.items():
         if kind == 'codebook_ema':
             continue
-        sd[name] = synth_tensor(name, shape, kind, dtype, seed)
+        sd[name] = synth_tensor(name, shape, kind, dtype, seed, window=getattr(spec, 'windows', {}).get(name))
     for name, (shape, kind, dtype) in spec.items():
         if kind == 'codebook_ema':               # embed_ema = weight[:-1] clone (tdcrqvae3_arch.py:96)
             sd[name] = sd[name.replace('embed_ema', 'weight')][:-1].clone()
