@@ -54,6 +54,8 @@ def _materialise(root, spec, seed):
     import weakref
     rootref = weakref.ref(root)
     for name, (shape, kind, dtype) in spec.items():
+        if spec.alias_of(name):
+            continue
         parts = name.split('.')
         node = root
         for part in parts[:-1]:
@@ -70,6 +72,16 @@ def _materialise(root, spec, seed):
             node.register_buffer(parts[-1], t)
         else:
             node.register_parameter(parts[-1], nn.Parameter(t, requires_grad=False))
+    # a shared codebook is the same module under every depth, as in the reference's ModuleList: state_dict() repeats its
+    # keys and load_state_dict(strict=True) loads each copy into the one tensor in turn (the last one wins)
+    for alias, target in spec.module_aliases.items():
+        *path, leaf = alias.split('.')
+        parent, node = root, root
+        for part in path:
+            parent = parent._modules[part]
+        for part in target.split('.'):
+            node = node._modules[part]
+        parent.add_module(leaf, node)
 
 
 class _B200Model(nn.Module):
@@ -80,8 +92,8 @@ class _B200Model(nn.Module):
         self.arch, self._spec = build_spec(network_g)
         _materialise(self, self._spec, seed)
         # embed_ema mirrors the codebook rows (tdcrqvae3_arch.py:96)
-        cb = self.quantizer.codebooks._modules['0']
-        cb.embed_ema.copy_(cb.weight.detach()[:-1])
+        for cb in self.quantizer.codebooks._modules.values():
+            cb.embed_ema.copy_(cb.weight.detach()[:-1])
         self._engine = None
         self.t = self.arch.tf
         self.code_shape = list(self.arch.code_shape)
@@ -120,7 +132,7 @@ class _B200Model(nn.Module):
         from pgtformer_b200.engine import Engine
         return Engine
 
-    # ---- depth-1 code helpers shared by the codecs.  Arguments are checked on the host before any launch: bad shapes
+    # ---- code helpers shared by the codecs.  Arguments are checked on the host before any launch: bad shapes
     # raise ValueError, codes outside [0, n_embed] IndexError (index n_embed is the codebook's padding row, which
     # nn.Embedding accepts).
     def _check_code(self, code):
@@ -136,19 +148,29 @@ class _B200Model(nn.Module):
 
     @torch.no_grad()
     def get_code_emb_with_depth(self, code):
-        """(codebook rows [F, h, w, 1, embed_dim] fp32, None), as RQBottleneck.embed_code_with_depth returns them."""
+        """(codebook rows [F, h, w, D, embed_dim] fp32, None), as RQBottleneck.embed_code_with_depth returns them."""
         self._check_code(code)
         Fr, h, w, d = code.shape
-        return self.engine().embed_code(code).view(Fr, h, w, d, self.arch.embed_dim), None
+        return self.engine().embed_code_with_depth(code).view(Fr, h, w, d, self.arch.embed_dim), None
 
     @torch.no_grad()
     def decode_partial_code(self, code, code_idx, decode_type='select'):
-        """Decodes with codebooks [0 .. code_idx]; with one codebook 'select' and 'add' are both decode_code."""
+        """RQBottleneck.embed_partial_code + decode (`archs/tdcrqvae3_arch.py:394-426, 855-863`): 'select' decodes the
+        code rows of depth code_idx alone, 'add' the sum of depths 0 .. code_idx; with one codebook both are
+        decode_code."""
         self._check_code(code)
         assert code_idx < code.shape[-1]
         if decode_type not in ('select', 'add'):
             raise NotImplementedError(f"{decode_type} is not implemented in partial decoding")
-        return self.decode_code(code)
+        if code.shape[-1] == 1:
+            return self.decode_code(code)
+        if isinstance(code_idx, bool) or not isinstance(code_idx, int) or code_idx < 0:
+            raise ValueError('code_idx must be an int in [0, %d), got %r' % (code.shape[-1], code_idx))
+        self._check_latent(*code.shape[:3])
+        eng = self.engine()
+        Fr, h, w, _ = code.shape
+        z_q = eng.embed_code(code, code_idx if decode_type == 'select' else 0, code_idx)
+        return eng.decode(z_q.view(Fr, h, w, self.arch.embed_dim))
 
     def train(self, mode=True):
         """The reference's train() forgets `return self` (archs/pgtformer_arch.py:577-581), so
@@ -162,7 +184,8 @@ class _B200Model(nn.Module):
 @ARCH_REGISTRY.register()
 class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
     """Registered stage-I autoencoder (`archs/tdcrqvae3_arch.py:710-872`): forward / get_codes run the encoder, the
-    nearest-codebook L2 argmin kernel and the decoder; encode / decode / decode_code / get_soft_codes and the partial-
+    residual quantiser (one exact nearest-codebook L2 argmin per code depth, `code_shape[2]`; separate codebooks, or one
+    shared by every depth with `shared_codebook=True`) and the decoder; encode / decode / decode_code / get_soft_codes and the partial-
     code methods expose the codec's parts (PGTFormer inherits them, as in the reference)."""
 
     def __init__(self, *, embed_dim=64, n_embed=512, decay=0.99, loss_type='mse', latent_loss_weight=0.25,
@@ -182,7 +205,7 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
     def get_codes(self, input):
         return self.engine().forward_vq(input, code_only=True)[2]
 
-    # ---- the rest of the stage-I codec surface (`archs/tdcrqvae3_arch.py:774-872`), depth-1 quantiser; arguments are
+    # ---- the rest of the stage-I codec surface (`archs/tdcrqvae3_arch.py:774-872`) at any quantiser depth; arguments are
     # checked on the host before any launch (see _B200Model._check_code).
     def _frames(self, x):
         """[b, t, 3, H, W] (the reference's form) or [b*t, 3, H, W] -> [b*t, 3, H, W]."""
@@ -218,7 +241,7 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
 
     @torch.no_grad()
     def decode_code(self, code):
-        """Codebook rows of the int codes [F, h, w, 1] (any h, w the decoder takes), decoded to frames."""
+        """The depth sum of the code rows of the int codes [F, h, w, D] (any h, w the decoder takes), decoded to frames."""
         self._check_code(code)
         self._check_latent(*code.shape[:3])
         eng = self.engine()
@@ -232,8 +255,9 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
 
     @torch.no_grad()
     def get_soft_codes(self, xs, temp=1.0, stochastic=False):
-        """(soft_code [F, h, w, 1, n_embed] fp32 = softmax(-||z_e - e_k||^2 / temp), code [F, h, w, 1] int64): the
-        exact nearest code (== get_codes), or with stochastic=True one draw per token from its soft_code row."""
+        """(soft_code [F, h, w, D, n_embed] fp32 = softmax(-||r_d - e_k||^2 / temp) over depth d's codebook, code
+        [F, h, w, D] int64), r_d the residual the earlier depths' codes left: the exact nearest code (== get_codes), or
+        with stochastic=True one draw per token and depth from its soft_code row."""
         try:
             t = float(temp)
         except (TypeError, ValueError):
@@ -245,7 +269,8 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
         z_e = eng.encode(x)
         Fr, h, w, E = z_e.shape
         p, code = eng.soft_codes(z_e.view(-1, E), t, stochastic=bool(stochastic))
-        return p.view(Fr, h, w, 1, -1), code.view(Fr, h, w, 1)
+        D = self.code_shape[-1]
+        return p.view(Fr, h, w, D, -1), code.view(Fr, h, w, D)
 
 
 @ARCH_REGISTRY.register()
@@ -276,9 +301,9 @@ class PGTFormer(TDCRQVAE3):
 
     def forward(self, x, w=None, detach_16=True, code_only=None, adain=None, force_codes=None):
         """`archs/pgtformer_arch.py:598-714`: returns (out, logits, lq_feat_nhwc), or
-        (logits, lq_feat_nhwc) when code_only.  `detach_16` only matters for autograd and is
-        accepted for signature compatibility.  `force_codes` (extension) teacher-forces the code
-        indices for decoder parity checks."""
+        (logits, lq_feat_nhwc) when code_only; logits are [b*3, h, w, D, codebook_size].  `detach_16` only
+        matters for autograd and is accepted for signature compatibility.  `force_codes` (extension, int64
+        [b*3, h, w, D]) teacher-forces the code indices for decoder parity checks."""
         if w is None:
             w = self.w
         if adain is None:

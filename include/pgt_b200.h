@@ -258,7 +258,7 @@ int64_t pgt_l2_argmin_ws_ints(int T);
 int pgt_l2_argmin_tc(const float* z, int T, int E, const float* codebook, const void* cb_bf16, const float* cb_norm,
                      int K, int64_t* idx, float* quant, int32_t* workspace, void* stream);
 
-/* ---- soft codes (RQBottleneck.get_soft_codes, archs/tdcrqvae3_arch.py:429-457, depth 1).
+/* ---- soft codes of one quantiser depth (RQBottleneck.get_soft_codes, archs/tdcrqvae3_arch.py:429-457).
  * pgt_soft_codes: out[t, k] = softmax_k((2 z[t].e_k - ||e_k||^2) / temp) = softmax_k(-||z[t] - e_k||^2 / temp) over the
  *   first K codebook rows; z fp32 [T, E]; codebook fp32 [K(+1), E]; cb_norm fp32 [>= K] = ||e_k||^2 (the norms
  *   pgt_codebook_pack writes); out fp32 [T, K].  3xTF32 tensor-core dot products (soft_codes.cu), fp32 softmax.
@@ -269,6 +269,31 @@ int pgt_l2_argmin_tc(const float* z, int T, int E, const float* codebook, const 
 int pgt_soft_codes(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
                    float* out, void* stream);
 int pgt_sample_codes(const float* p, int T, int K, const int64_t* seed, int64_t* idx, void* stream);
+/* The same two with a row pitch (elements, ldo / ldp >= K, ldo % 4 == 0): at quantiser depth D, depth d writes and
+ * reads the K-slice d of a contiguous [T, D, K] soft-code tensor (ldo = D * K), as RQBottleneck.get_soft_codes
+ * concatenates them (:429-457).  pgt_soft_codes / pgt_sample_codes are the pitch = K case. */
+int pgt_soft_codes_ld(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
+                      float* out, int ldo, void* stream);
+int pgt_sample_codes_ld(const float* p, int T, int K, int ldp, const int64_t* seed, int64_t* idx, void* stream);
+
+/* ---- residual quantisation over D code levels (rq.cu; RQBottleneck.quantize / embed_code / embed_partial_code /
+ * embed_code_with_depth, archs/tdcrqvae3_arch.py:294-426).  Level d's code is pgt_l2_argmin_tc of the level's residual.
+ * pgt_rq_residual: one quantiser step after that argmin: e = codebook_d[idx[t]] (codebook_d fp32 [K(+1), E], the
+ *   depth's own codebook), r_out = r_in - e (skipped when r_out == NULL, i.e. at the last depth), agg = first ? e :
+ *   agg + e (skipped when agg == NULL: the soft-code loop needs only the residual).  fp32, elementwise, one rounding per operation (no FMA): bit-identical to the reference's
+ *   residual_feature.sub_(quant) / aggregated_quants.add_(quant) (:319-324) wherever the codes agree.  r_in, r_out,
+ *   agg fp32 [T, E] contiguous; E % 4 == 0; r_in may equal r_out.
+ * pgt_rq_embed: out[t] = sum over d = d0 .. d1 of codebooks[d * cb_stride + idx[t * ldi + d * ldd] * E], accumulated in
+ *   depth order in fp32 from the first term, written fp32 or bf16 (out_dtype) with row pitch ldo.  codebooks: the
+ *   stacked [D, K + 1, E] fp32 codebooks (cb_stride = (K + 1) * E) or one shared codebook (cb_stride = 0); idx int64
+ *   with token pitch ldi and depth pitch ldd ([T, D] codes: ldi = D, ldd = 1; depth-major [D, T]: ldi = 1, ldd = T).
+ *   d0 = 0, d1 = D - 1 is embed_code (:355-368), d1 = j the 'add' mode of embed_partial_code, d0 = d1 = j its
+ *   'select' mode and one slice of embed_code_with_depth (:371-426).  Index n_embed reads the padding row; no range
+ *   check is made on the device. */
+int pgt_rq_residual(const float* r_in, float* r_out, const int64_t* idx, int T, int E, const float* codebook_d,
+                    float* agg, int first, void* stream);
+int pgt_rq_embed(const int64_t* idx, long long ldi, long long ldd, int T, int d0, int d1, const float* codebooks,
+                 long long cb_stride, int E, void* out, int ldo, int out_dtype, void* stream);
 
 /* ---- AdaIN: y = (q - mean_q)/std_q * std_l + mean_l per (frame, channel) over HW, unbiased
  * variance + eps.  q: bf16/fp32 [F, HW, ldq]; l (style) bf16 [F, HW, ldl]; y bf16.

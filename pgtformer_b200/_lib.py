@@ -77,6 +77,11 @@ SIGNATURES = {
                                  c_void_p, c_void_p]),
     'pgt_soft_codes': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p]),
     'pgt_sample_codes': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    'pgt_soft_codes_ld': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_void_p, c_int, c_void_p]),
+    'pgt_sample_codes_ld': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    'pgt_rq_residual': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
+    'pgt_rq_embed': (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_int, c_void_p, c_int,
+                             c_int, c_void_p]),
     'pgt_adain': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int,
                           c_void_p]),
     'pgt_maxpool3x3s2': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),

@@ -224,13 +224,15 @@ constexpr int AM_SHORT_LIST = 2048;
 // above the threshold the last code with p > 0 is taken.  A row without any positive entry yields -1.  The seed is read
 // on the device: no host synchronisation, and a CUDA graph replays fresh draws when seed is refilled before replay.
 __global__ void __launch_bounds__(256)
-sample_codes_kernel(const float* __restrict__ p, int T, int K, const int64_t* __restrict__ seed, int64_t* __restrict__ idx) {
+sample_codes_kernel(const float* __restrict__ p, int T, int K, const int64_t* __restrict__ seed, int64_t* __restrict__ idx,
+                    int ldp) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  p += (size_t)row * ldp;                                        // row pitch ldp: here, where ptxas keeps it out of the stack
   const int lane = threadIdx.x & 31;
   if (row >= T) return;
   const int per = (K + 31) / 32;
   const int c0 = min(K, lane * per), c1 = min(K, c0 + per);
-  const float* pr = p + (size_t)row * K;
+  const float* pr = p;
   float tot = 0.f;
   int lastnz = -1;
   for (int c = c0; c < c1; ++c) {
@@ -306,12 +308,17 @@ extern "C" int pgt_argmax_gather(const float* logits, int T, int K, const float*
   return PGT_OK;
 }
 
-extern "C" int pgt_sample_codes(const float* p, int T, int K, const int64_t* seed, int64_t* idx, void* stream) {
-  PGT_CHECK_ARG(p && seed && idx && T > 0 && K > 0);
+extern "C" int pgt_sample_codes_ld(const float* p, int T, int K, int ldp, const int64_t* seed, int64_t* idx,
+                                   void* stream) {
+  PGT_CHECK_ARG(p && seed && idx && T > 0 && K > 0 && ldp >= K);
   ProfScope ps(PGT_PROF_ARGMAX, (double)T * K * 4 + (double)T * 8, static_cast<cudaStream_t>(stream), "sample_codes");
-  sample_codes_kernel<<<ceil_div(T, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(p, T, K, seed, idx);
+  sample_codes_kernel<<<ceil_div(T, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(p, T, K, seed, idx, ldp);
   PGT_LAUNCH_OK();
   return PGT_OK;
+}
+
+extern "C" int pgt_sample_codes(const float* p, int T, int K, const int64_t* seed, int64_t* idx, void* stream) {
+  return pgt_sample_codes_ld(p, T, K, K, seed, idx, stream);
 }
 
 extern "C" int pgt_l2_argmin(const float* z, int T, int E, const float* codebook, int K, int64_t* idx, float* quant,

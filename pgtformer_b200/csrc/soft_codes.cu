@@ -59,7 +59,7 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
 
 __global__ void __launch_bounds__(256, 1)
 soft_codes_kernel(const float* __restrict__ z, int T, int E, const float* __restrict__ cb, const float* __restrict__ norm,
-                  int K, float temp, float* __restrict__ out) {
+                  int K, float temp, float* __restrict__ out, int ldo) {
   extern __shared__ __align__(16) float sm[];
   float* rstat = sm + SC_ST * SC_STAGE_FLOATS;            // [2][4][128]: per code-warp row max, row sum
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -177,7 +177,7 @@ soft_codes_kernel(const float* __restrict__ z, int T, int E, const float* __rest
           rmax[i][h] = m;
           rsum[i][h] = sum;
           if (t < T) {
-            float* o = out + (size_t)t * K + nt * SC_BN + wn * 32 + 2 * tq;
+            float* o = out + (size_t)t * ldo + nt * SC_BN + wn * 32 + 2 * tq;
 #pragma unroll
             for (int j = 0; j < 4; ++j) *reinterpret_cast<float2*>(o + 8 * j) = make_float2(s[2 * j], s[2 * j + 1]);
           }
@@ -220,7 +220,7 @@ soft_codes_kernel(const float* __restrict__ z, int T, int E, const float* __rest
     float s = 0.f;
 #pragma unroll
     for (int w = 0; w < 4; ++w) s += rstat[4 * SC_BM + w * SC_BM + r] * expf(rstat[w * SC_BM + r] - m);
-    float4* row = reinterpret_cast<float4*>(out + (size_t)t * K);
+    float4* row = reinterpret_cast<float4*>(out + (size_t)t * ldo);
     for (int c = lane; c < (K >> 2); c += 32) {
       float4 v = row[c];
       v.x = __fdiv_rn(expf(v.x - m), s);
@@ -236,9 +236,9 @@ soft_codes_kernel(const float* __restrict__ z, int T, int E, const float* __rest
 
 using namespace pgt;
 
-extern "C" int pgt_soft_codes(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
-                              float* out, void* stream) {
-  PGT_CHECK_ARG(z && codebook && cb_norm && out && T > 0 && K > 0 && E > 0);
+static int soft_codes_launch(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
+                             float* out, int ldo, void* stream) {
+  PGT_CHECK_ARG(z && codebook && cb_norm && out && T > 0 && K > 0 && E > 0 && ldo >= K && ldo % 4 == 0);
   PGT_CHECK_ARG(temp > 0.f && temp <= FLT_MAX);            // also rejects NaN
   PGT_CHECK_ARG((reinterpret_cast<uintptr_t>(z) & 15) == 0 && (reinterpret_cast<uintptr_t>(codebook) & 15) == 0 &&
                 (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(cb_norm) & 7) == 0);
@@ -247,7 +247,17 @@ extern "C" int pgt_soft_codes(const float* z, int T, int E, const float* codeboo
   static PerDeviceOnce once;
   PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(soft_codes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SC_SMEM); }));
   ProfScope ps(PGT_PROF_ARGMIN, 2.0 * T * (double)K * E, st, "soft_codes");
-  soft_codes_kernel<<<ceil_div(T, SC_BM), 256, SC_SMEM, st>>>(z, T, E, codebook, cb_norm, K, temp, out);
+  soft_codes_kernel<<<ceil_div(T, SC_BM), 256, SC_SMEM, st>>>(z, T, E, codebook, cb_norm, K, temp, out, ldo);
   PGT_LAUNCH_OK();
   return PGT_OK;
+}
+
+extern "C" int pgt_soft_codes(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
+                              float* out, void* stream) {
+  return soft_codes_launch(z, T, E, codebook, cb_norm, K, temp, out, K, stream);
+}
+
+extern "C" int pgt_soft_codes_ld(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K,
+                                 float temp, float* out, int ldo, void* stream) {
+  return soft_codes_launch(z, T, E, codebook, cb_norm, K, temp, out, ldo, stream);
 }

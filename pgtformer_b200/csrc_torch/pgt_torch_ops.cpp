@@ -99,6 +99,58 @@ void sample_codes(const at::Tensor& p, const at::Tensor& seed, at::Tensor idx) {
                          stream_of(p)), "sample_codes");
 }
 
+void soft_codes_ld(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor& norm, int64_t K, double temp,
+                   at::Tensor out) {
+  TORCH_CHECK(z.is_cuda() && z.scalar_type() == at::kFloat && z.is_contiguous() && codebook.scalar_type() == at::kFloat &&
+              codebook.is_contiguous() && norm.scalar_type() == at::kFloat && out.scalar_type() == at::kFloat &&
+              out.dim() == 2 && out.stride(1) == 1 && out.size(0) == z.size(0) && out.size(1) == K,
+              "soft_codes_ld: fp32 contiguous z [T, E], codebook, norm, row-pitched out [T, K]");
+  c10::cuda::CUDAGuard guard(z.device());
+  check(pgt_soft_codes_ld(z.data_ptr<float>(), (int)z.size(0), (int)z.size(1), codebook.data_ptr<float>(),
+                          norm.data_ptr<float>(), (int)K, (float)temp, out.data_ptr<float>(), (int)out.stride(0),
+                          stream_of(z)), "soft_codes_ld");
+}
+
+void sample_codes_ld(const at::Tensor& p, const at::Tensor& seed, at::Tensor idx) {
+  TORCH_CHECK(p.is_cuda() && p.scalar_type() == at::kFloat && p.dim() == 2 && p.stride(1) == 1 &&
+              seed.scalar_type() == at::kLong && seed.numel() == 2 && seed.device() == p.device() &&
+              idx.scalar_type() == at::kLong && idx.is_contiguous() && idx.numel() == p.size(0),
+              "sample_codes_ld: fp32 row-pitched p [T, K], device int64 seed [2], int64 idx [T]");
+  c10::cuda::CUDAGuard guard(p.device());
+  check(pgt_sample_codes_ld(p.data_ptr<float>(), (int)p.size(0), (int)p.size(1), (int)p.stride(0), seed.data_ptr<int64_t>(),
+                            idx.data_ptr<int64_t>(), stream_of(p)), "sample_codes_ld");
+}
+
+void rq_residual(const c10::optional<at::Tensor>& r_in, const c10::optional<at::Tensor>& r_out, const at::Tensor& idx,
+                 const at::Tensor& codebook, const c10::optional<at::Tensor>& agg, bool first) {
+  TORCH_CHECK(agg.has_value() || r_out.has_value(), "rq_residual: agg or r_out is needed");
+  const at::Tensor& ref = agg.has_value() ? *agg : *r_out;
+  TORCH_CHECK(ref.is_cuda() && ref.dim() == 2 && codebook.scalar_type() == at::kFloat && codebook.is_contiguous() &&
+              codebook.size(1) == ref.size(1) && idx.scalar_type() == at::kLong && idx.is_contiguous() &&
+              idx.numel() == ref.size(0), "rq_residual: codebook fp32 [K(+1), E], int64 idx [T]");
+  for (const auto* r : {&r_in, &r_out, &agg})
+    TORCH_CHECK(!r->has_value() || ((*r)->scalar_type() == at::kFloat && (*r)->is_contiguous() &&
+                                    (*r)->sizes() == ref.sizes()), "rq_residual: fp32 contiguous [T, E] tensors");
+  c10::cuda::CUDAGuard guard(ref.device());
+  auto ptr = [](const c10::optional<at::Tensor>& t) { return t.has_value() ? t->data_ptr<float>() : nullptr; };
+  check(pgt_rq_residual(ptr(r_in), ptr(r_out), idx.data_ptr<int64_t>(), (int)ref.size(0), (int)ref.size(1),
+                        codebook.data_ptr<float>(), ptr(agg), first ? 1 : 0, stream_of(ref)), "rq_residual");
+}
+
+void rq_embed(const at::Tensor& idx, int64_t d0, int64_t d1, const at::Tensor& codebooks, at::Tensor out, int64_t ldi,
+              int64_t ldd) {
+  TORCH_CHECK(idx.is_cuda() && idx.scalar_type() == at::kLong && idx.is_contiguous() && codebooks.scalar_type() == at::kFloat &&
+              codebooks.is_contiguous() && codebooks.dim() == 3 && out.dim() == 2 && out.size(1) == codebooks.size(2) &&
+              (out.scalar_type() == at::kFloat || out.scalar_type() == at::kBFloat16) && 0 <= d0 && d0 <= d1 &&
+              (codebooks.size(0) == 1 || d1 < codebooks.size(0)) && (out.size(0) - 1) * ldi + d1 * ldd < idx.numel(),
+              "rq_embed: int64 codes, fp32 codebooks [D or 1, K + 1, E], fp32 / bf16 out [T, E]");
+  c10::cuda::CUDAGuard guard(idx.device());
+  const int64_t cb_stride = codebooks.size(0) == 1 ? 0 : codebooks.size(1) * codebooks.size(2);
+  check(pgt_rq_embed(idx.data_ptr<int64_t>(), ldi, ldd, (int)out.size(0), (int)d0, (int)d1, codebooks.data_ptr<float>(),
+                     cb_stride, (int)out.size(1), out.data_ptr(), ld(out),
+                     out.scalar_type() == at::kBFloat16 ? PGT_BF16 : PGT_F32, stream_of(idx)), "rq_embed");
+}
+
 void linear(const at::Tensor& a, const at::Tensor& w, const c10::optional<at::Tensor>& bias, int64_t act,
             const c10::optional<at::Tensor>& residual, at::Tensor out) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16 && w.stride(1) == 1,
@@ -134,6 +186,10 @@ TORCH_LIBRARY(pgt, m) {
   m.def("linear(Tensor a, Tensor w, Tensor? bias, int act, Tensor? residual, Tensor(a!) out) -> ()");
   m.def("soft_codes(Tensor z, Tensor codebook, Tensor norm, int K, float temp, Tensor(a!) out) -> ()");
   m.def("sample_codes(Tensor p, Tensor seed, Tensor(a!) idx) -> ()");
+  m.def("soft_codes_ld(Tensor z, Tensor codebook, Tensor norm, int K, float temp, Tensor(a!) out) -> ()");
+  m.def("sample_codes_ld(Tensor p, Tensor seed, Tensor(a!) idx) -> ()");
+  m.def("rq_residual(Tensor? r_in, Tensor(a!)? r_out, Tensor idx, Tensor codebook, Tensor(b!)? agg, bool first) -> ()");
+  m.def("rq_embed(Tensor idx, int d0, int d1, Tensor codebooks, Tensor(a!) out, int ldi, int ldd) -> ()");
 }
 
 TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
@@ -145,4 +201,8 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("linear", linear);
   m.impl("soft_codes", soft_codes);
   m.impl("sample_codes", sample_codes);
+  m.impl("soft_codes_ld", soft_codes_ld);
+  m.impl("sample_codes_ld", sample_codes_ld);
+  m.impl("rq_residual", rq_residual);
+  m.impl("rq_embed", rq_embed);
 }

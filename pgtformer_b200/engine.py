@@ -124,6 +124,10 @@ class Engine:
             elif t.dtype.is_floating_point and t.dim() == 1:
                 w[name] = t.float().contiguous()
         w['codebook'] = self._f32('quantizer.codebooks.0.weight')
+        if self.depth > 1:
+            # every distinct codebook stacked once [D or 1, K + 1, E] (rq_embed reads a shared one with depth stride 0)
+            n = 1 if self.arch.shared_codebook else self.depth
+            w['codebooks'] = torch.stack([self._f32('quantizer.codebooks.%d.weight' % d) for d in range(n)]).contiguous()
         # Swin blocks: fused [q | k | v] projection and the expanded relative-position bias
         for name in list(sd):
             if name.endswith('.attn.relative_position_bias_table'):
@@ -161,6 +165,11 @@ class Engine:
         self._repack_parsing()
 
     # ------------------------------------------------------------------ small helpers
+    @property
+    def depth(self):
+        """Quantiser depth D = code_shape[2]: codes per token."""
+        return int(self.arch.code_shape[2])
+
     def _new(self, *shape, dtype=BF):
         return torch.empty(*shape, dtype=dtype, device=self.dev)
 
@@ -584,14 +593,14 @@ class Engine:
             m = self._lin(y, p + '.linear1', 2 * E, act=ops.ACT_GELU)
             q = self._lin(m, p + '.linear2', E, out_dtype=torch.float32, residual=q)
         y = ops.layernorm(q, wd['idx_pred_layer.0.weight'], wd['idx_pred_layer.0.bias'], self._new(T, E))
-        return self._lin(y, 'idx_pred_layer.1', a.n_embed, out_dtype=torch.float32)
+        return self._lin(y, 'idx_pred_layer.1', self.depth * a.n_embed, out_dtype=torch.float32)
 
     # ------------------------------------------------------------------ full forwards
     @_on_device
     @torch.no_grad()
     def forward(self, x, w=1.0, adain=True, code_only=False, force_codes=None, frame_index=None):
         """PGTFormer.forward (`archs/pgtformer_arch.py:598-714`).  x: fp32 [b*3,3,H,W] in [0,1] on the
-        device.  Returns (out, logits [b*3,h,w,1,K], lq_feat [b*3,h,w,E]) like the reference.
+        device.  Returns (out, logits [b*3,h,w,D,K], lq_feat [b*3,h,w,E]) like the reference; force_codes [b*3,h,w,D].
 
         frame_index (streaming, `pgtformer_b200/video.py`): device int32 [b*3]; x then holds DISTINCT frames and
         clip frame f is x[frame_index[f]] — the per-frame work (BiSeNet, attention-free encoder levels) runs once per
@@ -621,16 +630,25 @@ class Engine:
         lq32 = self._lin(h, 'quant_conv', a.embed_dim, out_dtype=torch.float32)
         lq = self._lin(h, 'quant_conv', a.embed_dim)
         logits = self.global_transformer(lq, pos, Fr // 3)
-        logits5 = logits.view(Fr, hh, ww, 1, a.n_embed)
+        D = self.depth
+        logits5 = logits.view(Fr, hh, ww, D, a.n_embed)
         lq_nhwc = lq32.view(Fr, hh, ww, a.embed_dim)
         if code_only:
             return logits5, lq_nhwc
         # quantise: argmax + codebook gather, AdaIN against lq, post_quant_conv
-        codes = torch.empty(T, dtype=torch.int64, device=self.dev)
+        codes = torch.empty(T * D, dtype=torch.int64, device=self.dev)
         quant = self._new(T, a.embed_dim, dtype=torch.float32)
-        idx_in = force_codes.to(self.dev).reshape(T).contiguous() if force_codes is not None else None
-        ops.argmax_gather(logits, wd['codebook'], codes, quant, idx_in=idx_in)
-        self.last_codes = codes.view(Fr, hh, ww, 1)
+        idx_in = force_codes.to(self.dev).reshape(T * D).contiguous() if force_codes is not None else None
+        if D == 1:
+            ops.argmax_gather(logits, wd['codebook'], codes, quant, idx_in=idx_in)
+        else:
+            # the [T, D*K] logits are [T*D, K] rows: one argmax per (token, depth), then the depth sum of the code rows
+            if idx_in is None:
+                ops.argmax_gather(logits.view(T * D, a.n_embed), wd['codebook'], codes, None)
+            else:
+                codes = idx_in
+            ops.rq_embed(codes, 0, D - 1, wd['codebooks'], quant, ldi=D, ldd=1)
+        self.last_codes = codes.view(Fr, hh, ww, D)
         if adain:
             quant = ops.adain(quant.view(Fr, hh * ww, -1), lq.view(Fr, hh * ww, -1), self._new(Fr, hh * ww, a.embed_dim))
         else:
@@ -669,11 +687,43 @@ class Engine:
         return outs
 
     # ------------------------------------------------------------------ stage-I codec (TDCRQVAE3 methods)
-    def _codebook_pack(self):
-        """bf16 copy + fp32 norms of the codebook (l2_argmin_tc, soft_codes), once per load."""
-        if 'codebook.pack' not in self.w:
-            self.w['codebook.pack'] = ops.codebook_pack(self.w['codebook'], self.arch.n_embed)
-        return self.w['codebook.pack']
+    def _codebook(self, d=0):
+        """fp32 codebook [K + 1, E] of depth d."""
+        if d == 0 or self.arch.shared_codebook:
+            return self.w['codebook']
+        return self.w['codebooks'][d]
+
+    def _codebook_pack(self, d=0):
+        """bf16 copy + fp32 norms of depth d's codebook (l2_argmin_tc, soft_codes), once per load and distinct codebook."""
+        key = 'codebook.pack' if d == 0 or self.arch.shared_codebook else 'codebook.pack.%d' % d
+        if key not in self.w:
+            self.w[key] = ops.codebook_pack(self._codebook(d), self.arch.n_embed)
+        return self.w[key]
+
+    def quantize(self, z):
+        """RQBottleneck.quantize + compute_commitment_loss (`archs/tdcrqvae3_arch.py:294-352`) of z fp32 [T, E]:
+        at each depth the exact L2 argmin of the residual over that depth's codebook, then residual -= e, aggregate
+        += e in fp32.  Returns (codes int64 [T, D], z_q fp32 [T, E] = the aggregate of all depths, loss = mean over
+        depths of mean((z - aggregate_d)^2))."""
+        a = self.arch
+        T, E = z.shape
+        D = self.depth
+        z_q = self._new(T, E, dtype=torch.float32)
+        if D == 1:
+            codes = torch.empty(T, dtype=torch.int64, device=self.dev)
+            ops.l2_argmin_tc(z, self.w['codebook'], self._codebook_pack(), a.n_embed, codes, z_q)
+            return codes.view(T, 1), z_q, (z - z_q).pow(2).mean()
+        # codes depth-major, as l2_argmin_tc writes them; the residual is a scratch buffer (z itself is never copied)
+        # and is updated after the argmin and its exhaustive fallback have both run
+        codes = torch.empty(D, T, dtype=torch.int64, device=self.dev)
+        r = self._new(T, E, dtype=torch.float32)
+        losses = []
+        for d in range(D):
+            src = z if d == 0 else r
+            ops.l2_argmin_tc(src, self._codebook(d), self._codebook_pack(d), a.n_embed, codes[d])
+            ops.rq_residual(src, r if d < D - 1 else None, codes[d], self._codebook(d), z_q, d == 0)
+            losses.append((z - z_q).pow(2).mean())
+        return codes.t().contiguous(), z_q, torch.stack(losses).mean()
 
     @_on_device
     @torch.no_grad()
@@ -700,25 +750,49 @@ class Engine:
 
     @_on_device
     @torch.no_grad()
-    def embed_code(self, codes):
-        """RQBottleneck.embed_code, depth 1 (`:355-368`): int64 codes [T] (each in [0, n_embed], the last row being
-        the padding row; the gather does no range check) -> fp32 [T, E] codebook rows."""
+    def embed_code(self, codes, d0=0, d1=None):
+        """RQBottleneck.embed_code (`:355-368`): int64 codes [..., D] (each in [0, n_embed], the last row being the
+        padding row; the gather does no range check) -> fp32 [T, E] = the sum of the code rows of depths d0 .. d1
+        (default all: embed_code; d1 = j: the 'add' mode of embed_partial_code; d0 = d1 = j: its 'select' mode)."""
         self._fusing = False
-        codes = codes.to(self.dev, torch.int64).reshape(-1).contiguous()
-        quant = self._new(codes.numel(), self.arch.embed_dim, dtype=torch.float32)
-        ops.argmax_gather(None, self.w['codebook'], None, quant, idx_in=codes)
+        D = self.depth
+        codes = codes.to(self.dev, torch.int64).reshape(-1, D).contiguous()
+        d1 = D - 1 if d1 is None else d1
+        quant = self._new(codes.shape[0], self.arch.embed_dim, dtype=torch.float32)
+        if D == 1:
+            ops.argmax_gather(None, self.w['codebook'], None, quant, idx_in=codes.view(-1))
+        else:
+            ops.rq_embed(codes, d0, d1, self.w['codebooks'], quant, ldi=D, ldd=1)
         return quant
 
     @_on_device
     @torch.no_grad()
+    def embed_code_with_depth(self, codes):
+        """RQBottleneck.embed_code_with_depth (`:371-391`): int64 codes [..., D] -> fp32 [T, D, E], one code row
+        per depth (not summed)."""
+        D = self.depth
+        if D == 1:
+            return self.embed_code(codes).unsqueeze(1)
+        self._fusing = False
+        codes = codes.to(self.dev, torch.int64).reshape(-1, D).contiguous()
+        out = self._new(codes.shape[0], D, self.arch.embed_dim, dtype=torch.float32)
+        for d in range(D):
+            ops.rq_embed(codes, d, d, self.w['codebooks'], out[:, d], ldi=D, ldd=1)
+        return out
+
+    @_on_device
+    @torch.no_grad()
     def soft_codes(self, z_e, temp, stochastic=False):
-        """RQBottleneck.get_soft_codes, depth 1 (`:429-457`): z_e fp32 [T, E] -> (p fp32 [T, K], codes int64 [T]).
-        Codes are the exact L2 argmin (== forward_vq's) or, stochastic, one draw per row from p with a seed taken on
-        the device from the default CUDA generator (reproducible under torch.manual_seed, no host sync)."""
+        """RQBottleneck.get_soft_codes (`:429-457`): z_e fp32 [T, E] -> (p fp32 [T, K], codes int64 [T]) at depth 1,
+        (p fp32 [T, D, K], codes int64 [T, D]) at depth D.  Codes are the exact L2 argmin (== forward_vq's) or,
+        stochastic, one draw per row from p with a seed taken on the device from the default CUDA generator
+        (reproducible under torch.manual_seed, no host sync); each depth works on the residual the earlier codes left."""
         a = self.arch
         self._fusing = False
         z = z_e.to(self.dev, torch.float32).reshape(-1, a.embed_dim).contiguous()
         T = z.shape[0]
+        if self.depth > 1:
+            return self._soft_codes_rq(z, temp, stochastic)
         pack = self._codebook_pack()
         p = self._new(T, a.n_embed, dtype=torch.float32)
         ops.soft_codes(z, self.w['codebook'], pack[1], a.n_embed, temp, p)
@@ -730,20 +804,36 @@ class Engine:
             ops.l2_argmin_tc(z, self.w['codebook'], pack, a.n_embed, codes)
         return p, codes
 
+    def _soft_codes_rq(self, z, temp, stochastic):
+        a = self.arch
+        T, D, K = z.shape[0], self.depth, a.n_embed
+        p = self._new(T, D, K, dtype=torch.float32)
+        codes = torch.empty(D, T, dtype=torch.int64, device=self.dev)
+        r = self._new(T, a.embed_dim, dtype=torch.float32)
+        for d in range(D):
+            src = z if d == 0 else r
+            pack = self._codebook_pack(d)
+            ops.soft_codes_ld(src, self._codebook(d), pack[1], K, temp, p[:, d])
+            if stochastic:
+                seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (2,), dtype=torch.int64, device=self.dev)
+                ops.sample_codes_ld(p[:, d], seed, codes[d])
+            else:
+                ops.l2_argmin_tc(src, self._codebook(d), pack, K, codes[d])
+            if d < D - 1:
+                ops.rq_residual(src, r, codes[d], self._codebook(d), None, d == 0)
+        return p, codes.t().contiguous()
+
     @_on_device
     @torch.no_grad()
     def forward_vq(self, x, code_only=False):
-        """TDCRQVAE3.forward (`archs/tdcrqvae3_arch.py:760-783`): encode -> L2 argmin -> embed -> decode."""
+        """TDCRQVAE3.forward (`archs/tdcrqvae3_arch.py:760-783`): encode -> residual quantiser -> decode."""
         a = self.arch
         z_e = self.encode(x)
         Fr, hh, ww, _ = z_e.shape
         T = Fr * hh * ww
         z_e = z_e.view(T, a.embed_dim)
-        codes = torch.empty(T, dtype=torch.int64, device=self.dev)
-        z_q = self._new(T, a.embed_dim, dtype=torch.float32)
-        ops.l2_argmin_tc(z_e, self.w['codebook'], self._codebook_pack(), a.n_embed, codes, z_q)
-        loss = (z_e - z_q).pow(2).mean()
-        codes = codes.view(Fr, hh, ww, 1)
+        codes, z_q, loss = self.quantize(z_e)
+        codes = codes.view(Fr, hh, ww, self.depth)
         z_q = z_q.view(Fr, hh, ww, -1)
         if code_only:
             return z_q, loss, codes

@@ -409,6 +409,57 @@ def sample_codes(p, seed, idx_out):
     return idx_out
 
 
+def soft_codes_ld(z, codebook, norm, K, temp, out):
+    """soft_codes into a row-pitched [T, K] view (one depth's K-slice of a contiguous [T, D, K] tensor)."""
+    lib = L.load()
+    T, E = z.shape
+    assert z.dtype == torch.float32 and z.is_contiguous() and codebook.dtype == torch.float32 and codebook.is_contiguous()
+    assert codebook.shape[1] == E and codebook.shape[0] >= K and norm.dtype == torch.float32 and norm.numel() >= K
+    assert out.dtype == torch.float32 and tuple(out.shape) == (T, K) and out.stride(1) == 1
+    L.check(lib.pgt_soft_codes_ld(_p(z), T, E, _p(codebook), _p(norm), K, float(temp), _p(out), out.stride(0), _stream(z)))
+    return out
+
+
+def sample_codes_ld(p, seed, idx_out):
+    """sample_codes over the rows of a row-pitched [T, K] view; idx_out int64 [T] contiguous."""
+    lib = L.load()
+    T, K = p.shape
+    assert p.dtype == torch.float32 and p.stride(1) == 1 and idx_out.dtype == torch.int64 and idx_out.numel() == T
+    assert idx_out.is_contiguous() and seed.dtype == torch.int64 and seed.numel() == 2 and seed.device == p.device
+    L.check(lib.pgt_sample_codes_ld(_p(p), T, K, p.stride(0), _p(seed), _p(idx_out), _stream(p)))
+    return idx_out
+
+
+def rq_residual(r_in, r_out, idx, codebook, agg, first):
+    """One residual-quantiser step (rq.cu): e = codebook[idx[t]]; r_out = r_in - e and agg = e if first else agg + e,
+    each skipped when its output is None.  fp32 [T, E] contiguous; idx int64 [T] contiguous."""
+    lib = L.load()
+    ref = agg if agg is not None else r_out
+    T, E = ref.shape
+    assert codebook.dtype == torch.float32 and codebook.is_contiguous() and codebook.shape[1] == E
+    assert idx.dtype == torch.int64 and idx.is_contiguous() and idx.numel() == T and idx.device == ref.device
+    for r in (r_in, r_out, agg):
+        assert r is None or (r.dtype == torch.float32 and r.is_contiguous() and tuple(r.shape) == (T, E))
+    L.check(lib.pgt_rq_residual(_p(r_in), _p(r_out), _p(idx), T, E, _p(codebook), _p(agg), int(bool(first)),
+                                _stream(ref)))
+    return agg
+
+
+def rq_embed(idx, d0, d1, codebooks, out, ldi, ldd):
+    """out[t] = sum_{d = d0..d1} codebooks[d or 0][idx[t * ldi + d * ldd]] (rq.cu); codebooks fp32 [D, K + 1, E], or
+    [1, K + 1, E] for a codebook shared by every depth (read with depth stride 0).  out fp32 / bf16 [T, E] rows."""
+    lib = L.load()
+    T, E, ldo = _rows(out)
+    assert codebooks.dtype == torch.float32 and codebooks.is_contiguous() and codebooks.dim() == 3 and codebooks.shape[2] == E
+    assert idx.dtype == torch.int64 and idx.device == out.device and 0 <= d0 <= d1
+    assert codebooks.shape[0] == 1 or d1 < codebooks.shape[0]
+    assert idx.is_contiguous() and (T - 1) * ldi + d1 * ldd < idx.numel()
+    cb_stride = 0 if codebooks.shape[0] == 1 else codebooks.shape[1] * E
+    L.check(lib.pgt_rq_embed(_p(idx), ldi, ldd, T, d0, d1, _p(codebooks), cb_stride, E, _p(out), ldo, _dt(out),
+                             _stream(out)))
+    return out
+
+
 def adain(q, style, out, eps=1e-5):
     lib = L.load()
     F = q.shape[0]

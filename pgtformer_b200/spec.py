@@ -20,6 +20,14 @@ class Spec(OrderedDict):
     def __init__(self, *a, **k):
         super().__init__(*a, **k)
         self.windows = {}         # name of a relative_position_index buffer -> its (D, H, W) window (default: WINDOW)
+        # module prefix -> the module it is: a shared codebook is one VQEmbedding listed under every depth
+        # (`archs/tdcrqvae3_arch.py:256-262`), so its state-dict keys repeat once per depth, all aliasing one tensor
+        self.module_aliases = {}
+
+    def alias_of(self, name):
+        """The key whose tensor `name` aliases, or None."""
+        mod, _, leaf = name.rpartition('.')
+        return self.module_aliases[mod] + '.' + leaf if mod in self.module_aliases else None
 
     def add(self, name, shape, kind, dtype='float32'):
         assert name not in self, name
@@ -126,6 +134,7 @@ class Arch:
         self.n_embed = int(g.get('n_embed', 512))
         self.code_shape = tuple(g['code_shape'])
         self.latent_shape = tuple(g['latent_shape'])
+        self.shared_codebook = bool(g.get('shared_codebook', True))       # the options files' setting
         self.dim_embd = int(g.get('dim_embd', 512))
         self.n_head = int(g.get('n_head', 8))
         self.n_layers = int(g.get('n_layers', 9))
@@ -152,8 +161,9 @@ class Arch:
             raise ValueError('incompatible code shape or latent shape')      # tdcrqvae3_arch.py:234
         if self.tf != 3 or self.num_frames != 3 or any(w != (4, 4) for w in self.window_sizes):
             raise ValueError('the CUDA path is built for 3-frame clips and 4x4x3 windows')
-        if self.code_shape[2] != 1:
-            raise ValueError('the CUDA path is built for quantiser depth 1')
+        if int(self.code_shape[2]) < 1:
+            raise ValueError('quantiser depth code_shape[2] must be >= 1, got %r' % (self.code_shape[2],))
+        self.depth = int(self.code_shape[2])
         # levels that carry a window-attention layer (curr_res walk of tdcrqvae3_arch.py:482-510)
         self.level_has_attn = tuple((self.resolution >> i) in self.attn_resolutions
                                     for i in range(self.num_levels))
@@ -203,11 +213,15 @@ def build_spec(network_g):
             _conv(s, 'decoder.up.%d.upsample.conv' % lvl, block_in, block_in, 3)
     _norm(s, 'decoder.norm_out', block_in)
     _conv(s, 'decoder.conv_out', block_in, a.out_ch, 3)
-    # ---- quantiser (tdcrqvae3_arch.py:80-97,215-271): shared codebook, depth 1
+    # ---- quantiser (tdcrqvae3_arch.py:80-97,215-271): one VQEmbedding per depth, or one shared by every depth
     e = a.embed_dim
-    s.add('quantizer.codebooks.0.weight', (a.n_embed + 1, e), 'codebook')
-    s.add('quantizer.codebooks.0.cluster_size_ema', (a.n_embed,), 'zeros')
-    s.add('quantizer.codebooks.0.embed_ema', (a.n_embed, e), 'codebook_ema')
+    for d in range(a.depth):
+        p = 'quantizer.codebooks.%d' % d
+        s.add(p + '.weight', (a.n_embed + 1, e), 'codebook')
+        s.add(p + '.cluster_size_ema', (a.n_embed,), 'zeros')
+        s.add(p + '.embed_ema', (a.n_embed, e), 'codebook_ema')
+        if a.shared_codebook and d > 0:
+            s.module_aliases[p] = 'quantizer.codebooks.0'
     _conv(s, 'quant_conv', a.z_channels, e, 1)
     _conv(s, 'post_quant_conv', e, a.z_channels, 1)
     # ---- PGTFormer head (pgtformer_arch.py:511-550)
@@ -294,7 +308,10 @@ class TDRQVAEArch:
         if any(y % x != 0 for x, y in zip(self.code_shape[:2], self.latent_shape[:2])):
             raise ValueError('incompatible code shape or latent shape')
         if self.code_shape[2] != 1:
-            raise ValueError('the CUDA path is built for quantiser depth 1')
+            # the reference's TDRQVAE.forward / get_codes reshape the codes with code.view(b, t, fh, fw, 1)
+            # (archs/tdrqvae_arch.py:852, 888), which fails for any deeper quantiser
+            raise ValueError('TDRQVAE runs quantiser depth 1 only: the reference reshapes its codes with '
+                             'view(b, t, h, w, 1) (archs/tdrqvae_arch.py:852, 888)')
         self.ch = int(dd['ch'])
         self.ch_mult = tuple(dd['ch_mult'])
         self.num_res_blocks = int(dd['num_res_blocks'])

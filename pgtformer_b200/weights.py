@@ -76,11 +76,15 @@ def synth_tensor(name, shape, kind, dtype, seed=0, window=None):
 
 def synth_state_dict(spec, seed=0):
     sd = {}
+    alias = getattr(spec, 'alias_of', lambda name: None)
     for name, (shape, kind, dtype) in spec.items():
-        if kind == 'codebook_ema':
+        if kind == 'codebook_ema' or alias(name):
             continue
         sd[name] = synth_tensor(name, shape, kind, dtype, seed, window=getattr(spec, 'windows', {}).get(name))
     for name, (shape, kind, dtype) in spec.items():
-        if kind == 'codebook_ema':               # embed_ema = weight[:-1] clone (tdcrqvae3_arch.py:96)
+        if kind == 'codebook_ema' and not alias(name):     # embed_ema = weight[:-1] clone (tdcrqvae3_arch.py:96)
             sd[name] = sd[name.replace('embed_ema', 'weight')][:-1].clone()
+    for name in spec:
+        if alias(name):                                    # a shared codebook: every depth's keys are one tensor
+            sd[name] = sd[alias(name)]
     return {k: sd[k] for k in spec}
