@@ -205,9 +205,10 @@ int pgt_window_attention(const void* qkv, int ldqkv, int clips, int H, int W, in
 
 /* The same core on TMA + wgmma (window_attn_tc.cu): a window's q / k / v rows of a 64-column chunk are one 5-D TMA box
  * of the qkv matrix (wrapped windows of a shifted block: 2 or 4 partial boxes), QK^T and PV run as wgmma with S / P / O
- * in registers, results are stored to the tokens' output rows.  tab: fp16 [4][heads][6][48][8] bias / mask tables
- * (pgtformer_b200/ops.py::window_tables — relative-position bias and the {0,-100} shift mask in the row order of the
- * four box layouts, times log2 e).  mode_n64: for d = 32 run P V with N = 64 instead of a half-atom N = 32 operand view.
+ * in registers, results are stored to the tokens' output rows.  tab: fp16 [4][heads][6][48][8] bias tables
+ * (pgtformer_b200/ops.py::window_tables — the relative-position bias in the row order of the four box layouts, times
+ * log2 e; the {0,-100} shift mask is not in the table, the kernel adds it in fp32).  mode_n64: for d = 32 run P V with
+ * N = 64 instead of a half-atom N = 32 operand view.
  * Returns PGT_ERR_UNSUPPORTED unless heads == 8, d in {32, 64}, C % 128 == 0, shift in {0, 2}. */
 int pgt_window_attention_tc(const void* qkv, int ldqkv, int clips, int H, int W, int C, int heads, int shift,
                             const void* tab, void* out, int ldo, int mode_n64, void* stream);

@@ -5,10 +5,15 @@
 //   warps 0..7  warpgroup h owns query rows [64h, 64h + 64): S = Q K_j^T (wgmma 64 x 128 x 16, fp32 in registers),
 //               one pass over S per key tile — p = 2^(s*c - m_ref) against a reference exponent m_ref that is the row
 //               maximum of the first tile and is only raised (by a whole power of two, so the rescale of O and L is
-//               exact) when a later tile produces p > 2^8 —, P packed to bf16 in registers as the A operand of
-//               O += P V_j (wgmma 64 x 64 x 16, V consumed MN-major straight from its TMA tile), and the denominator L
-//               summed over exactly the bf16 P that the numerator uses.  Each row's 128 scores of a tile live in the
-//               four lanes of a quad; row maxima and sums combine by shuffles.
+//               exact): lazily, for the following tiles, when a tile produces p > 2^8 —, P packed to bf16 in registers
+//               as the A operand of O += P V_j (wgmma 64 x 64 x 16, V consumed MN-major straight from its TMA tile), and
+//               the denominator L summed over exactly the bf16 P that the numerator uses.  Each row's 128 scores of a
+//               tile live in the four lanes of a quad; row maxima and sums combine by shuffles.
+//               A tile more than 2^64 above the reference (a key whose scaled logit exceeds the first tile's row maximum
+//               by ~44 or more; from ~88 on, p overflows fp32) is caught by one warp vote after the pass: the warp
+//               recomputes its rows of S from shared memory (fp32 FMAs), raises m_ref at once so that the tile's row
+//               maximum gives p <= 1, rescales O and L by the same power of two and exponentiates P again.  Inputs that
+//               never trigger it give the same bits as a kernel without it, and no score range overflows p.
 #include <cudaTypedefs.h>
 
 #include "common.cuh"
@@ -25,6 +30,7 @@ constexpr int FT_TILE = FT_BN * FT_D * 2;  // 16 KB: one 128 x 64 bf16 tile
 constexpr int FT_THREADS = 256 + 32;
 constexpr int FT_SMEM = FT_TILE /*Q*/ + FT_NST * 2 * FT_TILE /*K,V*/ + 256 + 1024;
 constexpr float FT_TAU = 256.f;              // p above this raises the reference exponent for the following tiles
+constexpr float FT_OVER = 18446744073709551616.f;   // 2^64: p above this raises it for the current tile (recomputed)
 
 __global__ void __launch_bounds__(FT_THREADS, 1)
 mha_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -131,6 +137,67 @@ mha_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ C
           pm[e] = fmaxf(pm[e], fmaxf(pr.x, pr.y));
           ts[e] += pr.x + pr.y;
           pa[c >> 1][(c & 1) * 2 + e] = pp;
+        }
+      }
+      // a tile far above the reference (p > 2^64, or overflowed to inf): raise the reference of those rows by the whole
+      // power of two that brings the tile's row maximum to p <= 1, fold it into the rescale of O and L, and exponentiate
+      // their P again.  Rare (the lazy raise below covers every tile within 2^64 of the reference): one warp vote on the
+      // common path.  S is not kept live through the pass (that costs spills): the warp recomputes the scores it needs
+      // from the Q and K tiles, which stay in shared memory until after P V, with fp32 FMAs on the bf16 values (no
+      // tensor cores, so the other warps of the warpgroup need not take the branch).  Other rows keep their P.
+      if (__any_sync(0xffffffffu, !(pm[0] <= FT_OVER) || !(pm[1] <= FT_OVER))) {
+        const uint8_t* sKt = sK + st * FT_TILE;
+        const int r0 = wg * 64 + 16 * w + (lane >> 2);         // Q rows r0, r0 + 8; keys 8c + 2 t4 + {0, 1}
+        auto score = [&](int r, int key) {                      // q_r . k_key over the 128B-swizzled 16-byte chunks
+          float acc = 0.f;
+#pragma unroll 1
+          for (int kc = 0; kc < FT_D / 8; ++kc) {
+            const uint4 a = *reinterpret_cast<const uint4*>(sQ + r * 128 + ((kc ^ (r & 7)) << 4));
+            const uint4 b = *reinterpret_cast<const uint4*>(sKt + key * 128 + ((kc ^ (key & 7)) << 4));
+            const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+            for (int x = 0; x < 4; ++x) {
+              const float2 fa = unpack_bf16x2(aw[x]), fb = unpack_bf16x2(bw[x]);
+              acc = fmaf(fa.y, fb.y, fmaf(fa.x, fb.x, acc));
+            }
+          }
+          return acc;
+        };
+        bool big[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float m = fmaxf(pm[e], __shfl_xor_sync(0xffffffffu, pm[e], 1));
+          m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+          big[e] = !(m <= FT_OVER);
+          float mx = -INFINITY;
+#pragma unroll 1
+          for (int key = 2 * t4; key < FT_BN; key += 8)
+            mx = fmaxf(mx, fmaxf(score(r0 + 8 * e, key), score(r0 + 8 * e, key + 1)));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          if (big[e]) {
+            const int r = (int)ceilf(fminf(fmaf(mx, sl2, -mb[e]), 1e6f));    // > 64 here
+            mb[e] += (float)r;
+            scale_due[e] *= r < 127 ? __int_as_float((127 - r) << 23) : 0.f;
+            pm[e] = 0.f;
+            ts[e] = 0.f;
+          }
+        }
+#pragma unroll
+        for (int c = 0; c < FT_BN / 8; ++c) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (big[e]) {
+              const int key = 8 * c + 2 * t4;
+              const float p0 = ex2_approx(fmaf(score(r0 + 8 * e, key), sl2, -mb[e]));
+              const float p1 = ex2_approx(fmaf(score(r0 + 8 * e, key + 1), sl2, -mb[e]));
+              const uint32_t pp = pack_bf16x2(p0, p1);
+              const float2 pr = unpack_bf16x2(pp);
+              pm[e] = fmaxf(pm[e], fmaxf(pr.x, pr.y));
+              ts[e] += pr.x + pr.y;
+              pa[c >> 1][(c & 1) * 2 + e] = pp;
+            }
+          }
         }
       }
       // exact power-of-two rescale of this row's O and L (rows with nothing due multiply by 1)

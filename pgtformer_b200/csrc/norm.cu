@@ -199,8 +199,10 @@ gn_apply_kernel(const __nv_bfloat16* __restrict__ x, int ldx, int HW, int C, int
 // One warp per token row, LN_ROWS rows per warp in flight (all loads issued before any reduction) so that
 // enough 16-byte requests are outstanding to approach HBM bandwidth; two-pass statistics in registers.
 constexpr int LN_ROWS = 4;
+// The minimum blocks per SM hold the register budget of the one-pass statistics (the rarely taken shifted pass below
+// would otherwise raise it and halve the occupancy of C = 512, the global transformer's width).
 template <int NV, bool POS>   // 8-element vectors per lane: C == 256 * NV; POS: second output LN(x) + pos
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(256, NV == 1 ? (POS ? 2 : 3) : (NV == 2 ? 2 : 1))
 layernorm_kernel(const void* __restrict__ xin, int ldx, int x_dtype, int T, const float* __restrict__ gamma,
                  const float* __restrict__ beta, float eps, __nv_bfloat16* __restrict__ y, int ldy,
                  const __nv_bfloat16* __restrict__ pos, int ldpos, __nv_bfloat16* __restrict__ y2, int ldy2) {
@@ -210,9 +212,12 @@ layernorm_kernel(const void* __restrict__ xin, int ldx, int x_dtype, int T, cons
   const int row0 = warp * LN_ROWS;
   if (row0 >= T) return;
   float v[LN_ROWS][NV][8];
+  float x0[LN_ROWS];                  // each row's first element: the shift of a row whose one-pass variance cancels
 #pragma unroll
   for (int r = 0; r < LN_ROWS; ++r) {
     const int row = min(row0 + r, T - 1);
+    x0[r] = x_dtype == PGT_BF16 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(xin)[(size_t)row * ldx])
+                                : __ldg(reinterpret_cast<const float*>(xin) + (size_t)row * ldx);
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
       const int c0 = (i * 32 + lane) * 8;
@@ -262,8 +267,35 @@ layernorm_kernel(const void* __restrict__ xin, int ldx, int x_dtype, int T, cons
       s += __shfl_xor_sync(0xffffffffu, s, o);
       q += __shfl_xor_sync(0xffffffffu, q, o);
     }
-    const float mean = s * (1.0f / C);
-    const float rstd = rsqrtf(fmaxf(q * (1.0f / C) - mean * mean, 0.f) + eps);
+    float mean = s * (1.0f / C);
+    float var = q * (1.0f / C) - mean * mean;
+    // A row far from zero next to its spread (|mean| >= 32 std, or constant; e.g. the global transformer's fp32
+    // residual stream) makes q / C - mean^2 cancel: a relative variance error of ~2^-24 (mean / std)^2, and worse from
+    // the fp32 sums.  Such a row is summed again, shifted by one of its own elements, and normalised shifted too: a
+    // constant row then gives exactly beta.  Every other row keeps the one-pass sums (and its bits).  The butterfly
+    // sums are identical on every lane, so the branch is warp-uniform.
+    float piv = 0.f;
+    if (!(var * 1024.f > mean * mean)) {
+      piv = x0[r];
+      s = 0.f;
+      q = 0.f;
+#pragma unroll
+      for (int i = 0; i < NV; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float d = v[r][i][j] - piv;
+          s += d;
+          q = fmaf(d, d, q);
+        }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        s += __shfl_xor_sync(0xffffffffu, s, o);
+        q += __shfl_xor_sync(0xffffffffu, q, o);
+      }
+      mean = s * (1.0f / C);
+      var = q * (1.0f / C) - mean * mean;
+    }
+    const float rstd = rsqrtf(fmaxf(var, 0.f) + eps);
     const float nm = -mean * rstd;
     if (row < T) {
 #pragma unroll
@@ -271,7 +303,7 @@ layernorm_kernel(const void* __restrict__ xin, int ldx, int x_dtype, int T, cons
         const int c0 = (i * 32 + lane) * 8;
         float o[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = fmaf(fmaf(v[r][i][j], rstd, nm), g[i][j], bt[i][j]);
+        for (int j = 0; j < 8; ++j) o[j] = fmaf(fmaf(v[r][i][j] - piv, rstd, nm), g[i][j], bt[i][j]);
         store8_bf16(y + (size_t)row * ldy + c0, o);
         if constexpr (POS) {
           const uint32_t pw[4] = {pr[r][i].x, pr[r][i].y, pr[r][i].z, pr[r][i].w};
@@ -295,7 +327,8 @@ __global__ void __launch_bounds__(ADAIN_THREADS)
 adain_kernel(const void* __restrict__ qin, int ldq, int q_dtype, const __nv_bfloat16* __restrict__ l, int ldl, int HW,
              int C, float eps, __nv_bfloat16* __restrict__ y, int ldy) {
   __shared__ float red[4][ADAIN_THREADS / 8][64];   // [stat][prow][channel]
-  __shared__ float sa[64], sb[64];
+  __shared__ float sa[64], sb[64], spiv[64];
+  __shared__ double sml[64], ssl[64];
   const int f = blockIdx.y;
   const int cbase = blockIdx.x * 64;
   const int vcol = threadIdx.x & 7;
@@ -331,6 +364,7 @@ adain_kernel(const void* __restrict__ qin, int ldq, int q_dtype, const __nv_bflo
 #pragma unroll
     for (int j = 0; j < 8; ++j) red[k][prow][vcol * 8 + j] = acc[k][j];
   __syncthreads();
+  bool shift = false;
   if (threadIdx.x < 64) {
     double s[4] = {0, 0, 0, 0};
     for (int r = 0; r < rows_par; ++r)
@@ -339,19 +373,61 @@ adain_kernel(const void* __restrict__ qin, int ldq, int q_dtype, const __nv_bflo
     const double n = (double)HW;
     const double mq = s[0] / n, ml = s[2] / n;
     double vq = (s[1] - n * mq * mq) / (n - 1.0), vl = (s[3] - n * ml * ml) / (n - 1.0);   // unbiased (torch.var)
+    // a content channel far from zero next to its spread (|mean| >= 32 std, or constant): its fp32 sums of squares
+    // cancel against n * mean^2, so it is summed again below, shifted by its value at pixel 0
+    shift = !(vq * 1024.0 > mq * mq);
     if (vq < 0) vq = 0;
     if (vl < 0) vl = 0;
     const double sq = sqrt(vq + (double)eps), sl = sqrt(vl + (double)eps);
     const double a = sl / sq;
     sa[threadIdx.x] = (float)a;
     sb[threadIdx.x] = (float)(ml - mq * a);
+    sml[threadIdx.x] = ml;
+    ssl[threadIdx.x] = sl;
+    float piv = 0.f;
+    if (shift) {
+      const size_t i0 = (size_t)f * HW * ldq + cbase + threadIdx.x;
+      piv = q_dtype == PGT_BF16 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(qin)[i0])
+                                : reinterpret_cast<const float*>(qin)[i0];
+    }
+    spiv[threadIdx.x] = piv;                            // 0 for every other channel: their bits are unchanged
+  }
+  if (__syncthreads_or(shift)) {                        // rare: a second pass over the content of this slab
+    float pq[8], a2[2][8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { pq[j] = spiv[vcol * 8 + j]; a2[0][j] = 0.f; a2[1][j] = 0.f; }
+    for (int p = prow; p < HW; p += rows_par) {
+      float vq[8];
+      load_q(p, vq);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float d = vq[j] - pq[j];
+        a2[0][j] += d; a2[1][j] += d * d;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) red[k][prow][vcol * 8 + j] = a2[k][j];
+    __syncthreads();
+    if (shift) {
+      double s0 = 0, s1 = 0;
+      for (int r = 0; r < rows_par; ++r) { s0 += (double)red[0][r][threadIdx.x]; s1 += (double)red[1][r][threadIdx.x]; }
+      const double n = (double)HW;
+      const double mq = s0 / n;                         // mean of the shifted channel
+      double vq = (s1 - n * mq * mq) / (n - 1.0);
+      if (vq < 0) vq = 0;
+      const double a = ssl[threadIdx.x] / sqrt(vq + (double)eps);
+      sa[threadIdx.x] = (float)a;
+      sb[threadIdx.x] = (float)(sml[threadIdx.x] - mq * a);   // applied to the shifted content
+    }
   }
   __syncthreads();
   for (int p = prow; p < HW; p += rows_par) {
     float vq[8];
     load_q(p, vq);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) vq[j] = vq[j] * sa[vcol * 8 + j] + sb[vcol * 8 + j];
+    for (int j = 0; j < 8; ++j) vq[j] = (vq[j] - spiv[vcol * 8 + j]) * sa[vcol * 8 + j] + sb[vcol * 8 + j];
     store8_bf16(y + ((size_t)f * HW + p) * ldy + c0, vq);
   }
 }

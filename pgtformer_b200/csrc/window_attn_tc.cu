@@ -8,19 +8,21 @@
 //              the [T, 3C] qkv matrix (128B swizzle) — the roll by -shift is a coordinate offset, window_partition is the
 //              box shape.  Windows in the last window row / column of a shifted block wrap around the frame: they are 2
 //              (or 4) half (quarter) boxes, landing one after the other, so their rows sit in a permuted order; attention
-//              does not care as long as bias and mask are permuted alike, which the host does once per layer (below).
+//              does not care as long as bias and mask follow it: the host permutes the bias table once per layer, the
+//              kernel labels the mask's halves / quarters in box order (below).
 //              4-deep ring of (k | v | q) chunk tiles.
 //   warps 0-3 / 4-7   two warpgroups that alternate chunks.  Per head and window: S = Q K^T as one wgmma 64 x 48 x d
 //              (window 0 from tile row 0, window 1 through a view that starts 16 rows before it, so that its 48 rows are
-//              rows 16..63 of the MMA), softmax on the register fragments (t = s * scale*log2e + table, exp2, row max and
-//              sum across the four lanes of a row), P converted in registers into the A operand of O = P V (wgmma
+//              rows 16..63 of the MMA), softmax on the register fragments (t = s * scale*log2e + table + mask, exp2, row
+//              max and sum across the four lanes of a row), P converted in registers into the A operand of O = P V (wgmma
 //              64 x 64 x 16 with A from registers, V read MN-major straight from its TMA tile; for d = 32 the N = 64
 //              view spans both heads of the chunk and the other head's half is ignored), then O * (1/sum) -> bf16 -> the
 //              token's output row in HBM (window_reverse + roll back are index math).
-// Bias / mask table (built at load time by the engine, fp16, already multiplied by log2 e):
+// Bias table (built at load time by the engine, fp16, already multiplied by log2 e):
 //   tab[type][head][j = key/8][row][8]   type 0 interior, 1 x-wrapped (right edge), 2 y-wrapped (bottom edge), 3 corner;
-//   entry = relative_position_bias[pi_t(row)][pi_t(key)] + (-100 where the reference's shift mask separates the two
-//   tokens), pi_t = the row permutation of the wrapped box order.  Type 0 lives in shared memory, the others in L2.
+//   entry = relative_position_bias[pi_t(row)][pi_t(key)], pi_t = the row permutation of the wrapped box order.  Type 0
+//   lives in shared memory, the others in L2.  The reference's shift mask (-100 between tokens it separates: the two
+//   halves or four quarters of a wrapped window, in box order) is added by the kernel as an exact fp32 constant.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -36,6 +38,9 @@ constexpr int WT_NST = 4;
 constexpr int WT_THREADS = 256 + 32;
 constexpr int WT_HEADS = 8;
 constexpr int WT_TAB_BYTES = WT_HEADS * 6 * WT_N * 16;            // 36 KB: one type of the fp16 table
+// the reference's -100 shift mask in the log2 domain, added in fp32: inside the fp16 table (ulp 0.125 near -144) it
+// would move a masked key's weight by up to 4 %, which matters once scores reach the size of the mask
+constexpr float WT_MASK = -144.26950408889634f;
 constexpr int WT_SMEM = 2048 /*pad*/ + WT_NST * WT_STAGE + WT_TAB_BYTES + 512 /*barriers*/ + 1024 /*align*/;
 
 struct WinParams {
@@ -63,6 +68,10 @@ __device__ __forceinline__ WinCoord win_coord(const WinParams& p, int w) {
   c.y0 = wy * 4 + p.shift;
   return c;
 }
+
+// Which part of a wrapped window (type 1 / 2: half, 3: quarter) row `rw` belongs to in the box order of the table: the
+// reference's shift mask separates tokens of different parts.
+__device__ __forceinline__ int wrap_label(int type, int rw) { return type == 3 ? rw / 12 : rw / 24; }
 
 // Token index (row of the [T, *] matrices) of row `rw` of a window, given its box layout (see the table comment).
 __device__ __forceinline__ int win_token(const WinParams& p, const WinCoord& wc, int rw) {
@@ -217,6 +226,23 @@ window_attn_tc_kernel(const __grid_constant__ CUtensorMap tmI0, const __grid_con
             s[4 * j + 2 * e] = fmaf(s[4 * j + 2 * e], p.sl2, b2.x);
             s[4 * j + 2 * e + 1] = fmaf(s[4 * j + 2 * e + 1], p.sl2, b2.y);
             mx[e] = fmaxf(mx[e], fmaxf(s[4 * j + 2 * e], s[4 * j + 2 * e + 1]));
+          }
+        }
+        if (type[wi] != 0) {
+          // a wrapped window: the reference's shift mask between its halves (x- or y-wrapped) or quarters (corner) in
+          // the table's box order, added here in fp32 (warp-uniform; interior windows skip it)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int rl = wrap_label(type[wi], rwin[wi][e]);
+            mx[e] = -1e30f;
+#pragma unroll
+            for (int j = 0; j < 6; ++j) {
+              if (wrap_label(type[wi], 8 * j + 2 * t4) != rl) {       // keys 8j + 2 t4 + {0, 1} share a label
+                s[4 * j + 2 * e] += WT_MASK;
+                s[4 * j + 2 * e + 1] += WT_MASK;
+              }
+              mx[e] = fmaxf(mx[e], fmaxf(s[4 * j + 2 * e], s[4 * j + 2 * e + 1]));
+            }
           }
         }
 #pragma unroll

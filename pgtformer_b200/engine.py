@@ -135,7 +135,7 @@ class Engine:
                 heads = sd[name].shape[1]
                 idx = sd[p + '.relative_position_index'].view(-1).long()
                 w[p + '.bias_tab'] = sd[name].float()[idx].view(48, 48, heads).permute(2, 0, 1).contiguous()
-                w[p + '.tab16'] = ops.window_tables(w[p + '.bias_tab'])     # wgmma window kernel: bias + mask, 4 box layouts
+                w[p + '.tab16'] = ops.window_tables(w[p + '.bias_tab'])     # wgmma window kernel: bias, 4 box layouts
                 w[p + '.qkv.weight'] = _pack_lin(torch.cat([sd[p + '.q.weight'], sd[p + '.kv.weight']], 0).float())
                 w[p + '.qkv.bias'] = torch.cat([sd[p + '.q.bias'], sd[p + '.kv.bias']], 0).float().contiguous()
                 blk = p[:-len('.attn')]

@@ -260,17 +260,17 @@ LOG2E = 1.4426950408889634
 
 
 def window_tables(bias):
-    """Bias / mask tables of pgt_window_attention_tc from the expanded relative-position bias [heads, 48, 48] fp32:
-    fp16 [4 types][heads][6][48][8] = (bias[pi(row)][pi(key)] - 100 * masked) * log2(e), where type 0 is an interior
-    window, 1 / 2 / 3 a window that wraps in x / y / both (last window column / row of a shifted block): the TMA boxes
-    of its halves land one after the other, which permutes the rows (pi), and the reference's {0, -100} shift mask
-    (`modules/rstt_layers.py:552-568`) separates tokens on different sides of the wrap."""
+    """Bias tables of pgt_window_attention_tc from the expanded relative-position bias [heads, 48, 48] fp32:
+    fp16 [4 types][heads][6][48][8] = bias[pi(row)][pi(key)] * log2(e), where type 0 is an interior window, 1 / 2 / 3 a
+    window that wraps in x / y / both (last window column / row of a shifted block): the TMA boxes of its halves land
+    one after the other, which permutes the rows (pi).  The reference's {0, -100} shift mask
+    (`modules/rstt_layers.py:552-568`), which separates tokens on different sides of the wrap, is not in the table: the
+    kernel adds it in fp32 (in fp16, near -144, it would be rounded by up to 0.0625 in the log2 domain)."""
     heads = bias.shape[0]
     dev = bias.device
     r = torch.arange(48, device=dev)
     tabs = []
     for t in range(4):
-        xs, ys = t & 1, (t >> 1) & 1
         if t == 0:
             f, iy, ix = r // 16, (r // 4) % 4, r % 4
         elif t == 1:                                   # parts x in {W-2, W-1} then {0, 1}: rows [f][y][x(2)]
@@ -283,10 +283,7 @@ def window_tables(bias):
             pp, rr = r // 12, r % 12
             f, iy, ix = rr // 4, (rr % 4) // 2 + 2 * (pp // 2), rr % 2 + 2 * (pp % 2)
         canon = f * 16 + iy * 4 + ix
-        b = bias[:, canon][:, :, canon].float()
-        lab = (iy >= 2).long() * 2 * ys + (ix >= 2).long() * xs
-        masked = (lab[:, None] != lab[None, :]).float() * -100.0
-        tt = (b + masked[None]) * LOG2E                                      # [heads, row, key]
+        tt = bias[:, canon][:, :, canon].float() * LOG2E                     # [heads, row, key]
         tabs.append(tt.view(heads, 48, 6, 8).permute(0, 2, 1, 3))             # [heads, 6, row, 8]
     return torch.stack(tabs, 0).to(torch.float16).contiguous()
 
