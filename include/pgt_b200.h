@@ -59,7 +59,8 @@ typedef struct pgt_epilogue {
   int32_t flags;         /* PGT_EPI_FLAG_*                                                  */
   float* gn_stats;       /* optional fp32 [rows/128, 4, 32, 2]: per-(tile, 32-row quadrant) (sum, sumsq) of the output per GroupNorm(32)
                           * group, produced by the epilogue for the NEXT Normalize() (bf16 NHWC output, N % 32 == 0,
-                          * every 128-row tile inside one frame: pgt_conv_tiles_per_frame() > 0, or HW % 128 == 0 for
+                          * every 128-row tile inside one frame: pgt_conv_tiles_per_frame() > 0 (exact statistics:
+                          * pgt_conv_tiles_exact() > 0), or HW % 128 == 0 for
                           * pgt_linear_bf16); consumed by pgt_groupnorm_apply_stats                         */
 } pgt_epilogue;
 
@@ -111,6 +112,10 @@ int pgt_conv_bf16(const void* x, int F, int Hin, int Win, int Cin, int ldx, cons
  * Cout <= 3, H % 16 == 0, W % 8 == 0. */
 int pgt_conv_out_gn(const void* x, int F, int H, int W, int Cin, int ldx, const float* gn_ab, const void* Wp, int ldw,
                     int Cout, const float* bias, float* out, void* stream);
+/* The same with the activation chosen: silu = 1 is pgt_conv_out_gn (same kernel, same bits); silu = 0 is
+ * GroupNorm -> conv with no SiLU, the end of VQGAN's / CodeFormer's generator (archs/vqgan_arch.py:329-332). */
+int pgt_conv_out_gn_act(const void* x, int F, int H, int W, int Cin, int ldx, const float* gn_ab, const void* Wp, int ldw,
+                        int Cout, const float* bias, float* out, int silu, void* stream);
 
 /* ---- GroupNorm(32)+SiLU of the INPUT fused into the 3x3 / stride 1 / pad 1 conv: the normalised activation is never
  * written to HBM — the kernel applies y = silu(x * a[f,c] + b[f,c]) to each input slab in shared memory (bit-identical
@@ -153,6 +158,9 @@ int pgt_conv_rgb_bf16(const float* x_nchw, int F, int H, int W, int ksize, int s
 int64_t pgt_groupnorm_ws_floats(int F, int HW, int C);
 /* tiles per frame of the conv launch (0 = tiles may span frames: no fused statistics for that shape) */
 int pgt_conv_tiles_per_frame(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo);
+/* the same, and 0 when the tile grid does not divide the output frame: a tile past the frame's right or bottom edge
+ * adds rows that are not output pixels to its statistics, so the fused statistics are exact only when this is > 0 */
+int pgt_conv_tiles_exact(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo);
 /* finalize + apply only, with the statistics already produced by the previous conv / linear epilogue
  * (stats: [F, chunks_per_frame, 32, 2], chunks_per_frame = 4 x tiles per frame); saves the statistics pass over the tensor (1/3 of the GroupNorm traffic) */
 int pgt_groupnorm_apply_stats(const void* x, int ldx, int F, int HW, int C, const float* gamma, const float* beta,
@@ -295,6 +303,19 @@ int pgt_rq_residual(const float* r_in, float* r_out, const int64_t* idx, int T, 
                     float* agg, int first, void* stream);
 int pgt_rq_embed(const int64_t* idx, long long ldi, long long ldd, int T, int d0, int d1, const float* codebooks,
                  long long cb_stride, int E, void* out, int ldo, int out_dtype, void* stream);
+
+/* ---- VectorQuantizer.forward of VQGAN / CodeFormer (vq.cu; archs/vqgan_arch.py:42-84) after the nearest-code argmin:
+ * z fp32 [T, E] token rows (T = b * HW, rows of image i are i*HW .. i*HW + HW - 1), codebook fp32 [K, E], idx int64 [T].
+ * Per token: zq_nchw fp32 [b, E, HW] and / or zq_bf16 [T, E] = z + (e - z) (fp32, one rounding per operation);
+ * min_enc fp32 [T, K] one-hot rows; scores fp32 [T] = exp(-d / 10), d = |z|^2 + |e|^2 - 2 z.e in fp64 rounded to fp32;
+ * usage int32 [K] += code counts.  Any of these may be NULL.  hist int32 [K] must be zero on entry (it receives this
+ * call's counts); ws: pgt_vq_stats_ws_doubles(T, E) doubles.  scalars fp32 [3] = (loss = m + beta m with
+ * m = mean((e - z)^2), perplexity of this call's counts, mean_distance = mean of d over all [T, K] pairs, in closed
+ * form), finished on the device; the scalars are deterministic.  E % 32 == 0, E <= 512, K % 4 == 0. */
+long long pgt_vq_stats_ws_doubles(int T, int E);
+int pgt_vq_stats(const float* z, int T, int E, int HW, const float* codebook, int K, const int64_t* idx, float beta,
+                 float* zq_nchw, void* zq_bf16, float* min_enc, float* scores, int* usage, int* hist, double* ws,
+                 float* scalars, void* stream);
 
 /* ---- AdaIN: y = (q - mean_q)/std_q * std_l + mean_l per (frame, channel) over HW, unbiased
  * variance + eps.  q: bf16/fp32 [F, HW, ldq]; l (style) bf16 [F, HW, ldl]; y bf16.

@@ -42,6 +42,8 @@ SIGNATURES = {
                                  c_void_p]),
     'pgt_conv_out_gn': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
                                 c_void_p, c_void_p]),
+    'pgt_conv_out_gn_act': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                                    c_void_p, c_void_p, c_int, c_void_p]),
     'pgt_groupnorm_ab': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int,
                                  c_void_p, c_void_p, c_void_p]),
     'pgt_conv_up2x_bf16': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int,
@@ -50,6 +52,7 @@ SIGNATURES = {
                                   c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     'pgt_groupnorm_ws_floats': (c_int64, [c_int, c_int, c_int]),
     'pgt_conv_tiles_per_frame': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    'pgt_conv_tiles_exact': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int]),
     'pgt_groupnorm_apply_stats': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int,
                                           c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     'pgt_groupnorm_silu': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int,
@@ -82,6 +85,9 @@ SIGNATURES = {
     'pgt_rq_residual': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     'pgt_rq_embed': (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_int, c_void_p, c_int,
                              c_int, c_void_p]),
+    'pgt_vq_stats_ws_doubles': (c_int64, [c_int, c_int]),
+    'pgt_vq_stats': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_float, c_void_p, c_void_p,
+                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'pgt_adain': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int,
                           c_void_p]),
     'pgt_maxpool3x3s2': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),

@@ -1,5 +1,7 @@
 // decoder.norm_out -> SiLU -> conv_out (3x3, 64 -> 3 channels, fp32 NCHW result) as ONE wgmma kernel
 // (`archs/pgtformer_arch.py:707-710`, `archs/tdcrqvae3_arch.py:700-706`: GroupNorm(32, eps 1e-6), swish, Conv2d).
+// The activation is a template parameter: VQGAN's and CodeFormer's generator ends in GroupNorm -> Conv2d with no swish
+// (`archs/vqgan_arch.py:329-332`, last_silu=False), the SILU = false instantiation.
 //
 // Why its own kernel: with Cout = 3 the generic halo conv computes a 64-wide tile for 3 useful columns and stores
 // fp32 NCHW through its slow path (2.3 ms per 16 clips of 512^2), after a separate GroupNorm apply pass over the
@@ -49,6 +51,7 @@ struct ConvOutParams {
   int tiles_x, tiles_y, num_tiles;
 };
 
+template <bool SILU>
 __global__ void __launch_bounds__(CO_THREADS, 2)
 conv_out_gn_kernel(const ConvOutParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -124,7 +127,7 @@ conv_out_gn_kernel(const ConvOutParams p) {
             for (int e = 0; e < 4; ++e) {
               const float2 xv = unpack_bf16x2(u[e]);
               const float v0 = fmaf(xv.x, a[2 * e], b[2 * e]), v1 = fmaf(xv.y, a[2 * e + 1], b[2 * e + 1]);
-              q[e] = pack_bf16x2(silu_tanh(v0), silu_tanh(v1));
+              q[e] = SILU ? pack_bf16x2(silu_tanh(v0), silu_tanh(v1)) : pack_bf16x2(v0, v1);
             }
             o = make_uint4(q[0], q[1], q[2], q[3]);
           }
@@ -189,8 +192,9 @@ conv_out_gn_kernel(const ConvOutParams p) {
 
 using namespace pgt;
 
-extern "C" int pgt_conv_out_gn(const void* x, int F, int H, int W, int Cin, int ldx, const float* gn_ab, const void* Wp,
-                               int ldw, int Cout, const float* bias, float* out, void* stream) {
+template <bool SILU>
+static int conv_out_gn_run(const void* x, int F, int H, int W, int Cin, int ldx, const float* gn_ab, const void* Wp, int ldw,
+                           int Cout, const float* bias, float* out, void* stream) {
   PGT_CHECK_ARG(x && gn_ab && Wp && out && F > 0);
   if (Cin != 64 || Cout < 1 || Cout > 3 || H % CO_TH != 0 || W % CO_TW != 0 || ldx % 8 != 0 || ldw % 8 != 0)
     return PGT_ERR_UNSUPPORTED;
@@ -202,12 +206,24 @@ extern "C" int pgt_conv_out_gn(const void* x, int F, int H, int W, int Cin, int 
   p.ab = gn_ab; p.w = reinterpret_cast<const __nv_bfloat16*>(Wp); p.ldw = ldw; p.bias = bias; p.out = out;
   p.tiles_x = W / CO_TW; p.tiles_y = H / CO_TH; p.num_tiles = F * p.tiles_x * p.tiles_y;
   static PerDeviceOnce once;
-  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(conv_out_gn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CO_SMEM); }));
+  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(conv_out_gn_kernel<SILU>, cudaFuncAttributeMaxDynamicSharedMemorySize, CO_SMEM); }));
   const int grid = p.num_tiles < 2 * num_sms() ? p.num_tiles : 2 * num_sms();   // 2 CTAs per SM (66 KB smem each)
   char desc[64];
-  snprintf(desc, sizeof(desc), "conv_out_gn F%d H%d W%d N%d", F, H, W, Cout);
+  snprintf(desc, sizeof(desc), "conv_out_gn%s F%d H%d W%d N%d", SILU ? "" : "_nosilu", F, H, W, Cout);
   ProfScope ps(PGT_PROF_GEMM, 2.0 * F * (double)H * W * Cout * 9 * Cin, st, desc);
-  conv_out_gn_kernel<<<grid, CO_THREADS, CO_SMEM, st>>>(p);
+  conv_out_gn_kernel<SILU><<<grid, CO_THREADS, CO_SMEM, st>>>(p);
   PGT_LAUNCH_OK();
   return PGT_OK;
+}
+
+extern "C" int pgt_conv_out_gn(const void* x, int F, int H, int W, int Cin, int ldx, const float* gn_ab, const void* Wp,
+                               int ldw, int Cout, const float* bias, float* out, void* stream) {
+  return conv_out_gn_run<true>(x, F, H, W, Cin, ldx, gn_ab, Wp, ldw, Cout, bias, out, stream);
+}
+
+extern "C" int pgt_conv_out_gn_act(const void* x, int F, int H, int W, int Cin, int ldx, const float* gn_ab, const void* Wp,
+                                   int ldw, int Cout, const float* bias, float* out, int silu, void* stream) {
+  PGT_CHECK_ARG(silu == 0 || silu == 1);
+  return silu ? conv_out_gn_run<true>(x, F, H, W, Cin, ldx, gn_ab, Wp, ldw, Cout, bias, out, stream)
+              : conv_out_gn_run<false>(x, F, H, W, Cin, ldx, gn_ab, Wp, ldw, Cout, bias, out, stream);
 }

@@ -1442,21 +1442,37 @@ static int conv_impl(const void* x, int F, int Hin, int Win, int Cin, int ldx, c
   return dispatch_gemm(tmA, Wp, ldw, p, static_cast<cudaStream_t>(stream));
 }
 
-// 128-row tiles per frame of the conv the library would launch for this shape (0: a tile may span frames, so the
-// fused GroupNorm statistics are unavailable).  Mirrors the tile selection of conv_impl.
-extern "C" int pgt_conv_tiles_per_frame(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo) {
+// Tile shape (tw x th pixels) of the conv the library would launch for this shape, 0 when a 128-row tile may span
+// frames.  Mirrors the tile selection of conv_impl.
+static int conv_tile_shape(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo, int& tw, int& th) {
   static const bool no_halo = getenv("PGT_NO_HALO") != nullptr;
   const int H = Hin / stride, W = Win / stride;
   const bool halo = !no_halo && stride == 1 && ((ksize == 3 && pad_lo == 1) || ksize == 2) && Cout <= 128 && Hin >= HALO_TH &&
                     Win >= HALO_TW;      // ksize 2: an upsample phase (pgt_conv_up2x_bf16)
-  int tw = 1, th = 1;
+  tw = 1; th = 1;
   if (halo) { tw = HALO_TW; th = HALO_TH; }
   else {
     while (tw * 2 <= W && tw * 2 <= BM) tw *= 2;
     while (th * 2 <= H && tw * th * 2 <= BM) th *= 2;
   }
-  if (tw * th != BM) return 0;
-  return ceil_div(W, tw) * ceil_div(H, th);
+  return tw * th == BM ? 1 : 0;
+}
+
+// 128-row tiles per frame of the conv the library would launch for this shape (0: a tile may span frames, so the
+// fused GroupNorm statistics are unavailable).
+extern "C" int pgt_conv_tiles_per_frame(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo) {
+  int tw, th;
+  if (!conv_tile_shape(Hin, Win, Cout, ksize, stride, pad_lo, tw, th)) return 0;
+  return ceil_div(Win / stride, tw) * ceil_div(Hin / stride, th);
+}
+
+// The same, and 0 also when the tile grid does not divide the frame: the epilogue sums all 128 rows of a tile into the
+// statistics, so a tile that reaches past the frame's right or bottom edge adds rows that are not output pixels.
+extern "C" int pgt_conv_tiles_exact(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo) {
+  int tw, th;
+  if (!conv_tile_shape(Hin, Win, Cout, ksize, stride, pad_lo, tw, th)) return 0;
+  const int H = Hin / stride, W = Win / stride;
+  return (W % tw == 0 && H % th == 0) ? (W / tw) * (H / th) : 0;
 }
 
 extern "C" int pgt_conv_bf16(const void* x, int F, int Hin, int Win, int Cin, int ldx, const void* Wp, int ldw,

@@ -175,6 +175,56 @@ void linear(const at::Tensor& a, const at::Tensor& w, const c10::optional<at::Te
                         stream_of(a)), "linear");
 }
 
+void conv_out_gn_act(const at::Tensor& x, const at::Tensor& ab, const at::Tensor& wp, int64_t cout,
+                     const c10::optional<at::Tensor>& bias, bool silu, at::Tensor out) {
+  TORCH_CHECK(x.is_cuda() && x.dim() == 4 && x.scalar_type() == at::kBFloat16 && x.stride(3) == 1 &&
+              x.stride(1) == x.size(2) * x.stride(2) && (x.size(0) == 1 || x.stride(0) == x.size(1) * x.stride(1)) &&
+              ab.scalar_type() == at::kFloat && wp.scalar_type() == at::kBFloat16 && wp.stride(1) == 1 &&
+              out.scalar_type() == at::kFloat && out.is_contiguous() && out.dim() == 4 && out.size(0) == x.size(0) &&
+              out.size(1) == cout && out.size(2) == x.size(1) && out.size(3) == x.size(2),
+              "conv_out_gn_act: bf16 x [F, H, W, 64], fp32 ab [F, 2, 64], bf16 packed wp, fp32 out [F, cout, H, W]");
+  TORCH_CHECK(ab.device() == x.device() && wp.device() == x.device() && out.device() == x.device() &&
+              (!bias.has_value() || (bias->device() == x.device() && bias->scalar_type() == at::kFloat)),
+              "conv_out_gn_act: every tensor on x's device, fp32 bias");
+  c10::cuda::CUDAGuard guard(x.device());
+  check(pgt_conv_out_gn_act(x.data_ptr(), (int)x.size(0), (int)x.size(1), (int)x.size(2), (int)x.size(3), (int)x.stride(2),
+                            ab.data_ptr<float>(), wp.data_ptr(), (int)wp.stride(0), (int)cout,
+                            bias.has_value() ? bias->data_ptr<float>() : nullptr, out.data_ptr<float>(), silu ? 1 : 0,
+                            stream_of(x)), "conv_out_gn_act");
+}
+
+void vq_stats(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor& idx, int64_t HW, double beta,
+              at::Tensor scalars, const c10::optional<at::Tensor>& zq_nchw, const c10::optional<at::Tensor>& zq_bf16,
+              const c10::optional<at::Tensor>& min_enc, const c10::optional<at::Tensor>& scores,
+              const c10::optional<at::Tensor>& usage) {
+  TORCH_CHECK(z.is_cuda() && z.dim() == 2 && z.scalar_type() == at::kFloat && z.is_contiguous() &&
+              codebook.scalar_type() == at::kFloat && codebook.is_contiguous() && codebook.dim() == 2 &&
+              codebook.size(1) == z.size(1) && idx.scalar_type() == at::kLong && idx.is_contiguous() &&
+              idx.numel() == z.size(0) && scalars.scalar_type() == at::kFloat && scalars.is_contiguous() &&
+              scalars.numel() >= 3, "vq_stats: fp32 z [T, E], codebook [K, E], int64 idx [T], fp32 scalars [3]");
+  const int64_t T = z.size(0), E = z.size(1), K = codebook.size(0);
+  TORCH_CHECK(codebook.device() == z.device() && idx.device() == z.device() && scalars.device() == z.device(),
+              "vq_stats: codebook, idx and scalars must be on z's device");
+  auto opt = [&z](const c10::optional<at::Tensor>& t, at::ScalarType dt, int64_t n) -> void* {
+    if (!t.has_value()) return nullptr;
+    TORCH_CHECK(t->scalar_type() == dt && t->is_contiguous() && t->numel() == n, "vq_stats: optional output dtype / size");
+    TORCH_CHECK(t->device() == z.device(), "vq_stats: every output must be on z's device");
+    return t->data_ptr();
+  };
+  void* zn = opt(zq_nchw, at::kFloat, T * E);
+  void* zb = opt(zq_bf16, at::kBFloat16, T * E);
+  void* me = opt(min_enc, at::kFloat, T * K);
+  void* sc = opt(scores, at::kFloat, T);
+  void* us = opt(usage, at::kInt, K);
+  c10::cuda::CUDAGuard guard(z.device());
+  auto hist = at::zeros({K}, z.options().dtype(at::kInt));
+  auto ws = at::empty({std::max<int64_t>(pgt_vq_stats_ws_doubles((int)T, (int)E), 1)}, z.options().dtype(at::kDouble));
+  check(pgt_vq_stats(z.data_ptr<float>(), (int)T, (int)E, (int)HW, codebook.data_ptr<float>(), (int)K,
+                     idx.data_ptr<int64_t>(), (float)beta, static_cast<float*>(zn), zb, static_cast<float*>(me),
+                     static_cast<float*>(sc), static_cast<int*>(us), hist.data_ptr<int>(), ws.data_ptr<double>(),
+                     scalars.data_ptr<float>(), stream_of(z)), "vq_stats");
+}
+
 }  // namespace
 
 TORCH_LIBRARY(pgt, m) {
@@ -190,6 +240,9 @@ TORCH_LIBRARY(pgt, m) {
   m.def("sample_codes_ld(Tensor p, Tensor seed, Tensor(a!) idx) -> ()");
   m.def("rq_residual(Tensor? r_in, Tensor(a!)? r_out, Tensor idx, Tensor codebook, Tensor(b!)? agg, bool first) -> ()");
   m.def("rq_embed(Tensor idx, int d0, int d1, Tensor codebooks, Tensor(a!) out, int ldi, int ldd) -> ()");
+  m.def("conv_out_gn_act(Tensor x, Tensor ab, Tensor wp, int cout, Tensor? bias, bool silu, Tensor(a!) out) -> ()");
+  m.def("vq_stats(Tensor z, Tensor codebook, Tensor idx, int HW, float beta, Tensor(a!) scalars, Tensor(b!)? zq_nchw, "
+        "Tensor(c!)? zq_bf16, Tensor(d!)? min_enc, Tensor(e!)? scores, Tensor(f!)? usage) -> ()");
 }
 
 TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
@@ -205,4 +258,6 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("sample_codes_ld", sample_codes_ld);
   m.impl("rq_residual", rq_residual);
   m.impl("rq_embed", rq_embed);
+  m.impl("conv_out_gn_act", conv_out_gn_act);
+  m.impl("vq_stats", vq_stats);
 }

@@ -186,6 +186,10 @@ class Engine:
     fuse_gn_min_hw = int(os.environ.get('PGT_FUSE_GN', '0') or 0)       # fuse only for feature maps at least this tall
     fuse_gn_stats = True      # GroupNorm statistics from the producing conv / linear epilogue (saves one pass)
 
+    def _stats_tiles(self, H, W, cout, ksize, stride, pad_lo):
+        """Tiles per frame of a conv whose epilogue emits the next GroupNorm's statistics; 0: no fused statistics."""
+        return ops.conv_tiles_per_frame(H, W, cout, ksize, stride, pad_lo)
+
     def _gn(self, x, p, silu=True):
         gn = getattr(x, '_pgt_gn', None)
         if gn is not None:
@@ -193,26 +197,28 @@ class Engine:
                                              silu=silu)
         return ops.groupnorm_silu(x, self.w[p + '.weight'], self.w[p + '.bias'], self._new(*x.shape), silu=silu)
 
-    def _conv3(self, x, p, cout, out=None, gn_out=False, gn=None, **kw):
+    def _conv3(self, x, p, cout, out=None, gn_out=False, gn=None, gn_silu=True, **kw):
         """3x3 conv; gn: name of the Normalize() whose GroupNorm+SiLU precedes it — applied inside the conv kernel
-        where the halo path exists (the normalised tensor never reaches HBM), as a separate pass otherwise."""
+        where the halo path exists (the normalised tensor never reaches HBM), as a separate pass otherwise.  With
+        gn_silu=False the GroupNorm has no SiLU after it (VQGAN's encoder tail); the fused kernel always applies SiLU,
+        so that case takes the separate pass."""
         Fr, H, W, cin = x.shape
         stride = kw.get('stride', 1)
         fused_ab = None
         if gn is not None:
-            if self.fuse_gn_apply and H >= self.fuse_gn_min_hw and stride == 1 and kw.get('ksize', 3) == 3 and kw.get('pad_lo', 1) == 1 and \
+            if gn_silu and self.fuse_gn_apply and H >= self.fuse_gn_min_hw and stride == 1 and kw.get('ksize', 3) == 3 and kw.get('pad_lo', 1) == 1 and \
                     'act' not in kw and not kw.get('relu_after_res') and ops.conv_gn_supported(H, W, cin, cout):
                 st = getattr(x, '_pgt_gn', None)
                 fused_ab = ops.groupnorm_ab(x, self.w[gn + '.weight'], self.w[gn + '.bias'],
                                             self._new(Fr * 2 * cin, dtype=torch.float32),
                                             stats=st[0] if st else None, chunks_per_frame=st[1] if st else 0)
             else:
-                x = self._gn(x, gn)
+                x = self._gn(x, gn, silu=gn_silu)
         if out is None:
             out = self._new(Fr, H // stride, W // stride, cout)
         stats = None
         if gn_out and self.fuse_gn_stats and cout % 32 == 0 and cout // 32 in (2, 4, 8, 16, 32) and out.is_contiguous():
-            tpf = ops.conv_tiles_per_frame(H, W, cout, kw.get('ksize', 3), stride, kw.get('pad_lo', 1))
+            tpf = self._stats_tiles(H, W, cout, kw.get('ksize', 3), stride, kw.get('pad_lo', 1))
             if tpf > 0:
                 stats = self._new(Fr * tpf * 4 * 64, dtype=torch.float32)      # [tile][32-row quadrant][32 groups][2]
                 out._pgt_gn = (stats, tpf * 4)
@@ -234,12 +240,13 @@ class Engine:
         return ops.linear(x, self.w[p + '.weight'], out, bias=self.w.get(p + '.bias'), N=n, gn_stats=stats, **kw)
 
     # ------------------------------------------------------------------ blocks
-    def td_resblock(self, x, p, cout, gn_next=False, out=None):
-        """TDResnetBlock (`modules/rstt_layers.py:875-904`): 2 x (GN+SiLU -> conv3x3), residual in the
-        second conv's epilogue (1x1 nin_shortcut first when the width changes).  conv1's epilogue also emits the
-        GroupNorm statistics norm2 needs; with gn_next the block output carries them for the next Normalize()."""
+    def td_resblock(self, x, p, cout, gn_next=False, out=None, shortcut='nin_shortcut'):
+        """TDResnetBlock (`modules/rstt_layers.py:875-904`) / VQGAN's ResBlock (`archs/vqgan_arch.py:155-178`,
+        shortcut='conv_out'): 2 x (GN+SiLU -> conv3x3), residual in the second conv's epilogue (the 1x1 shortcut first
+        when the width changes).  conv1's epilogue also emits the GroupNorm statistics norm2 needs; with gn_next the
+        block output carries them for the next Normalize()."""
         h = self._conv3(x, p + '.conv1', cout, gn=p + '.norm1', gn_out=True)
-        sc = self._lin(x, p + '.nin_shortcut', cout) if (p + '.nin_shortcut.weight') in self.w else x
+        sc = self._lin(x, p + '.' + shortcut, cout) if (p + '.' + shortcut + '.weight') in self.w else x
         return self._conv3(h, p + '.conv2', cout, gn=p + '.norm2', residual=sc, gn_out=gn_next, out=out)
 
     def swin_block(self, x, p, heads, shift, gn_next=False, out=None):
@@ -279,6 +286,26 @@ class Engine:
         m = self._lin(y, p + '.mlp.fc1', C, act=ops.ACT_GELU)
         return self._lin(m, p + '.mlp.fc2', C, residual=x, gn_out=gn_next, out=out)
 
+    def _repack_attn_qkv(self):
+        """AttnBlock: q, k and v (1x1 convs of the same normalised input) as one [3C, C] projection."""
+        sd, w = self._sd, self.w
+        for name in list(sd):
+            if name.endswith('.proj_out.weight'):
+                p = name[:-len('.proj_out.weight')]
+                w[p + '.qkv.weight'] = _pack_lin(torch.cat([sd[p + '.%s.weight' % n] for n in 'qkv'], 0).float())
+                w[p + '.qkv.bias'] = torch.cat([sd[p + '.%s.bias' % n] for n in 'qkv'], 0).float().contiguous()
+
+    def attn_block(self, x, p, gn_next=False):
+        """AttnBlock (`archs/tdrqvae_arch.py:179-203`, `archs/vqgan_arch.py:181-240`): GroupNorm (no SiLU) -> q | k | v
+        -> softmax(q k^T C^-1/2) v over all H*W tokens of each frame (one head of width C) -> proj_out + x.  The
+        GroupNorm statistics come from the producing epilogue; with gn_next the output carries them for the next
+        Normalize()."""
+        Fr, H, W, C = x.shape
+        y = self._gn(x, p + '.norm', silu=False)
+        qkv = self._lin(y, p + '.qkv', 3 * C)
+        a = ops.mha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], Fr, H * W, 1, C, self._new(Fr, H, W, C))
+        return self._lin(a, p + '.proj_out', C, residual=x, gn_out=gn_next)
+
     def encoder_layer(self, x, p, heads, depth, gn_next=False, out=None):
         for i in range(depth):
             x = self.swin_block(x, '%s.blocks.%d' % (p, i), heads, 2 if i % 2 == 1 else 0,
@@ -307,6 +334,13 @@ class Engine:
         ops.regroup_frames(self._lin(dec, p + '.tconvdec', 32), tcat[..., 96:], b, P, 32, 0)
         fut = ops.regroup_frames(self._lin(tcat, p + '.tfusion0', 96), self._new(Fr, P, 32), b, P, 32, 1)
         self._lin(fut, p + '.tfusion1', 32, out=cat.view(Fr, P, 2 * C + 32)[..., 2 * C:])
+        return self.sft_tail(cat, dec, p, wgt, gn_next)
+
+    def sft_tail(self, cat, dec, p, wgt, gn_next=False):
+        """The part of Fuse_sft_block PGTFormer (`archs/pgtformer_arch.py:476-484`) and CodeFormer
+        (`archs/codeformer_arch.py:218-226`) share: encode_enc (ResBlock of the concat, 1x1 conv_out shortcut) ->
+        scale / shift branches -> dec + w*(dec*scale + shift) in the epilogue of the last `shift` conv."""
+        C = dec.shape[-1]
         e = p + '.encode_enc'
         h = self._conv3(cat, e + '.conv1', C, gn=e + '.norm1', gn_out=True)
         sc = self._lin(cat, e + '.conv_out', C)
@@ -440,7 +474,7 @@ class Engine:
             lvl += 1
         return h, feats, lvl
 
-    def conv_in(self, x):
+    def conv_in(self, x, p='encoder.conv_in'):
         """encoder.conv_in on the fp32 NCHW frames.  Cin = 3: the kernel builds the patch rows itself; its epilogue also
         yields block 0's GroupNorm statistics."""
         a = self.arch
@@ -451,7 +485,7 @@ class Engine:
             tpf = H * W // 128
             stats = self._new(Fr * tpf * 4 * 64, dtype=torch.float32)
             h._pgt_gn = (stats, tpf * 4)
-        ops.conv_rgb(x, self.w['encoder.conv_in.weight'], self.w['encoder.conv_in.bias'], h, 3, 1, 1, gn_stats=stats)
+        ops.conv_rgb(x, self.w[p + '.weight'], self.w[p + '.bias'], h, 3, 1, 1, gn_stats=stats)
         return h
 
     def _encoder_level(self, h, lvl, feats):
@@ -543,27 +577,27 @@ class Engine:
         Fr, H, W, C = h.shape
         out = self._new(Fr, 2 * H, 2 * W, C)
         stats = None
-        tpf = ops.conv_tiles_per_frame(H, W, C, 2, 1, 1)
+        tpf = self._stats_tiles(H, W, C, 2, 1, 1)
         if self.fuse_gn_stats and tpf > 0 and C // 32 in (2, 4, 8, 16, 32):
             stats = self._new(Fr * 16 * tpf * 64, dtype=torch.float32)     # [frame][phase][tile][quadrant][32][2]
             out._pgt_gn = (stats, 16 * tpf)
         return ops.conv_up2x(h, self.w[p + '.weight'], C, out, bias=self.w[p + '.bias'], gn_stats=stats)
 
-    def decoder_out(self, h):
-        """decoder.norm_out + SiLU + decoder.conv_out -> fp32 NCHW [F, out_ch, H, W]."""
-        a = self.arch
+    def decoder_out(self, h, norm='decoder.norm_out', conv='decoder.conv_out', silu=True, out_ch=None):
+        """norm (GroupNorm) + SiLU (unless silu=False) + conv -> fp32 NCHW [F, out_ch, H, W]."""
+        out_ch = self.arch.out_ch if out_ch is None else out_ch
         Fr, H, W, _ = h.shape
-        out = self._new(Fr, a.out_ch, H, W, dtype=torch.float32)
+        out = self._new(Fr, out_ch, H, W, dtype=torch.float32)
         if self.fuse_conv_out:
-            # norm_out + SiLU + conv_out in one kernel: the normalised 512^2 tensor never reaches HBM
+            # norm + SiLU + conv in one kernel: the normalised 512^2 tensor never reaches HBM
             st = getattr(h, '_pgt_gn', None)
-            ab = ops.groupnorm_ab(h, self.w['decoder.norm_out.weight'], self.w['decoder.norm_out.bias'],
+            ab = ops.groupnorm_ab(h, self.w[norm + '.weight'], self.w[norm + '.bias'],
                                   self._new(Fr * 2 * h.shape[-1], dtype=torch.float32),
                                   stats=st[0] if st else None, chunks_per_frame=st[1] if st else 0)
-            if ops.conv_out_gn(h, ab, self.w['decoder.conv_out.weight'], a.out_ch, self.w.get('decoder.conv_out.bias'),
-                               out) is not None:
+            if ops.conv_out_gn(h, ab, self.w[conv + '.weight'], out_ch, self.w.get(conv + '.bias'), out,
+                               silu=silu) is not None:
                 return out
-        self._conv3(h, 'decoder.conv_out', a.out_ch, out=out, gn='decoder.norm_out', nchw=True)
+        self._conv3(h, conv, out_ch, out=out, gn=norm, gn_silu=silu, nchw=True)
         return out
 
     def parse_pos(self, x):

@@ -151,6 +151,12 @@ def conv_tiles_per_frame(H, W, cout, ksize=3, stride=1, pad_lo=1):
     return int(L.load().pgt_conv_tiles_per_frame(H, W, cout, ksize, stride, pad_lo))
 
 
+def conv_tiles_exact(H, W, cout, ksize=3, stride=1, pad_lo=1):
+    """conv_tiles_per_frame, or 0 when the tile grid does not divide the frame (the fused statistics would then include
+    rows past the frame's edge)."""
+    return int(L.load().pgt_conv_tiles_exact(H, W, cout, ksize, stride, pad_lo))
+
+
 def groupnorm_apply_stats(x, gamma, beta, out, stats, chunks_per_frame, eps=1e-6, silu=True):
     """GroupNorm(32)+SiLU whose statistics were produced by the previous conv / linear epilogue."""
     lib = L.load()
@@ -187,15 +193,20 @@ def groupnorm_ab(x, gamma, beta, ab, stats=None, chunks_per_frame=0, eps=1e-6):
     return ab
 
 
-def conv_out_gn(x, ab, wp, cout, bias, out):
-    """conv3x3(silu(groupnorm(x))) -> fp32 NCHW for the decoder tail (Cin = 64, Cout <= 3); None when not covered."""
+def conv_out_gn(x, ab, wp, cout, bias, out, silu=True):
+    """conv3x3(silu(groupnorm(x))) -> fp32 NCHW for the decoder tail (Cin = 64, Cout <= 3); with silu=False
+    conv3x3(groupnorm(x)) (VQGAN's generator tail).  None when not covered."""
     lib = L.load()
     F, H, W, Cin = x.shape
     assert x.dtype == torch.bfloat16 and x.stride(3) == 1 and x.stride(1) == W * x.stride(2) and \
         (F == 1 or x.stride(0) == H * x.stride(1))
     assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (F, cout, H, W)
-    rc = lib.pgt_conv_out_gn(_p(x), F, H, W, Cin, x.stride(2), _p(ab), _p(wp), wp.stride(0), cout, _p(bias), _p(out),
-                             _stream(x))
+    if silu:
+        rc = lib.pgt_conv_out_gn(_p(x), F, H, W, Cin, x.stride(2), _p(ab), _p(wp), wp.stride(0), cout, _p(bias), _p(out),
+                                 _stream(x))
+    else:
+        rc = lib.pgt_conv_out_gn_act(_p(x), F, H, W, Cin, x.stride(2), _p(ab), _p(wp), wp.stride(0), cout, _p(bias),
+                                     _p(out), 0, _stream(x))
     if rc == -3:
         return None
     L.check(rc)
@@ -455,6 +466,32 @@ def rq_embed(idx, d0, d1, codebooks, out, ldi, ldd):
     L.check(lib.pgt_rq_embed(_p(idx), ldi, ldd, T, d0, d1, _p(codebooks), cb_stride, E, _p(out), ldo, _dt(out),
                              _stream(out)))
     return out
+
+
+def vq_stats(z, codebook, idx, HW, beta, scalars, zq_nchw=None, zq_bf16=None, min_enc=None, scores=None, usage=None):
+    """VectorQuantizer.forward's outputs after the argmin (vq.cu): z fp32 [T, E] rows (T = b * HW), codebook fp32 [K, E],
+    idx int64 [T].  Writes the straight-through z + (e - z) (fp32 NCHW [b, E, h, w] and / or bf16 [T, E] rows), the
+    one-hot min_enc [T, K], scores [T], adds the counts to usage (int32 [K]) and writes scalars fp32 [3] = (loss,
+    perplexity, mean_distance).  Outputs left None are not written."""
+    lib = L.load()
+    T, E = z.shape
+    K = codebook.shape[0]
+    assert z.dtype == torch.float32 and z.is_contiguous() and codebook.dtype == torch.float32 and codebook.is_contiguous()
+    assert codebook.shape[1] == E and idx.dtype == torch.int64 and idx.is_contiguous() and idx.numel() == T
+    assert scalars.dtype == torch.float32 and scalars.numel() >= 3 and scalars.is_contiguous()
+    assert zq_nchw is None or (zq_nchw.dtype == torch.float32 and zq_nchw.is_contiguous() and zq_nchw.numel() == T * E
+                               and zq_nchw.shape[1] == E)
+    assert zq_bf16 is None or (zq_bf16.dtype == torch.bfloat16 and zq_bf16.is_contiguous() and zq_bf16.numel() == T * E)
+    assert min_enc is None or (min_enc.dtype == torch.float32 and min_enc.is_contiguous() and min_enc.numel() == T * K)
+    assert scores is None or (scores.dtype == torch.float32 and scores.is_contiguous() and scores.numel() == T)
+    assert usage is None or (usage.dtype == torch.int32 and usage.is_contiguous() and usage.numel() == K)
+    for t in (idx, zq_nchw, zq_bf16, min_enc, scores, usage, scalars):
+        assert t is None or t.device == z.device
+    hist = torch.zeros(K, dtype=torch.int32, device=z.device)
+    ws = torch.empty(max(int(lib.pgt_vq_stats_ws_doubles(T, E)), 1), dtype=torch.float64, device=z.device)
+    L.check(lib.pgt_vq_stats(_p(z), T, E, int(HW), _p(codebook), K, _p(idx), float(beta), _p(zq_nchw), _p(zq_bf16),
+                             _p(min_enc), _p(scores), _p(usage), _p(hist), _p(ws), _p(scalars), _stream(z)))
+    return scalars
 
 
 def adain(q, style, out, eps=1e-5):

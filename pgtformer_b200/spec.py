@@ -397,3 +397,178 @@ def build_tdrqvae_spec(network_g):
     for p in ('tdswin_pre', 'tdswin_post'):
         _swin3d_layer(s, p, e, a.stages_atten, a.num_head, a.window_size)
     return a, s
+
+
+# --------------------------------------------------------------------------- VQGAN / CodeFormer (archs/vqgan_arch.py,
+# archs/codeformer_arch.py)
+CODEFORMER_CHANNELS = {'16': 512, '32': 256, '64': 256, '128': 128, '256': 128, '512': 64}   # codeformer_arch.py:268-275
+CODEFORMER_ENC_BLOCK = {'512': 2, '256': 5, '128': 8, '64': 11, '32': 14, '16': 18}         # :278
+CODEFORMER_GEN_BLOCK = {'16': 6, '32': 9, '64': 12, '128': 15, '256': 18, '512': 21}        # :280
+
+
+def _res_block(s, p, cin, cout):
+    """ResBlock (`archs/vqgan_arch.py:155-178`): the 1x1 shortcut is `conv_out`."""
+    _norm(s, p + '.norm1', cin)
+    _conv(s, p + '.conv1', cin, cout, 3)
+    _norm(s, p + '.norm2', cout)
+    _conv(s, p + '.conv2', cout, cout, 3)
+    if cin != cout:
+        _conv(s, p + '.conv_out', cin, cout, 1)
+
+
+class VQGANArch:
+    """Resolved constants of VQAutoEncoder (`archs/vqgan_arch.py:344-411`) and, with codeformer=True, CodeFormer
+    (`archs/codeformer_arch.py:229-286`).  `enc_blocks` / `gen_blocks` are the flat `encoder.blocks` / `generator.blocks`
+    ModuleLists as (kind, cin, cout, res) tuples, kind in conv_in, res, attn, down, up, norm, conv_out; `res` is the
+    constructor's curr_res (img_size-relative), which places the AttnBlocks.  Raises ValueError for what the reference
+    rejects and for what the CUDA kernels cannot run."""
+
+    def __init__(self, g, codeformer=False):
+        g = dict(g)
+        self.codeformer = codeformer
+        self.img_size = int(g.get('img_size', 512))
+        self.nf = int(g.get('nf', 64))
+        self.ch = self.nf                                              # Engine.conv_in's name for the first width
+        self.ch_mult = tuple(int(m) for m in g.get('ch_mult', [1, 2, 2, 4, 4, 8]))
+        self.quantizer = g.get('quantizer', 'nearest')
+        self.res_blocks = int(g.get('res_blocks', 2))
+        self.attn_resolutions = tuple(int(r) for r in g.get('attn_resolutions', [16]))
+        self.n_embed = int(g.get('codebook_size', 1024))
+        self.embed_dim = int(g.get('emb_dim', 256))
+        self.beta = float(g.get('beta', 0.25))
+        self.last_silu = bool(g.get('last_silu', False))
+        self.num_levels = len(self.ch_mult)
+        self.down = 2 ** (self.num_levels - 1)
+        self.level_ch = tuple(self.nf * m for m in self.ch_mult)
+        if self.quantizer == 'gumbel':
+            raise ValueError("quantizer='gumbel': its eval forward draws Gumbel noise from torch's RNG; only 'nearest' "
+                             "runs on the GPU")
+        if self.quantizer != 'nearest':
+            raise ValueError("quantizer must be 'nearest', got %r" % (self.quantizer,))
+        if self.nf != 64:
+            raise ValueError('nf = %d: the CUDA path is built for nf = 64 (the 64-channel convs and the generator tail)'
+                             % self.nf)
+        if any(c % 32 for c in self.level_ch):
+            raise ValueError('GroupNorm(32): every level width must be a multiple of 32, got %s' % (self.level_ch,))
+        if self.embed_dim % 32 or self.embed_dim > 512 or self.n_embed % 256:
+            raise ValueError('emb_dim %d, codebook_size %d: the quantiser kernels take emb_dim a multiple of 32 up to 512 '
+                             'and codebook_size a multiple of 256' % (self.embed_dim, self.n_embed))
+        enc, res = [('conv_in', 3, self.nf, self.img_size)], self.img_size
+        cin = self.nf
+        for i in range(self.num_levels):                               # Encoder.__init__ (vqgan_arch.py:252-282)
+            cout = self.level_ch[i]
+            for _ in range(self.res_blocks):
+                enc.append(('res', cin, cout, res))
+                cin = cout
+                if res in self.attn_resolutions:
+                    enc.append(('attn', cin, cin, res))
+            if i != self.num_levels - 1:
+                enc.append(('down', cin, cin, res))
+                res //= 2
+        enc += [('res', cin, cin, res), ('attn', cin, cin, res), ('res', cin, cin, res), ('norm', cin, cin, res)]
+        if self.last_silu:
+            raise ValueError('last_silu=True adds an nn.SiLU block the CUDA path does not run')
+        enc.append(('conv_out', cin, self.embed_dim, res))
+        gen, res = [], self.img_size // self.down                      # Generator.__init__ (:303-334)
+        cin = self.level_ch[-1]
+        gen += [('conv_in', self.embed_dim, cin, res), ('res', cin, cin, res), ('attn', cin, cin, res),
+                ('res', cin, cin, res)]
+        for i in reversed(range(self.num_levels)):
+            cout = self.level_ch[i]
+            for _ in range(self.res_blocks):
+                gen.append(('res', cin, cout, res))
+                cin = cout
+                if res in self.attn_resolutions:
+                    gen.append(('attn', cin, cin, res))
+            if i != 0:
+                gen.append(('up', cin, cin, res))
+                res *= 2
+        gen += [('norm', cin, cin, res), ('conv_out', cin, 3, res)]
+        self.enc_blocks, self.gen_blocks = tuple(enc), tuple(gen)
+        widths = {b[1] for b in enc + gen if b[0] == 'attn'}
+        if not widths <= set(ATTN_WIDTHS):
+            raise ValueError('AttnBlock widths %s: the attention kernel takes %s' % (sorted(widths), ATTN_WIDTHS))
+        self.code_shape = (self.img_size // self.down, self.img_size // self.down, 1)
+        if not codeformer:
+            return
+        self.dim_embd = int(g.get('dim_embd', 512))
+        self.n_head = int(g.get('n_head', 8))
+        self.n_layers = int(g.get('n_layers', 9))
+        self.latent_size = int(g.get('latent_size', 256))
+        self.connect_list = [str(c) for c in g.get('connect_list', ['32', '64', '128', '256'])]
+        hw = self.code_shape[0] * self.code_shape[1]
+        if self.latent_size != hw:
+            raise ValueError('latent_size %d != (img_size / 2^(levels - 1))^2 = %d: position_emb has latent_size rows, '
+                             'one per token' % (self.latent_size, hw))
+        if self.embed_dim != 256 or self.code_shape[0] != 16:
+            # feat_emb is nn.Linear(256, dim_embd) and forward reshapes the codes to [b, 16, 16, 256] (:257, :345)
+            raise ValueError('CodeFormer runs emb_dim = 256 on a 16 x 16 latent only (codeformer_arch.py:257, 345)')
+        if self.dim_embd % self.n_head or self.dim_embd // self.n_head != 64:
+            raise ValueError('dim_embd %d with %d heads: the transformer kernel takes head width 64'
+                             % (self.dim_embd, self.n_head))
+        self.fuse_enc, self.fuse_gen = {}, {}                          # flat block index -> size key
+        for key in self.connect_list:
+            if key not in CODEFORMER_CHANNELS:
+                raise ValueError('connect_list entry %r: CodeFormer has fusion layers for %s'
+                                 % (key, sorted(CODEFORMER_CHANNELS, key=int)))
+            ei, gi = CODEFORMER_ENC_BLOCK[key], CODEFORMER_GEN_BLOCK[key]
+            c = CODEFORMER_CHANNELS[key]
+            # the reference keys a tapped feature by its width (`codeformer_arch.py:316, 361`): the block at the table's
+            # index must give the key's resolution and CodeFormer's channel count for it
+            if ei >= len(enc) or gi >= len(gen) or enc[ei][0] != 'res' or gen[gi][0] != 'res' or \
+                    enc[ei][2] != c or gen[gi][2] != c or enc[ei][3] != int(key) or gen[gi][3] != int(key):
+                raise ValueError('connect_list entry %r does not fit this encoder / generator' % key)
+            self.fuse_enc[ei], self.fuse_gen[gi] = key, key
+
+
+def _vqgan_blocks(s, prefix, blocks):
+    for i, (kind, cin, cout, _) in enumerate(blocks):
+        p = '%s.blocks.%d' % (prefix, i)
+        if kind in ('conv_in', 'conv_out'):
+            _conv(s, p, cin, cout, 3)
+        elif kind == 'res':
+            _res_block(s, p, cin, cout)
+        elif kind == 'attn':
+            _attn_block(s, p, cin)
+        elif kind in ('down', 'up'):
+            _conv(s, p + '.conv', cin, cin, 3)
+        else:
+            _norm(s, p, cin)
+
+
+def build_vqgan_spec(g, codeformer=False):
+    """State-dict layout of VQAutoEncoder (`archs/vqgan_arch.py:344-391`), or with codeformer=True of CodeFormer
+    (`archs/codeformer_arch.py:229-286`), from the constructor keywords."""
+    a = VQGANArch(g, codeformer)
+    s = Spec()
+    if codeformer:
+        s.add('position_emb', (a.latent_size, a.dim_embd), 'pos_emb')
+    _vqgan_blocks(s, 'encoder', a.enc_blocks)
+    s.add('quantize.embedding.weight', (a.n_embed, a.embed_dim), 'codebook_nopad')
+    _vqgan_blocks(s, 'generator', a.gen_blocks)
+    if not codeformer:
+        return a, s
+    _linear(s, 'feat_emb', 256, a.dim_embd)
+    for i in range(a.n_layers):
+        p = 'ft_layers.%d' % i
+        s.add(p + '.self_attn.in_proj_weight', (3 * a.dim_embd, a.dim_embd), 'linear_w')
+        s.add(p + '.self_attn.in_proj_bias', (3 * a.dim_embd,), 'bias')
+        _linear(s, p + '.self_attn.out_proj', a.dim_embd, a.dim_embd)
+        _linear(s, p + '.linear1', a.dim_embd, 2 * a.dim_embd)
+        _linear(s, p + '.linear2', 2 * a.dim_embd, a.dim_embd)
+        _norm(s, p + '.norm1', a.dim_embd)
+        _norm(s, p + '.norm2', a.dim_embd)
+    _norm(s, 'idx_pred_layer.0', a.dim_embd)
+    _linear(s, 'idx_pred_layer.1', a.dim_embd, a.n_embed, bias=False)
+    for key in a.connect_list:                                         # Fuse_sft_block (:200-213)
+        c = CODEFORMER_CHANNELS[key]
+        p = 'fuse_convs_dict.' + key
+        _res_block(s, p + '.encode_enc', 2 * c, c)
+        for br in ('scale', 'shift'):
+            _conv(s, '%s.%s.0' % (p, br), c, c, 3)
+            _conv(s, '%s.%s.2' % (p, br), c, c, 3)
+    return a, s
+
+
+def build_codeformer_spec(g):
+    return build_vqgan_spec(g, codeformer=True)

@@ -35,25 +35,10 @@ class TDRQVAEEngine(Engine):
             elif t.dtype.is_floating_point and t.dim() == 1:
                 w[name] = t.float().contiguous()
         w['codebook'] = self._f32('quantizer.codebooks.0.weight')
-        # AttnBlock: q, k and v (1x1 convs of the same normalised input) as one [3C, C] projection
-        for name in list(sd):
-            if name.endswith('.proj_out.weight'):
-                p = name[:-len('.proj_out.weight')]
-                w[p + '.qkv.weight'] = _pack_lin(torch.cat([sd[p + '.%s.weight' % n] for n in 'qkv'], 0).float())
-                w[p + '.qkv.bias'] = torch.cat([sd[p + '.%s.bias' % n] for n in 'qkv'], 0).float().contiguous()
+        self._repack_attn_qkv()
         self.swin = {p: pack_blocks(lambda k, p=p: sd.get(p + '.' + k), self.arch.stages_atten) for p in SWIN_LAYERS}
 
     # ------------------------------------------------------------------ blocks
-    def attn_block(self, x, p, gn_next=False):
-        """AttnBlock (`archs/tdrqvae_arch.py:179-203`): GroupNorm (no SiLU) -> q | k | v -> softmax(q k^T C^-1/2) v over
-        all H*W tokens of each frame (one head of width C) -> proj_out + x.  The GroupNorm statistics come from the
-        producing epilogue; with gn_next the output carries them for the next Normalize()."""
-        Fr, H, W, C = x.shape
-        y = self._gn(x, p + '.norm', silu=False)
-        qkv = self._lin(y, p + '.qkv', 3 * C)
-        a = ops.mha(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], Fr, H * W, 1, C, self._new(Fr, H, W, C))
-        return self._lin(a, p + '.proj_out', C, residual=x, gn_out=gn_next)
-
     def encoder(self, x):
         """Encoder.forward (`archs/tdrqvae_arch.py:650-680`); x fp32 NCHW [F,3,H,W] -> (h [F,H/16,W/16,z], [])."""
         a = self.arch

@@ -69,6 +69,10 @@ def synth_tensor(name, shape, kind, dtype, seed=0, window=None):
         w = torch.randn(shape, generator=g)
         w[-1].zero_()
         return w
+    if kind == 'codebook_nopad':                 # VQGAN's nn.Embedding: N(0,1) init, no padding row
+        return torch.randn(shape, generator=g)
+    if kind == 'pos_emb':                        # non-zero (the reference initialises zeros, which hides indexing errors)
+        return 0.5 * torch.randn(shape, generator=g)
     if kind == 'zeros':
         return torch.zeros(shape)
     raise ValueError(kind)
