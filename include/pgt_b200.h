@@ -117,16 +117,6 @@ int pgt_conv_out_gn(const void* x, int F, int H, int W, int Cin, int ldx, const 
 int pgt_conv_out_gn_act(const void* x, int F, int H, int W, int Cin, int ldx, const float* gn_ab, const void* Wp, int ldw,
                         int Cout, const float* bias, float* out, int silu, void* stream);
 
-/* ---- GroupNorm(32)+SiLU of the INPUT fused into the 3x3 / stride 1 / pad 1 conv: the normalised activation is never
- * written to HBM — the kernel applies y = silu(x * a[f,c] + b[f,c]) to each input slab in shared memory (bit-identical
- * to pgt_groupnorm_silu's apply pass) before the MMAs read it.  gn_ab: fp32 [F][2][Cin] from pgt_groupnorm_ab.
- * Available where the halo-reuse kernel is (pgt_conv_gn_supported: Cout <= 128, Hin >= 16, Win >= 8, Cin % 8 == 0);
- * PGT_ERR_UNSUPPORTED otherwise.  Replaces  Normalize -> swish -> conv  of TDResnetBlock (modules/rstt_layers.py:
- * 875-904), ResBlock (archs/pgtformer_arch.py:421-432) and norm_out -> conv_out (archs/tdcrqvae3_arch.py:569-572). */
-int pgt_conv_gn_supported(int Hin, int Win, int Cin, int Cout);
-int pgt_conv_gn_bf16(const void* x, int F, int Hin, int Win, int Cin, int ldx, const float* gn_ab, const void* Wp,
-                     int ldw, int Cout, const pgt_epilogue* ep, void* stream);
-
 /* ---- nearest-x2 upsample + 3x3 conv as ONE op, without materialising the upsampled tensor: the output
  * pixel (2y+py, 2x+px) only sees a 2x2 neighbourhood of the source, so the op is four 2x2 convolutions
  * (one per output phase) over the SOURCE resolution with tap-summed weights: 4/9 of the FLOPs, 1/4 of the
@@ -168,7 +158,7 @@ int pgt_groupnorm_apply_stats(const void* x, int ldx, int F, int HW, int C, cons
                               float* ws, void* stream);
 
 /* GroupNorm statistics -> per-(frame, channel) affine terms only: ab[f][0][c] = rstd*gamma, ab[f][1][c] = beta -
- * mean*rstd*gamma (fp32 [F][2][C]), for pgt_conv_gn_bf16.  stats/chunks_per_frame as in pgt_groupnorm_apply_stats, or
+ * mean*rstd*gamma (fp32 [F][2][C]), for pgt_conv_out_gn[_act].  stats/chunks_per_frame as in pgt_groupnorm_apply_stats, or
  * stats == NULL to compute them from x (ws: pgt_groupnorm_ws_floats floats). */
 int pgt_groupnorm_ab(const void* x, int ldx, int F, int HW, int C, const float* gamma, const float* beta, float eps,
                      const float* stats, int chunks_per_frame, float* ws, float* ab, void* stream);
@@ -215,11 +205,10 @@ int pgt_window_attention(const void* qkv, int ldqkv, int clips, int H, int W, in
  * of the qkv matrix (wrapped windows of a shifted block: 2 or 4 partial boxes), QK^T and PV run as wgmma with S / P / O
  * in registers, results are stored to the tokens' output rows.  tab: fp16 [4][heads][6][48][8] bias tables
  * (pgtformer_b200/ops.py::window_tables — the relative-position bias in the row order of the four box layouts, times
- * log2 e; the {0,-100} shift mask is not in the table, the kernel adds it in fp32).  mode_n64: for d = 32 run P V with
- * N = 64 instead of a half-atom N = 32 operand view.
+ * log2 e; the {0,-100} shift mask is not in the table, the kernel adds it in fp32).
  * Returns PGT_ERR_UNSUPPORTED unless heads == 8, d in {32, 64}, C % 128 == 0, shift in {0, 2}. */
 int pgt_window_attention_tc(const void* qkv, int ldqkv, int clips, int H, int W, int C, int heads, int shift,
-                            const void* tab, void* out, int ldo, int mode_n64, void* stream);
+                            const void* tab, void* out, int ldo, void* stream);
 
 /* ---- generic 3-D shifted-window attention core of the Video-Swin BasicLayer (window3d.cu; modules/swin.py:136-166,
  * 214-250, 309-323; used by TDRQVAE, archs/tdrqvae_arch.py:834-835): window (wd, wh, ww) with wd*wh*ww <= 128, shift

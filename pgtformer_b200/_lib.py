@@ -37,9 +37,6 @@ SIGNATURES = {
     'pgt_linear_bf16': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, POINTER(Epilogue), c_void_p]),
     'pgt_conv_bf16': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
                               c_int, POINTER(Epilogue), c_void_p]),
-    'pgt_conv_gn_supported': (c_int, [c_int, c_int, c_int, c_int]),
-    'pgt_conv_gn_bf16': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
-                                 c_void_p]),
     'pgt_conv_out_gn': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
                                 c_void_p, c_void_p]),
     'pgt_conv_out_gn_act': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
@@ -66,7 +63,7 @@ SIGNATURES = {
     'pgt_window_attention': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                      c_int, c_void_p]),
     'pgt_window_attention_tc': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
-                                        c_int, c_int, c_void_p]),
+                                        c_int, c_void_p]),
     'pgt_window3d_attention': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                        c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     'pgt_mha_fwd': (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,

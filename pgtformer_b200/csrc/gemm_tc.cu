@@ -2,7 +2,7 @@
 //
 //   out[rows, N] = epilogue( A[rows, K] * W[N, K]^T )          bf16 operands, fp32 accumulate in registers
 //
-// Persistent, warp-specialised kernels (384 threads = three warpgroups; the GroupNorm-fused halo variant keeps 320 + 128):
+// Persistent, warp-specialised kernels (384 threads = three warpgroups):
 //   warps 0..7  two consumer warpgroups, raised to CONSUMER_REGS registers with setmaxnreg: warpgroup h issues wgmma
 //               64 x BN x 16 for rows [64h, 64h + 64) of the 128-row tile over the whole k loop, then runs the epilogue:
 //               the accumulators go through a 128 x 64 fp32 shared-memory exchange (one row per thread, 32 columns per
@@ -15,14 +15,14 @@
 //     warps 10, 11 idle (setmaxnreg acts on whole warpgroups)
 // Pipelines: smem full/empty ring (TMA <-> wgmma) and a staging ring of 4 slots (2 at BN = 256) (epilogue <-> DMA warp);
 // the producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
-// conv_halo_kernel<BN, false> runs the consumers PING-PONG instead: each warpgroup owns alternate tiles (all 128 rows)
+// conv_halo_kernel<BN> runs the consumers PING-PONG instead: each warpgroup owns alternate tiles (all 128 rows)
 // and its epilogue (epilogue_tile_wg) runs under the other warpgroup's MMAs.
 // Consumer waits do not time out (a reachable trap would hold ptxas to the launch-bound register count); the producer
 // and the DMA warp wait with a bound, and the producer ends by waiting until every stage it filled has been released,
 // so a transaction that never completes traps the launch instead of hanging it.
 //
 // Kernels in this file: gemm_tc_kernel<BN> (linear / generic implicit-GEMM conv; BN = 64, 128 or 256),
-// conv_halo_kernel<BN, GN> (3x3 and upsample-phase convs with Cout <= 128: one halo slab serves every tap).
+// conv_halo_kernel<BN> (3x3 and upsample-phase convs with Cout <= 128: one halo slab serves every tap).
 //
 // The A operand is produced by TMA in three addressing modes:
 //   LINEAR   2-D map [K, rows]
@@ -88,8 +88,6 @@ struct GemmParams {
   float* gn_stats;       // optional: per-(tile, group) partial (sum, sumsq) of the OUTPUT for the next GroupNorm(32)
   int gn_cpg;            // channels per group = N / 32
   int ntaps, tap_kw, tap_oy, tap_ox;   // halo conv: 9 taps of a 3x3, or the 4 taps (kw = 2) of an upsample phase at slab offset (oy, ox)
-  const float* gn_ab;    // halo conv only: GroupNorm+SiLU of the INPUT applied to the slab in smem, [F][2][gn_c] (a, b)
-  int gn_c;              //   channels of that GroupNorm (= Cin)
   int gn_tpf;            // > 0: statistics rows are laid out [frame][gn_fstride] (several launches share one buffer)
   int gn_fstride;        //      chunk = (m_blk / gn_tpf) * gn_fstride + (m_blk % gn_tpf) * 4 + quad
   int relu_after_res;    // ResNet BasicBlock: out = relu(conv + shortcut) — ReLU applied after the residual add
@@ -809,19 +807,19 @@ constexpr int HALO_PITCH = (HALO_TW + 2) * 128;                     // bytes bet
 constexpr int HALO_A_BYTES = (HALO_TH + 2) * HALO_PITCH;            // 23040
 constexpr int HALO_A_STRIDE = ((HALO_A_BYTES + 1023) / 1024) * 1024; // 23552: keep every slab 1024-aligned
 
-// The ping-pong variant (GN = false) gives each consumer warpgroup its own exchange (2 x 18 KB instead of 34 KB).  At
-// BN = 128 that costs a weight stage: the ring keeps 4 of 16 KB.  A 3x3 tap of BN = 128 is never resident (9 > 5) and
-// the 4-tap upsample phases with Cin <= 64 still are; with the previous schedule, 4 stages timed the same as 5 on every
-// BN = 128 shape of tools/micro_conv.py halo (H100 80GB HBM3, 700 W).  The staging ring keeps its 4 slots, because an
-// SFT item takes two of them.
-template <int BN, bool GN>
+// Each consumer warpgroup has its own accumulator exchange (2 x 18 KB, where one shared exchange takes 34 KB).  At
+// BN = 128 that costs a weight stage: the ring keeps 4 of 16 KB instead of 5.  A 3x3 tap of BN = 128 is never resident
+// (9 > 5) and the 4-tap upsample phases with Cin <= 64 still are; under the earlier schedule with one shared exchange,
+// 4 stages timed the same as 5 on every BN = 128 shape of tools/micro_conv.py halo (H100 80GB HBM3, 700 W).  The
+// staging ring keeps its 4 slots, because an SFT item takes two of them.
+template <int BN>
 struct HaloCfg {
   static constexpr int B_BYTES = BN * 128;
   static constexpr int A_STAGES = 2;
-  static constexpr int B_STAGES = (BN == 64) ? 9 : GN ? 5 : 4;
+  static constexpr int B_STAGES = (BN == 64) ? 9 : 4;
   static constexpr int SLOTS = staging_slots<BN>();
   static constexpr int STAGING_BYTES = SLOTS * PANEL_BYTES;
-  static constexpr int XCH = GN ? XCH_BYTES : 2 * XCH_WG_BYTES;
+  static constexpr int XCH = 2 * XCH_WG_BYTES;
   static constexpr int SMEM_BYTES = A_STAGES * HALO_A_STRIDE + B_STAGES * B_BYTES + STAGING_BYTES + XCH + 512 + 1024;
   static_assert(SMEM_BYTES <= 232448, "halo conv smem budget");
 };
@@ -834,20 +832,14 @@ __device__ __forceinline__ void ring_skip(int& s, uint32_t& ph, int n) {
   s = t % S;
 }
 
-// The GroupNorm-fused variant keeps its own layout without setmaxnreg: warps 0..9 as above, then four GroupNorm warps.
-constexpr int HALO_GN_THREADS = 128;             // extra warps of the GroupNorm-fused variant
-constexpr int HALO_GN_FIRST = (DMA_WARP + 1) * 32;
-template <bool GN>
-constexpr int halo_threads() { return GN ? HALO_GN_FIRST + HALO_GN_THREADS : GEMM_THREADS; }
-
-template <int BN, bool GN>
-__global__ void __launch_bounds__(halo_threads<GN>(), 1)
+template <int BN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
                  const __grid_constant__ CUtensorMap tmX, const GemmParams p) {
-  using Cfg = HaloCfg<BN, GN>;
+  using Cfg = HaloCfg<BN>;
   constexpr int AS = Cfg::A_STAGES, BS = Cfg::B_STAGES;
-  constexpr int RELEASERS = GN ? EPI_WARPS : 4;   // warps releasing a ring stage: both warpgroups, or the ping-pong owner
+  constexpr int RELEASERS = 4;                    // warps releasing a ring stage: the four of the tile's warpgroup
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
@@ -861,7 +853,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* b_empty = bars + 2 * AS + BS;
   uint64_t* res_bar = bars + 2 * AS + 2 * BS;                          // [Cfg::SLOTS]
   uint64_t* slot_ready = res_bar + Cfg::SLOTS;                         // [Cfg::SLOTS]
-  uint64_t* a_ready = slot_ready + Cfg::SLOTS;                         // [AS] GN variant: slab normalised in place
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -874,7 +865,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (p.fast_epi) tma_prefetch_desc(&tmO);
     if (p.has_res_map) tma_prefetch_desc(&tmR);
     if (p.fast_epi && p.epi_mode == PGT_EPI_SFT) tma_prefetch_desc(&tmX);
-    for (int i = 0; i < AS; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], RELEASERS); mbar_init(&a_ready[i], HALO_GN_THREADS); }
+    for (int i = 0; i < AS; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], RELEASERS); }
     for (int i = 0; i < BS; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], RELEASERS); }
     for (int i = 0; i < Cfg::SLOTS; ++i) {
       mbar_init(&res_bar[i], 1);
@@ -885,7 +876,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   __syncthreads();
 
   if (warp >= EPI_WARPS) {
-    if constexpr (!GN) setmaxnreg_dec<PRODUCER_REGS>();
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == PRODUCER_WARP) {
       // ---------------------------------------------------------------- TMA producer
       int as = 0, bs = 0;
@@ -941,64 +932,8 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     } else if (warp == DMA_WARP) {
       const EpiCtx ctx{staging, xch, res_bar, slot_ready};
       epilogue_dma_loop<BN>(p, ctx, tmO, tmR, tmX, lane, num_tiles);
-    } else if (GN) {
-      // ------------------------------------------------------------------ GroupNorm + SiLU of the input, in the slab
-      // y = silu(x * a[f,c] + b[f,c]) exactly as gn_apply_kernel computes it, applied to every in-image pixel of the
-      // slab once it has landed (the zero padding TMA wrote for out-of-image pixels must stay zero), then handed to the
-      // MMA lane through a_ready.  Thread = one 16-byte channel chunk column (fixed 8 channels) x every 16th pixel row.
-      const int t = threadIdx.x - HALO_GN_FIRST;
-      const int c = t & 7, rl = t >> 3;
-      int as = 0;
-      uint32_t aph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int n0, y0, x0;
-        decode_conv_tile(p, tile / p.n_tiles, n0, y0, x0);
-        for (int cb = 0; cb < p.cin_blocks; ++cb) {
-          float ah[8], bh[8];
-          const int ch0 = cb * BK + c * 8;
-          if (ch0 < p.gn_c) {
-            const float4* pa = reinterpret_cast<const float4*>(p.gn_ab + ((size_t)n0 * 2 + 0) * p.gn_c + ch0);
-            const float4* pb = reinterpret_cast<const float4*>(p.gn_ab + ((size_t)n0 * 2 + 1) * p.gn_c + ch0);
-            const float4 a0 = __ldg(pa), a1 = __ldg(pa + 1), b0 = __ldg(pb), b1 = __ldg(pb + 1);
-            ah[0] = a0.x; ah[1] = a0.y; ah[2] = a0.z; ah[3] = a0.w; ah[4] = a1.x; ah[5] = a1.y; ah[6] = a1.z; ah[7] = a1.w;
-            bh[0] = b0.x; bh[1] = b0.y; bh[2] = b0.z; bh[3] = b0.w; bh[4] = b1.x; bh[5] = b1.y; bh[6] = b1.z; bh[7] = b1.w;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { ah[j] *= 0.5f; bh[j] *= 0.5f; }     // silu(v) = h + h tanh(h), h = v / 2
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { ah[j] = 0.f; bh[j] = 0.f; }         // channel padding stays zero
-          }
-          mbar_wait(&a_full[as], aph);
-          uint8_t* slab = smem_a + as * HALO_A_STRIDE;
-#pragma unroll 4
-          for (int j = 0; j < 12; ++j) {
-            const int r = rl + 16 * j;
-            if (r >= (HALO_TH + 2) * (HALO_TW + 2)) break;
-            const int sy = r / (HALO_TW + 2), sx = r - sy * (HALO_TW + 2);
-            if ((unsigned)(y0 - 1 + sy) >= (unsigned)p.H || (unsigned)(x0 - 1 + sx) >= (unsigned)p.W) continue;
-            uint4* ptr = reinterpret_cast<uint4*>(slab + r * 128 + ((c ^ (r & 7)) << 4));
-            const uint4 u = *ptr;
-            const float2 q0 = unpack_bf16x2(u.x), q1 = unpack_bf16x2(u.y), q2 = unpack_bf16x2(u.z), q3 = unpack_bf16x2(u.w);
-            float v[8] = {q0.x, q0.y, q1.x, q1.y, q2.x, q2.y, q3.x, q3.y};
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const float h = fmaf(v[e], ah[e], bh[e]);
-              float th;
-              asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(h));
-              v[e] = fmaf(h, th, h);
-            }
-            uint4 o;
-            o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]);
-            o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
-            *ptr = o;
-          }
-          fence_proxy_async();
-          mbar_arrive(&a_ready[as]);
-          if (++as == AS) { as = 0; aph ^= 1; }
-        }
-      }
     }
-  } else if constexpr (!GN) {
+  } else {
     // ------------------------------------------------------------------ ping-pong consumer warpgroups
     // The j-th tile of the CTA belongs to warpgroup j & 1, which multiplies all 128 rows (two m64 row blocks on one B
     // descriptor; block 1 = image rows [8, 16) of the patch, 8 slab rows further down) and runs the whole epilogue.
@@ -1079,64 +1014,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       epilogue_tile_wg<BN>(p, ctx, warp & 3, PP_XCH_BAR + wg, tile, k, acc);
       if (has_next) named_bar_arrive(PP_EPI_BAR + (wg ^ 1), 256);
       k += items;
-    }
-  } else {
-    // ------------------------------------------------------------------ GroupNorm-fused variant: consumer warpgroups
-    // Warpgroup h multiplies tile rows [64h, 64h + 64) = image rows [8h, 8h + 8) of the patch: its view of a tap starts
-    // 8 slab rows further down.
-    const EpiCtx ctx{staging, xch, res_bar, slot_ready};
-    const int wg = warp >> 2;
-    const uint32_t a_view = smem_u32(smem_a) + wg * 8 * HALO_PITCH;
-    const uint32_t b_base = smem_u32(smem_b);
-    int as = 0, bs = 0;
-    uint32_t aph = 0, bph = 0;
-    int k = 0;
-    bool first = true;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      float acc[BN / 2];
-      for (int cb = 0; cb < p.cin_blocks; ++cb) {
-        mbar_wait_spin(GN ? &a_ready[as] : &a_full[as], aph);
-        const uint64_t da0 = wgmma_desc_k_sw128(a_view + as * HALO_A_STRIDE, HALO_PITCH);
-        auto tap_desc = [&](int t) -> uint64_t {       // slab row offset of tap t, in 16-byte descriptor units
-          const int dy = t / p.tap_kw, dx = t - dy * p.tap_kw;
-          return da0 + (uint64_t)(((dy + p.tap_oy) * (HALO_TW + 2) + dx + p.tap_ox) * 8);
-        };
-        if (p.b_resident) {
-          if (first) {
-            for (int t = 0; t < p.ntaps * p.cin_blocks; ++t) mbar_wait_spin(&b_full[t], 0);
-            first = false;
-          }
-          wgmma_fence();
-          for (int t = 0; t < p.ntaps; ++t) {
-            const uint64_t da = tap_desc(t);
-            const uint64_t db = wgmma_desc_k_sw128(b_base + (cb * p.ntaps + t) * Cfg::B_BYTES);
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk) wgmma_bf16<BN>(acc, da + 2 * kk, db + 2 * kk, (cb | t | kk) != 0 ? 1u : 0u);
-          }
-          wgmma_commit();
-          wgmma_wait<0>();
-        } else {
-          int prev = -1;
-          for (int t = 0; t < p.ntaps; ++t) {
-            mbar_wait_spin(&b_full[bs], bph);
-            const uint64_t da = tap_desc(t);
-            const uint64_t db = wgmma_desc_k_sw128(b_base + bs * Cfg::B_BYTES);
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk) wgmma_bf16<BN>(acc, da + 2 * kk, db + 2 * kk, (cb | t | kk) != 0 ? 1u : 0u);
-            wgmma_commit();
-            wgmma_wait<1>();                             // the previous tap's weight stage is free
-            if (prev >= 0) release_stage(&b_empty[prev], lane);
-            prev = bs;
-            if (++bs == BS) { bs = 0; bph ^= 1; }
-          }
-          wgmma_wait<0>();
-          release_stage(&b_empty[prev], lane);
-        }
-        release_stage(&a_empty[as], lane);
-        if (++as == AS) { as = 0; aph ^= 1; }
-      }
-      epilogue_tile<BN>(p, ctx, warp, lane, tile, k, acc);
     }
   }
 }
@@ -1244,9 +1121,9 @@ static int launch_gemm(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
   return PGT_OK;
 }
 
-template <int BN, bool GN>
+template <int BN>
 static int launch_halo(const CUtensorMap& tmA, const void* W, int ldw, GemmParams& p, cudaStream_t stream) {
-  using Cfg = HaloCfg<BN, GN>;
+  using Cfg = HaloCfg<BN>;
   CUtensorMap tmB, tmO, tmR, tmX;
   int rc = encode_weight_map(&tmB, W, ldw, p.K, p.N, BN);
   if (rc != PGT_OK) return rc;
@@ -1255,17 +1132,16 @@ static int launch_halo(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
   p.n_tiles = ceil_div(p.N, BN);
   p.b_resident = (p.ntaps * p.cin_blocks <= Cfg::B_STAGES && p.n_tiles == 1) ? 1 : 0;
   static PerDeviceOnce once;
-  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(conv_halo_kernel<BN, GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); }));
+  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(conv_halo_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); }));
   const int tiles = p.m_tiles * p.n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
   {
     char desc[96];
     if (prof_enabled())
-      snprintf(desc, sizeof(desc), "halo3%s F%d H%d W%d K%d N%d BN%d e%d r%d", GN ? "+gn" : "", p.F, p.H, p.W, p.K, p.N, BN,
-               p.fast_epi, p.b_resident);
+      snprintf(desc, sizeof(desc), "halo3 F%d H%d W%d K%d N%d BN%d e%d r%d", p.F, p.H, p.W, p.K, p.N, BN, p.fast_epi,
+               p.b_resident);
     ProfScope ps(PGT_PROF_GEMM, p.flops, stream, desc);
-    conv_halo_kernel<BN, GN><<<grid, halo_threads<GN>(), Cfg::SMEM_BYTES, stream>>>(
-        tmA, tmB, tmO, tmR, tmX, p);
+    conv_halo_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
   }
   PGT_LAUNCH_OK();
   return PGT_OK;
@@ -1342,8 +1218,7 @@ extern "C" int pgt_linear_bf16(const void* A, int lda, const void* W, int ldw, i
 // pad_y/pad_x: zero rows/cols before the input (stride 1); up_phase >= 0: phase (py = up_phase>>1, px = up_phase&1)
 // of a nearest-x2-upsample-folded conv — the [F,Hin,Win,Cout] result is scattered to out[F, 2y+py, 2x+px, :].
 static int conv_impl(const void* x, int F, int Hin, int Win, int Cin, int ldx, const void* Wp, int ldw, int Cout,
-                     int ksize, int stride, int pad_y, int pad_x, int up_phase, const pgt_epilogue* ep, void* stream,
-                     const float* gn_ab = nullptr) {
+                     int ksize, int stride, int pad_y, int pad_x, int up_phase, const pgt_epilogue* ep, void* stream) {
   const int pad_lo = pad_y;
   PGT_CHECK_ARG(x && Wp && F > 0 && Hin > 0 && Win > 0 && Cin > 0 && Cout > 0);
   PGT_CHECK_ARG((ksize >= 1 && ksize <= 3) && (stride == 1 || stride == 2) && pad_y >= 0 && pad_y <= 1 && pad_x >= 0 && pad_x <= 1);
@@ -1418,12 +1293,7 @@ static int conv_impl(const void* x, int F, int Hin, int Win, int Cin, int ldx, c
     rc = encode_map(&tmA, x, 4, dims, str, box);
     if (rc == PGT_OK && halo) {
       cudaStream_t st = static_cast<cudaStream_t>(stream);
-      if (gn_ab != nullptr) {
-        p.gn_ab = gn_ab;
-        p.gn_c = Cin;
-        return Cout <= 64 ? launch_halo<64, true>(tmA, Wp, ldw, p, st) : launch_halo<128, true>(tmA, Wp, ldw, p, st);
-      }
-      return Cout <= 64 ? launch_halo<64, false>(tmA, Wp, ldw, p, st) : launch_halo<128, false>(tmA, Wp, ldw, p, st);
+      return Cout <= 64 ? launch_halo<64>(tmA, Wp, ldw, p, st) : launch_halo<128>(tmA, Wp, ldw, p, st);
     }
   } else {
     uint64_t dims[5] = {(uint64_t)2 * ldx, (uint64_t)Win / 2, 2, (uint64_t)Hin / 2, (uint64_t)F};
@@ -1433,7 +1303,6 @@ static int conv_impl(const void* x, int F, int Hin, int Win, int Cin, int ldx, c
     rc = encode_map(&tmA, x, 5, dims, str, box);
   }
   if (rc != PGT_OK) return rc;
-  if (gn_ab != nullptr) return PGT_ERR_UNSUPPORTED;          // the fused input GroupNorm exists on the halo path only
   if (up_phase >= 0) {
     // strided placement exists only on the TMA-store path
     const int esz = p.out_dtype == PGT_BF16 ? 2 : 4;
@@ -1479,18 +1348,6 @@ extern "C" int pgt_conv_bf16(const void* x, int F, int Hin, int Win, int Cin, in
                              int Cout, int ksize, int stride, int pad_lo, const pgt_epilogue* ep, void* stream) {
   PGT_CHECK_ARG(ksize == 1 || ksize == 3);
   return conv_impl(x, F, Hin, Win, Cin, ldx, Wp, ldw, Cout, ksize, stride, pad_lo, pad_lo, -1, ep, stream);
-}
-
-extern "C" int pgt_conv_gn_supported(int Hin, int Win, int Cin, int Cout) {
-  static const bool no_halo = getenv("PGT_NO_HALO") != nullptr;
-  return (!no_halo && Cout <= 128 && Hin >= HALO_TH && Win >= HALO_TW && Cin % 8 == 0) ? 1 : 0;
-}
-
-extern "C" int pgt_conv_gn_bf16(const void* x, int F, int Hin, int Win, int Cin, int ldx, const float* gn_ab, const void* Wp,
-                                int ldw, int Cout, const pgt_epilogue* ep, void* stream) {
-  PGT_CHECK_ARG(gn_ab != nullptr && Cin % 8 == 0);
-  if (!pgt_conv_gn_supported(Hin, Win, Cin, Cout)) return PGT_ERR_UNSUPPORTED;
-  return conv_impl(x, F, Hin, Win, Cin, ldx, Wp, ldw, Cout, 3, 1, 1, 1, -1, ep, stream, gn_ab);
 }
 
 extern "C" int pgt_conv_up2x_bf16(const void* x, int F, int Hin, int Win, int Cin, int ldx, const void* Wp4, int ldw,

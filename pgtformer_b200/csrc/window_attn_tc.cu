@@ -311,8 +311,7 @@ static int win_map(CUtensorMap* map, const void* base, int ld, int cols, int cli
 }
 
 extern "C" int pgt_window_attention_tc(const void* qkv, int ldqkv, int clips, int H, int W, int C, int heads, int shift,
-                                       const void* tab, void* out, int ldo, int mode_n64, void* stream) {
-  (void)mode_n64;                                           // kept in the ABI: the N = 64 fallback view proved unnecessary
+                                       const void* tab, void* out, int ldo, void* stream) {
   PGT_CHECK_ARG(qkv && tab && out && clips > 0 && H > 0 && W > 0 && heads > 0);
   PGT_CHECK_ARG(H % 4 == 0 && W % 4 == 0 && C % heads == 0 && ldqkv % 8 == 0 && ldo % 8 == 0 && ldqkv >= 3 * C);
   if (H <= 4 || W <= 4) shift = 0;                         // get_window_size(): no shift when the map is one window

@@ -32,7 +32,7 @@ void window_attention(const at::Tensor& qkv, int64_t clips, int64_t H, int64_t W
               tab16.scalar_type() == at::kHalf && tab16.is_contiguous(), "window_attention: bf16 qkv / out, fp16 table");
   c10::cuda::CUDAGuard guard(qkv.device());
   check(pgt_window_attention_tc(qkv.data_ptr(), ld(qkv), (int)clips, (int)H, (int)W, (int)C, (int)heads, (int)shift,
-                                tab16.data_ptr(), out.data_ptr(), ld(out), 0, stream_of(qkv)), "window_attention");
+                                tab16.data_ptr(), out.data_ptr(), ld(out), stream_of(qkv)), "window_attention");
 }
 
 void mha_fwd(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v, int64_t clips, int64_t L, int64_t heads, int64_t d,

@@ -11,8 +11,6 @@ natural row order and no permute is ever materialised.
 Every op — including the BiSeNet parsing net, whose eval-mode BatchNorms are folded at load time — is a call
 into the C ABI; there is no PyTorch / cuDNN / CPU fallback: without the CUDA library construction fails.
 """
-import os
-
 import torch
 import torch.nn.functional as F  # noqa: F401  (load-time weight padding only)
 
@@ -139,7 +137,7 @@ class Engine:
                 w[p + '.qkv.weight'] = _pack_lin(torch.cat([sd[p + '.q.weight'], sd[p + '.kv.weight']], 0).float())
                 w[p + '.qkv.bias'] = torch.cat([sd[p + '.q.bias'], sd[p + '.kv.bias']], 0).float().contiguous()
                 blk = p[:-len('.attn')]
-                if self.fuse_ln_qkv and sd[p + '.q.weight'].shape[1] == 256 and (blk + '.norm1.weight') in sd:
+                if sd[p + '.q.weight'].shape[1] == 256 and (blk + '.norm1.weight') in sd:
                     # norm1's affine folded into the projection the fused kernel applies to the normalised tile:
                     # (xh * g + b) W^T + c = xh (W * g)^T + (W b + c); products and sums in fp32, one bf16 rounding of W * g
                     wf = torch.cat([sd[p + '.q.weight'], sd[p + '.kv.weight']], 0)
@@ -153,15 +151,14 @@ class Engine:
             w[p + '.qk.weight'], w[p + '.qk.bias'] = _pack_lin(wi[:2 * E]), bi[:2 * E].contiguous()
             w[p + '.v.weight'], w[p + '.v.bias'] = _pack_lin(wi[2 * E:]), bi[2 * E:].contiguous()
         # Swin MLP halves: norm2's affine folded into fc1 (same algebra as norm1 -> q/kv above)
-        if self.fuse_swin_mlp:
-            for name in list(sd):
-                if name.endswith('.mlp.fc1.weight') and sd[name].shape == (256, 256):
-                    blk = name[:-len('.mlp.fc1.weight')]
-                    if (blk + '.norm2.weight') not in sd:
-                        continue
-                    wg, bg = fold_layernorm_affine(sd[name], sd[blk + '.mlp.fc1.bias'], sd[blk + '.norm2.weight'],
-                                                   sd[blk + '.norm2.bias'])
-                    w[blk + '.mlp.fc1_ln.weight'], w[blk + '.mlp.fc1_ln.bias'] = _pack_lin(wg), bg
+        for name in list(sd):
+            if name.endswith('.mlp.fc1.weight') and sd[name].shape == (256, 256):
+                blk = name[:-len('.mlp.fc1.weight')]
+                if (blk + '.norm2.weight') not in sd:
+                    continue
+                wg, bg = fold_layernorm_affine(sd[name], sd[blk + '.mlp.fc1.bias'], sd[blk + '.norm2.weight'],
+                                               sd[blk + '.norm2.bias'])
+                w[blk + '.mlp.fc1_ln.weight'], w[blk + '.mlp.fc1_ln.bias'] = _pack_lin(wg), bg
         self._repack_parsing()
 
     # ------------------------------------------------------------------ small helpers
@@ -173,22 +170,22 @@ class Engine:
     def _new(self, *shape, dtype=BF):
         return torch.empty(*shape, dtype=dtype, device=self.dev)
 
-    fuse_cat_in_place = True  # SFT concat: encoder / decoder level outputs written straight into the concat buffer
     _fusing = False           # set per forward: SFT fusion active (w > 0)
-    fuse_conv_out = True      # decoder norm_out + SiLU + conv_out (64 -> 3) as one kernel (conv_out.cu)
-    window_tc = True          # window attention core on TMA + wgmma (window_attn_tc.cu)
-    fuse_ln_qkv = True        # norm1 + q/kv projection of the C=256 Swin blocks as one kernel
-    fuse_swin_mlp = True      # LN + fc1 + GELU + fc2 + residual of the C=256 Swin blocks as one kernel
-    # GroupNorm+SiLU applied inside the consuming 3x3 conv (pgt_conv_gn_bf16, bit-identical).  Off by default: the
-    # narrow (Cout <= 128) halo convs are bound by shared-memory operand reads, so the in-place slab transform costs
-    # them more (+10 ms at 16 clips of 512^2) than the GroupNorm apply passes it removes (-6.8 ms); see DESIGN.md.
-    fuse_gn_apply = os.environ.get('PGT_FUSE_GN', '') != ''
-    fuse_gn_min_hw = int(os.environ.get('PGT_FUSE_GN', '0') or 0)       # fuse only for feature maps at least this tall
-    fuse_gn_stats = True      # GroupNorm statistics from the producing conv / linear epilogue (saves one pass)
 
     def _stats_tiles(self, H, W, cout, ksize, stride, pad_lo):
         """Tiles per frame of a conv whose epilogue emits the next GroupNorm's statistics; 0: no fused statistics."""
         return ops.conv_tiles_per_frame(H, W, cout, ksize, stride, pad_lo)
+
+    def _gn_stats(self, out, chunks_per_frame):
+        """The next GroupNorm's statistics, filled by the epilogue that writes `out` (saves that GroupNorm a pass over
+        the tensor): allocates the fp32 buffer [frame][chunk][32 groups][2], attaches it as out._pgt_gn and returns it
+        for the producer's gn_stats.  None, with nothing attached, when out's channel count has no fused statistics,
+        out is not contiguous or chunks_per_frame (32-row chunks per frame, 4 per 128-row tile) is 0."""
+        if chunks_per_frame <= 0 or not ops.gn_stats_supported(out.shape[-1]) or not out.is_contiguous():
+            return None
+        stats = self._new(out.shape[0] * chunks_per_frame * 64, dtype=torch.float32)
+        out._pgt_gn = (stats, chunks_per_frame)
+        return stats
 
     def _gn(self, x, p, silu=True):
         gn = getattr(x, '_pgt_gn', None)
@@ -198,45 +195,25 @@ class Engine:
         return ops.groupnorm_silu(x, self.w[p + '.weight'], self.w[p + '.bias'], self._new(*x.shape), silu=silu)
 
     def _conv3(self, x, p, cout, out=None, gn_out=False, gn=None, gn_silu=True, **kw):
-        """3x3 conv; gn: name of the Normalize() whose GroupNorm+SiLU precedes it — applied inside the conv kernel
-        where the halo path exists (the normalised tensor never reaches HBM), as a separate pass otherwise.  With
-        gn_silu=False the GroupNorm has no SiLU after it (VQGAN's encoder tail); the fused kernel always applies SiLU,
-        so that case takes the separate pass."""
-        Fr, H, W, cin = x.shape
+        """3x3 conv; gn: name of the Normalize() that precedes it, run as a separate pass: GroupNorm, then SiLU unless
+        gn_silu=False (VQGAN's encoder tail).  gn_out: the epilogue also emits the next GroupNorm's statistics."""
+        Fr, H, W, _ = x.shape
         stride = kw.get('stride', 1)
-        fused_ab = None
         if gn is not None:
-            if gn_silu and self.fuse_gn_apply and H >= self.fuse_gn_min_hw and stride == 1 and kw.get('ksize', 3) == 3 and kw.get('pad_lo', 1) == 1 and \
-                    'act' not in kw and not kw.get('relu_after_res') and ops.conv_gn_supported(H, W, cin, cout):
-                st = getattr(x, '_pgt_gn', None)
-                fused_ab = ops.groupnorm_ab(x, self.w[gn + '.weight'], self.w[gn + '.bias'],
-                                            self._new(Fr * 2 * cin, dtype=torch.float32),
-                                            stats=st[0] if st else None, chunks_per_frame=st[1] if st else 0)
-            else:
-                x = self._gn(x, gn, silu=gn_silu)
+            x = self._gn(x, gn, silu=gn_silu)
         if out is None:
             out = self._new(Fr, H // stride, W // stride, cout)
         stats = None
-        if gn_out and self.fuse_gn_stats and cout % 32 == 0 and cout // 32 in (2, 4, 8, 16, 32) and out.is_contiguous():
-            tpf = self._stats_tiles(H, W, cout, kw.get('ksize', 3), stride, kw.get('pad_lo', 1))
-            if tpf > 0:
-                stats = self._new(Fr * tpf * 4 * 64, dtype=torch.float32)      # [tile][32-row quadrant][32 groups][2]
-                out._pgt_gn = (stats, tpf * 4)
-        if fused_ab is not None:
-            kw.pop('ksize', None); kw.pop('stride', None); kw.pop('pad_lo', None)
-            return ops.conv_gn(x, fused_ab, self.w[p + '.weight'], cout, out, bias=self.w.get(p + '.bias'),
-                               gn_stats=stats, **kw)
+        if gn_out:
+            stats = self._gn_stats(out, 4 * self._stats_tiles(H, W, cout, kw.get('ksize', 3), stride, kw.get('pad_lo', 1)))
         return ops.conv(x, self.w[p + '.weight'], cout, out, bias=self.w.get(p + '.bias'), gn_stats=stats, **kw)
 
     def _lin(self, x, p, n, out=None, out_dtype=BF, gn_out=False, **kw):
         if out is None:
             out = self._new(*x.shape[:-1], n, dtype=out_dtype)
         stats = None
-        if gn_out and self.fuse_gn_stats and out.dim() == 4 and out.dtype == BF and n % 32 == 0 and \
-                n // 32 in (2, 4, 8, 16, 32) and (out.shape[1] * out.shape[2]) % 128 == 0 and out.is_contiguous():
-            tpf = out.shape[1] * out.shape[2] // 128
-            stats = self._new(out.shape[0] * tpf * 4 * 64, dtype=torch.float32)
-            out._pgt_gn = (stats, tpf * 4)
+        if gn_out and out.dim() == 4 and out.dtype == BF and (out.shape[1] * out.shape[2]) % 128 == 0:
+            stats = self._gn_stats(out, out.shape[1] * out.shape[2] // 32)
         return ops.linear(x, self.w[p + '.weight'], out, bias=self.w.get(p + '.bias'), N=n, gn_stats=stats, **kw)
 
     # ------------------------------------------------------------------ blocks
@@ -253,7 +230,7 @@ class Engine:
         """VSTSREncoderTransformerBlock (`modules/rstt_layers.py:284-338`) on [F,H,W,C]."""
         Fr, H, W, C = x.shape
         w = self.w
-        if C == 256 and self.fuse_ln_qkv:
+        if C == 256:
             # norm1 + the fused q/kv projection in one kernel (LN applied to the tile in shared memory)
             if (p + '.attn.qkv_ln.weight') in w:      # gamma / beta already inside the weights (see _repack)
                 qkv = ops.ln_linear(x, None, None, w[p + '.attn.qkv_ln.weight'], w[p + '.attn.qkv_ln.bias'],
@@ -265,17 +242,13 @@ class Engine:
             y = ops.layernorm(x, w[p + '.norm1.weight'], w[p + '.norm1.bias'], self._new(Fr, H, W, C))
             qkv = self._lin(y, p + '.attn.qkv', 3 * C)
         a = self._new(Fr, H, W, C)
-        if not self.window_tc or ops.window_attention_tc(qkv, Fr // 3, H, W, C, heads, shift, w[p + '.attn.tab16'], a) is None:
+        if ops.window_attention_tc(qkv, Fr // 3, H, W, C, heads, shift, w[p + '.attn.tab16'], a) is None:
             ops.window_attention(qkv, Fr // 3, H, W, C, heads, shift, w[p + '.attn.bias_tab'], a)   # shapes the TMA kernel does not cover
         x = self._lin(a, p + '.attn.proj', C, residual=x)
-        if C == 256 and self.fuse_swin_mlp:
+        if C == 256:
             # norm2 + fc1 + GELU + fc2 + residual in one kernel (the hidden tile never leaves the SM)
             out = self._new(Fr, H, W, C) if out is None else out
-            stats = None
-            if gn_next and self.fuse_gn_stats and (H * W) % 128 == 0 and out.is_contiguous():
-                tpf = H * W // 128
-                stats = self._new(Fr * tpf * 4 * 64, dtype=torch.float32)
-                out._pgt_gn = (stats, tpf * 4)
+            stats = self._gn_stats(out, H * W // 32) if gn_next and (H * W) % 128 == 0 else None
             if (p + '.mlp.fc1_ln.weight') in w:       # gamma / beta already inside fc1 (see _repack)
                 return ops.swin_mlp(x, None, None, w[p + '.mlp.fc1_ln.weight'], w[p + '.mlp.fc1_ln.bias'],
                                     w[p + '.mlp.fc2.weight'], w[p + '.mlp.fc2.bias'], out, gn_stats=stats)
@@ -480,11 +453,7 @@ class Engine:
         a = self.arch
         Fr, _, H, W = x.shape
         h = self._new(Fr, H, W, a.ch)
-        stats = None
-        if self.fuse_gn_stats and (H * W) % 128 == 0 and a.ch == 64:
-            tpf = H * W // 128
-            stats = self._new(Fr * tpf * 4 * 64, dtype=torch.float32)
-            h._pgt_gn = (stats, tpf * 4)
+        stats = self._gn_stats(h, H * W // 32) if (H * W) % 128 == 0 and a.ch == 64 else None
         ops.conv_rgb(x, self.w[p + '.weight'], self.w[p + '.bias'], h, 3, 1, 1, gn_stats=stats)
         return h
 
@@ -495,7 +464,7 @@ class Engine:
         # a level whose output is an SFT skip tensor writes it into the [enc | dec | t] concat buffer of that fusion
         # (not the last level: its output carries GroupNorm statistics for mid.block_1 and must stay contiguous)
         slot = None
-        if self.fuse_cat_in_place and self._fusing and lvl in a.fuse_level_key and not last:
+        if self._fusing and lvl in a.fuse_level_key and not last:
             cat = self._cat_slot(Fr, H, W, a.level_ch[lvl])
             slot = cat[..., :a.level_ch[lvl]]
         for blk in range(a.num_res_blocks):
@@ -576,11 +545,7 @@ class Engine:
         """Upsample (nearest x2 + conv3x3) as four 2x2 phase convs; the epilogue emits the next norm1's statistics."""
         Fr, H, W, C = h.shape
         out = self._new(Fr, 2 * H, 2 * W, C)
-        stats = None
-        tpf = self._stats_tiles(H, W, C, 2, 1, 1)
-        if self.fuse_gn_stats and tpf > 0 and C // 32 in (2, 4, 8, 16, 32):
-            stats = self._new(Fr * 16 * tpf * 64, dtype=torch.float32)     # [frame][phase][tile][quadrant][32][2]
-            out._pgt_gn = (stats, 16 * tpf)
+        stats = self._gn_stats(out, 16 * self._stats_tiles(H, W, C, 2, 1, 1))     # [frame][phase][tile][quadrant]
         return ops.conv_up2x(h, self.w[p + '.weight'], C, out, bias=self.w[p + '.bias'], gn_stats=stats)
 
     def decoder_out(self, h, norm='decoder.norm_out', conv='decoder.conv_out', silu=True, out_ch=None):
@@ -588,15 +553,14 @@ class Engine:
         out_ch = self.arch.out_ch if out_ch is None else out_ch
         Fr, H, W, _ = h.shape
         out = self._new(Fr, out_ch, H, W, dtype=torch.float32)
-        if self.fuse_conv_out:
-            # norm + SiLU + conv in one kernel: the normalised 512^2 tensor never reaches HBM
-            st = getattr(h, '_pgt_gn', None)
-            ab = ops.groupnorm_ab(h, self.w[norm + '.weight'], self.w[norm + '.bias'],
-                                  self._new(Fr * 2 * h.shape[-1], dtype=torch.float32),
-                                  stats=st[0] if st else None, chunks_per_frame=st[1] if st else 0)
-            if ops.conv_out_gn(h, ab, self.w[conv + '.weight'], out_ch, self.w.get(conv + '.bias'), out,
-                               silu=silu) is not None:
-                return out
+        # norm + SiLU + conv in one kernel: the normalised 512^2 tensor never reaches HBM
+        st = getattr(h, '_pgt_gn', None)
+        ab = ops.groupnorm_ab(h, self.w[norm + '.weight'], self.w[norm + '.bias'],
+                              self._new(Fr * 2 * h.shape[-1], dtype=torch.float32),
+                              stats=st[0] if st else None, chunks_per_frame=st[1] if st else 0)
+        if ops.conv_out_gn(h, ab, self.w[conv + '.weight'], out_ch, self.w.get(conv + '.bias'), out,
+                           silu=silu) is not None:
+            return out
         self._conv3(h, conv, out_ch, out=out, gn=norm, gn_silu=silu, nchw=True)
         return out
 

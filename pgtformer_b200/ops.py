@@ -75,6 +75,12 @@ def make_epilogue(out, bias=None, act=ACT_NONE, residual=None, sft_scale=None, s
     return ep
 
 
+def gn_stats_supported(C):
+    """Whether a C-channel output can carry fused GroupNorm(32) statistics (the gn_stats argument below): 2, 4, 8, 16
+    or 32 channels per group, as setup_epilogue_maps in gemm_tc.cu requires."""
+    return C % 32 == 0 and C // 32 in (2, 4, 8, 16, 32)
+
+
 def linear(a, w, out, bias=None, act=ACT_NONE, residual=None, K=None, N=None, relu_after_res=False, gn_stats=None):
     """out[T,N] = act(a[T,K] @ w[N,K]^T + bias) (+ residual).  a, w bf16; out bf16 / fp32."""
     lib = L.load()
@@ -129,6 +135,17 @@ def conv_up2x(x, wp4, cout, out, bias=None, act=ACT_NONE, gn_stats=None):
 _gn_ws = {}
 
 
+def _gn_workspace(kind, x, n):
+    """fp32 GroupNorm scratch of at least n floats, one per (kind, device, current stream), grown on demand: 'stats'
+    holds pgt_groupnorm_ws_floats partial statistics, 'ab' the [F, 2, C] affine terms of groupnorm_apply_stats."""
+    key = (kind, x.device.index, torch.cuda.current_stream().cuda_stream)
+    ws = _gn_ws.get(key)
+    if ws is None or ws.numel() < n:
+        ws = torch.empty(max(n, 1 << 16), dtype=torch.float32, device=x.device)
+        _gn_ws[key] = ws
+    return ws
+
+
 def groupnorm_silu(x, gamma, beta, out, eps=1e-6, silu=True):
     lib = L.load()
     F = x.shape[0]
@@ -136,12 +153,7 @@ def groupnorm_silu(x, gamma, beta, out, eps=1e-6, silu=True):
     HW = x.numel() // (F * C) if x.is_contiguous() else x.shape[1] * x.shape[2]
     _, _, ldx = _rows(x)
     _, _, ldy = _rows(out)
-    n = lib.pgt_groupnorm_ws_floats(F, HW, C)
-    key = (x.device.index, torch.cuda.current_stream().cuda_stream)
-    ws = _gn_ws.get(key)
-    if ws is None or ws.numel() < n:
-        ws = torch.empty(max(n, 1 << 16), dtype=torch.float32, device=x.device)
-        _gn_ws[key] = ws
+    ws = _gn_workspace('stats', x, lib.pgt_groupnorm_ws_floats(F, HW, C))
     L.check(lib.pgt_groupnorm_silu(_p(x), ldx, F, HW, C, _p(gamma), _p(beta), eps, int(silu), _p(out), ldy, _p(ws),
                                    _stream()))
     return out
@@ -163,30 +175,20 @@ def groupnorm_apply_stats(x, gamma, beta, out, stats, chunks_per_frame, eps=1e-6
     F = x.shape[0]
     C = x.shape[-1]
     HW = x.shape[1] * x.shape[2]
-    key = ('ab', x.device.index, torch.cuda.current_stream().cuda_stream)
-    ws = _gn_ws.get(key)
-    if ws is None or ws.numel() < F * 2 * C:
-        ws = torch.empty(max(F * 2 * C, 1 << 16), dtype=torch.float32, device=x.device)
-        _gn_ws[key] = ws
+    ws = _gn_workspace('ab', x, F * 2 * C)
     L.check(lib.pgt_groupnorm_apply_stats(_p(x), _rows(x)[2], F, HW, C, _p(gamma), _p(beta), eps, int(silu), _p(out),
                                           _rows(out)[2], _p(stats), chunks_per_frame, _p(ws), _stream()))
     return out
 
 
 def groupnorm_ab(x, gamma, beta, ab, stats=None, chunks_per_frame=0, eps=1e-6):
-    """Per-(frame, channel) GroupNorm affine terms ab [F, 2, C] fp32 (for conv_gn), from fused statistics or from x."""
+    """Per-(frame, channel) GroupNorm affine terms ab [F, 2, C] fp32 (for conv_out_gn), from fused statistics or from
+    x."""
     lib = L.load()
     F = x.shape[0]
     C = x.shape[-1]
     HW = x.shape[1] * x.shape[2]
-    ws = None
-    if stats is None:
-        n = lib.pgt_groupnorm_ws_floats(F, HW, C)
-        key = (x.device.index, torch.cuda.current_stream().cuda_stream)
-        ws = _gn_ws.get(key)
-        if ws is None or ws.numel() < n:
-            ws = torch.empty(max(n, 1 << 16), dtype=torch.float32, device=x.device)
-            _gn_ws[key] = ws
+    ws = None if stats is not None else _gn_workspace('stats', x, lib.pgt_groupnorm_ws_floats(F, HW, C))
     assert ab.dtype == torch.float32 and ab.numel() >= F * 2 * C and ab.is_contiguous()
     L.check(lib.pgt_groupnorm_ab(_p(x), _rows(x)[2], F, HW, C, _p(gamma), _p(beta), eps, _p(stats), chunks_per_frame,
                                  _p(ws), _p(ab), _stream()))
@@ -210,23 +212,6 @@ def conv_out_gn(x, ab, wp, cout, bias, out, silu=True):
     if rc == -3:
         return None
     L.check(rc)
-    return out
-
-
-def conv_gn_supported(H, W, cin, cout):
-    return bool(L.load().pgt_conv_gn_supported(H, W, cin, cout))
-
-
-def conv_gn(x, ab, wp, cout, out, bias=None, act=ACT_NONE, residual=None, sft_scale=None, sft_w=0.0, nchw=False,
-            gn_stats=None):
-    """conv3x3(silu(groupnorm(x))) with the normalisation applied to the input slabs in shared memory."""
-    lib = L.load()
-    F, H, W, Cin = x.shape
-    assert x.dtype == torch.bfloat16 and x.stride(3) == 1 and x.stride(1) == W * x.stride(2) and \
-        (F == 1 or x.stride(0) == H * x.stride(1))
-    ep = make_epilogue(out, bias, act, residual, sft_scale, sft_w, nchw, False, gn_stats)
-    L.check(lib.pgt_conv_gn_bf16(_p(x), F, H, W, Cin, x.stride(2), _p(ab), _p(wp), wp.stride(0), cout,
-                                 ctypes.byref(ep), _stream()))
     return out
 
 
@@ -299,15 +284,12 @@ def window_tables(bias):
     return torch.stack(tabs, 0).to(torch.float16).contiguous()
 
 
-WINDOW_MODE_N64 = 0          # d = 32 heads: 0 = P V with a half-atom N = 32 view of V, 1 = N = 64 (both heads' columns)
-
-
-def window_attention_tc(qkv, clips, H, W, C, heads, shift, tab16, out, mode_n64=None):
+def window_attention_tc(qkv, clips, H, W, C, heads, shift, tab16, out):
     """TMA + wgmma window attention core; returns None when the shape is not covered (caller uses window_attention)."""
     lib = L.load()
     assert qkv.dtype == torch.bfloat16 and tab16.dtype == torch.float16 and tab16.is_contiguous()
     rc = lib.pgt_window_attention_tc(_p(qkv), _rows(qkv)[2], clips, H, W, C, heads, shift, _p(tab16), _p(out),
-                                     _rows(out)[2], WINDOW_MODE_N64 if mode_n64 is None else int(mode_n64), _stream(qkv))
+                                     _rows(out)[2], _stream(qkv))
     if rc == -3:
         return None
     L.check(rc)

@@ -85,7 +85,7 @@ class VQGANEngine(Engine):
 
     def encoder_out(self, h, out, nchw=False):
         """The encoder tail: GroupNorm (no SiLU) -> conv 3x3 to emb_dim, into out (fp32 NHWC rows, fp32 NCHW with
-        nchw, or bf16 NHWC).  The GroupNorm runs on its own pass: the fused conv_gn kernel always applies SiLU."""
+        nchw, or bf16 NHWC).  The GroupNorm runs on its own pass."""
         n = len(self.arch.enc_blocks)
         y = getattr(h, '_pgt_normed', None)
         if y is None:

@@ -523,56 +523,6 @@ def test_conv_rgb_tensor_core(ks, stride, pad, norm, Fr, H, W):
         check_close(y, gref, 'rgb conv fused-stats groupnorm', bf16_out=True, rel=3e-3)
 
 
-@pytest.mark.parametrize('Fr,H,W,Cin,Cout,res,nchw,fused_stats', [
-    (3, 32, 24, 64, 64, True, False, True), (2, 16, 8, 160, 64, False, False, False),
-    (3, 40, 20, 128, 128, True, False, False), (2, 32, 32, 288, 128, False, False, True),
-    (3, 48, 16, 64, 3, False, True, False)])
-def test_conv_with_fused_input_groupnorm(Fr, H, W, Cin, Cout, res, nchw, fused_stats):
-    """conv3x3(silu(GroupNorm(x))) with the normalisation applied to the slabs in shared memory must equal the
-    two-pass path (GroupNorm+SiLU written to HBM, then the conv) bit for bit: same affine terms, same rounding,
-    same MMA order; zero padding and channel padding stay zero."""
-    o = ops()
-    x = bf(rnd((Fr, H, W, Cin), 190) * 1.3 + 0.2).to(DEV)
-    gam, bet = (1 + 0.1 * rnd((Cin,), 191)).to(DEV), (0.1 * rnd((Cin,), 192)).to(DEV)
-    w = pack_conv_weight(bf(rnd((Cout, Cin, 3, 3), 193, (9 * Cin) ** -0.5)).float()).to(DEV)
-    b = rnd((Cout,), 194, 0.1).to(DEV)
-    r = bf(rnd((Fr, H, W, Cout), 195)).to(DEV) if res else None
-    if not o.conv_gn_supported(H, W, Cin, Cout):
-        pytest.skip('halo-reuse conv disabled (PGT_NO_HALO): the fused-GroupNorm variant does not exist')
-
-    def mk():
-        return (torch.empty(Fr, Cout, H, W, dtype=torch.float32, device=DEV) if nchw
-                else torch.empty(Fr, H, W, Cout, dtype=torch.bfloat16, device=DEV))
-    xn = torch.empty_like(x)
-    o.groupnorm_silu(x, gam, bet, xn)
-    ref = o.conv(xn, w, Cout, mk(), bias=b, residual=r, nchw=nchw)
-    ab = torch.empty(Fr * 2 * Cin, dtype=torch.float32, device=DEV)
-    o.groupnorm_ab(x, gam, bet, ab)
-    stats = None
-    if fused_stats:
-        tpf = o.conv_tiles_per_frame(H, W, Cout)
-        stats = torch.zeros(Fr * tpf * 4 * 64, dtype=torch.float32, device=DEV)
-    got = o.conv_gn(x, ab, w, Cout, mk(), bias=b, residual=r, nchw=nchw, gn_stats=stats)
-    torch.cuda.synchronize()
-    assert torch.equal(got, ref), 'fused-GN conv differs: max |d| = %g' % (got.float() - ref.float()).abs().max().item()
-    # and against the fp32 composition
-    xr = F.silu(F.group_norm(x.float().cpu().permute(0, 3, 1, 2), 32, gam.cpu(), bet.cpu(), eps=1e-6))
-    wr = bf(rnd((Cout, Cin, 3, 3), 193, (9 * Cin) ** -0.5)).float()
-    full = F.conv2d(bf(xr).float(), wr, b.cpu(), padding=1)
-    if res:
-        full = full + r.float().cpu().permute(0, 3, 1, 2)
-    if nchw:
-        check_close(got, full, 'fused-GN conv vs fp32', rel=4e-3)
-    else:
-        check_close(got, full.permute(0, 2, 3, 1), 'fused-GN conv vs fp32', bf16_out=True, rel=4e-3)
-    if stats is not None:
-        y = torch.empty_like(got)
-        g2, b2 = (1 + 0.1 * rnd((Cout,), 196)).to(DEV), (0.1 * rnd((Cout,), 197)).to(DEV)
-        o.groupnorm_apply_stats(got, g2, b2, y, stats, tpf * 4)
-        gref = F.silu(F.group_norm(got.float().cpu().permute(0, 3, 1, 2), 32, g2.cpu(), b2.cpu(), eps=1e-6)).permute(0, 2, 3, 1)
-        check_close(y, gref, 'stats after fused-GN conv', bf16_out=True, rel=3e-3)
-
-
 @pytest.mark.parametrize('T,N', [(128, 768), (1000, 768), (12288, 256), (5000, 512)])
 def test_ln_linear_fused(T, N):
     """out = LN(x) W^T + b in one kernel vs the fp32 composition on bf16-rounded operands."""

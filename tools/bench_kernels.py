@@ -65,9 +65,7 @@ def bench_window(C, H, clips, shift, pk, out):
     bytes_ = T * 4 * C * 2                                        # read q,k,v + write o (SURVEY 8d)
     flops = 4.0 * 48 * 48 * C * (T // 48)
     cases = [('mma_sync', lambda: ops.window_attention(qkv, clips, H, H, C, heads, shift, bias, o)),
-             ('wgmma', lambda: ops.window_attention_tc(qkv, clips, H, H, C, heads, shift, tab16, o, mode_n64=0))]
-    if C // heads == 32:
-        cases.append(('wgmma_n64', lambda: ops.window_attention_tc(qkv, clips, H, H, C, heads, shift, tab16, o, mode_n64=1)))
+             ('wgmma', lambda: ops.window_attention_tc(qkv, clips, H, H, C, heads, shift, tab16, o))]
     for name, fn in cases:
         ms = timed(fn)
         out({'kernel': 'window_attention', 'impl': name, 'C': C, 'H': H, 'clips': clips, 'shift': shift, 'ms': ms,

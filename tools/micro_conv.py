@@ -131,4 +131,3 @@ if len(sys.argv) > 1 and sys.argv[1] == 'wide':
 for args in [(12, 512, 64, 64, False), (12, 512, 64, 64, True), (12, 512, 128, 64, False), (12, 256, 128, 128, False),
              (12, 256, 128, 128, True), (12, 128, 256, 256, True), (12, 128, 256, 256, False)]:
     conv_case(*args)
-os.environ['PGT_NO_HALO'] = '1'
