@@ -255,6 +255,14 @@ int pgt_codebook_pack(const float* codebook, int K, int E, void* cb_bf16, float*
 int64_t pgt_l2_argmin_ws_ints(int T);
 int pgt_l2_argmin_tc(const float* z, int T, int E, const float* codebook, const void* cb_bf16, const float* cb_norm,
                      int K, int64_t* idx, float* quant, int32_t* workspace, void* stream);
+/* pgt_l2_argmin_tc with the codebook split into `splits` ranges of whole 128-code tiles (the last one ragged; more
+ * splits than tiles are clamped), one CTA per (128-token tile, range), and a merge kernel (one warp per token) that
+ * resolves the union of the ranges' candidate windows exactly: the same result (fp64 argmin, first-index tie-break) for
+ * any splits >= 1.  For small T, where the unsplit sweep leaves most SMs idle.
+ *   workspace: int32 [pgt_l2_argmin_split_ws_ints(T, splits)]. */
+int64_t pgt_l2_argmin_split_ws_ints(int T, int splits);
+int pgt_l2_argmin_tc_split(const float* z, int T, int E, const float* codebook, const void* cb_bf16, const float* cb_norm,
+                           int K, int splits, int64_t* idx, float* quant, int32_t* workspace, void* stream);
 
 /* ---- soft codes of one quantiser depth (RQBottleneck.get_soft_codes, archs/tdcrqvae3_arch.py:429-457).
  * pgt_soft_codes: out[t, k] = softmax_k((2 z[t].e_k - ||e_k||^2) / temp) = softmax_k(-||z[t] - e_k||^2 / temp) over the

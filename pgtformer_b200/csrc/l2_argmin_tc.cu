@@ -24,6 +24,14 @@
 //   index on ties).  Rows whose window holds more than 16 codes or whose list overflowed (degenerate codebooks: many
 //   duplicated / zero rows) are appended to a list for the exhaustive fp32+fp64 kernel in codebook.cu.
 // The result therefore equals an fp64 argmin of ||z - e_k||^2 with first-index tie-break for every input.
+//
+// Codebook split (pgt_l2_argmin_tc_split, small T): the grid is token tiles x S code ranges of whole 128-code N-tiles
+// (the last one ragged).  Each CTA runs the same scan over its range and writes, per (token, range, list owner), its
+// running minimum d~, its candidate list and the list length (> LT_LIST: overflow) to the workspace instead of merging.
+// l2_argmin_merge_kernel (one warp per token) takes the global minimum, keeps every list's entries within W of it and
+// resolves them exactly as above; overflowed lists and windows of more than LT_TOP codes go to the exhaustive kernel.
+// Exact for any S: each list is a superset of {k in its range : d~_k <= its range's min + W}, and the global minimum is
+// <= every range's minimum, so the lists together hold the whole global window.
 #include <float.h>
 
 #include "common.cuh"
@@ -252,12 +260,22 @@ __device__ __forceinline__ int argmin_resolve_exact(const float* __restrict__ z,
   return best;
 }
 
+// per-(token, range, owner) scan results of the split sweep
+struct SplitOut {
+  int S, per;                  // code ranges, N-tiles per range
+  float* win;                  // [T] W of each token
+  float* mins;                 // [T][S][2] running minima
+  int* cnt;                    // [T][S][2] list lengths (> LT_LIST: overflowed)
+  float2* lists;               // [T][S][2][LT_LIST] (d~, code)
+};
+
 // ------------------------------------------------------------------------------ the sweep
+template <bool SPLIT>
 __global__ void __launch_bounds__(LT_THREADS, 1)
 l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const float* __restrict__ z, const float2* __restrict__ zn2, int T, int E,
                     const float* __restrict__ cb, const float* __restrict__ norm, int K, int64_t* __restrict__ idx,
-                    float* __restrict__ quant, int* __restrict__ fb_count, int* __restrict__ fb_list) {
+                    float* __restrict__ quant, int* __restrict__ fb_count, int* __restrict__ fb_list, const SplitOut so) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                                          // [E/64][128 rows][128 B]: this CTA's 128 tokens
@@ -278,6 +296,11 @@ l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   const int KB = E / LT_BK;                                    // k-blocks
   const int NT = K / LT_BN;                                    // N-tiles
   const int n_t = (T + LT_BM - 1) / LT_BM;                     // 128-token tiles
+  // work items: token tiles, or with SPLIT (token tile, code range) pairs, range-minor
+  const int n_items = SPLIT ? n_t * so.S : n_t;
+  auto item_tile = [&](int wi) { return SPLIT ? wi / so.S : wi; };
+  auto item_nt0 = [&](int wi) { return SPLIT ? (wi % so.S) * so.per : 0; };
+  auto item_nt1 = [&](int wi) { return SPLIT ? min(NT, (wi % so.S + 1) * so.per) : NT; };
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
@@ -293,8 +316,9 @@ l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     // ---------------------------------------------------------------- codebook producer
     int st = 0;
     uint32_t ph = 0;
-    for (int tt = blockIdx.x; tt < n_t; tt += gridDim.x) {
-      for (int nt = 0; nt < NT; ++nt) {
+    for (int wi = blockIdx.x; wi < n_items; wi += gridDim.x) {
+      const int nt1 = item_nt1(wi);
+      for (int nt = item_nt0(wi); nt < nt1; ++nt) {
         for (int kb = 0; kb < KB; ++kb) {
           mbar_wait(&b_empty[st], ph ^ 1);
           if (elect_one()) {
@@ -309,8 +333,8 @@ l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   } else if (warp == 9) {
     // ---------------------------------------------------------------- A producer: the bf16 z rows of this CTA's 128 tokens
     int it = 0;
-    for (int tt = blockIdx.x; tt < n_t; tt += gridDim.x, ++it) {
-      const int t0 = tt * LT_BM;
+    for (int wi = blockIdx.x; wi < n_items; wi += gridDim.x, ++it) {
+      const int t0 = item_tile(wi) * LT_BM;
       for (int kb = 0; kb < KB; ++kb) {
         if (it > 0) mbar_wait(&a_empty[kb], (it - 1) & 1);       // the previous tile's last N-tile has read this k-block
         if (elect_one()) {
@@ -335,8 +359,9 @@ l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     int st = 0;
     uint32_t ph = 0;
     int it = 0;
-    for (int tt = blockIdx.x; tt < n_t; tt += gridDim.x, ++it) {
-      const int t0 = tt * LT_BM;
+    for (int wi = blockIdx.x; wi < n_items; wi += gridDim.x, ++it) {
+      const int t0 = item_tile(wi) * LT_BM;
+      const int nt0 = item_nt0(wi), nt1 = item_nt1(wi);
       const bool live = t0 + r < T;
       float W;
       {
@@ -347,11 +372,11 @@ l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       }
       float runmin = live ? FLT_MAX : -FLT_MAX, thr = runmin;  // rows past T never pass the chunk test
       int cnt = 0;
-      for (int nt = 0; nt < NT; ++nt) {
+      for (int nt = nt0; nt < nt1; ++nt) {
         float acc[LT_BN / 2];
         int prev = -1;
         for (int kb = 0; kb < KB; ++kb) {
-          if (nt == 0) mbar_wait(&a_full[kb], it & 1);
+          if (nt == nt0) mbar_wait(&a_full[kb], it & 1);
           mbar_wait(&b_full[st], ph);
           const uint64_t da = wgmma_desc_k_sw128(a_rows + kb * LT_A_KB_BYTES);
           const uint64_t db = wgmma_desc_k_sw128(smem_u32(sB) + st * LT_BST);
@@ -368,7 +393,7 @@ l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         __syncwarp();
         if (lane == 0) {
           mbar_arrive(&b_empty[prev]);
-          if (nt == NT - 1)
+          if (nt == nt1 - 1)
             for (int kb = 0; kb < KB; ++kb) mbar_arrive(&a_empty[kb]);   // the tile is done with its A k-blocks
         }
         static_for<0, LT_BN / 32>([&](auto rc) {
@@ -387,6 +412,18 @@ l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           const int c = nt * LT_BN + 32 * R + g * LT_SCH;
           argmin_scan_chunk(v, norm + c, c, W, smem_u32(lst), runmin, thr, cnt);
         });
+      }
+      if constexpr (SPLIT) {
+        // this range's scan results, merged across ranges by l2_argmin_merge_kernel
+        if (live) {
+          const int t = t0 + r, s = wi % so.S;
+          const size_t o = ((size_t)t * so.S + s) * 2 + g;
+          if (s == 0 && g == 0) so.win[t] = W;
+          so.mins[o] = runmin;
+          so.cnt[o] = cnt;
+          for (int j = 0; j < min(cnt, LT_LIST); ++j) so.lists[o * LT_LIST + j] = lst[j * 2 * LT_BM];
+        }
+        continue;
       }
       // merge: every thread filters its own list against the row's minimum over both owners
       xmin[g * LT_BM + r] = runmin;
@@ -446,6 +483,62 @@ l2_argmin_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 
 }
 
+// Merge of the split sweep: one warp per token.  Lanes take the (range, owner) lists in turn; entries within W of the
+// global minimum are gathered into shared memory in (range, owner, list) order and resolved as in the sweep.
+constexpr int LM_WARPS = 8;
+__global__ void __launch_bounds__(LM_WARPS * 32)
+l2_argmin_merge_kernel(const float* __restrict__ z, int T, int E, const float* __restrict__ cb, const SplitOut so,
+                       int64_t* __restrict__ idx, float* __restrict__ quant, int* __restrict__ fb_count,
+                       int* __restrict__ fb_list) {
+  __shared__ int mi[LM_WARPS][LT_TOP];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t = blockIdx.x * LM_WARPS + warp;
+  if (t >= T) return;
+  const int nl = 2 * so.S;                                       // lists of this token
+  const size_t o0 = (size_t)t * nl;
+  float gmin = FLT_MAX;
+  bool ovf = false;
+  for (int l = lane; l < nl; l += 32) {
+    gmin = fminf(gmin, so.mins[o0 + l]);
+    ovf |= so.cnt[o0 + l] > LT_LIST;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) gmin = fminf(gmin, __shfl_xor_sync(0xffffffffu, gmin, o));
+  ovf = __any_sync(0xffffffffu, ovf);
+  const float win = gmin + so.win[t];
+  int n = 0;                                                     // window members found so far (warp-uniform)
+  for (int l0 = 0; l0 < nl && !ovf; l0 += 32) {
+    const int l = l0 + lane;
+    const int c = l < nl ? so.cnt[o0 + l] : 0;
+    for (int j = 0; j < LT_LIST; ++j) {
+      bool in = false;
+      int code = 0;
+      if (j < c) {
+        const float2 e = so.lists[(o0 + l) * LT_LIST + j];
+        in = e.x <= win;
+        code = __float_as_int(e.y);
+      }
+      const unsigned m = __ballot_sync(0xffffffffu, in);
+      const int pos = n + __popc(m & ((1u << lane) - 1u));
+      if (in && pos < LT_TOP) mi[warp][pos] = code;
+      n += __popc(m);
+    }
+  }
+  __syncwarp();
+  int best;
+  if (ovf || n > LT_TOP || n == 0) {
+    if (lane == 0) fb_list[atomicAdd(fb_count, 1)] = t;         // exhaustive kernel
+    return;
+  }
+  best = n == 1 ? mi[warp][0] : argmin_resolve_exact(z, cb, E, t, n, mi[warp], lane);
+  if (lane == 0) idx[t] = best;
+  if (quant != nullptr) {
+    const float4* src = reinterpret_cast<const float4*>(cb + (size_t)best * E);
+    float4* dst = reinterpret_cast<float4*>(quant + (size_t)t * E);
+    for (int e = lane; e < (E >> 2); e += 32) dst[e] = __ldg(src + e);
+  }
+}
+
 int l2_argmin_list_launch(const float* z, int T, int E, const float* codebook, int K, int64_t* idx, float* quant,
                           const int* list, const int* count, int grid, cudaStream_t st);      // codebook.cu
 
@@ -491,7 +584,7 @@ extern "C" int pgt_l2_argmin_tc(const float* z, int T, int E, const float* codeb
   if (rc == PGT_OK) rc = tmap_rows_bf16(&tmB, cb_bf16, E, K, E, LT_BN);
   if (rc != PGT_OK) return rc;
   static PerDeviceOnce once;
-  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(l2_argmin_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM); }));
+  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(l2_argmin_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM); }));
   PGT_CUDA_OK(cudaMemsetAsync(workspace, 0, sizeof(int32_t), st));
   const int n_t = ceil_div(T, LT_BM);
   const int grid = n_t < num_sms() ? n_t : num_sms();
@@ -509,10 +602,69 @@ extern "C" int pgt_l2_argmin_tc(const float* z, int T, int E, const float* codeb
       }
     }
     z_pack_kernel<<<pack_ctas, 256, 0, st>>>(z, T, E, zb, zn2);
-    l2_argmin_tc_kernel<<<grid, LT_THREADS, LT_SMEM, st>>>(tmA, tmB, z, zn2, T, E, codebook, cb_norm, K, idx, quant,
-                                                           fb_count, fb_list);
+    l2_argmin_tc_kernel<false><<<grid, LT_THREADS, LT_SMEM, st>>>(tmA, tmB, z, zn2, T, E, codebook, cb_norm, K, idx, quant,
+                                                                  fb_count, fb_list, SplitOut{});
     PGT_LAUNCH_OK();
   }
   // tokens whose certificate window did not fit the shortlist (degenerate codebooks): exhaustive exact kernel
+  return l2_argmin_list_launch(z, T, E, codebook, K, idx, quant, fb_list, fb_count, num_sms(), st);
+}
+
+// ------------------------------------------------------------------------------ codebook split (small T)
+// workspace (int32 units): the unsplit layout, then [win: T][mins: T x 2S][cnt: T x 2S][lists: T x 2S x LT_LIST float2]
+static inline int64_t ws_off_split(int T) { return ws_align4(pgt_l2_argmin_ws_ints(T)); }
+
+static inline int split_ranges(int K, int splits, int* per) {
+  const int NT = K / LT_BN;
+  const int s = splits < 1 ? 1 : (splits > NT ? NT : splits);
+  *per = ceil_div(NT, s);
+  return ceil_div(NT, *per);                     // ranges actually used: every one non-empty
+}
+
+extern "C" int64_t pgt_l2_argmin_split_ws_ints(int T, int splits) {
+  const int64_t L = (int64_t)T * 2 * (splits < 1 ? 1 : splits);
+  return ws_off_split(T) + ws_align4(T) + ws_align4(L) + ws_align4(L) + L * LT_LIST * 2;
+}
+
+extern "C" int pgt_l2_argmin_tc_split(const float* z, int T, int E, const float* codebook, const void* cb_bf16,
+                                      const float* cb_norm, int K, int splits, int64_t* idx, float* quant,
+                                      int32_t* workspace, void* stream) {
+  PGT_CHECK_ARG(z && codebook && cb_bf16 && cb_norm && idx && workspace && T > 0 && splits >= 1);
+  if (K % LT_BN != 0 || E % LT_BK != 0 || E > LT_EMAX || E % 128 != 0) return PGT_ERR_UNSUPPORTED;
+  PGT_CHECK_ARG((reinterpret_cast<uintptr_t>(z) & 15) == 0 && (reinterpret_cast<uintptr_t>(codebook) & 15) == 0 &&
+                (reinterpret_cast<uintptr_t>(cb_bf16) & 15) == 0 && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0 &&
+                (quant == nullptr || (reinterpret_cast<uintptr_t>(quant) & 15) == 0));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int* fb_count = workspace;
+  int* fb_list = workspace + ws_off_list(T);
+  float2* zn2 = reinterpret_cast<float2*>(workspace + ws_off_zn2(T));
+  __nv_bfloat16* zb = reinterpret_cast<__nv_bfloat16*>(workspace + ws_off_zb(T));
+  SplitOut so{};
+  so.S = split_ranges(K, splits, &so.per);
+  // sections sized for `splits` lists per token (>= so.S), so the layout matches pgt_l2_argmin_split_ws_ints
+  const int64_t L = (int64_t)T * 2 * splits;
+  int32_t* base = workspace + ws_off_split(T);
+  so.win = reinterpret_cast<float*>(base);
+  so.mins = reinterpret_cast<float*>(base + ws_align4(T));
+  so.cnt = base + ws_align4(T) + ws_align4(L);
+  so.lists = reinterpret_cast<float2*>(base + ws_align4(T) + 2 * ws_align4(L));
+  CUtensorMap tmA, tmB;
+  int rc = tmap_rows_bf16(&tmA, zb, E, T, E, LT_BM);
+  if (rc == PGT_OK) rc = tmap_rows_bf16(&tmB, cb_bf16, E, K, E, LT_BN);
+  if (rc != PGT_OK) return rc;
+  static PerDeviceOnce once;
+  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(l2_argmin_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM); }));
+  PGT_CUDA_OK(cudaMemsetAsync(workspace, 0, sizeof(int32_t), st));
+  const int items = ceil_div(T, LT_BM) * so.S;
+  const int grid = items < num_sms() ? items : num_sms();
+  {
+    ProfScope ps(PGT_PROF_ARGMIN, 2.0 * T * (double)K * E, st, "l2_argmin_tc_split");
+    z_pack_kernel<<<num_sms() * 2, 256, 0, st>>>(z, T, E, zb, zn2);
+    l2_argmin_tc_kernel<true><<<grid, LT_THREADS, LT_SMEM, st>>>(tmA, tmB, z, zn2, T, E, codebook, cb_norm, K, idx, nullptr,
+                                                                 fb_count, fb_list, so);
+    l2_argmin_merge_kernel<<<ceil_div(T, LM_WARPS), LM_WARPS * 32, 0, st>>>(z, T, E, codebook, so, idx, quant, fb_count,
+                                                                            fb_list);
+    PGT_LAUNCH_OK();
+  }
   return l2_argmin_list_launch(z, T, E, codebook, K, idx, quant, fb_list, fb_count, num_sms(), st);
 }

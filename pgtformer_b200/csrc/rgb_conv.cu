@@ -7,12 +7,15 @@
 //                output pixel; gathers its 3 k^2 inputs (coalesced across the warp: lanes are neighbouring pixels),
 //                optional (x - mean) / std, bf16, and writes the row of the 128 x K A tile straight into the
 //                128B-swizzled K-major layout the wgmma descriptor expects (double buffered)
-//   last 4 warps one warpgroup: 2 x K/16 wgmma 64 x 64 x 16 per tile (both 64-row halves) against the weight tile
-//                resident in smem, [128 x 64] fp32 accumulator in registers -> shared-memory exchange (thread = row)
+//   last 4 warps one warpgroup: 2 x K/16 wgmma 64 x N x 16 per tile (both 64-row halves) against the weight tile
+//                resident in smem, [128 x N] fp32 accumulator in registers -> shared-memory exchange (thread = row)
 //                -> bias (+ReLU) -> optional GroupNorm(32) partial statistics -> bf16 -> swizzled staging tile -> one
-//                TMA store per tile
-// The 3x3 kernel runs two CTAs per SM (109 KB of shared memory each): a tile's chain gather -> MMA -> epilogue -> store
-// is latency-bound, a second CTA fills the gaps.
+//                TMA store per 64-channel panel
+// N = 64 output channels for both layers; the 3x3 stem also has N = 128 (ch = 128 RQ-VAEs, archs/rqvae_arch.py:592-596).
+// The 3x3 N = 64 kernel runs two CTAs per SM (109 KB of shared memory each): a tile's chain gather -> MMA -> epilogue ->
+// store is latency-bound, a second CTA fills the gaps.  At N = 128 the staging tiles and the fp32 exchange double
+// (179 KB), so one CTA per SM: two would need a single-buffered staging tile and a half-width exchange, i.e. a second
+// barrier round per tile, for a layer that is ~1 % of an RQ-VAE forward.
 #include <cudaTypedefs.h>
 
 #include "common.cuh"
@@ -22,11 +25,7 @@
 
 namespace pgt {
 
-constexpr int RC_N = 64;                 // output channels (both layers)
-constexpr int RC_SUB = 128 * 128;        // [128 rows x 64 k] bf16 A sub-tile
-constexpr int RC_BSUB = RC_N * 128;      // [64 rows x 64 k] bf16 weight sub-tile
-constexpr int RC_XLD = RC_N + 4;         // accumulator exchange pitch (fp32)
-constexpr int RC_XCH = 128 * RC_XLD * 4;
+constexpr int RC_SUB = 128 * 128;        // [128 rows x 64 k] bf16 A sub-tile; also one 64-channel staging panel
 
 struct RgbConvParams {
   const float* x;                        // [F, 3, H, W] fp32
@@ -39,19 +38,25 @@ struct RgbConvParams {
   float* gn_stats;                       // optional [m_tiles][4][32][2]
 };
 
-template <int KS>
+template <int KS, int N>
 struct RgbCfg {
+  static_assert(N == 64 || N == 128, "output channels");
   static constexpr int K = 3 * KS * KS;
   static constexpr int KSTEPS = (K + 15) / 16;
   static constexpr int NSUB = (KSTEPS + 3) / 4;
   static constexpr int NCH = KSTEPS * 2;                        // 16-byte chunks written per row
+  static constexpr int BSUB = N * 128;                          // [N rows x 64 k] bf16 weight sub-tile
+  static constexpr int PANELS = N / 64;                         // 64-channel panels of a staged output tile
+  static constexpr int XLD = N + 4;                             // accumulator exchange pitch (fp32)
+  static constexpr int XCH = 128 * XLD * 4;
   static constexpr int A_BYTES = NSUB * RC_SUB;
-  static constexpr int B_BYTES = NSUB * RC_BSUB;
-  static constexpr int SMEM = 2 * A_BYTES + B_BYTES + 2 * RC_SUB /*staging*/ + RC_XCH + 256;
+  static constexpr int B_BYTES = NSUB * BSUB;
+  static constexpr int STG = PANELS * RC_SUB;                   // one staging tile
+  static constexpr int SMEM = 2 * A_BYTES + B_BYTES + 2 * STG + XCH + 256;
   static constexpr int BW = KS == 3 ? 4 : 8;                    // builder warps
   static constexpr int PARTS = BW / 4;                          // threads per output pixel
   static constexpr int THREADS = (BW + 4) * 32;
-  static constexpr int PER_SM = KS == 3 ? 2 : 1;                // resident CTAs per SM
+  static constexpr int PER_SM = KS == 3 && N == 64 ? 2 : 1;     // resident CTAs per SM
 };
 
 // 16-byte chunks [CH0, CH1) of one A row (one output pixel): every tap offset is a compile-time constant
@@ -81,17 +86,17 @@ __device__ __forceinline__ void rgb_build_chunks(const RgbConvParams& p, const f
   }
 }
 
-template <int KS, int STRIDE, int PAD>
-__global__ void __launch_bounds__(RgbCfg<KS>::THREADS, RgbCfg<KS>::PER_SM)
+template <int KS, int STRIDE, int PAD, int N>
+__global__ void __launch_bounds__(RgbCfg<KS, N>::THREADS, RgbCfg<KS, N>::PER_SM)
 rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO, const RgbConvParams p) {
-  using Cfg = RgbCfg<KS>;
+  using Cfg = RgbCfg<KS, N>;
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sA = smem;                                   // [2][NSUB] sub-tiles
   uint8_t* sB = sA + 2 * Cfg::A_BYTES;                  // [NSUB] weight sub-tiles
   uint8_t* sO = sB + Cfg::B_BYTES;                      // [2] staging tiles
-  float* xch = reinterpret_cast<float*>(sO + 2 * RC_SUB);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sO + 2 * RC_SUB + RC_XCH);
+  float* xch = reinterpret_cast<float*>(sO + 2 * Cfg::STG);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sO + 2 * Cfg::STG + Cfg::XCH);
   uint64_t* a_full = bars;           // [2] builders -> MMA warpgroup
   uint64_t* a_free = bars + 2;       // [2] MMA warpgroup (one arrive per warp) -> builders
   uint64_t* b_full = bars + 4;
@@ -105,7 +110,7 @@ rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       mbar_init(b_full, 1);
       fence_barrier_init();
       mbar_arrive_expect_tx(b_full, Cfg::B_BYTES);
-      for (int s = 0; s < Cfg::NSUB; ++s) tma_load_2d(sB + s * RC_BSUB, &tmW, b_full, s * 64, 0);
+      for (int s = 0; s < Cfg::NSUB; ++s) tma_load_2d(sB + s * Cfg::BSUB, &tmW, b_full, s * 64, 0);
     }
     __syncwarp();
   }
@@ -140,20 +145,20 @@ rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
     const int quad = warp & 3;
     const int r = quad * 32 + lane;
     const int et = threadIdx.x - BW * 32;
-    const float* xrow = xch + r * RC_XLD;
+    const float* xrow = xch + r * Cfg::XLD;
     mbar_wait(b_full, 0);
     int it = 0;
     for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x, ++it) {
       const int buf = it & 1;
       mbar_wait(&a_full[buf], (it >> 1) & 1);
-      float acc0[RC_N / 2], acc1[RC_N / 2];               // rows [0, 64) and [64, 128) of the tile
+      float acc0[N / 2], acc1[N / 2];                     // rows [0, 64) and [64, 128) of the tile
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < Cfg::KSTEPS; ++ks) {
         const uint32_t a = smem_u32(sA + buf * Cfg::A_BYTES + (ks >> 2) * RC_SUB);
-        const uint64_t db = wgmma_desc_k_sw128(smem_u32(sB + (ks >> 2) * RC_BSUB)) + 2 * (ks & 3);
-        wgmma_bf16<RC_N>(acc0, wgmma_desc_k_sw128(a) + 2 * (ks & 3), db, ks != 0 ? 1u : 0u);
-        wgmma_bf16<RC_N>(acc1, wgmma_desc_k_sw128(a + 64 * 128) + 2 * (ks & 3), db, ks != 0 ? 1u : 0u);
+        const uint64_t db = wgmma_desc_k_sw128(smem_u32(sB + (ks >> 2) * Cfg::BSUB)) + 2 * (ks & 3);
+        wgmma_bf16<N>(acc0, wgmma_desc_k_sw128(a) + 2 * (ks & 3), db, ks != 0 ? 1u : 0u);
+        wgmma_bf16<N>(acc1, wgmma_desc_k_sw128(a + 64 * 128) + 2 * (ks & 3), db, ks != 0 ? 1u : 0u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -162,12 +167,12 @@ rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
       // staging[buf] was last read by the store two tiles back; the exchange by the previous tile's epilogue
       if (et == 0) bulk_wait_read<1>();
       named_bar_sync(1, 128);
-      acc_to_smem<0, RC_N>(acc0, xch, RC_XLD, quad, lane);
-      acc_to_smem<0, RC_N>(acc1, xch + 64 * RC_XLD, RC_XLD, quad, lane);
+      acc_to_smem<0, N>(acc0, xch, Cfg::XLD, quad, lane);
+      acc_to_smem<0, N>(acc1, xch + 64 * Cfg::XLD, Cfg::XLD, quad, lane);
       named_bar_sync(1, 128);
-      uint8_t* srow = sO + buf * RC_SUB + r * 128;
+      uint8_t* srow = sO + buf * Cfg::STG + r * 128;
 #pragma unroll
-      for (int hb = 0; hb < 2; ++hb) {
+      for (int hb = 0; hb < N / 32; ++hb) {
         uint32_t v[32];
         smem_row_32(xrow + hb * 32, v);
         float f[32];
@@ -189,15 +194,17 @@ rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
           uint4 o;
           o.x = pack_bf16x2(f[8 * i + 0], f[8 * i + 1]); o.y = pack_bf16x2(f[8 * i + 2], f[8 * i + 3]);
           o.z = pack_bf16x2(f[8 * i + 4], f[8 * i + 5]); o.w = pack_bf16x2(f[8 * i + 6], f[8 * i + 7]);
-          *reinterpret_cast<uint4*>(srow + (((hb * 4 + i) ^ (r & 7)) << 4)) = o;
+          *reinterpret_cast<uint4*>(srow + (hb >> 1) * RC_SUB + (((((hb & 1) * 4) + i) ^ (r & 7)) << 4)) = o;
         }
+        // GroupNorm(32): N / 32 channels per group, so a 32-column chunk holds 1024 / N groups
         if (p.gn_stats != nullptr)
-          gn_chunk_stats<2>(f, p.gn_stats + (((size_t)tile * 4 + quad) * 32 + hb * 16) * 2, 0, lane);
+          gn_chunk_stats<N / 32>(f, p.gn_stats + (((size_t)tile * 4 + quad) * 32 + hb * (1024 / N)) * 2, 0, lane);
       }
       fence_proxy_async();
       named_bar_sync(1, 128);
       if (et == 0) {
-        tma_store_2d(&tmO, sO + buf * RC_SUB, 0, tile * 128);
+#pragma unroll
+        for (int pn = 0; pn < Cfg::PANELS; ++pn) tma_store_2d(&tmO, sO + buf * Cfg::STG + pn * RC_SUB, pn * 64, tile * 128);
         bulk_commit();
       }
     }
@@ -209,22 +216,22 @@ static int rc_enc2d(CUtensorMap* map, const void* base, long long ld, long long 
   return tmap_rows_bf16(map, base, ld, rows, cols, box_rows);
 }
 
-template <int KS, int STRIDE, int PAD>
+template <int KS, int STRIDE, int PAD, int N>
 static int launch_rgb(const CUtensorMap& tw, const CUtensorMap& to, const RgbConvParams& p, cudaStream_t st, const char* desc) {
-  using Cfg = RgbCfg<KS>;
+  using Cfg = RgbCfg<KS, N>;
   static PerDeviceOnce once;
   PGT_CUDA_OK(once.run([] {
-    cudaError_t e = cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     if (e != cudaSuccess) return e;
     // the resident-CTA count is fixed by the kernel's own budget (__launch_bounds__, shared memory), not
     // asked of the occupancy calculator: it answered 1 for the 3x3 kernel and left half of every SM idle
-    return cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD>, cudaFuncAttributePreferredSharedMemoryCarveout,
+    return cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD, N>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                 cudaSharedmemCarveoutMaxShared);
   }));
   const int grid = p.m_tiles < num_sms() * Cfg::PER_SM ? p.m_tiles : num_sms() * Cfg::PER_SM;
   {
-    ProfScope ps(PGT_PROF_GEMM, 2.0 * (double)p.M * RC_N * Cfg::K, st, desc);
-    rgb_conv_kernel<KS, STRIDE, PAD><<<grid, Cfg::THREADS, Cfg::SMEM, st>>>(tw, to, p);
+    ProfScope ps(PGT_PROF_GEMM, 2.0 * (double)p.M * N * Cfg::K, st, desc);
+    rgb_conv_kernel<KS, STRIDE, PAD, N><<<grid, Cfg::THREADS, Cfg::SMEM, st>>>(tw, to, p);
   }
   PGT_LAUNCH_OK();
   return PGT_OK;
@@ -238,8 +245,8 @@ extern "C" int pgt_conv_rgb_bf16(const float* x_nchw, int F, int H, int W, int k
                                  const float* mean3, const float* std3, const void* Wp, int ldw, int Cout,
                                  const float* bias, int act, void* out, int ldo, float* gn_stats, void* stream) {
   PGT_CHECK_ARG(x_nchw && Wp && bias && out && F > 0 && H > 0 && W > 0);
-  if (Cout != RC_N || !((ksize == 3 && stride == 1 && pad == 1) || (ksize == 7 && stride == 2 && pad == 3)))
-    return PGT_ERR_UNSUPPORTED;
+  const bool k3 = ksize == 3 && stride == 1 && pad == 1, k7 = ksize == 7 && stride == 2 && pad == 3;
+  if (!((Cout == 64 && (k3 || k7)) || (Cout == 128 && k3))) return PGT_ERR_UNSUPPORTED;
   PGT_CHECK_ARG(act == PGT_ACT_NONE || act == PGT_ACT_RELU);
   auto al = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   PGT_CHECK_ARG(al(Wp) && al(out) && ldw % 8 == 0 && ldo % 8 == 0 && ldw >= 3 * ksize * ksize && ldo >= Cout);
@@ -258,9 +265,11 @@ extern "C" int pgt_conv_rgb_bf16(const float* x_nchw, int F, int H, int W, int k
   if (gn_stats != nullptr && (p.Ho * p.Wo) % 128 != 0) return PGT_ERR_UNSUPPORTED;   // a tile must not straddle frames
   CUtensorMap tw, to;
   // weight rows beyond K inside the last 64-wide box are zero-filled by TMA
-  int rc = rc_enc2d(&tw, Wp, ldw, Cout, 3 * ksize * ksize, RC_N);
+  int rc = rc_enc2d(&tw, Wp, ldw, Cout, 3 * ksize * ksize, Cout);
   if (rc == PGT_OK) rc = rc_enc2d(&to, out, ldo, p.M, Cout, 128);
   if (rc != PGT_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return ksize == 3 ? launch_rgb<3, 1, 1>(tw, to, p, st, "rgb_conv 3x3/1 N64") : launch_rgb<7, 2, 3>(tw, to, p, st, "rgb_conv 7x7/2 N64");
+  if (Cout == 128) return launch_rgb<3, 1, 1, 128>(tw, to, p, st, "rgb_conv 3x3/1 N128");
+  return ksize == 3 ? launch_rgb<3, 1, 1, 64>(tw, to, p, st, "rgb_conv 3x3/1 N64")
+                    : launch_rgb<7, 2, 3, 64>(tw, to, p, st, "rgb_conv 7x7/2 N64");
 }

@@ -79,6 +79,19 @@ void l2_argmin(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor
   check(rc, "l2_argmin");
 }
 
+void l2_argmin_split(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor& cb16, const at::Tensor& norm,
+                     int64_t K, int64_t splits, at::Tensor idx, const c10::optional<at::Tensor>& quant) {
+  TORCH_CHECK(z.is_cuda() && z.scalar_type() == at::kFloat && z.is_contiguous() && codebook.is_contiguous() &&
+              idx.scalar_type() == at::kLong && splits >= 1, "l2_argmin_split: fp32 contiguous z / codebook, int64 idx");
+  c10::cuda::CUDAGuard guard(z.device());
+  const int T = (int)z.size(0), E = (int)z.size(1);
+  auto ws = at::empty({pgt_l2_argmin_split_ws_ints(T, (int)splits)}, z.options().dtype(at::kInt));
+  float* qp = quant.has_value() ? quant->data_ptr<float>() : nullptr;
+  check(pgt_l2_argmin_tc_split(z.data_ptr<float>(), T, E, codebook.data_ptr<float>(), cb16.data_ptr(),
+                               norm.data_ptr<float>(), (int)K, (int)splits, idx.data_ptr<int64_t>(), qp, ws.data_ptr<int>(),
+                               stream_of(z)), "l2_argmin_split");
+}
+
 void soft_codes(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor& norm, int64_t K, double temp,
                 at::Tensor out) {
   TORCH_CHECK(z.is_cuda() && z.scalar_type() == at::kFloat && z.is_contiguous() && codebook.scalar_type() == at::kFloat &&
@@ -233,6 +246,8 @@ TORCH_LIBRARY(pgt, m) {
   m.def("argmax_gather(Tensor logits, Tensor codebook, Tensor(a!) idx, Tensor(b!) quant) -> ()");
   m.def("codebook_pack(Tensor codebook, int K) -> (Tensor, Tensor)");
   m.def("l2_argmin(Tensor z, Tensor codebook, Tensor cb16, Tensor norm, int K, Tensor(a!) idx, Tensor(b!)? quant) -> ()");
+  m.def("l2_argmin_split(Tensor z, Tensor codebook, Tensor cb16, Tensor norm, int K, int splits, Tensor(a!) idx, "
+        "Tensor(b!)? quant) -> ()");
   m.def("linear(Tensor a, Tensor w, Tensor? bias, int act, Tensor? residual, Tensor(a!) out) -> ()");
   m.def("soft_codes(Tensor z, Tensor codebook, Tensor norm, int K, float temp, Tensor(a!) out) -> ()");
   m.def("sample_codes(Tensor p, Tensor seed, Tensor(a!) idx) -> ()");
@@ -251,6 +266,7 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("argmax_gather", argmax_gather);
   m.impl("codebook_pack", codebook_pack);
   m.impl("l2_argmin", l2_argmin);
+  m.impl("l2_argmin_split", l2_argmin_split);
   m.impl("linear", linear);
   m.impl("soft_codes", soft_codes);
   m.impl("sample_codes", sample_codes);

@@ -449,11 +449,11 @@ class Engine:
 
     def conv_in(self, x, p='encoder.conv_in'):
         """encoder.conv_in on the fp32 NCHW frames.  Cin = 3: the kernel builds the patch rows itself; its epilogue also
-        yields block 0's GroupNorm statistics."""
+        yields block 0's GroupNorm statistics (a.ch = 64 or 128)."""
         a = self.arch
         Fr, _, H, W = x.shape
         h = self._new(Fr, H, W, a.ch)
-        stats = self._gn_stats(h, H * W // 32) if (H * W) % 128 == 0 and a.ch == 64 else None
+        stats = self._gn_stats(h, H * W // 32) if (H * W) % 128 == 0 and a.ch in (64, 128) else None
         ops.conv_rgb(x, self.w[p + '.weight'], self.w[p + '.bias'], h, 3, 1, 1, gn_stats=stats)
         return h
 
@@ -691,25 +691,32 @@ class Engine:
             return self.w['codebook']
         return self.w['codebooks'][d]
 
+    def _n_embed(self, d=0):
+        """Codes in depth d's codebook (the rows before its padding row)."""
+        return self.arch.n_embed
+
     def _codebook_pack(self, d=0):
         """bf16 copy + fp32 norms of depth d's codebook (l2_argmin_tc, soft_codes), once per load and distinct codebook."""
         key = 'codebook.pack' if d == 0 or self.arch.shared_codebook else 'codebook.pack.%d' % d
         if key not in self.w:
-            self.w[key] = ops.codebook_pack(self._codebook(d), self.arch.n_embed)
+            self.w[key] = ops.codebook_pack(self._codebook(d), self._n_embed(d))
         return self.w[key]
+
+    def _argmin(self, *a, **k):
+        """The exact L2 argmin quantize runs (RQVAEEngine: the codebook-split one)."""
+        return ops.l2_argmin_tc(*a, **k)
 
     def quantize(self, z):
         """RQBottleneck.quantize + compute_commitment_loss (`archs/tdcrqvae3_arch.py:294-352`) of z fp32 [T, E]:
         at each depth the exact L2 argmin of the residual over that depth's codebook, then residual -= e, aggregate
         += e in fp32.  Returns (codes int64 [T, D], z_q fp32 [T, E] = the aggregate of all depths, loss = mean over
         depths of mean((z - aggregate_d)^2))."""
-        a = self.arch
         T, E = z.shape
         D = self.depth
         z_q = self._new(T, E, dtype=torch.float32)
         if D == 1:
             codes = torch.empty(T, dtype=torch.int64, device=self.dev)
-            ops.l2_argmin_tc(z, self.w['codebook'], self._codebook_pack(), a.n_embed, codes, z_q)
+            self._argmin(z, self.w['codebook'], self._codebook_pack(), self._n_embed(0), codes, z_q)
             return codes.view(T, 1), z_q, (z - z_q).pow(2).mean()
         # codes depth-major, as l2_argmin_tc writes them; the residual is a scratch buffer (z itself is never copied)
         # and is updated after the argmin and its exhaustive fallback have both run
@@ -718,7 +725,7 @@ class Engine:
         losses = []
         for d in range(D):
             src = z if d == 0 else r
-            ops.l2_argmin_tc(src, self._codebook(d), self._codebook_pack(d), a.n_embed, codes[d])
+            self._argmin(src, self._codebook(d), self._codebook_pack(d), self._n_embed(d), codes[d])
             ops.rq_residual(src, r if d < D - 1 else None, codes[d], self._codebook(d), z_q, d == 0)
             losses.append((z - z_q).pow(2).mean())
         return codes.t().contiguous(), z_q, torch.stack(losses).mean()
@@ -726,14 +733,15 @@ class Engine:
     @_on_device
     @torch.no_grad()
     def encode(self, x):
-        """TDCRQVAE3.encode (`archs/tdcrqvae3_arch.py:774-777`): x fp32 [F,3,H,W] -> z_e fp32 NHWC [F,H/16,W/16,E]."""
+        """TDCRQVAE3.encode (`archs/tdcrqvae3_arch.py:774-777`): x fp32 [F,3,H,W] -> z_e fp32 NHWC [F,h,w,E], h x w the
+        encoder's latent map (H/16 x W/16 for the four-downsample encoders)."""
         a = self.arch
         x = x.to(self.dev, torch.float32).contiguous()
-        Fr, _, H, W = x.shape
         self._fusing = False                                   # the plain autoencoder has no SFT fusion
         h, _ = self.encoder(x)
-        z_e = self._lin(h.view(Fr * (H // 16) * (W // 16), -1), 'quant_conv', a.embed_dim, out_dtype=torch.float32)
-        return z_e.view(Fr, H // 16, W // 16, a.embed_dim)
+        Fr, hh, ww, _ = h.shape
+        z_e = self._lin(h.view(Fr * hh * ww, -1), 'quant_conv', a.embed_dim, out_dtype=torch.float32)
+        return z_e.view(Fr, hh, ww, a.embed_dim)
 
     @_on_device
     @torch.no_grad()

@@ -109,7 +109,8 @@ def conv(x, wp, cout, out, ksize=3, stride=1, pad_lo=1, bias=None, act=ACT_NONE,
 
 
 def conv_rgb(x_nchw, wp, bias, out, ksize, stride, pad, act=ACT_NONE, mean3=None, std3=None, gn_stats=None):
-    """Cin = 3 conv on the tensor cores straight from the fp32 NCHW image; wp [64, Kpad] bf16 (engine._pack_rgb)."""
+    """Cin = 3 conv on the tensor cores straight from the fp32 NCHW image; wp [Cout, Kpad] bf16 (engine._pack_rgb), Cout 64
+    (3x3 / 1 and 7x7 / 2) or 128 (3x3 / 1)."""
     lib = L.load()
     F, C, H, W = x_nchw.shape
     assert C == 3 and x_nchw.dtype == torch.float32 and x_nchw.is_contiguous() and wp.dtype == torch.bfloat16
@@ -196,7 +197,7 @@ def groupnorm_ab(x, gamma, beta, ab, stats=None, chunks_per_frame=0, eps=1e-6):
 
 
 def conv_out_gn(x, ab, wp, cout, bias, out, silu=True):
-    """conv3x3(silu(groupnorm(x))) -> fp32 NCHW for the decoder tail (Cin = 64, Cout <= 3); with silu=False
+    """conv3x3(silu(groupnorm(x))) -> fp32 NCHW for the decoder tail (Cin = 64 or 128, Cout <= 3); with silu=False
     conv3x3(groupnorm(x)) (VQGAN's generator tail).  None when not covered."""
     lib = L.load()
     F, H, W, Cin = x.shape
@@ -373,6 +374,31 @@ def l2_argmin_tc(z, codebook, pack, K, idx_out, quant=None):
     if rc == L2_ARGMIN_UNSUPPORTED:
         return l2_argmin(z, codebook, K, idx_out, quant)
     L.check(rc)
+    return idx_out, quant
+
+
+ARGMIN_MIN_CODES_PER_SPLIT = 512     # floor on codes per range of l2_argmin_tc_split (DESIGN §6, item 8)
+
+
+def argmin_splits(T, K, device=None):
+    """Code ranges for l2_argmin_tc_split: enough (token tile, range) CTAs to cover the SMs, min(K / 128, SMs / tiles),
+    but no range below ARGMIN_MIN_CODES_PER_SPLIT codes; 1 once the token tiles alone fill the GPU."""
+    sms = torch.cuda.get_device_properties(device if device is not None else torch.cuda.current_device()).multi_processor_count
+    tiles = (T + 127) // 128
+    return max(1, min(K // 128, sms // tiles, K // ARGMIN_MIN_CODES_PER_SPLIT))
+
+
+def l2_argmin_tc_split(z, codebook, pack, K, idx_out, quant=None, splits=None):
+    """l2_argmin_tc with the codebook split over `splits` code ranges (default argmin_splits(T, K)): the same codes, more
+    CTAs at small T (l2_argmin_tc.cu).  K a multiple of 128, E a multiple of 128 up to 512."""
+    lib = L.load()
+    T, E = z.shape
+    assert z.dtype == torch.float32 and z.is_contiguous() and codebook.is_contiguous() and idx_out.dtype == torch.int64
+    if splits is None:
+        splits = argmin_splits(T, K, z.device)
+    ws = torch.empty(int(lib.pgt_l2_argmin_split_ws_ints(T, int(splits))), dtype=torch.int32, device=z.device)
+    L.check(lib.pgt_l2_argmin_tc_split(_p(z), T, E, _p(codebook), _p(pack[0]), _p(pack[1]), K, int(splits), _p(idx_out),
+                                       _p(quant), _p(ws), _stream(z)))
     return idx_out, quant
 
 

@@ -350,6 +350,22 @@ class TDRQVAEArch:
 def build_tdrqvae_spec(network_g):
     a = TDRQVAEArch(network_g)
     s = Spec()
+    _rqvae_autoencoder(s, a)
+    # ---- quantiser (:206-223, 381-394): one shared codebook of depth 1
+    e = a.embed_dim
+    s.add('quantizer.codebooks.0.weight', (a.n_embed + 1, e), 'codebook')
+    s.add('quantizer.codebooks.0.cluster_size_ema', (a.n_embed,), 'zeros')
+    s.add('quantizer.codebooks.0.embed_ema', (a.n_embed, e), 'codebook_ema')
+    _conv(s, 'quant_conv', a.z_channels, e, 1)
+    _conv(s, 'post_quant_conv', e, a.z_channels, 1)
+    for p in ('tdswin_pre', 'tdswin_post'):
+        _swin3d_layer(s, p, e, a.stages_atten, a.num_head, a.window_size)
+    return a, s
+
+
+def _rqvae_autoencoder(s, a):
+    """The 2-D RQ-VAE Encoder and Decoder TDRQVAE and RQVAE share (`archs/tdrqvae_arch.py:587-751`,
+    `archs/rqvae_arch.py:579-743`)."""
     in_mult = (1,) + a.ch_mult
     # ---- Encoder (tdrqvae_arch.py:587-648)
     _conv(s, 'encoder.conv_in', a.in_channels, a.ch, 3)
@@ -387,15 +403,97 @@ def build_tdrqvae_spec(network_g):
             _conv(s, 'decoder.up.%d.upsample.conv' % lvl, block_in, block_in, 3)
     _norm(s, 'decoder.norm_out', block_in)
     _conv(s, 'decoder.conv_out', block_in, a.out_ch, 3)
-    # ---- quantiser (:206-223, 381-394): one shared codebook of depth 1
-    e = a.embed_dim
-    s.add('quantizer.codebooks.0.weight', (a.n_embed + 1, e), 'codebook')
-    s.add('quantizer.codebooks.0.cluster_size_ema', (a.n_embed,), 'zeros')
-    s.add('quantizer.codebooks.0.embed_ema', (a.n_embed, e), 'codebook_ema')
-    _conv(s, 'quant_conv', a.z_channels, e, 1)
-    _conv(s, 'post_quant_conv', e, a.z_channels, 1)
-    for p in ('tdswin_pre', 'tdswin_post'):
-        _swin3d_layer(s, p, e, a.stages_atten, a.num_head, a.window_size)
+
+
+class RQVAEArch:
+    """Resolved constants of the registered RQVAE (`archs/rqvae_arch.py:779-931`): the 2-D Encoder / Decoder around an
+    RQBottleneck of depth D = code_shape[2], one codebook per depth (`n_embed` an int or a list of D sizes) or one shared
+    by every depth.  Raises ValueError for what the reference rejects, for what it accepts but fails on at forward, and
+    for what the CUDA kernels cannot run."""
+
+    def __init__(self, network_g):
+        g = dict(network_g)
+        dd = dict(g['ddconfig'])
+        if g.get('bottleneck_type', 'rq') != 'rq':
+            raise ValueError("invalid 'bottleneck_type' (must be 'rq')")     # rqvae_arch.py:820
+        self.embed_dim = int(g.get('embed_dim', 64))
+        self.latent_shape = tuple(int(v) for v in g['latent_shape'])
+        self.code_shape = tuple(int(v) for v in g['code_shape'])
+        self.shared_codebook = bool(g['shared_codebook'])
+        if not len(self.code_shape) == len(self.latent_shape) == 3:
+            raise ValueError('incompatible code shape or latent shape')      # rqvae_arch.py:350-353
+        if any(y % x != 0 for x, y in zip(self.code_shape[:2], self.latent_shape[:2])):
+            raise ValueError('incompatible code shape or latent shape')
+        self.depth = self.code_shape[2]
+        n = g.get('n_embed', 512)
+        if isinstance(n, (list, tuple)):
+            if self.shared_codebook:
+                raise ValueError('Shared codebooks are incompatible with list types of momentums or sizes: '
+                                 'Change it into int')                      # rqvae_arch.py:363-366
+            if len(n) != self.depth:
+                raise ValueError('n_embed lists one size per code depth: %d sizes for depth %d' % (len(n), self.depth))
+            self.n_embeds = tuple(int(k) for k in n)
+        else:
+            self.n_embeds = (int(n),) * self.depth
+        self.n_embed = max(self.n_embeds)                                    # rows of the padded per-depth codebook stack
+        self.ch = int(dd['ch'])
+        self.ch_mult = tuple(dd['ch_mult'])
+        self.num_res_blocks = int(dd['num_res_blocks'])
+        self.resolution = int(dd['resolution'])
+        self.attn_resolutions = tuple(dd['attn_resolutions'])
+        self.z_channels = int(dd['z_channels'])
+        self.in_channels = int(dd['in_channels'])
+        self.out_ch = int(dd['out_ch'])
+        self.double_z = bool(dd.get('double_z', True))
+        self.num_levels = len(self.ch_mult)
+        self.down = 2 ** (self.num_levels - 1)
+        self.level_ch = tuple(self.ch * m for m in self.ch_mult)
+        self.level_has_attn = tuple((self.resolution >> i) in self.attn_resolutions for i in range(self.num_levels))
+        if self.depth < 1:
+            raise ValueError('quantiser depth code_shape[2] must be >= 1, got %d' % self.depth)
+        if self.code_shape[:2] != self.latent_shape[:2]:
+            raise ValueError('code_shape %s, latent_shape %s: code-shape divisors > 1 are not supported'
+                             % (self.code_shape, self.latent_shape))
+        if self.latent_shape[2] != self.embed_dim:
+            # the codebooks are latent_shape[2] wide and quantise quant_conv's embed_dim channels (rqvae_arch.py:356)
+            raise ValueError('latent_shape[2] = %d must equal embed_dim = %d' % (self.latent_shape[2], self.embed_dim))
+        if self.double_z:
+            raise ValueError('double_z: Encoder.conv_out would give 2 * z_channels, quant_conv reads z_channels')
+        if not dd.get('resamp_with_conv', True):
+            raise ValueError('resamp_with_conv=False (average-pool / nearest resampling) is not supported')
+        if dd.get('give_pre_end', False):
+            raise ValueError('give_pre_end=True (the decoder without its norm_out / conv_out tail) is not supported')
+        if self.in_channels != 3 or self.ch not in RGB_STEM_WIDTHS:
+            raise ValueError('the CUDA path is built for RGB input and ch in %s' % (RGB_STEM_WIDTHS,))
+        if any(c % 32 for c in self.level_ch):
+            raise ValueError('GroupNorm(32): every level width must be a multiple of 32')
+        widths = {c for c, a in zip(self.level_ch, self.level_has_attn) if a} | {self.level_ch[-1]}
+        if not widths <= set(ATTN_WIDTHS):
+            raise ValueError('AttnBlock widths %s: the attention kernel takes %s' % (sorted(widths), ATTN_WIDTHS))
+        if self.embed_dim % 128 or self.embed_dim > 512 or any(k % 128 or k < 128 for k in self.n_embeds):
+            raise ValueError('embed_dim %d, n_embed %s: the argmin takes codebooks of a multiple of 128 up to 512 '
+                             'channels and a multiple of 128 codes' % (self.embed_dim, list(self.n_embeds)))
+
+
+RGB_STEM_WIDTHS = (64, 128)           # pgt_conv_rgb_bf16 3x3 output widths
+
+
+def build_rqvae_spec(network_g):
+    a = RQVAEArch(network_g)
+    s = Spec()
+    _rqvae_autoencoder(s, a)
+    # ---- RQBottleneck (rqvae_arch.py:199-216, 374-387): one VQEmbedding per depth, or one shared by every depth
+    e = a.latent_shape[2]
+    for d in range(a.depth):
+        p = 'quantizer.codebooks.%d' % d
+        k = a.n_embeds[d]
+        s.add(p + '.weight', (k + 1, e), 'codebook')
+        s.add(p + '.cluster_size_ema', (k,), 'zeros')
+        s.add(p + '.embed_ema', (k, e), 'codebook_ema')
+        if a.shared_codebook and d > 0:
+            s.module_aliases[p] = 'quantizer.codebooks.0'
+    _conv(s, 'quant_conv', a.z_channels, a.embed_dim, 1)
+    _conv(s, 'post_quant_conv', a.embed_dim, a.z_channels, 1)
     return a, s
 
 

@@ -19,6 +19,11 @@ class TDRQVAEEngine(Engine):
     arch_class = TDRQVAEArch
 
     def _repack(self):
+        self._repack_autoencoder()
+        self.swin = {p: pack_blocks(lambda k, p=p: self._sd.get(p + '.' + k), self.arch.stages_atten) for p in SWIN_LAYERS}
+
+    def _repack_autoencoder(self):
+        """Encoder / decoder convs, AttnBlock projections and codebook 0 in kernel layouts (RQVAEEngine shares it)."""
         sd, w = self._sd, self.w
         for name, t in sd.items():
             if name.startswith(SWIN_LAYERS):
@@ -36,7 +41,6 @@ class TDRQVAEEngine(Engine):
                 w[name] = t.float().contiguous()
         w['codebook'] = self._f32('quantizer.codebooks.0.weight')
         self._repack_attn_qkv()
-        self.swin = {p: pack_blocks(lambda k, p=p: sd.get(p + '.' + k), self.arch.stages_atten) for p in SWIN_LAYERS}
 
     # ------------------------------------------------------------------ blocks
     def encoder(self, x):
