@@ -267,20 +267,17 @@ int pgt_l2_argmin_tc_split(const float* z, int T, int E, const float* codebook, 
 /* ---- soft codes of one quantiser depth (RQBottleneck.get_soft_codes, archs/tdcrqvae3_arch.py:429-457).
  * pgt_soft_codes: out[t, k] = softmax_k((2 z[t].e_k - ||e_k||^2) / temp) = softmax_k(-||z[t] - e_k||^2 / temp) over the
  *   first K codebook rows; z fp32 [T, E]; codebook fp32 [K(+1), E]; cb_norm fp32 [>= K] = ||e_k||^2 (the norms
- *   pgt_codebook_pack writes); out fp32 [T, K].  3xTF32 tensor-core dot products (soft_codes.cu), fp32 softmax.
- *   temp must be finite and > 0.  Returns PGT_ERR_UNSUPPORTED unless K % 128 == 0 and E % 32 == 0.
- * pgt_sample_codes: idx[t] = one draw from row t of p fp32 [T, K] (non-negative, any positive sum), Philox keyed by the
- *   DEVICE int64 seed[2]; a zero-probability index is never drawn; a row with no positive entry yields -1.  Replaces
- *   torch.multinomial(soft_code, 1) (:441-444). */
+ *   pgt_codebook_pack writes); out fp32 [T, K] with row pitch ldo.  3xTF32 tensor-core dot products (soft_codes.cu),
+ *   fp32 softmax.  temp must be finite and > 0.  Returns PGT_ERR_UNSUPPORTED unless K % 128 == 0 and E % 32 == 0.
+ * pgt_sample_codes: idx[t] = one draw from row t of p fp32 [T, K] with row pitch ldp (non-negative, any positive sum),
+ *   Philox keyed by the DEVICE int64 seed[2]; a zero-probability index is never drawn; a row with no positive entry
+ *   yields -1.  Replaces torch.multinomial(soft_code, 1) (:441-444).
+ * Row pitches are in elements, ldo / ldp >= K, ldo % 4 == 0: at quantiser depth D, depth d writes and reads the K-slice
+ * d of a contiguous [T, D, K] soft-code tensor (ldo = D * K), as RQBottleneck.get_soft_codes concatenates them
+ * (:429-457); a contiguous [T, K] tensor is the pitch = K case. */
 int pgt_soft_codes(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
-                   float* out, void* stream);
-int pgt_sample_codes(const float* p, int T, int K, const int64_t* seed, int64_t* idx, void* stream);
-/* The same two with a row pitch (elements, ldo / ldp >= K, ldo % 4 == 0): at quantiser depth D, depth d writes and
- * reads the K-slice d of a contiguous [T, D, K] soft-code tensor (ldo = D * K), as RQBottleneck.get_soft_codes
- * concatenates them (:429-457).  pgt_soft_codes / pgt_sample_codes are the pitch = K case. */
-int pgt_soft_codes_ld(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
-                      float* out, int ldo, void* stream);
-int pgt_sample_codes_ld(const float* p, int T, int K, int ldp, const int64_t* seed, int64_t* idx, void* stream);
+                   float* out, int ldo, void* stream);
+int pgt_sample_codes(const float* p, int T, int K, int ldp, const int64_t* seed, int64_t* idx, void* stream);
 
 /* ---- residual quantisation over D code levels (rq.cu; RQBottleneck.quantize / embed_code / embed_partial_code /
  * embed_code_with_depth, archs/tdcrqvae3_arch.py:294-426).  Level d's code is pgt_l2_argmin_tc of the level's residual.

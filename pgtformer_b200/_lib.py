@@ -78,10 +78,8 @@ SIGNATURES = {
     'pgt_l2_argmin_split_ws_ints': (c_int64, [c_int, c_int]),
     'pgt_l2_argmin_tc_split': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
                                        c_void_p, c_void_p, c_void_p]),
-    'pgt_soft_codes': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p]),
-    'pgt_sample_codes': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
-    'pgt_soft_codes_ld': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_void_p, c_int, c_void_p]),
-    'pgt_sample_codes_ld': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    'pgt_soft_codes': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_void_p, c_int, c_void_p]),
+    'pgt_sample_codes': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'pgt_rq_residual': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     'pgt_rq_embed': (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_int, c_void_p, c_int,
                              c_int, c_void_p]),

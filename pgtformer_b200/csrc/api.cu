@@ -96,7 +96,7 @@ extern "C" const char* pgt_strerror(int status) {
   }
 }
 extern "C" const char* pgt_last_cuda_error(void) { return pgt::g_last_error; }
-extern "C" int pgt_version(void) { return 201; }
+extern "C" int pgt_version(void) { return 202; }
 extern "C" void pgt_tmap_cache_stats(int64_t* hits, int64_t* misses) {
   long long h = 0, m = 0;
   pgt::tmap_cache_stats(&h, &m);

@@ -308,17 +308,13 @@ extern "C" int pgt_argmax_gather(const float* logits, int T, int K, const float*
   return PGT_OK;
 }
 
-extern "C" int pgt_sample_codes_ld(const float* p, int T, int K, int ldp, const int64_t* seed, int64_t* idx,
-                                   void* stream) {
+extern "C" int pgt_sample_codes(const float* p, int T, int K, int ldp, const int64_t* seed, int64_t* idx,
+                                void* stream) {
   PGT_CHECK_ARG(p && seed && idx && T > 0 && K > 0 && ldp >= K);
   ProfScope ps(PGT_PROF_ARGMAX, (double)T * K * 4 + (double)T * 8, static_cast<cudaStream_t>(stream), "sample_codes");
   sample_codes_kernel<<<ceil_div(T, 8), 256, 0, static_cast<cudaStream_t>(stream)>>>(p, T, K, seed, idx, ldp);
   PGT_LAUNCH_OK();
   return PGT_OK;
-}
-
-extern "C" int pgt_sample_codes(const float* p, int T, int K, const int64_t* seed, int64_t* idx, void* stream) {
-  return pgt_sample_codes_ld(p, T, K, K, seed, idx, stream);
 }
 
 extern "C" int pgt_l2_argmin(const float* z, int T, int E, const float* codebook, int K, int64_t* idx, float* quant,

@@ -236,8 +236,8 @@ soft_codes_kernel(const float* __restrict__ z, int T, int E, const float* __rest
 
 using namespace pgt;
 
-static int soft_codes_launch(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
-                             float* out, int ldo, void* stream) {
+extern "C" int pgt_soft_codes(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
+                              float* out, int ldo, void* stream) {
   PGT_CHECK_ARG(z && codebook && cb_norm && out && T > 0 && K > 0 && E > 0 && ldo >= K && ldo % 4 == 0);
   PGT_CHECK_ARG(temp > 0.f && temp <= FLT_MAX);            // also rejects NaN
   PGT_CHECK_ARG((reinterpret_cast<uintptr_t>(z) & 15) == 0 && (reinterpret_cast<uintptr_t>(codebook) & 15) == 0 &&
@@ -250,14 +250,4 @@ static int soft_codes_launch(const float* z, int T, int E, const float* codebook
   soft_codes_kernel<<<ceil_div(T, SC_BM), 256, SC_SMEM, st>>>(z, T, E, codebook, cb_norm, K, temp, out, ldo);
   PGT_LAUNCH_OK();
   return PGT_OK;
-}
-
-extern "C" int pgt_soft_codes(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K, float temp,
-                              float* out, void* stream) {
-  return soft_codes_launch(z, T, E, codebook, cb_norm, K, temp, out, K, stream);
-}
-
-extern "C" int pgt_soft_codes_ld(const float* z, int T, int E, const float* codebook, const float* cb_norm, int K,
-                                 float temp, float* out, int ldo, void* stream) {
-  return soft_codes_launch(z, T, E, codebook, cb_norm, K, temp, out, ldo, stream);
 }

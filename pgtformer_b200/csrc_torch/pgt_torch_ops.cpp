@@ -96,42 +96,22 @@ void soft_codes(const at::Tensor& z, const at::Tensor& codebook, const at::Tenso
                 at::Tensor out) {
   TORCH_CHECK(z.is_cuda() && z.scalar_type() == at::kFloat && z.is_contiguous() && codebook.scalar_type() == at::kFloat &&
               codebook.is_contiguous() && norm.scalar_type() == at::kFloat && out.scalar_type() == at::kFloat &&
-              out.is_contiguous() && out.size(0) == z.size(0) && out.size(1) == K,
-              "soft_codes: fp32 contiguous z [T, E], codebook, norm, out [T, K]");
+              out.dim() == 2 && out.stride(1) == 1 && out.size(0) == z.size(0) && out.size(1) == K,
+              "soft_codes: fp32 contiguous z [T, E], codebook, norm, row-pitched out [T, K]");
   c10::cuda::CUDAGuard guard(z.device());
-  check(pgt_soft_codes(z.data_ptr<float>(), (int)z.size(0), (int)z.size(1), codebook.data_ptr<float>(), norm.data_ptr<float>(),
-                       (int)K, (float)temp, out.data_ptr<float>(), stream_of(z)), "soft_codes");
+  check(pgt_soft_codes(z.data_ptr<float>(), (int)z.size(0), (int)z.size(1), codebook.data_ptr<float>(),
+                       norm.data_ptr<float>(), (int)K, (float)temp, out.data_ptr<float>(), (int)out.stride(0),
+                       stream_of(z)), "soft_codes");
 }
 
 void sample_codes(const at::Tensor& p, const at::Tensor& seed, at::Tensor idx) {
-  TORCH_CHECK(p.is_cuda() && p.scalar_type() == at::kFloat && p.is_contiguous() && seed.scalar_type() == at::kLong &&
-              seed.numel() == 2 && seed.device() == p.device() && idx.scalar_type() == at::kLong && idx.numel() == p.size(0),
-              "sample_codes: fp32 contiguous p [T, K], device int64 seed [2], int64 idx [T]");
-  c10::cuda::CUDAGuard guard(p.device());
-  check(pgt_sample_codes(p.data_ptr<float>(), (int)p.size(0), (int)p.size(1), seed.data_ptr<int64_t>(), idx.data_ptr<int64_t>(),
-                         stream_of(p)), "sample_codes");
-}
-
-void soft_codes_ld(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor& norm, int64_t K, double temp,
-                   at::Tensor out) {
-  TORCH_CHECK(z.is_cuda() && z.scalar_type() == at::kFloat && z.is_contiguous() && codebook.scalar_type() == at::kFloat &&
-              codebook.is_contiguous() && norm.scalar_type() == at::kFloat && out.scalar_type() == at::kFloat &&
-              out.dim() == 2 && out.stride(1) == 1 && out.size(0) == z.size(0) && out.size(1) == K,
-              "soft_codes_ld: fp32 contiguous z [T, E], codebook, norm, row-pitched out [T, K]");
-  c10::cuda::CUDAGuard guard(z.device());
-  check(pgt_soft_codes_ld(z.data_ptr<float>(), (int)z.size(0), (int)z.size(1), codebook.data_ptr<float>(),
-                          norm.data_ptr<float>(), (int)K, (float)temp, out.data_ptr<float>(), (int)out.stride(0),
-                          stream_of(z)), "soft_codes_ld");
-}
-
-void sample_codes_ld(const at::Tensor& p, const at::Tensor& seed, at::Tensor idx) {
   TORCH_CHECK(p.is_cuda() && p.scalar_type() == at::kFloat && p.dim() == 2 && p.stride(1) == 1 &&
               seed.scalar_type() == at::kLong && seed.numel() == 2 && seed.device() == p.device() &&
               idx.scalar_type() == at::kLong && idx.is_contiguous() && idx.numel() == p.size(0),
-              "sample_codes_ld: fp32 row-pitched p [T, K], device int64 seed [2], int64 idx [T]");
+              "sample_codes: fp32 row-pitched p [T, K], device int64 seed [2], int64 idx [T]");
   c10::cuda::CUDAGuard guard(p.device());
-  check(pgt_sample_codes_ld(p.data_ptr<float>(), (int)p.size(0), (int)p.size(1), (int)p.stride(0), seed.data_ptr<int64_t>(),
-                            idx.data_ptr<int64_t>(), stream_of(p)), "sample_codes_ld");
+  check(pgt_sample_codes(p.data_ptr<float>(), (int)p.size(0), (int)p.size(1), (int)p.stride(0), seed.data_ptr<int64_t>(),
+                         idx.data_ptr<int64_t>(), stream_of(p)), "sample_codes");
 }
 
 void rq_residual(const c10::optional<at::Tensor>& r_in, const c10::optional<at::Tensor>& r_out, const at::Tensor& idx,
@@ -251,8 +231,6 @@ TORCH_LIBRARY(pgt, m) {
   m.def("linear(Tensor a, Tensor w, Tensor? bias, int act, Tensor? residual, Tensor(a!) out) -> ()");
   m.def("soft_codes(Tensor z, Tensor codebook, Tensor norm, int K, float temp, Tensor(a!) out) -> ()");
   m.def("sample_codes(Tensor p, Tensor seed, Tensor(a!) idx) -> ()");
-  m.def("soft_codes_ld(Tensor z, Tensor codebook, Tensor norm, int K, float temp, Tensor(a!) out) -> ()");
-  m.def("sample_codes_ld(Tensor p, Tensor seed, Tensor(a!) idx) -> ()");
   m.def("rq_residual(Tensor? r_in, Tensor(a!)? r_out, Tensor idx, Tensor codebook, Tensor(b!)? agg, bool first) -> ()");
   m.def("rq_embed(Tensor idx, int d0, int d1, Tensor codebooks, Tensor(a!) out, int ldi, int ldd) -> ()");
   m.def("conv_out_gn_act(Tensor x, Tensor ab, Tensor wp, int cout, Tensor? bias, bool silu, Tensor(a!) out) -> ()");
@@ -270,8 +248,6 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("linear", linear);
   m.impl("soft_codes", soft_codes);
   m.impl("sample_codes", sample_codes);
-  m.impl("soft_codes_ld", soft_codes_ld);
-  m.impl("sample_codes_ld", sample_codes_ld);
   m.impl("rq_residual", rq_residual);
   m.impl("rq_embed", rq_embed);
   m.impl("conv_out_gn_act", conv_out_gn_act);

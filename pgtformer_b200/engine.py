@@ -16,6 +16,7 @@ import torch.nn.functional as F  # noqa: F401  (load-time weight padding only)
 
 from . import ops
 from .spec import Arch
+from .swin3d import pack_blocks
 
 BF = torch.bfloat16
 
@@ -104,30 +105,35 @@ class Engine:
         return self._sd[name].float().contiguous()
 
     def _repack(self):
-        sd, w = self._sd, self.w
-        for name, t in sd.items():
-            if name.startswith('conditionnet.'):
-                continue
-            if name.endswith('.weight') and t.dim() == 4:
-                if name == 'encoder.conv_in.weight':
-                    w[name] = _pack_rgb(t.float())
-                elif t.shape[2] == 3 and '.upsample.conv.' in name:
-                    w[name] = _pack_up2x(t.float())
-                elif t.shape[2] == 3:
-                    w[name] = _pack_conv(t.float())
-                else:
-                    w[name] = _pack_lin(t.float())
-            elif name.endswith('.weight') and t.dim() == 2 and 'codebooks' not in name:
+        """Every model's weights into kernel layouts by one rule.  The arch names the RGB stem, the upsample convs and
+        the codebooks; any other 4-D weight is a 3x3 conv or a 1x1 conv (a linear), any other 2-D weight a linear, any
+        1-D float tensor an fp32 vector.  The fused projections follow from the names present; the prefixes in
+        arch.packed_apart are packed by a rule of their own."""
+        a, sd, w = self.arch, self._sd, self.w
+        names = [n for n in sd if not n.startswith(a.packed_apart)]
+        for name in names:
+            t = sd[name]
+            if name == a.stem:
+                w[name] = _pack_rgb(t.float())
+            elif name in a.upsample_convs:
+                w[name] = _pack_up2x(t.float())
+            elif name.endswith('.weight') and t.dim() == 4:
+                w[name] = _pack_conv(t.float()) if t.shape[2] == 3 else _pack_lin(t.float())
+            elif name.endswith('.weight') and t.dim() == 2 and name not in a.codebooks:
                 w[name] = _pack_lin(t.float())
             elif t.dtype.is_floating_point and t.dim() == 1:
                 w[name] = t.float().contiguous()
-        w['codebook'] = self._f32('quantizer.codebooks.0.weight')
+        w['codebook'] = self._f32(a.codebooks[0])
         if self.depth > 1:
-            # every distinct codebook stacked once [D or 1, K + 1, E] (rq_embed reads a shared one with depth stride 0)
-            n = 1 if self.arch.shared_codebook else self.depth
-            w['codebooks'] = torch.stack([self._f32('quantizer.codebooks.%d.weight' % d) for d in range(n)]).contiguous()
+            # every distinct codebook stacked once [D or 1, K + 1, E], each zero-padded to the largest K + 1 rows: rq_embed
+            # reads a shared one with depth stride 0, and depth d's padding row stays at index K_d
+            cbs = [self._f32(k) for k in a.codebooks[:1 if a.shared_codebook else self.depth]]
+            w['codebooks'] = torch.zeros(len(cbs), max(c.shape[0] for c in cbs), cbs[0].shape[1], dtype=torch.float32,
+                                         device=self.dev)
+            for d, cb in enumerate(cbs):
+                w['codebooks'][d, :cb.shape[0]] = cb
         # Swin blocks: fused [q | k | v] projection and the expanded relative-position bias
-        for name in list(sd):
+        for name in names:
             if name.endswith('.attn.relative_position_bias_table'):
                 p = name[:-len('.relative_position_bias_table')]
                 heads = sd[name].shape[1]
@@ -143,15 +149,22 @@ class Engine:
                     wf = torch.cat([sd[p + '.q.weight'], sd[p + '.kv.weight']], 0)
                     wg, bg = fold_layernorm_affine(wf, w[p + '.qkv.bias'], sd[blk + '.norm1.weight'], sd[blk + '.norm1.bias'])
                     w[p + '.qkv_ln.weight'], w[p + '.qkv_ln.bias'] = _pack_lin(wg), bg
+        # AttnBlock: q, k and v (1x1 convs of the same normalised input) as one [3C, C] projection
+        for name in names:
+            if name.endswith('.proj_out.weight'):
+                p = name[:-len('.proj_out.weight')]
+                w[p + '.qkv.weight'] = _pack_lin(torch.cat([sd[p + '.%s.weight' % n] for n in 'qkv'], 0).float())
+                w[p + '.qkv.bias'] = torch.cat([sd[p + '.%s.bias' % n] for n in 'qkv'], 0).float().contiguous()
         # global transformer: in_proj split into the (q,k) projection of LN(x)+pos and the v projection of LN(x)
-        E = self.arch.dim_embd
-        for i in range(self.arch.n_layers):
-            p = 'ft_layers.%d.self_attn' % i
-            wi, bi = sd[p + '.in_proj_weight'].float(), sd[p + '.in_proj_bias'].float()
-            w[p + '.qk.weight'], w[p + '.qk.bias'] = _pack_lin(wi[:2 * E]), bi[:2 * E].contiguous()
-            w[p + '.v.weight'], w[p + '.v.bias'] = _pack_lin(wi[2 * E:]), bi[2 * E:].contiguous()
+        for name in names:
+            if name.endswith('.self_attn.in_proj_weight'):
+                p = name[:-len('.in_proj_weight')]
+                wi, bi = sd[name].float(), sd[p + '.in_proj_bias'].float()
+                E = wi.shape[1]
+                w[p + '.qk.weight'], w[p + '.qk.bias'] = _pack_lin(wi[:2 * E]), bi[:2 * E].contiguous()
+                w[p + '.v.weight'], w[p + '.v.bias'] = _pack_lin(wi[2 * E:]), bi[2 * E:].contiguous()
         # Swin MLP halves: norm2's affine folded into fc1 (same algebra as norm1 -> q/kv above)
-        for name in list(sd):
+        for name in names:
             if name.endswith('.mlp.fc1.weight') and sd[name].shape == (256, 256):
                 blk = name[:-len('.mlp.fc1.weight')]
                 if (blk + '.norm2.weight') not in sd:
@@ -159,7 +172,16 @@ class Engine:
                 wg, bg = fold_layernorm_affine(sd[name], sd[blk + '.mlp.fc1.bias'], sd[blk + '.norm2.weight'],
                                                sd[blk + '.norm2.bias'])
                 w[blk + '.mlp.fc1_ln.weight'], w[blk + '.mlp.fc1_ln.bias'] = _pack_lin(wg), bg
-        self._repack_parsing()
+        # the prefixes packed by a rule of their own (BiSeNet, or one of TDRQVAE's Video-Swin BasicLayers), and
+        # CodeFormer's learned positions
+        self.swin = {}
+        for prefix in a.packed_apart:
+            if prefix == 'conditionnet.':
+                self._repack_parsing()
+            else:
+                self.swin[prefix[:-1]] = pack_blocks(lambda k, p=prefix: sd.get(p + k), a.stages_atten)
+        if 'position_emb' in sd:
+            w['position_emb'] = sd['position_emb'].to(BF).contiguous()
 
     # ------------------------------------------------------------------ small helpers
     @property
@@ -231,13 +253,10 @@ class Engine:
         Fr, H, W, C = x.shape
         w = self.w
         if C == 256:
-            # norm1 + the fused q/kv projection in one kernel (LN applied to the tile in shared memory)
-            if (p + '.attn.qkv_ln.weight') in w:      # gamma / beta already inside the weights (see _repack)
-                qkv = ops.ln_linear(x, None, None, w[p + '.attn.qkv_ln.weight'], w[p + '.attn.qkv_ln.bias'],
-                                    self._new(Fr, H, W, 3 * C))
-            else:
-                qkv = ops.ln_linear(x, w[p + '.norm1.weight'], w[p + '.norm1.bias'], w[p + '.attn.qkv.weight'],
-                                    w[p + '.attn.qkv.bias'], self._new(Fr, H, W, 3 * C))
+            # norm1 + the fused q/kv projection in one kernel (LN applied to the tile in shared memory; gamma / beta
+            # already inside the weights, see _repack)
+            qkv = ops.ln_linear(x, None, None, w[p + '.attn.qkv_ln.weight'], w[p + '.attn.qkv_ln.bias'],
+                                self._new(Fr, H, W, 3 * C))
         else:
             y = ops.layernorm(x, w[p + '.norm1.weight'], w[p + '.norm1.bias'], self._new(Fr, H, W, C))
             qkv = self._lin(y, p + '.attn.qkv', 3 * C)
@@ -246,27 +265,15 @@ class Engine:
             ops.window_attention(qkv, Fr // 3, H, W, C, heads, shift, w[p + '.attn.bias_tab'], a)   # shapes the TMA kernel does not cover
         x = self._lin(a, p + '.attn.proj', C, residual=x)
         if C == 256:
-            # norm2 + fc1 + GELU + fc2 + residual in one kernel (the hidden tile never leaves the SM)
+            # norm2 + fc1 + GELU + fc2 + residual in one kernel (the hidden tile never leaves the SM; gamma / beta
+            # already inside fc1, see _repack)
             out = self._new(Fr, H, W, C) if out is None else out
             stats = self._gn_stats(out, H * W // 32) if gn_next and (H * W) % 128 == 0 else None
-            if (p + '.mlp.fc1_ln.weight') in w:       # gamma / beta already inside fc1 (see _repack)
-                return ops.swin_mlp(x, None, None, w[p + '.mlp.fc1_ln.weight'], w[p + '.mlp.fc1_ln.bias'],
-                                    w[p + '.mlp.fc2.weight'], w[p + '.mlp.fc2.bias'], out, gn_stats=stats)
-            return ops.swin_mlp(x, w[p + '.norm2.weight'], w[p + '.norm2.bias'], w[p + '.mlp.fc1.weight'],
-                                w[p + '.mlp.fc1.bias'], w[p + '.mlp.fc2.weight'], w[p + '.mlp.fc2.bias'], out,
-                                gn_stats=stats)
+            return ops.swin_mlp(x, None, None, w[p + '.mlp.fc1_ln.weight'], w[p + '.mlp.fc1_ln.bias'],
+                                w[p + '.mlp.fc2.weight'], w[p + '.mlp.fc2.bias'], out, gn_stats=stats)
         y = ops.layernorm(x, w[p + '.norm2.weight'], w[p + '.norm2.bias'], self._new(Fr, H, W, C))
         m = self._lin(y, p + '.mlp.fc1', C, act=ops.ACT_GELU)
         return self._lin(m, p + '.mlp.fc2', C, residual=x, gn_out=gn_next, out=out)
-
-    def _repack_attn_qkv(self):
-        """AttnBlock: q, k and v (1x1 convs of the same normalised input) as one [3C, C] projection."""
-        sd, w = self._sd, self.w
-        for name in list(sd):
-            if name.endswith('.proj_out.weight'):
-                p = name[:-len('.proj_out.weight')]
-                w[p + '.qkv.weight'] = _pack_lin(torch.cat([sd[p + '.%s.weight' % n] for n in 'qkv'], 0).float())
-                w[p + '.qkv.bias'] = torch.cat([sd[p + '.%s.bias' % n] for n in 'qkv'], 0).float().contiguous()
 
     def attn_block(self, x, p, gn_next=False):
         """AttnBlock (`archs/tdrqvae_arch.py:179-203`, `archs/vqgan_arch.py:181-240`): GroupNorm (no SiLU) -> q | k | v
@@ -789,40 +796,24 @@ class Engine:
     @_on_device
     @torch.no_grad()
     def soft_codes(self, z_e, temp, stochastic=False):
-        """RQBottleneck.get_soft_codes (`:429-457`): z_e fp32 [T, E] -> (p fp32 [T, K], codes int64 [T]) at depth 1,
-        (p fp32 [T, D, K], codes int64 [T, D]) at depth D.  Codes are the exact L2 argmin (== forward_vq's) or,
-        stochastic, one draw per row from p with a seed taken on the device from the default CUDA generator
-        (reproducible under torch.manual_seed, no host sync); each depth works on the residual the earlier codes left."""
+        """RQBottleneck.get_soft_codes (`:429-457`): z_e fp32 [T, E] -> (p fp32 [T, D, K], codes int64 [T, D]).  Codes
+        are the exact L2 argmin (== forward_vq's) or, stochastic, one draw per row from p with a seed taken on the device
+        from the default CUDA generator (reproducible under torch.manual_seed, no host sync); each depth works on the
+        residual the earlier codes left and writes K-slice d of p."""
         a = self.arch
         self._fusing = False
         z = z_e.to(self.dev, torch.float32).reshape(-1, a.embed_dim).contiguous()
-        T = z.shape[0]
-        if self.depth > 1:
-            return self._soft_codes_rq(z, temp, stochastic)
-        pack = self._codebook_pack()
-        p = self._new(T, a.n_embed, dtype=torch.float32)
-        ops.soft_codes(z, self.w['codebook'], pack[1], a.n_embed, temp, p)
-        codes = torch.empty(T, dtype=torch.int64, device=self.dev)
-        if stochastic:
-            seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (2,), dtype=torch.int64, device=self.dev)
-            ops.sample_codes(p, seed, codes)
-        else:
-            ops.l2_argmin_tc(z, self.w['codebook'], pack, a.n_embed, codes)
-        return p, codes
-
-    def _soft_codes_rq(self, z, temp, stochastic):
-        a = self.arch
         T, D, K = z.shape[0], self.depth, a.n_embed
         p = self._new(T, D, K, dtype=torch.float32)
         codes = torch.empty(D, T, dtype=torch.int64, device=self.dev)
-        r = self._new(T, a.embed_dim, dtype=torch.float32)
+        r = self._new(T, a.embed_dim, dtype=torch.float32) if D > 1 else None
         for d in range(D):
             src = z if d == 0 else r
             pack = self._codebook_pack(d)
-            ops.soft_codes_ld(src, self._codebook(d), pack[1], K, temp, p[:, d])
+            ops.soft_codes(src, self._codebook(d), pack[1], K, temp, p[:, d])
             if stochastic:
                 seed = torch.randint(-2 ** 63, 2 ** 63 - 1, (2,), dtype=torch.int64, device=self.dev)
-                ops.sample_codes_ld(p[:, d], seed, codes[d])
+                ops.sample_codes(p[:, d], seed, codes[d])
             else:
                 ops.l2_argmin_tc(src, self._codebook(d), pack, K, codes[d])
             if d < D - 1:

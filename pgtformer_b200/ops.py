@@ -404,45 +404,25 @@ def l2_argmin_tc_split(z, codebook, pack, K, idx_out, quant=None, splits=None):
 
 def soft_codes(z, codebook, norm, K, temp, out):
     """out[T, K] = softmax_k(-||z - e_k||^2 / temp) over the first K codebook rows (soft_codes.cu); norm: the fp32
-    ||e_k||^2 of codebook_pack."""
-    lib = L.load()
-    T, E = z.shape
-    assert z.dtype == torch.float32 and z.is_contiguous() and codebook.dtype == torch.float32 and codebook.is_contiguous()
-    assert codebook.shape[1] == E and codebook.shape[0] >= K and norm.dtype == torch.float32 and norm.numel() >= K
-    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (T, K)
-    L.check(lib.pgt_soft_codes(_p(z), T, E, _p(codebook), _p(norm), K, float(temp), _p(out), _stream(z)))
-    return out
-
-
-def sample_codes(p, seed, idx_out):
-    """idx_out[t] = one draw from the distribution in row t of p (codebook.cu sample_codes_kernel); seed: device int64
-    [2] (Philox key and offset), read on the device."""
-    lib = L.load()
-    T, K = p.shape
-    assert p.dtype == torch.float32 and p.is_contiguous() and idx_out.dtype == torch.int64 and idx_out.numel() == T
-    assert seed.dtype == torch.int64 and seed.numel() == 2 and seed.device == p.device and idx_out.device == p.device
-    L.check(lib.pgt_sample_codes(_p(p), T, K, _p(seed), _p(idx_out), _stream(p)))
-    return idx_out
-
-
-def soft_codes_ld(z, codebook, norm, K, temp, out):
-    """soft_codes into a row-pitched [T, K] view (one depth's K-slice of a contiguous [T, D, K] tensor)."""
+    ||e_k||^2 of codebook_pack.  out may be row-pitched (one depth's K-slice of a contiguous [T, D, K] tensor)."""
     lib = L.load()
     T, E = z.shape
     assert z.dtype == torch.float32 and z.is_contiguous() and codebook.dtype == torch.float32 and codebook.is_contiguous()
     assert codebook.shape[1] == E and codebook.shape[0] >= K and norm.dtype == torch.float32 and norm.numel() >= K
     assert out.dtype == torch.float32 and tuple(out.shape) == (T, K) and out.stride(1) == 1
-    L.check(lib.pgt_soft_codes_ld(_p(z), T, E, _p(codebook), _p(norm), K, float(temp), _p(out), out.stride(0), _stream(z)))
+    L.check(lib.pgt_soft_codes(_p(z), T, E, _p(codebook), _p(norm), K, float(temp), _p(out), out.stride(0), _stream(z)))
     return out
 
 
-def sample_codes_ld(p, seed, idx_out):
-    """sample_codes over the rows of a row-pitched [T, K] view; idx_out int64 [T] contiguous."""
+def sample_codes(p, seed, idx_out):
+    """idx_out[t] = one draw from the distribution in row t of p (codebook.cu sample_codes_kernel), p [T, K] possibly
+    row-pitched; seed: device int64 [2] (Philox key and offset), read on the device; idx_out int64 [T] contiguous."""
     lib = L.load()
     T, K = p.shape
     assert p.dtype == torch.float32 and p.stride(1) == 1 and idx_out.dtype == torch.int64 and idx_out.numel() == T
     assert idx_out.is_contiguous() and seed.dtype == torch.int64 and seed.numel() == 2 and seed.device == p.device
-    L.check(lib.pgt_sample_codes_ld(_p(p), T, K, p.stride(0), _p(seed), _p(idx_out), _stream(p)))
+    assert idx_out.device == p.device
+    L.check(lib.pgt_sample_codes(_p(p), T, K, p.stride(0), _p(seed), _p(idx_out), _stream(p)))
     return idx_out
 
 

@@ -6,8 +6,6 @@ reads every depth's rows (the padding row of depth d stays at index K_d) and the
 codes.  The argmins run split over code ranges (ops.l2_argmin_tc_split): RQ-VAE latents are small (64 tokens per 256^2
 image at f = 32), so the unsplit sweep would scan each large codebook on a handful of SMs.  Every op is a call into the
 C ABI; there is no PyTorch / CPU fallback."""
-import torch
-
 from . import ops
 from .spec import RQVAEArch
 from .tdrqvae import TDRQVAEEngine
@@ -15,17 +13,6 @@ from .tdrqvae import TDRQVAEEngine
 
 class RQVAEEngine(TDRQVAEEngine):
     arch_class = RQVAEArch
-
-    def _repack(self):
-        a = self.arch
-        self._repack_autoencoder()
-        if self.depth > 1:
-            n = 1 if a.shared_codebook else self.depth
-            cbs = torch.zeros(n, a.n_embed + 1, a.latent_shape[2], dtype=torch.float32, device=self.dev)
-            for d in range(n):
-                cb = self._f32('quantizer.codebooks.%d.weight' % d)
-                cbs[d, :cb.shape[0]] = cb
-            self.w['codebooks'] = cbs
 
     def _n_embed(self, d=0):
         return self.arch.n_embeds[d]

@@ -7,8 +7,9 @@ parameter/buffer names below are the reference's: they follow the module attribu
 attention / Swin block / EncoderLayer / TDResnetBlock ctors), `archs/codeformer_arch.py:102-117`
 (TransformerSALayer) and `archs/pgtformer_arch.py:34-397` (BiSeNet / ResNet18).
 
-`kind` drives the deterministic synthetic initialisation in weights.py and the kernel-layout
-repack in engine.py.
+`kind` drives the deterministic synthetic initialisation in weights.py.  The arch classes name what the
+kernel-layout repack (Engine._repack) cannot tell from a tensor's name and shape: the RGB stem, the upsample convs,
+the codebook key of each depth and the prefixes packed by a rule of their own.
 """
 from collections import OrderedDict
 
@@ -172,6 +173,20 @@ class Arch:
         self.fuse_level_key = {i: str(self.resolution >> i) for i in range(self.num_levels)
                                if str(self.resolution >> i) in self.connect_list}
         self.fuse_channels = {'16': 512, '32': 512, '64': 256, '128': 256, '256': 128, '512': 64}
+        self.stem = 'encoder.conv_in.weight'
+        self.upsample_convs = _upsample_convs(self.num_levels)
+        self.codebooks = _codebooks(self.depth)
+        self.packed_apart = ('conditionnet.',)                      # BiSeNet: BatchNorms folded into its convs
+
+
+def _upsample_convs(num_levels):
+    """The decoder's Upsample convs (nearest x2 + conv3x3, packed as 2x2 phase convs)."""
+    return tuple('decoder.up.%d.upsample.conv.weight' % lvl for lvl in range(1, num_levels))
+
+
+def _codebooks(depth):
+    """The codebook key of each quantiser depth (a shared codebook's keys alias the first)."""
+    return tuple('quantizer.codebooks.%d.weight' % d for d in range(depth))
 
 
 def build_spec(network_g):
@@ -345,6 +360,10 @@ class TDRQVAEArch:
         if len(self.window_size) != 3 or min(self.window_size) < 1 or \
                 self.window_size[0] * self.window_size[1] * self.window_size[2] > SWIN_MAX_TOKENS:
             raise ValueError('Video-Swin window %s: at most %d tokens' % (self.window_size, SWIN_MAX_TOKENS))
+        self.stem = 'encoder.conv_in.weight'
+        self.upsample_convs = _upsample_convs(self.num_levels)
+        self.codebooks = _codebooks(1)
+        self.packed_apart = ('tdswin_pre.', 'tdswin_post.')         # Video-Swin BasicLayers: swin3d.pack_blocks
 
 
 def build_tdrqvae_spec(network_g):
@@ -473,6 +492,10 @@ class RQVAEArch:
         if self.embed_dim % 128 or self.embed_dim > 512 or any(k % 128 or k < 128 for k in self.n_embeds):
             raise ValueError('embed_dim %d, n_embed %s: the argmin takes codebooks of a multiple of 128 up to 512 '
                              'channels and a multiple of 128 codes' % (self.embed_dim, list(self.n_embeds)))
+        self.stem = 'encoder.conv_in.weight'
+        self.upsample_convs = _upsample_convs(self.num_levels)
+        self.codebooks = _codebooks(self.depth)
+        self.packed_apart = ()
 
 
 RGB_STEM_WIDTHS = (64, 128)           # pgt_conv_rgb_bf16 3x3 output widths
@@ -587,6 +610,14 @@ class VQGANArch:
         if not widths <= set(ATTN_WIDTHS):
             raise ValueError('AttnBlock widths %s: the attention kernel takes %s' % (sorted(widths), ATTN_WIDTHS))
         self.code_shape = (self.img_size // self.down, self.img_size // self.down, 1)
+        # an Upsample conv is `generator.blocks.N.conv`, a Downsample conv `encoder.blocks.N.conv`: the block list tells
+        # them apart, no name pattern does
+        self.stem = 'encoder.blocks.0.weight'
+        self.upsample_convs = tuple('%s.blocks.%d.conv.weight' % (prefix, i)
+                                    for prefix, blocks in (('encoder', enc), ('generator', gen))
+                                    for i, b in enumerate(blocks) if b[0] == 'up')
+        self.codebooks = ('quantize.embedding.weight',)
+        self.packed_apart = ()
         if not codeformer:
             return
         self.dim_embd = int(g.get('dim_embd', 512))

@@ -8,39 +8,13 @@ the C ABI; there is no PyTorch / CPU fallback."""
 import torch
 
 from . import ops
-from .engine import BF, Engine, _on_device, _pack_conv, _pack_lin, _pack_rgb, _pack_up2x
+from .engine import BF, Engine, _on_device
 from .spec import TDRQVAEArch
-from .swin3d import basic_layer_rows, pack_blocks
-
-SWIN_LAYERS = ('tdswin_pre', 'tdswin_post')
+from .swin3d import basic_layer_rows
 
 
 class TDRQVAEEngine(Engine):
     arch_class = TDRQVAEArch
-
-    def _repack(self):
-        self._repack_autoencoder()
-        self.swin = {p: pack_blocks(lambda k, p=p: self._sd.get(p + '.' + k), self.arch.stages_atten) for p in SWIN_LAYERS}
-
-    def _repack_autoencoder(self):
-        """Encoder / decoder convs, AttnBlock projections and codebook 0 in kernel layouts (RQVAEEngine shares it)."""
-        sd, w = self._sd, self.w
-        for name, t in sd.items():
-            if name.startswith(SWIN_LAYERS):
-                continue
-            if name.endswith('.weight') and t.dim() == 4:
-                if name == 'encoder.conv_in.weight':
-                    w[name] = _pack_rgb(t.float())
-                elif t.shape[2] == 3 and '.upsample.conv.' in name:
-                    w[name] = _pack_up2x(t.float())
-                elif t.shape[2] == 3:
-                    w[name] = _pack_conv(t.float())
-                else:
-                    w[name] = _pack_lin(t.float())
-            elif t.dtype.is_floating_point and t.dim() == 1:
-                w[name] = t.float().contiguous()
-        w['codebook'] = self._f32('quantizer.codebooks.0.weight')
-        self._repack_attn_qkv()
 
     # ------------------------------------------------------------------ blocks
     def encoder(self, x):
@@ -106,7 +80,7 @@ class TDRQVAEEngine(Engine):
         z = self.tdswin('tdswin_pre', z, b, t, hh, ww, out_dtype=torch.float32)
         codes = torch.empty(T, dtype=torch.int64, device=self.dev)
         z_q = self._new(T, a.embed_dim, dtype=torch.float32)
-        ops.l2_argmin_tc(z, self.w['codebook'], self._codebook_pack(), a.n_embed, codes, z_q)
+        self._argmin(z, self.w['codebook'], self._codebook_pack(), self._n_embed(0), codes, z_q)
         return z, codes, z_q, (b, t, hh, ww)
 
     @_on_device

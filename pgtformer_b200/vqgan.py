@@ -9,7 +9,7 @@ reference's b(hw) order of logits and codes.  Every op is a call into the C ABI;
 import torch
 
 from . import ops
-from .engine import BF, Engine, _on_device, _pack_conv, _pack_lin, _pack_rgb, _pack_up2x
+from .engine import Engine, _on_device
 from .spec import VQGANArch
 
 F32 = torch.float32
@@ -21,37 +21,11 @@ class VQGANEngine(Engine):
     def arch_class(self, g):
         return VQGANArch(g, self.codeformer)
 
-    def _repack(self):
-        """Kernel layouts by the spec's block kinds (an Upsample conv is `generator.blocks.N.conv`, a Downsample conv
-        `encoder.blocks.N.conv`: no name pattern tells them apart)."""
-        sd, w = self._sd, self.w
-        for name, t in sd.items():
-            if t.dtype.is_floating_point and t.dim() == 1:
-                w[name] = t.float().contiguous()
-            elif name.endswith('.weight') and t.dim() == 4:
-                w[name] = _pack_conv(t.float()) if t.shape[2] == 3 else _pack_lin(t.float())
-            elif name.endswith('.weight') and t.dim() == 2 and name != 'quantize.embedding.weight':
-                w[name] = _pack_lin(t.float())
-        for prefix, blocks in (('encoder', self.arch.enc_blocks), ('generator', self.arch.gen_blocks)):
-            for i, (kind, *_rest) in enumerate(blocks):
-                p = '%s.blocks.%d' % (prefix, i)
-                if kind == 'up':
-                    w[p + '.conv.weight'] = _pack_up2x(sd[p + '.conv.weight'].float())
-                elif kind == 'conv_in' and prefix == 'encoder':
-                    w[p + '.weight'] = _pack_rgb(sd[p + '.weight'].float())
-        w['codebook'] = self._f32('quantize.embedding.weight')
-        self._repack_attn_qkv()
-
     def _stats_tiles(self, H, W, cout, ksize, stride, pad_lo):
         """Fused statistics only where the conv's tile grid divides the frame: VQAutoEncoder takes any multiple of 128,
         and at, say, 256 x 384 the 256-channel levels (48 and 24 columns) get 32- and 16-column tiles, whose last
         column of tiles would add rows past the frame's edge to the statistics (pgt_conv_tiles_exact)."""
         return ops.conv_tiles_exact(H, W, cout, ksize, stride, pad_lo)
-
-    def _codebook_pack(self, d=0):
-        if 'codebook.pack' not in self.w:
-            self.w['codebook.pack'] = ops.codebook_pack(self.w['codebook'], self.arch.n_embed)
-        return self.w['codebook.pack']
 
     # ------------------------------------------------------------------ encoder / generator
     def _walk(self, prefix, blocks, h, lo, hi, taps=None):
@@ -152,7 +126,7 @@ class VQGANEngine(Engine):
         T, K = b * hh * ww, a.n_embed
         codes = torch.empty(T, dtype=torch.int64, device=self.dev)
         zr = z.view(T, E)
-        ops.l2_argmin_tc(zr, self.w['codebook'], self._codebook_pack(), K, codes)
+        self._argmin(zr, self.w['codebook'], self._codebook_pack(), self._n_embed(0), codes)
         if force_codes is not None:
             codes = force_codes.to(self.dev, torch.int64).reshape(T).contiguous()
         scalars = self._new(3, dtype=F32)
@@ -173,23 +147,12 @@ class VQGANEngine(Engine):
 class CodeFormerEngine(VQGANEngine):
     codeformer = True
 
-    def _repack(self):
-        super()._repack()
-        sd, w = self._sd, self.w
-        E = self.arch.dim_embd
-        for i in range(self.arch.n_layers):
-            p = 'ft_layers.%d.self_attn' % i
-            wi, bi = sd[p + '.in_proj_weight'].float(), sd[p + '.in_proj_bias'].float()
-            w[p + '.qk.weight'], w[p + '.qk.bias'] = _pack_lin(wi[:2 * E]), bi[:2 * E].contiguous()
-            w[p + '.v.weight'], w[p + '.v.bias'] = _pack_lin(wi[2 * E:]), bi[2 * E:].contiguous()
-        w['position_emb'] = sd['position_emb'].to(BF).contiguous()
-        self._pos = {}
-
     def pos(self, b):
         """position_emb tiled over the batch: [b * L, dim_embd] bf16, built once per batch size."""
-        if b not in self._pos:
-            self._pos[b] = self.w['position_emb'].repeat(b, 1).contiguous()
-        return self._pos[b]
+        key = 'position_emb.%d' % b
+        if key not in self.w:
+            self.w[key] = self.w['position_emb'].repeat(b, 1).contiguous()
+        return self.w[key]
 
     @_on_device
     @torch.no_grad()

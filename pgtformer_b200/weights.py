@@ -1,4 +1,4 @@
-"""Deterministic synthetic checkpoints and the kernel-layout repack helpers.
+"""Deterministic synthetic checkpoints (the kernel-layout repack is Engine._repack, pgtformer_b200/engine.py).
 
 No trained weights are reachable offline (SURVEY F10), so every test / bench uses a synthetic
 state dict that is a pure function of (name, shape, kind, seed): independent of module

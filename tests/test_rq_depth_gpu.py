@@ -130,7 +130,7 @@ def test_rq_embed_every_mode_is_a_sequential_fp32_sum(shared, out_dtype):
         assert torch.equal(got, want)
 
 
-def test_bindings_agree_on_the_new_entries():
+def test_bindings_agree_on_the_rq_entries():
     from pgtformer_b200 import ops, torch_ops
     tops = torch_ops.load()
     K, E, D, T = 1024, 512, 3, 2000
@@ -151,13 +151,13 @@ def test_bindings_agree_on_the_new_entries():
     assert torch.equal(r1, r2) and torch.equal(g1, g2)
     _, norm = ops.codebook_pack(cb, K)
     p1, p2 = torch.zeros(T, 2, K, device=DEV), torch.zeros(T, 2, K, device=DEV)
-    ops.soft_codes_ld(z, cb, norm, K, 3.0, p1[:, 1])
-    tops.soft_codes_ld(z, cb, norm, K, 3.0, p2[:, 1])
+    ops.soft_codes(z, cb, norm, K, 3.0, p1[:, 1])
+    tops.soft_codes(z, cb, norm, K, 3.0, p2[:, 1])
     assert torch.equal(p1, p2) and (p1[:, 0] == 0).all()
     seed = torch.tensor([5, 6], dtype=torch.int64, device=DEV)
     i1, i2 = torch.empty(T, dtype=torch.int64, device=DEV), torch.empty(T, dtype=torch.int64, device=DEV)
-    ops.sample_codes_ld(p1[:, 1], seed, i1)
-    tops.sample_codes_ld(p2[:, 1], seed, i2)
+    ops.sample_codes(p1[:, 1], seed, i1)
+    tops.sample_codes(p2[:, 1], seed, i2)
     assert torch.equal(i1, i2)
 
 
