@@ -63,5 +63,6 @@ class CodeFormer(VQAutoEncoder):
             lo, hi = torch.aminmax(force_codes)
             if int(lo) < 0 or int(hi) >= self.codebook_size:
                 raise IndexError('code out of range [0, %d)' % self.codebook_size)
-        return self.engine().forward(x, w=float(w), adain=bool(adain), code_only=bool(code_only),
-                                     force_codes=force_codes)
+            return self.engine().forward(x, w=float(w), adain=bool(adain), code_only=bool(code_only),
+                                         force_codes=force_codes)
+        return self._run('forward', x, w=float(w), adain=bool(adain), code_only=bool(code_only))

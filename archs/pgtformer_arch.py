@@ -86,6 +86,10 @@ def _materialise(root, spec, seed):
 
 class _B200Model(nn.Module):
     _PGT_KEYS = ()
+    # replay the model's calls from CUDA graphs (Engine.graphed): their outputs are then the graphs' static tensors, to
+    # be consumed before the next call.  Off by default; PGTFormer reads PGT_CUDA_GRAPH and replays its forward only.
+    cuda_graph = False
+    _graph_calls = True       # whether cuda_graph covers the codec calls routed through _run (not for PGTFormer)
 
     def _setup(self, network_g, seed=0):
         self._network_g = network_g
@@ -132,6 +136,15 @@ class _B200Model(nn.Module):
         from pgtformer_b200.engine import Engine
         return Engine
 
+    def _run(self, name, *tensors, writes=(), **scalars):
+        """The engine's method `name` on the tensors and scalars: eager, or with cuda_graph replayed from the engine's
+        graph for this key (Engine.graphed; `writes`: the tensors the method updates in place).  The caller has checked
+        the arguments on the host."""
+        eng = self.engine()
+        if self.cuda_graph and self._graph_calls:
+            return eng.graphed(getattr(eng, name), tensors, writes=writes, **scalars)
+        return getattr(eng, name)(*tensors, **scalars)
+
     # ---- code helpers shared by the codecs.  Arguments are checked on the host before any launch: bad shapes
     # raise ValueError, codes outside [0, n_embed] IndexError (index n_embed is the codebook's padding row, which
     # nn.Embedding accepts).
@@ -163,7 +176,8 @@ class _B200Model(nn.Module):
         if decode_type not in ('select', 'add'):
             raise NotImplementedError(f"{decode_type} is not implemented in partial decoding")
         if code.shape[-1] == 1:
-            return self.decode_code(code)
+            self._check_latent(*code.shape[:3])
+            return self.engine().decode_code(code)
         if isinstance(code_idx, bool) or not isinstance(code_idx, int) or code_idx < 0:
             raise ValueError('code_idx must be an int in [0, %d), got %r' % (code.shape[-1], code_idx))
         self._check_latent(*code.shape[:3])
@@ -199,11 +213,13 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
         self._setup(g)
 
     def forward(self, input, code_only=False):
-        return self.engine().forward_vq(input, code_only=code_only)
+        x = self._frames(input)
+        return self._run('forward_vq', x, code_only=bool(code_only))
 
     @torch.no_grad()
     def get_codes(self, input):
-        return self.engine().forward_vq(input, code_only=True)[2]
+        x = self._frames(input)
+        return self._run('forward_vq', x, code_only=True)[2]
 
     # ---- the rest of the stage-I codec surface (`archs/tdcrqvae3_arch.py:774-872`) at any quantiser depth; arguments are
     # checked on the host before any launch (see _B200Model._check_code).
@@ -228,7 +244,7 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
     def encode(self, x):
         """z_e = quant_conv(Encoder(x)) as NHWC fp32 [b*t, H/16, W/16, embed_dim]."""
         x = self._frames(x)
-        return self.engine().encode(x)
+        return self._run('encode', x)
 
     @torch.no_grad()
     def decode(self, z_q):
@@ -237,20 +253,19 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
                 not z_q.dtype.is_floating_point:
             raise ValueError('expected z_q [F, h, w, %d] floating point, got %s' % (self.arch.embed_dim, _shape(z_q)))
         self._check_latent(*z_q.shape[:3])
-        return self.engine().decode(z_q)
+        return self._run('decode', z_q)
 
     @torch.no_grad()
     def decode_code(self, code):
         """The depth sum of the code rows of the int codes [F, h, w, D] (any h, w the decoder takes), decoded to frames."""
         self._check_code(code)
         self._check_latent(*code.shape[:3])
-        eng = self.engine()
-        Fr, h, w, _ = code.shape
-        return eng.decode(eng.embed_code(code).view(Fr, h, w, self.arch.embed_dim))
+        return self._run('decode_code', code)
 
     @torch.no_grad()
     def forward_partial_code(self, xs, code_idx, decode_type='select'):
-        code = self.get_codes(self._frames(xs))
+        x = self._frames(xs)
+        code = self.engine().forward_vq(x, code_only=True)[2]
         return self.decode_partial_code(code, code_idx, decode_type)
 
     @torch.no_grad()
@@ -275,6 +290,8 @@ class TDCRQVAE3(_B200Model, PyTorchModelHubMixin):
 
 @ARCH_REGISTRY.register()
 class PGTFormer(TDCRQVAE3):
+    _graph_calls = False      # cuda_graph replays forward alone: the inherited codec methods keep fresh outputs
+
     def __init__(self, ddconfig, dim_embd=512, n_head=8, n_layers=9, connect_list=['32', '64', '128', '256'],
                  fix_modules=['quantizer', 'decoder', 'conditionnet'], w=0, detach_16=True, adain=False, tf=3,
                  droprate=0.0, **kwargs):

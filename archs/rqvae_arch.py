@@ -79,13 +79,13 @@ class RQVAE(_B200Model, PyTorchModelHubMixin):
         """(out fp32 [B,3,H,W], quant_loss, code int64 [B,h,w,D]); with code_only, (z_q fp32 [B,h,w,embed_dim],
         quant_loss, code)."""
         x = self._images(xs)
-        return self.engine().forward_vq(x, code_only=bool(code_only))
+        return self._run('forward_vq', x, code_only=bool(code_only))
 
     @torch.no_grad()
     def encode(self, x):
         """z_e = quant_conv(Encoder(x)) as NHWC fp32 [B, h, w, embed_dim]."""
         x = self._images(x)
-        return self.engine().encode(x)
+        return self._run('encode', x)
 
     @torch.no_grad()
     def decode(self, z_q):
@@ -94,19 +94,19 @@ class RQVAE(_B200Model, PyTorchModelHubMixin):
                 not z_q.dtype.is_floating_point:
             raise ValueError('expected z_q [B, h, w, %d] floating point, got %s' % (self.arch.embed_dim, _shape(z_q)))
         self._check_latent(*z_q.shape[:3])
-        return self.engine().decode(z_q)
+        return self._run('decode', z_q)
 
     @torch.no_grad()
     def get_codes(self, xs):
         """Codes [B, h, w, D] int64 (those forward returns)."""
         x = self._images(xs)
-        return self.engine().forward_vq(x, code_only=True)[2]
+        return self._run('forward_vq', x, code_only=True)[2]
 
     @torch.no_grad()
     def get_codesbt(self, xs):
         """get_codes of clips [b, t, 3, H, W] as [b*t, h, w, D]."""
         x = self._images(xs, dims=5)
-        return self.engine().forward_vq(x.reshape(-1, *x.shape[2:]), code_only=True)[2]
+        return self._run('forward_vq', x.reshape(-1, *x.shape[2:]), code_only=True)[2]
 
     @torch.no_grad()
     def get_soft_codes(self, xs, temp=1.0, stochastic=False):
@@ -135,11 +135,11 @@ class RQVAE(_B200Model, PyTorchModelHubMixin):
         """The depth sum of the code rows of the int codes [B, h, w, D], decoded to images."""
         self._check_code(code)
         self._check_latent(*code.shape[:3])
-        eng = self.engine()
-        B, h, w, _ = code.shape
-        return eng.decode(eng.embed_code(code).view(B, h, w, self.arch.embed_dim))
+        return self._run('decode_code', code)
 
     @torch.no_grad()
     def forward_partial_code(self, xs, code_idx, decode_type='select'):
-        """decode_partial_code of get_codes(xs)."""
-        return self.decode_partial_code(self.get_codes(xs), code_idx, decode_type)
+        """decode_partial_code of get_codes(xs), both eager."""
+        x = self._images(xs)
+        code = self.engine().forward_vq(x, code_only=True)[2]
+        return self.decode_partial_code(code, code_idx, decode_type)

@@ -81,13 +81,13 @@ class TDRQVAE(_B200Model, PyTorchModelHubMixin):
         """(out [b,t,3,H,W], quant_loss, code [b,t,h,w,1]); with code_only, (z_q after tdswin_post [b,t,h,w,E],
         quant_loss, code)."""
         x = self._clips(input)
-        return self.engine().forward(x, code_only=bool(code_only))
+        return self._run('forward', x, code_only=bool(code_only))
 
     @torch.no_grad()
     def get_codes(self, input):
         """Codes [b,t,h,w,1] of the tdswin_pre output (the codes forward returns)."""
         x = self._clips(input)
-        return self.engine().codes(x)
+        return self._run('codes', x)
 
     @torch.no_grad()
     def get_codesbt(self, input):
@@ -99,7 +99,7 @@ class TDRQVAE(_B200Model, PyTorchModelHubMixin):
     def encode(self, x):
         """z_e = quant_conv(Encoder(x)) of frames [F,3,H,W] as NHWC fp32 [F, H/16, W/16, embed_dim]; no Swin layer."""
         x = self._frames(x)
-        return self.engine().encode(x)
+        return self._run('encode', x)
 
     @torch.no_grad()
     def decode(self, z_q):
@@ -108,16 +108,14 @@ class TDRQVAE(_B200Model, PyTorchModelHubMixin):
                 not z_q.dtype.is_floating_point:
             raise ValueError('expected z_q [F, h, w, %d] floating point, got %s' % (self.arch.embed_dim, _shape(z_q)))
         self._check_latent(*z_q.shape[:3])
-        return self.engine().decode(z_q)
+        return self._run('decode', z_q)
 
     @torch.no_grad()
     def decode_code(self, code):
         """Codebook rows of the int codes [F, h, w, 1], decoded to frames without tdswin_post."""
         self._check_code(code)
         self._check_latent(*code.shape[:3])
-        eng = self.engine()
-        Fr, h, w, _ = code.shape
-        return eng.decode(eng.embed_code(code).view(Fr, h, w, self.arch.embed_dim))
+        return self._run('decode_code', code)
 
     @torch.no_grad()
     def get_soft_codes(self, xs, temp=1.0, stochastic=False):

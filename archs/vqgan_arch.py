@@ -104,4 +104,5 @@ class VQAutoEncoder(_B200Model):
         usage = self.quantize.usage
         if usage.device != eng.dev:
             raise RuntimeError('quantize.usage is on %s, the model on %s' % (usage.device, eng.dev))
-        return eng.forward(x, code_only=bool(code_only), usage=usage)
+        # a replay adds its counts to the buffer held now (reset_usage() replaces it), through the graph's own copy
+        return self._run('counted_forward', x, usage, writes=(1,), code_only=bool(code_only))

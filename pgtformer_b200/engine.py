@@ -664,32 +664,56 @@ class Engine:
 
     @_on_device
     @torch.no_grad()
-    def forward_graphed(self, x, w=1.0, adain=True):
-        """The same launch sequence replayed from a CUDA graph captured once per (shape, w, adain): removes the
-        ~700 per-launch host costs (what bounds the reference's own b=1 sliding-window loop, `inference.py:47-74`).
-        Returned tensors are the graph's static outputs: consume them before the next call."""
-        x = x.to(self.dev, torch.float32).contiguous()
-        key = (tuple(x.shape), float(w), bool(adain))
+    def graphed(self, method, tensors, writes=(), **scalars):
+        """method(*tensors, **scalars) replayed from a CUDA graph: removes the host cost of every launch (Python, ctypes,
+        the output allocations and tensor-map lookups), up to a third of a call at b = 1 (DESIGN §6c).
+
+        One graph per key = (method, shapes and dtypes of the tensors, scalars), kept by this engine: a new key runs the
+        method twice on a side stream (the lazy one-time set-up: kernel attributes, constant tables, codebook packs,
+        workspaces) and then captures it on this engine's capture stream (on its device), into a memory pool of its own;
+        scratch taken during the capture comes from that pool (ops._gn_workspace).  Every call copies the tensors into the graph's
+        static inputs and replays it; tensors at the indices in `writes` are ones the method updates in place, copied
+        back after the replay.  Returns the graph's static outputs: consume them before the next call.  Arguments are
+        checked by the caller before this: a capture never starts on an argument the method would reject, and a key
+        whose warm-up raises stores nothing."""
+        tensors = [t.to(self.dev) for t in tensors]
+        key = (method.__name__, tuple((tuple(t.shape), t.dtype) for t in tensors), tuple(sorted(scalars.items())))
         if not hasattr(self, '_graphs'):
             self._graphs = {}
+            self.capture_stream = torch.cuda.Stream(device=self.dev)
         entry = self._graphs.get(key)
         if entry is None:
-            static_x = x.clone()
+            static = [torch.empty(t.shape, dtype=t.dtype, device=self.dev) for t in tensors]
+            for s, t in zip(static, tensors):
+                s.copy_(t)
+            cur = torch.cuda.current_stream(self.dev)
             side = torch.cuda.Stream(device=self.dev)
-            side.wait_stream(torch.cuda.current_stream(self.dev))
-            with torch.cuda.stream(side):                      # warm-up outside capture (lazy attribute / workspace setup)
-                for _ in range(2):
-                    self.forward(static_x, w=w, adain=adain)
-            torch.cuda.current_stream(self.dev).wait_stream(side)
+            side.wait_stream(cur)
+            try:
+                with torch.cuda.stream(side):
+                    for _ in range(2):
+                        method(*static, **scalars)
+            finally:
+                cur.wait_stream(side)
             graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                outs = self.forward(static_x, w=w, adain=adain)
-            entry = (graph, static_x, outs)
+            with torch.cuda.graph(graph, stream=self.capture_stream):
+                outs = method(*static, **scalars)
+            entry = (graph, static, outs)
             self._graphs[key] = entry
-        graph, static_x, outs = entry
-        static_x.copy_(x, non_blocking=True)
+        graph, static, outs = entry
+        for s, t in zip(static, tensors):
+            s.copy_(t, non_blocking=True)
         graph.replay()
+        for i in writes:
+            tensors[i].copy_(static[i], non_blocking=True)
         return outs
+
+    def forward_graphed(self, x, w=1.0, adain=True):
+        """forward replayed from a CUDA graph captured once per (shape, w, adain) (graphed): removes the ~700
+        per-launch host costs (what bounds the reference's own b=1 sliding-window loop, `inference.py:47-74`).
+        Returned tensors are the graph's static outputs: consume them before the next call."""
+        x = x.to(self.dev, torch.float32).contiguous()
+        return self.graphed(self.forward, (x,), w=float(w), adain=bool(adain))
 
     # ------------------------------------------------------------------ stage-I codec (TDCRQVAE3 methods)
     def _codebook(self, d=0):
@@ -777,6 +801,13 @@ class Engine:
         else:
             ops.rq_embed(codes, d0, d1, self.w['codebooks'], quant, ldi=D, ldd=1)
         return quant
+
+    @_on_device
+    @torch.no_grad()
+    def decode_code(self, codes):
+        """decode of embed_code: int64 codes [F, h, w, D] -> the depth sum of their code rows, decoded to fp32 NCHW."""
+        Fr, hh, ww, _ = codes.shape
+        return self.decode(self.embed_code(codes).view(Fr, hh, ww, self.arch.embed_dim))
 
     @_on_device
     @torch.no_grad()

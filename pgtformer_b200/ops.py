@@ -138,7 +138,13 @@ _gn_ws = {}
 
 def _gn_workspace(kind, x, n):
     """fp32 GroupNorm scratch of at least n floats, one per (kind, device, current stream), grown on demand: 'stats'
-    holds pgt_groupnorm_ws_floats partial statistics, 'ab' the [F, 2, C] affine terms of groupnorm_apply_stats."""
+    holds pgt_groupnorm_ws_floats partial statistics, 'ab' the [F, 2, C] affine terms of groupnorm_apply_stats.
+
+    Under CUDA-graph capture the scratch is a fresh tensor from the capturing graph's own memory pool and is not cached:
+    a cached one would be shared by every graph captured on that stream and could be freed (grown, or released with
+    the pool of a destroyed graph) while another graph still replays into it."""
+    if torch.cuda.is_current_stream_capturing():
+        return torch.empty(max(n, 1), dtype=torch.float32, device=x.device)
     key = (kind, x.device.index, torch.cuda.current_stream().cuda_stream)
     ws = _gn_ws.get(key)
     if ws is None or ws.numel() < n:

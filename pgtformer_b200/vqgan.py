@@ -143,6 +143,10 @@ class VQGANEngine(Engine):
             return zq, scalars[0], stats
         return self.generator(zq16), scalars[0], stats
 
+    def counted_forward(self, x, usage, code_only=False):
+        """forward with the usage buffer as a positional tensor argument (the form Engine.graphed replays)."""
+        return self.forward(x, code_only=code_only, usage=usage)
+
 
 class CodeFormerEngine(VQGANEngine):
     codeformer = True
