@@ -195,8 +195,11 @@ class Engine:
     _fusing = False           # set per forward: SFT fusion active (w > 0)
 
     def _stats_tiles(self, H, W, cout, ksize, stride, pad_lo):
-        """Tiles per frame of a conv whose epilogue emits the next GroupNorm's statistics; 0: no fused statistics."""
-        return ops.conv_tiles_per_frame(H, W, cout, ksize, stride, pad_lo)
+        """Tiles per frame of a conv whose epilogue emits the next GroupNorm's statistics; 0: no fused statistics.
+        Fused statistics only where the conv's tile grid divides the frame: the models take frames of any multiple of
+        64 (or 128), and at, say, 192 x 192 PGTFormer's level-0 Downsample (96 columns) gets 64-column tiles, whose
+        last column of tiles would add rows past the frame's edge to the statistics (pgt_conv_tiles_exact)."""
+        return ops.conv_tiles_exact(H, W, cout, ksize, stride, pad_lo)
 
     def _gn_stats(self, out, chunks_per_frame):
         """The next GroupNorm's statistics, filled by the epilogue that writes `out` (saves that GroupNorm a pass over

@@ -21,12 +21,6 @@ class VQGANEngine(Engine):
     def arch_class(self, g):
         return VQGANArch(g, self.codeformer)
 
-    def _stats_tiles(self, H, W, cout, ksize, stride, pad_lo):
-        """Fused statistics only where the conv's tile grid divides the frame: VQAutoEncoder takes any multiple of 128,
-        and at, say, 256 x 384 the 256-channel levels (48 and 24 columns) get 32- and 16-column tiles, whose last
-        column of tiles would add rows past the frame's edge to the statistics (pgt_conv_tiles_exact)."""
-        return ops.conv_tiles_exact(H, W, cout, ksize, stride, pad_lo)
-
     # ------------------------------------------------------------------ encoder / generator
     def _walk(self, prefix, blocks, h, lo, hi, taps=None):
         """Runs blocks[lo:hi] of `prefix` on h; with taps (flat index -> key) returns {key: output after that block}."""

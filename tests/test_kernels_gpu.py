@@ -424,9 +424,12 @@ def test_conv_relu_after_residual():
 
 @pytest.mark.parametrize('Fr,H,W,Cin,Cout,lin', [(3, 16, 16, 64, 64, False), (3, 32, 32, 128, 256, False),
                                                 (6, 16, 16, 256, 512, False), (3, 16, 32, 64, 128, False),
-                                                (3, 16, 16, 256, 256, True)])
+                                                (3, 32, 64, 128, 256, False), (3, 16, 24, 64, 128, False),
+                                                (2, 48, 16, 128, 64, False), (3, 16, 16, 256, 256, True)])
 def test_groupnorm_stats_fused_in_epilogue(Fr, H, W, Cin, Cout, lin):
-    """conv / linear epilogue emits per-tile (sum, sumsq) per GroupNorm group; finalize+apply consumes them."""
+    """conv / linear epilogue emits per-tile (sum, sumsq) per GroupNorm group; finalize+apply consumes them.  The
+    non-square conv frames are ones whose tile grid divides the frame (32 x 64 at 256 channels: 64 x 2 tiles; 16 x 24
+    and 48 x 16 on the halo kernel's 8 x 16 tiles), the only frames the engines fuse statistics for."""
     o = ops()
     x = bf(rnd((Fr, H, W, Cin), 150))
     gam, bet = 1 + 0.1 * rnd((Cout,), 153), 0.1 * rnd((Cout,), 154)
@@ -442,8 +445,8 @@ def test_groupnorm_stats_fused_in_epilogue(Fr, H, W, Cin, Cout, lin):
     else:
         w = bf(rnd((Cout, Cin, 3, 3), 151, (9 * Cin) ** -0.5)).float()
         b = rnd((Cout,), 152, 0.1)
-        tpf = o.conv_tiles_per_frame(H, W, Cout)
-        assert tpf > 0
+        tpf = o.conv_tiles_exact(H, W, Cout)
+        assert tpf == o.conv_tiles_per_frame(H, W, Cout) > 0
         stats = torch.zeros(Fr * tpf * 4 * 64, dtype=torch.float32, device=DEV)
         o.conv(x.to(DEV), pack_conv_weight(w).to(DEV), Cout, y, bias=b.to(DEV), residual=res.to(DEV), gn_stats=stats)
         ref = conv_ref(x, w, b) + res.float()
@@ -472,17 +475,19 @@ def test_swin_mlp_fused(T):
     check_close(out, ref, 'fused swin mlp', bf16_out=True, rel=4e-3)
 
 
-@pytest.mark.parametrize('Fr,H,W,C', [(3, 16, 16, 128), (2, 32, 64, 64), (3, 16, 16, 512)])
+@pytest.mark.parametrize('Fr,H,W,C', [(3, 16, 16, 128), (2, 32, 64, 64), (3, 16, 16, 512), (3, 16, 24, 128),
+                                      (2, 8, 32, 256)])
 def test_conv_up2x_groupnorm_stats(Fr, H, W, C):
-    """The four phase launches of the upsample conv fill one statistics buffer [frame][phase][tile][quad][32][2]."""
+    """The four phase launches of the upsample conv fill one statistics buffer [frame][phase][tile][quad][32][2].
+    From a 16 x 24 source the halo phases run 3 tiles each; from 8 x 32 at 256 channels, 32 x 4 tiles."""
     from pgtformer_b200.engine import _pack_up2x
     o = ops()
     x = bf(rnd((Fr, H, W, C), 170))
     w = bf(rnd((C, C, 3, 3), 171, (9 * C) ** -0.5)).float()
     b = rnd((C,), 172, 0.1)
     gam, bet = 1 + 0.1 * rnd((C,), 173), 0.1 * rnd((C,), 174)
-    tpf = o.conv_tiles_per_frame(H, W, C, 2, 1, 1)
-    assert tpf > 0
+    tpf = o.conv_tiles_exact(H, W, C, 2, 1, 1)
+    assert tpf == o.conv_tiles_per_frame(H, W, C, 2, 1, 1) > 0
     stats = torch.zeros(Fr * 16 * tpf * 64, dtype=torch.float32, device=DEV)
     y = torch.empty(Fr, 2 * H, 2 * W, C, dtype=torch.bfloat16, device=DEV)
     o.conv_up2x(x.to(DEV), _pack_up2x(w.to(DEV)), C, y, bias=b.to(DEV), gn_stats=stats)

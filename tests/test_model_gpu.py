@@ -138,19 +138,23 @@ def test_global_transformer(eng, bf_sd, arch_spec):
 
 
 def test_encoder_decoder_stages(eng, bf_sd, arch_spec):
+    """At 128 x 128 and at 64 x 192, where the tile grids of several levels do not divide the frame (level 0's
+    Downsample: 64-column tiles over 96 columns)."""
     from oracle import pgt_oracle as O
     arch, _ = arch_spec
-    x = torch.rand(3, 3, 128, 128, generator=torch.Generator().manual_seed(8))
-    h, feats = eng.encoder(x.to(DEV))
-    rh, rfeats = O.encoder_forward(bf_sd, arch, x)
-    assert relerr(h, nhwc(rh)) < 3e-2
-    for a, b in zip(feats, rfeats):
-        assert relerr(a, nhwc(b)) < 3e-2
-    z = rand_fm((3, 8, 8, 256), 9, 0.5)
-    efeats = [nhwc(f).bfloat16() for f in rfeats]
-    out = eng.decoder(z.to(DEV), [f.to(DEV) for f in efeats], 1.0)
-    ref = O.decoder_forward(bf_sd, arch, z.float().permute(0, 3, 1, 2), [f.float().permute(0, 3, 1, 2) for f in efeats], 1.0)
-    assert relerr(out, ref) < 4e-2 and psnr(out, ref) > 38.0
+    for H, W in ((128, 128), (64, 192)):
+        x = torch.rand(3, 3, H, W, generator=torch.Generator().manual_seed(8))
+        h, feats = eng.encoder(x.to(DEV))
+        rh, rfeats = O.encoder_forward(bf_sd, arch, x)
+        assert relerr(h, nhwc(rh)) < 3e-2, (H, W)
+        for a, b in zip(feats, rfeats):
+            assert relerr(a, nhwc(b)) < 3e-2, (H, W, tuple(a.shape))
+        z = rand_fm((3, H // 16, W // 16, 256), 9, 0.5)
+        efeats = [nhwc(f).bfloat16() for f in rfeats]
+        out = eng.decoder(z.to(DEV), [f.to(DEV) for f in efeats], 1.0)
+        ref = O.decoder_forward(bf_sd, arch, z.float().permute(0, 3, 1, 2),
+                                [f.float().permute(0, 3, 1, 2) for f in efeats], 1.0)
+        assert relerr(out, ref) < 4e-2 and psnr(out, ref) > 38.0, (H, W)
 
 
 @pytest.mark.parametrize('fixture', ['pgtformer_ref_b1_128_seed1.pt', 'pgtformer_ref_b2_128_seed2.pt'])

@@ -184,13 +184,16 @@ def test_batch_equals_per_clip(model):
     assert torch.equal(model(x[1:], code_only=True)[0], zq[1:])
 
 
+@pytest.mark.parametrize('H,W', [(128, 64), (64, 192)])
 @pytest.mark.parametrize('b,t', [(1, 1), (3, 2), (1, 5)])
-def test_any_clip_length(model, sd64_cpu, b, t):
-    """Any b, t >= 1 (t >= 5 fills the 5-frame window in depth); against the oracle with the same codes."""
-    x = torch.rand(b, t, 3, 128, 64, generator=torch.Generator().manual_seed(b * 10 + t)).to(DEV)
+def test_any_clip_length(model, sd64_cpu, b, t, H, W):
+    """Any b, t >= 1 (t >= 5 fills the 5-frame window in depth); against the oracle with the same codes.  At 64 x 192
+    the tile grids of several levels do not divide the frame."""
+    x = torch.rand(b, t, 3, H, W, generator=torch.Generator().manual_seed(b * 10 + t)).to(DEV)
     out, loss, code = model(x)
-    assert out.shape == (b, t, 3, 128, 64) and code.shape == (b, t, 8, 4, 1)
-    (ref, _, ref_code), lat = O.forward(sd64_cpu, model.arch, x.double().cpu(), force_codes=code.cpu().view(b * t, 8, 4, 1),
+    h, w = H // 16, W // 16
+    assert out.shape == (b, t, 3, H, W) and code.shape == (b, t, h, w, 1)
+    (ref, _, ref_code), lat = O.forward(sd64_cpu, model.arch, x.double().cpu(), force_codes=code.cpu().view(b * t, h, w, 1),
                                         return_latents=True)
     agree = (code.cpu() == ref_code).float().mean().item()
     print('b=%d t=%d: code agreement %.3f, out PSNR %.1f dB' % (b, t, agree, psnr(out, ref)))
