@@ -195,7 +195,9 @@ int pgt_swin_mlp_bf16(const void* x, int ldx, int T, int C, const float* ln_g, c
  * qkv: bf16 [F*H*W, 3C] = [q | k | v] per token in natural (frame, y, x) order; the cyclic
  * shift, window partition / reverse and the {0,-100} shift mask are index math inside the
  * kernel; out: bf16 [F*H*W, C] in natural order.  bias_tab: fp32 [heads, 48, 48] (the 245x8
- * relative-position table expanded through relative_position_index at load time).
+ * relative-position table expanded through relative_position_index at load time).  shift applies per
+ * axis as get_window_size (modules/rstt_layers.py:90-114) does: an axis of 4 (one window) is not
+ * shifted, the other still is.
  * Replaces window_partition/roll/WindowAttention3D core/window_reverse
  * (modules/rstt_layers.py:55-88,213-230,301-329,552-568). */
 int pgt_window_attention(const void* qkv, int ldqkv, int clips, int H, int W, int C, int heads, int shift,

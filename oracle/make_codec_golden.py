@@ -6,8 +6,9 @@ module with the deterministic synthetic checkpoint (seed 0) and the size patch, 
 
 64^2, b = 1 (kept whole): encode, decode of the quantiser's z_q, decode_code of a seeded code map that includes the
 padding row, and get_soft_codes at three temperatures (in a file of their own, so each file stays below 1 MB).
-128^2, b = 2: strided samples of encode and of decode of the codebook rows of the reference's own codes.
-Inputs are not stored: `oracle.make_golden.golden_input(seed, b, H)` regenerates them bit-exactly."""
+128^2, b = 2 and 64x192, b = 1: strided samples of encode and of decode of the codebook rows of the reference's own
+codes; at 64x192 also decode_code of a seeded code map.
+Inputs are not stored: `oracle.make_golden.golden_input(seed, b, H, W)` regenerates them bit-exactly."""
 import os
 
 import torch
@@ -16,7 +17,7 @@ import torch.nn.functional as F
 from oracle.make_golden import GOLDEN, _reference_model, golden_input, sample_into
 
 CODEC_TEMPS = (1.0, 10.0, 100.0)
-CODEC_STRIDES = {'z_e': 4, 'out': 4}                # 128^2, b = 2
+CODEC_STRIDES = {'z_e': 4, 'out': 4}                # 128^2, b = 2 and 64x192
 
 
 def codec_code_map(seed, Fr, h, w, n_embed):
@@ -70,6 +71,23 @@ def main():
     sample_into(rec, 'z_e', torch.cat(zs, 0), CODEC_STRIDES['z_e'])
     sample_into(rec, 'out', torch.cat(outs, 0), CODEC_STRIDES['out'])
     path = os.path.join(GOLDEN, 'tdcrqvae3_codec_b%d_%d_seed%d.pt' % (b, H, seed))
+    torch.save(rec, path)
+    print('wrote %s (%.0f KB)' % (path, os.path.getsize(path) / 1e3))
+    # 64x192: level 4 and the mid layers are one window row deep, where only x is shifted (get_window_size per axis)
+    seed, H, W = 23, 64, 192
+    generalise_size(m, H, W)
+    x = golden_input(seed, 1, H, W)
+    with torch.no_grad():
+        z_e = V.encode(m, x.view(1, 3, 3, H, W))
+        codes = m.quantizer(z_e)[2]
+        out = V.decode(m, F.embedding(codes[..., 0], m.quantizer.codebooks[0].weight))
+        code = codec_code_map(seed, 3, H // 16, W // 16, n_embed)
+        out_code = V.decode_code(m, code)
+    rec = {'seed': seed, 'b': 1, 'H': H, 'W': W, 'codes': codes, 'code': code}
+    sample_into(rec, 'z_e', z_e, CODEC_STRIDES['z_e'])
+    sample_into(rec, 'out', out, CODEC_STRIDES['out'])
+    sample_into(rec, 'out_code', out_code, CODEC_STRIDES['out'])
+    path = os.path.join(GOLDEN, 'tdcrqvae3_codec_b1_%dx%d_seed%d.pt' % (H, W, seed))
     torch.save(rec, path)
     print('wrote %s (%.0f KB)' % (path, os.path.getsize(path) / 1e3))
 

@@ -7,8 +7,9 @@ Run where the reference checkout is available (PGT_REFERENCE_ROOT); the tests on
     python -m oracle.make_golden --full     # 512^2 (the reference's native size, NO size patch) and 1024^2 (size patch)
     python -m oracle.make_golden --video    # first 8 frames of assets/inputdemovideo.mp4, downscaled to 128^2, through
                                             # inference.py's loop
+    python -m oracle.make_golden --nonsquare  # 64x192, 192x64 and 64x128 (b = 2), strided samples as at 128^2
     python -m oracle.make_golden --swin     # the Video-Swin BasicLayer of modules/swin.py (TDRQVAE) on stand-in weights
-Inputs are not stored: `golden_input(seed, b, H)` regenerates them bit-exactly.
+Inputs are not stored: `golden_input(seed, b, H, W)` regenerates them bit-exactly.
 
 The full-size fixtures are stored compactly (the raw outputs are 50-200 MB): every code index (int16), the top-2
 logit values of every token (the margin that decides whether a code flip is a real error), full logit rows for a
@@ -42,9 +43,9 @@ def load_network_g():
         return yaml.safe_load(f)['network_g']
 
 
-def golden_input(seed, b, H):
+def golden_input(seed, b, H, W=None):
     g = torch.Generator().manual_seed(seed)
-    return torch.rand(b * 3, 3, H, H, generator=g)
+    return torch.rand(b * 3, 3, H, H if W is None else W, generator=g)
 
 
 def sampled_rows(T, seed):
@@ -61,8 +62,8 @@ def sample_into(rec, key, t, stride):
     rec[key + '_absmax'] = t.abs().max().item()
 
 
-def small_record(out, logits, lq, vq_out, vq_loss, vq_codes, seed, b, H):
-    rec = {'seed': seed, 'b': b, 'H': H, 'w': 1.0, 'adain': True, 'codes': logits.argmax(-1),
+def small_record(out, logits, lq, vq_out, vq_loss, vq_codes, seed, b, H, W):
+    rec = {'seed': seed, 'b': b, 'H': H, 'W': W, 'w': 1.0, 'adain': True, 'codes': logits.argmax(-1),
            'vq_loss': vq_loss, 'vq_codes': vq_codes}
     for key, t in (('out', out), ('logits', logits), ('lq_feat', lq.contiguous()), ('vq_out', vq_out)):
         sample_into(rec, key, t.float(), SMALL_STRIDES[key] * b)
@@ -80,24 +81,30 @@ def _reference_model():
     return build_reference_model(opt, sd)
 
 
-def small():
+def small_cases(m, cases, name):
+    """Strided-sample fixtures (small_record) of the reference forward and TDCRQVAE3.forward at (seed, b, H, W)."""
     from oracle.reference_loader import reference_forward, import_reference, generalise_size
-    m = _reference_model()
     ref_mod = import_reference()
-    for (seed, b, H) in ((1, 1, 128), (2, 2, 128)):
-        x = golden_input(seed, b, H)
+    for (seed, b, H, W) in cases:
+        x = golden_input(seed, b, H, W)
         out, logits, lq = reference_forward(m, x, w=1.0, adain=True)
         # the registered TDCRQVAE3.forward (L2-argmin path) on the same module / weights
         vq = []
         with torch.no_grad():
             for i in range(b):
-                generalise_size(m, H, H)
+                generalise_size(m, H, W)
                 vq.append(ref_mod.TDCRQVAE3.forward(m, x[i * 3:(i + 1) * 3]))
         rec = small_record(out, logits, lq, torch.cat([v[0] for v in vq], 0), torch.stack([v[1] for v in vq]),
-                           torch.cat([v[2] for v in vq], 0), seed, b, H)
-        path = os.path.join(GOLDEN, 'pgtformer_ref_b%d_%d_seed%d.pt' % (b, H, seed))
+                           torch.cat([v[2] for v in vq], 0), seed, b, H, W)
+        path = os.path.join(GOLDEN, name(seed, b, H, W))
         torch.save(rec, path)
         print('wrote', path, {k: tuple(v.shape) for k, v in rec.items() if torch.is_tensor(v)})
+
+
+def small():
+    from oracle.reference_loader import reference_forward
+    m = _reference_model()
+    small_cases(m, ((1, 1, 128, 128), (2, 2, 128, 128)), lambda s, b, H, W: 'pgtformer_ref_b%d_%d_seed%d.pt' % (b, H, s))
     # 64^2, small enough to keep whole
     seed, H = 7, 64
     out, logits, lq = reference_forward(m, golden_input(seed, 1, H), w=1.0, adain=True)
@@ -105,6 +112,19 @@ def small():
     torch.save({'seed': seed, 'b': 1, 'H': H, 'w': 1.0, 'adain': True, 'out': out, 'logits': logits,
                 'lq_feat': lq.contiguous()}, path)
     print('wrote', path)
+
+
+# Non-square frames: one 64-pixel side puts a single window row (or column) at level 4 and in the mid layers, where
+# get_window_size shifts only the other axis.  The reference runs one clip at a time; b = 2 checks the clip loop.
+NONSQUARE_CASES = ((11, 1, 64, 192), (12, 1, 192, 64), (13, 2, 64, 128))
+
+
+def nonsquare_name(seed, b, H, W):
+    return 'pgtformer_ref_b%d_%dx%d_seed%d.pt' % (b, H, W, seed)
+
+
+def nonsquare():
+    small_cases(_reference_model(), NONSQUARE_CASES, nonsquare_name)
 
 
 def compact_record(out, logits, lq, seed, H, lq_stride):
@@ -221,6 +241,7 @@ if __name__ == '__main__':
     ap.add_argument('--full', action='store_true')
     ap.add_argument('--video', action='store_true')
     ap.add_argument('--swin', action='store_true')
+    ap.add_argument('--nonsquare', action='store_true')
     a = ap.parse_args()
     if a.full:
         full()
@@ -228,5 +249,7 @@ if __name__ == '__main__':
         video()
     if a.swin:
         swin()
-    if not (a.full or a.video or a.swin):
+    if a.nonsquare:
+        nonsquare()
+    if not (a.full or a.video or a.swin or a.nonsquare):
         small()

@@ -8,9 +8,10 @@ from this repo's `network_g` with `type: TDRQVAE` and loaded with the determinis
 The reference's TDRQVAE runs any b and t.  forward and get_codes need no size patch; decode_code away from 512^2 needs
 the `quantizer.code_shape` patch of reference_loader.generalise_size (applied here alone: TDRQVAE has no parsing net).
 
-Fixtures (inputs are not stored: `golden_clips(seed, b, t, H)` regenerates them bit-exactly):
+Fixtures (inputs are not stored: `golden_clips(seed, b, t, H, W)` regenerates them bit-exactly):
   64^2,  b = 1, t = 3: whole tensors;
   128^2, b = 2, t = 7: the depth is padded 7 -> 10 and the windows are shifted in depth; strided samples;
+  64x192, b = 1, t = 3: H != W; strided samples;
   512^2, b = 1, t = 3: the reference's native size, compact: frame samples as fp16 (the reference materialises
   [F, 16384, 16384] fp32 scores at its 128^2 AttnBlocks, so F stays 3).
 Each records z_e = encode(frames), the same after tdswin_pre, every code with its top-2 distance margin, quant_loss, the
@@ -27,10 +28,11 @@ import torch
 from oracle.make_golden import GOLDEN, load_network_g, sample_into
 
 SPEC_JSON = os.path.join(GOLDEN, 'tdrqvae_state_dict_spec.json')
-# (seed, b, t, H) -> flat sample strides of the large tensors; None keeps the tensor whole
+# (seed, b, t, H[, W]) -> flat sample strides of the large tensors; None keeps the tensor whole
 CASES = {(31, 1, 3, 64): None,
          (32, 2, 7, 128): {'z': 16, 'out': 32, 'soft': 64},
-         (33, 1, 3, 512): {'z': 64, 'out': 64, 'soft': 256}}
+         (33, 1, 3, 512): {'z': 64, 'out': 64, 'soft': 256},
+         (34, 1, 3, 64, 192): {'z': 4, 'out': 4, 'soft': 16}}
 
 
 def network_g():
@@ -39,13 +41,14 @@ def network_g():
     return g
 
 
-def golden_clips(seed, b, t, H):
+def golden_clips(seed, b, t, H, W=None):
     g = torch.Generator().manual_seed(seed)
-    return torch.rand(b, t, 3, H, H, generator=g)
+    return torch.rand(b, t, 3, H, H if W is None else W, generator=g)
 
 
-def golden_name(seed, b, t, H):
-    return 'tdrqvae_ref_b%d_t%d_%d_seed%d.pt' % (b, t, H, seed)
+def golden_name(seed, b, t, H, W=None):
+    size = '%d' % H if W is None else '%dx%d' % (H, W)
+    return 'tdrqvae_ref_b%d_t%d_%s_seed%d.pt' % (b, t, size, seed)
 
 
 def import_reference_tdrqvae():
@@ -106,26 +109,29 @@ def write_spec(m):
     print('wrote %s (%d entries)' % (SPEC_JSON, len(spec)))
 
 
-def mint(m, seed, b, t, H, strides):
-    x = golden_clips(seed, b, t, H)
-    Fr, h = b * t, H // 16
-    m.quantizer.code_shape = torch.Size([h, h, 1])           # generalise_size's patch (decode_code only)
+def mint(m, seed, b, t, H, strides, W=None):
+    x = golden_clips(seed, b, t, H, W)
+    W = H if W is None else W
+    Fr, h, w = b * t, H // 16, W // 16
+    m.quantizer.code_shape = torch.Size([h, w, 1])           # generalise_size's patch (decode_code only)
     t0 = time.time()
     with torch.no_grad():
         out, loss, code = m(x)
         z_q, loss2, code2 = m(x, code_only=True)
         assert torch.equal(code, code2) and torch.equal(loss, loss2)
-        z_e = m.encode(x.view(Fr, 3, H, H))
-        z_pre = m.tdswin_pre(z_e.view(b, t, h, h, -1).permute(0, 4, 1, 2, 3)).permute(0, 2, 3, 4, 1)
+        z_e = m.encode(x.view(Fr, 3, H, W))
+        z_pre = m.tdswin_pre(z_e.view(b, t, h, w, -1).permute(0, 4, 1, 2, 3)).permute(0, 2, 3, 4, 1)
         dist = m.quantizer.codebooks[0].compute_distances(z_pre)
         top2 = dist.topk(2, dim=-1, largest=False).values
-        assert torch.equal(dist.argmin(-1), code.view(b, t, h, h))
-        out_code = m.decode_code(code.view(Fr, h, h, 1))
-        soft, soft_code = m.get_soft_codes(x.view(Fr, 3, H, H), temp=1.0)
+        assert torch.equal(dist.argmin(-1), code.view(b, t, h, w))
+        out_code = m.decode_code(code.view(Fr, h, w, 1))
+        soft, soft_code = m.get_soft_codes(x.view(Fr, 3, H, W), temp=1.0)
     rec = {'seed': seed, 'b': b, 't': t, 'H': H, 'quant_loss': loss, 'codes': code.to(torch.int16),
            'margin': (top2[..., 1] - top2[..., 0]).contiguous(), 'soft_codes': soft_code.to(torch.int16)}
     tensors = {'z_e': (z_e, 'z'), 'z_pre': (z_pre.contiguous(), 'z'), 'z_q': (z_q.contiguous(), 'z'),
                'out': (out, 'out'), 'out_code': (out_code, 'out'), 'soft': (soft, 'soft')}
+    if W != H:
+        rec['W'] = W
     for key, (v, kind) in tensors.items():
         if strides is None:
             rec[key] = v.contiguous()
@@ -134,7 +140,7 @@ def mint(m, seed, b, t, H, strides):
     if H >= 512:                                             # the compact fixture keeps its frame samples as fp16
         for key in ('out', 'out_code'):
             rec[key] = rec[key].to(torch.float16)
-    path = os.path.join(GOLDEN, golden_name(seed, b, t, H))
+    path = os.path.join(GOLDEN, golden_name(seed, b, t, H, W if W != H else None))
     torch.save(rec, path)
     print('wrote %s in %.0f s (%.0f KB)' % (path, time.time() - t0, os.path.getsize(path) / 1e3))
 
@@ -144,9 +150,9 @@ def main():
     m = reference_model()
     write_spec(m)
     only = [int(a) for a in sys.argv[1:]]
-    for (seed, b, t, H), strides in CASES.items():
+    for (seed, b, t, H, *W), strides in CASES.items():
         if not only or H in only:
-            mint(m, seed, b, t, H, strides)
+            mint(m, seed, b, t, H, strides, *W)
 
 
 if __name__ == '__main__':

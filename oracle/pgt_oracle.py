@@ -74,16 +74,24 @@ def upsample(sd, p, x):
 # --------------------------------------------------------------------------- window attention
 def shift_mask(Hp, Wp, dtype=torch.float32):
     """(nW,48,48) mask of {0,-100}: 3x3 region labels of the rolled map, window-partitioned
-    (`modules/rstt_layers.py:552-568`)."""
+    (`modules/rstt_layers.py:552-568`), with the shifts of `window_shift(Hp, Wp)`.  An unshifted axis has one region:
+    the reference's slice(-0, None) covers it whole."""
+    sy, sx = window_shift(Hp, Wp)
     img = torch.zeros((1, FRAMES, Hp, Wp, 1), dtype=dtype)
     cnt = 0
-    for hs in (slice(0, -WIN[0]), slice(-WIN[0], -SHIFT[0]), slice(-SHIFT[0], None)):
-        for ws in (slice(0, -WIN[1]), slice(-WIN[1], -SHIFT[1]), slice(-SHIFT[1], None)):
+    for hs in (slice(0, -WIN[0]), slice(-WIN[0], -sy), slice(-sy, None)):
+        for ws in (slice(0, -WIN[1]), slice(-WIN[1], -sx), slice(-sx, None)):
             img[:, :, hs, ws, :] = cnt
             cnt += 1
     mw = window_partition(img).view(-1, FRAMES * WIN[0] * WIN[1])
     am = mw.unsqueeze(1) - mw.unsqueeze(2)
     return torch.where(am != 0, torch.full_like(am, -100.0), torch.zeros_like(am))
+
+
+def window_shift(H, W):
+    """get_window_size (`modules/rstt_layers.py:90-114`), per axis: an axis no larger than the window is not shifted,
+    whatever the other axis is."""
+    return (SHIFT[0] if H > WIN[0] else 0), (SHIFT[1] if W > WIN[1] else 0)
 
 
 def window_partition(x):
@@ -124,15 +132,16 @@ def swin_block(sd, p, x, heads, shifted, mask):
     H, W are multiples of 4 on this path so the pad branch is a no-op."""
     B, D, H, W, C = x.shape
     assert H % WIN[0] == 0 and W % WIN[1] == 0
-    do_shift = shifted and H > WIN[0] and W > WIN[1]       # get_window_size (:90-114)
+    sy, sx = window_shift(H, W) if shifted else (0, 0)
+    do_shift = sy > 0 or sx > 0
     h = layer_norm(sd, p + '.norm1', x)
     if do_shift:
-        h = torch.roll(h, shifts=(-SHIFT[0], -SHIFT[1]), dims=(2, 3))
+        h = torch.roll(h, shifts=(-sy, -sx), dims=(2, 3))
     xw = window_partition(h).view(-1, D * WIN[0] * WIN[1], C)
     aw = window_attention(sd, p + '.attn', xw, heads, mask if do_shift else None)
     h = window_reverse(aw.view(-1, D, WIN[0], WIN[1], C), B, D, H, W)
     if do_shift:
-        h = torch.roll(h, shifts=SHIFT, dims=(2, 3))
+        h = torch.roll(h, shifts=(sy, sx), dims=(2, 3))
     x = x + h
     m = linear(sd, p + '.mlp.fc1', layer_norm(sd, p + '.norm2', x))
     m = linear(sd, p + '.mlp.fc2', F.gelu(m))                # exact-erf GELU (:116-132)
@@ -143,7 +152,7 @@ def encoder_layer(sd, p, x4, heads, depth=2):
     """EncoderLayer.forward (`modules/rstt_layers.py:535-575`); x4 is [b*3,C,H,W]."""
     BD, C, H, W = x4.shape
     x = x4.view(BD // FRAMES, FRAMES, C, H, W).permute(0, 1, 3, 4, 2)
-    mask = shift_mask(H, W, x4.dtype) if (H > WIN[0] and W > WIN[1]) else None
+    mask = shift_mask(H, W, x4.dtype) if any(window_shift(H, W)) else None
     for i in range(depth):
         x = swin_block(sd, '%s.blocks.%d' % (p, i), x, heads, shifted=(i % 2 == 1), mask=mask)
     return x.permute(0, 1, 4, 2, 3).reshape(BD, C, H, W)

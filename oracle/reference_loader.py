@@ -8,7 +8,7 @@ Recipe (SURVEY.md Appendix C):
     (`archs/pgtformer_arch.py:15-16`, `archs/tdcrqvae3_arch.py:32`);
   * the reference is 512x512-only in three places (`archs/pgtformer_arch.py:375-378`, `:649`,
     `:535-550,698-700`); `generalise_size` applies the three run-time patches (bit-identical at
-    512x512) so that 128x128 / 256x256 fixtures can be generated;
+    512x512) so that fixtures at other sizes, H != W included, can be generated;
   * the reference crashes for clip-batch b>1 (`modules/rstt_layers.py:896-904`): callers loop
     over clips (b=1).
 """
@@ -88,10 +88,11 @@ def build_reference_model(network_g, state_dict=None, seed=0):
 
 def generalise_size(m, H, W):
     """Three run-time patches that lift the 512x512 restriction (SURVEY F4 / Appendix C step 4).
-    Bit-identical to the unpatched model at 512x512."""
+    Bit-identical to the unpatched model at 512x512.  H and W may differ: the fusion keys the reference looks up are
+    feature widths (`feat.shape[-1]`), which the rescaled keys below follow."""
     import torch
     import torch.nn.functional as F
-    assert H == W and H % 64 == 0
+    assert H % 64 == 0 and W % 64 == 0
     cn = m.conditionnet
 
     def bisenet_forward(self, x):           # `archs/pgtformer_arch.py:365-379` with (32,32)->(H/16,W/16)

@@ -37,7 +37,7 @@ constexpr int WIN_N = 48;
 
 template <int D>
 __global__ void __launch_bounds__(256)
-window_attn_kernel(const __nv_bfloat16* __restrict__ qkv, int ldqkv, int H, int W, int C, int heads, int shift,
+window_attn_kernel(const __nv_bfloat16* __restrict__ qkv, int ldqkv, int H, int W, int C, int heads, int sy, int sx,
                    const float* __restrict__ bias_tab, __nv_bfloat16* __restrict__ out, int ldo) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ int tok[WIN_N];
@@ -50,10 +50,10 @@ window_attn_kernel(const __nv_bfloat16* __restrict__ qkv, int ldqkv, int H, int 
     const int i = threadIdx.x;
     const int fr = i >> 4, iy = (i >> 2) & 3, ix = i & 3;
     const int ys = wy * 4 + iy, xs = wx * 4 + ix;         // coordinates in the rolled (shifted) frame
-    const int y = (ys + shift) % H, x = (xs + shift) % W; // source / destination pixel (roll by -shift, then back)
+    const int y = (ys + sy) % H, x = (xs + sx) % W;       // source / destination pixel (roll by -shift, then back)
     tok[i] = ((clip * 3 + fr) * H + y) * W + x;
-    const int hr = ys < H - 4 ? 0 : (ys < H - shift ? 1 : 2);
-    const int wr = xs < W - 4 ? 0 : (xs < W - shift ? 1 : 2);
+    const int hr = ys < H - 4 ? 0 : (ys < H - sy ? 1 : 2); // an unshifted axis is one region
+    const int wr = xs < W - 4 ? 0 : (xs < W - sx ? 1 : 2);
     lab[i] = hr * 3 + wr;
   }
   __syncthreads();
@@ -109,7 +109,7 @@ window_attn_kernel(const __nv_bfloat16* __restrict__ qkv, int ldqkv, int H, int 
         s[nt][1] = s[nt][1] * scale + bb0.y;
         s[nt][2] = s[nt][2] * scale + bb1.x;
         s[nt][3] = s[nt][3] * scale + bb1.y;
-        if (shift > 0) {
+        if (sy > 0 || sx > 0) {
           const int lc0 = lab[c], lc1 = lab[c + 1];
           if (lc0 != l0) s[nt][0] += -100.f;
           if (lc1 != l0) s[nt][1] += -100.f;
@@ -311,7 +311,8 @@ extern "C" int pgt_window_attention(const void* qkv, int ldqkv, int clips, int H
   PGT_CHECK_ARG(qkv && bias_tab && out && clips > 0 && H > 0 && W > 0 && heads > 0);
   PGT_CHECK_ARG(H % 4 == 0 && W % 4 == 0 && C % heads == 0 && ldqkv % 8 == 0 && ldo % 8 == 0 && ldqkv >= 3 * C);
   PGT_CHECK_ARG(shift >= 0 && shift < 4);
-  if (H <= 4 || W <= 4) shift = 0;                         // get_window_size(): no shift when the map is one window
+  // get_window_size(), per axis: an axis that is one window deep is not shifted, whatever the other axis is
+  const int sy = H > 4 ? shift : 0, sx = W > 4 ? shift : 0;
   const int d = C / heads;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   dim3 grid((H / 4) * (W / 4), clips);
@@ -324,7 +325,7 @@ extern "C" int pgt_window_attention(const void* qkv, int ldqkv, int clips, int H
       attr32 = true;
     }
     window_attn_kernel<32><<<grid, 256, smem, st>>>(reinterpret_cast<const __nv_bfloat16*>(qkv), ldqkv, H, W, C, heads,
-                                                    shift, bias_tab, reinterpret_cast<__nv_bfloat16*>(out), ldo);
+                                                    sy, sx, bias_tab, reinterpret_cast<__nv_bfloat16*>(out), ldo);
   } else if (d == 64) {
     static bool attr = false;
     if (!attr) {
@@ -332,7 +333,7 @@ extern "C" int pgt_window_attention(const void* qkv, int ldqkv, int clips, int H
       attr = true;
     }
     window_attn_kernel<64><<<grid, 256, smem, st>>>(reinterpret_cast<const __nv_bfloat16*>(qkv), ldqkv, H, W, C, heads,
-                                                    shift, bias_tab, reinterpret_cast<__nv_bfloat16*>(out), ldo);
+                                                    sy, sx, bias_tab, reinterpret_cast<__nv_bfloat16*>(out), ldo);
   } else {
     return PGT_ERR_UNSUPPORTED;
   }

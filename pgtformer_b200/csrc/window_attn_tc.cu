@@ -44,7 +44,8 @@ constexpr float WT_MASK = -144.26950408889634f;
 constexpr int WT_SMEM = 2048 /*pad*/ + WT_NST * WT_STAGE + WT_TAB_BYTES + 512 /*barriers*/ + 1024 /*align*/;
 
 struct WinParams {
-  int clips, H, W, C, heads, d, shift;
+  int clips, H, W, C, heads, d;
+  int sy, sx;                                        // shift per axis (get_window_size)
   int nwx, nwy, n_windows, n_pairs, n_chunks, hpc;   // hpc: heads per 64-column chunk
   int ldo;                                           // output row pitch (elements)
   __nv_bfloat16* out;
@@ -62,10 +63,10 @@ __device__ __forceinline__ WinCoord win_coord(const WinParams& p, int w) {
   c.clip = w / per_clip;
   const int r = w - c.clip * per_clip;
   const int wy = r / p.nwx, wx = r - wy * p.nwx;
-  c.xs = (p.shift > 0 && wx == p.nwx - 1) ? 1 : 0;
-  c.ys = (p.shift > 0 && wy == p.nwy - 1) ? 1 : 0;
-  c.x0 = wx * 4 + p.shift;
-  c.y0 = wy * 4 + p.shift;
+  c.xs = (p.sx > 0 && wx == p.nwx - 1) ? 1 : 0;
+  c.ys = (p.sy > 0 && wy == p.nwy - 1) ? 1 : 0;
+  c.x0 = wx * 4 + p.sx;
+  c.y0 = wy * 4 + p.sy;
   return c;
 }
 
@@ -314,7 +315,6 @@ extern "C" int pgt_window_attention_tc(const void* qkv, int ldqkv, int clips, in
                                        const void* tab, void* out, int ldo, void* stream) {
   PGT_CHECK_ARG(qkv && tab && out && clips > 0 && H > 0 && W > 0 && heads > 0);
   PGT_CHECK_ARG(H % 4 == 0 && W % 4 == 0 && C % heads == 0 && ldqkv % 8 == 0 && ldo % 8 == 0 && ldqkv >= 3 * C);
-  if (H <= 4 || W <= 4) shift = 0;                         // get_window_size(): no shift when the map is one window
   const int d = C / heads;
   if ((d != 32 && d != 64) || heads != WT_HEADS || C % 128 != 0 || (shift != 0 && shift != 2)) return PGT_ERR_UNSUPPORTED;
   auto al = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
@@ -327,7 +327,9 @@ extern "C" int pgt_window_attention_tc(const void* qkv, int ldqkv, int clips, in
     if (rc != PGT_OK) return rc;
   }
   WinParams p{};
-  p.clips = clips; p.H = H; p.W = W; p.C = C; p.heads = heads; p.d = d; p.shift = shift;
+  p.clips = clips; p.H = H; p.W = W; p.C = C; p.heads = heads; p.d = d;
+  // get_window_size(), per axis: an axis that is one window deep is not shifted, whatever the other axis is
+  p.sy = H > 4 ? shift : 0; p.sx = W > 4 ? shift : 0;
   p.nwx = W / 4; p.nwy = H / 4;
   p.n_windows = clips * p.nwx * p.nwy;
   p.n_pairs = (p.n_windows + 1) / 2;

@@ -25,8 +25,9 @@ def window_reference(qkv, clips, H, W, C, heads, bias_tab, shifted):
     from oracle import pgt_oracle as O
     d = C // heads
     x = qkv.float().view(clips, 3, H, W, 3 * C)
-    do_shift = shifted and H > 4 and W > 4
-    xs = torch.roll(x, (-2, -2), (2, 3)) if do_shift else x
+    sy, sx = O.window_shift(H, W) if shifted else (0, 0)      # get_window_size: each axis on its own
+    do_shift = sy > 0 or sx > 0
+    xs = torch.roll(x, (-sy, -sx), (2, 3))
     xw = O.window_partition(xs).view(-1, 48, 3 * C)
     q = xw[..., :C].view(-1, 48, heads, d).permute(0, 2, 1, 3) * d ** -0.5
     k = xw[..., C:2 * C].view(-1, 48, heads, d).permute(0, 2, 1, 3)
@@ -38,8 +39,7 @@ def window_reference(qkv, clips, H, W, C, heads, bias_tab, shifted):
         attn = (attn.view(-1, nW, heads, 48, 48) + mask[None, :, None]).view(-1, heads, 48, 48)
     ow = (attn.softmax(-1) @ v).transpose(1, 2).reshape(-1, 48, C)
     ref = O.window_reverse(ow.view(-1, 3, 4, 4, C), clips, 3, H, W)
-    if do_shift:
-        ref = torch.roll(ref, (2, 2), (2, 3))
+    ref = torch.roll(ref, (sy, sx), (2, 3))
     return ref.reshape(-1, C)
 
 

@@ -9,7 +9,7 @@ import torch
 
 from conftest import ROOT, golden_sample, load_golden
 
-SMALL = [('tdrqvae_ref_b1_t3_64_seed31.pt'), ('tdrqvae_ref_b2_t7_128_seed32.pt')]
+SMALL = [('tdrqvae_ref_b1_t3_64_seed31.pt'), ('tdrqvae_ref_b2_t7_128_seed32.pt'), ('tdrqvae_ref_b1_t3_64x192_seed34.pt')]
 
 
 @pytest.fixture(scope='module')
@@ -57,13 +57,13 @@ def test_oracle_matches_reference_golden(name, tdrq_spec, tdrq_sd):
     from oracle.make_tdrqvae_golden import golden_clips
     arch = tdrq_spec[0]
     g = load_golden(name)
-    b, t, H = g['b'], g['t'], g['H']
-    x = golden_clips(g['seed'], b, t, H)
+    b, t, H, W = g['b'], g['t'], g['H'], g.get('W', g['H'])
+    x = golden_clips(g['seed'], b, t, H, W)
     with torch.no_grad():
         (out, loss, code), lat = O.forward(tdrq_sd, arch, x, return_latents=True)
         z_q = O.forward(tdrq_sd, arch, x, code_only=True)[0]
-        out_code = O.decode_code(tdrq_sd, arch, code.view(b * t, H // 16, H // 16, 1))
-        soft, soft_code = O.get_soft_codes(tdrq_sd, arch, x.view(b * t, 3, H, H), 1.0)
+        out_code = O.decode_code(tdrq_sd, arch, code.view(b * t, H // 16, W // 16, 1))
+        soft, soft_code = O.get_soft_codes(tdrq_sd, arch, x.view(b * t, 3, H, W), 1.0)
     errs = {k: _cmp(v, g, k) for k, v in (('z_e', lat['z_e']), ('z_pre', lat['z_pre']), ('z_q', z_q), ('out', out),
                                           ('out_code', out_code), ('soft', soft))}
     print(name, errs)

@@ -17,7 +17,8 @@ from test_swin3d_gpu import test_window3d_attention_core as window3d_core
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-FIXTURES = ['tdrqvae_ref_b1_t3_64_seed31.pt', 'tdrqvae_ref_b2_t7_128_seed32.pt', 'tdrqvae_ref_b1_t3_512_seed33.pt']
+FIXTURES = ['tdrqvae_ref_b1_t3_64_seed31.pt', 'tdrqvae_ref_b2_t7_128_seed32.pt', 'tdrqvae_ref_b1_t3_512_seed33.pt',
+            'tdrqvae_ref_b1_t3_64x192_seed34.pt']
 
 
 @pytest.fixture(scope='module')
@@ -127,18 +128,18 @@ def _take(t, g, key):
 def test_methods_against_reference_golden(model, name):
     from oracle.make_tdrqvae_golden import golden_clips
     g = load_golden(name)
-    b, t, H = g['b'], g['t'], g['H']
-    h = H // 16
-    x = golden_clips(g['seed'], b, t, H).to(DEV)
+    b, t, H, W = g['b'], g['t'], g['H'], g.get('W', g['H'])
+    h, w = H // 16, W // 16
+    x = golden_clips(g['seed'], b, t, H, W).to(DEV)
     eng = model.engine()
     z_e, z_pre = eng.latents(x)
     res = {}
     for key, v in (('z_e', z_e), ('z_pre', z_pre)):
         s, ref, amax = _take(v, g, key)
         res[key] = ((s - ref).abs().max() / amax).item()
-    assert torch.equal(model.encode(x.view(b * t, 3, H, H)), z_e)
+    assert torch.equal(model.encode(x.view(b * t, 3, H, W)), z_e)
     out, loss, code = model(x)
-    assert out.shape == (b, t, 3, H, H) and out.dtype == torch.float32 and code.shape == (b, t, h, h, 1)
+    assert out.shape == (b, t, 3, H, W) and out.dtype == torch.float32 and code.shape == (b, t, h, w, 1)
     ref_code = g['codes'].long()
     agree = (code.cpu() == ref_code).float().mean().item()
     # codes must match wherever the reference's top-2 distance margin clearly exceeds the distance error our z error
@@ -159,10 +160,10 @@ def test_methods_against_reference_golden(model, name):
     res.update(out_psnr=psnr(s, ref), out_err=((s - ref).abs().max() / amax).item())
     s, ref, amax = _take(zq_tf, g, 'z_q')
     res['z_q_err'] = ((s - ref).abs().max() / amax).item()
-    out_code = model.decode_code(ref_code.view(b * t, h, h, 1))
+    out_code = model.decode_code(ref_code.view(b * t, h, w, 1))
     s, ref, amax = _take(out_code, g, 'out_code')
     res.update(out_code_psnr=psnr(s, ref), out_code_err=((s - ref).abs().max() / amax).item())
-    soft, soft_code = model.get_soft_codes(x.view(b * t, 3, H, H), 1.0)
+    soft, soft_code = model.get_soft_codes(x.view(b * t, 3, H, W), 1.0)
     res['soft_code_agree'] = (soft_code.cpu() == g['soft_codes'].long()).float().mean().item()
     print('%s: %s' % (name, res))
     assert res['z_e'] < 2.5e-2 and res['z_pre'] < 2.5e-2
