@@ -1215,6 +1215,23 @@ extern "C" int pgt_linear_bf16(const void* A, int lda, const void* W, int ldw, i
   return dispatch_gemm(tmA, W, ldw, p, static_cast<cudaStream_t>(stream));
 }
 
+// Tile (tw x th pixels) of a conv of this shape: the 16 x 8 halo tile for the stride-1 3x3 convs (pad 1) and the
+// upsample phases (ksize 2, pgt_conv_up2x_bf16) of up to 128 output channels, otherwise the widest power-of-two
+// rows of at most 128 pixels.  tw * th < 128 when a 128-row tile spans frames.  Returns whether it is a halo conv.
+static bool conv_tile_shape(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo, int& tw, int& th) {
+  static const bool no_halo = getenv("PGT_NO_HALO") != nullptr;
+  const int H = Hin / stride, W = Win / stride;
+  const bool halo = !no_halo && stride == 1 && ((ksize == 3 && pad_lo == 1) || ksize == 2) && Cout <= 128 && Hin >= HALO_TH &&
+                    Win >= HALO_TW;
+  tw = 1; th = 1;
+  if (halo) { tw = HALO_TW; th = HALO_TH; }
+  else {
+    while (tw * 2 <= W && tw * 2 <= BM) tw *= 2;
+    while (th * 2 <= H && tw * th * 2 <= BM) th *= 2;
+  }
+  return halo;
+}
+
 // pad_y/pad_x: zero rows/cols before the input (stride 1); up_phase >= 0: phase (py = up_phase>>1, px = up_phase&1)
 // of a nearest-x2-upsample-folded conv — the [F,Hin,Win,Cout] result is scattered to out[F, 2y+py, 2x+px, :].
 static int conv_impl(const void* x, int F, int Hin, int Win, int Cin, int ldx, const void* Wp, int ldw, int Cout,
@@ -1257,21 +1274,14 @@ static int conv_impl(const void* x, int F, int Hin, int Win, int Cin, int ldx, c
     p.out = static_cast<char*>(p.out) + ((long long)py * Wo + px) * p.ldo * esz;
     p.o_sx = 2LL * p.ldo; p.o_sy = 2LL * Wo * p.ldo; p.o_sf = 4LL * Hin * Win * p.ldo;
   }
-  // 128-pixel tile = tn frames x th rows x tw columns
-  static const bool no_halo = getenv("PGT_NO_HALO") != nullptr;
-  const bool halo = !no_halo && stride == 1 && Cout <= 128 && Hin >= HALO_TH && Win >= HALO_TW &&
-                    ((up_phase < 0 && ksize == 3 && pad_y == 1 && pad_x == 1) || (up_phase >= 0 && ksize == 2));
+  // 128-pixel tile = tn frames x th rows x tw columns (ksize 2 is only ever an upsample phase, and pad_x == pad_y
+  // otherwise)
+  int tw, th;
+  const bool halo = conv_tile_shape(Hin, Win, Cout, ksize, stride, pad_y, tw, th);
   p.ntaps = ksize * ksize; p.tap_kw = ksize;
   p.tap_oy = up_phase >= 0 ? (up_phase >> 1) : 0;          // phase (py, px): tap (dy, dx) reads slab row dy + py, col dx + px
   p.tap_ox = up_phase >= 0 ? (up_phase & 1) : 0;
-  int tw = 1, th = 1, tn;
-  if (halo) {
-    tw = HALO_TW; th = HALO_TH;
-  } else {
-    while (tw * 2 <= p.W && tw * 2 <= BM) tw *= 2;
-    while (th * 2 <= p.H && tw * th * 2 <= BM) th *= 2;
-  }
-  tn = BM / (tw * th);
+  const int tn = BM / (tw * th);
   p.tw = tw; p.th = th; p.tn = tn;
   p.tiles_x = ceil_div(p.W, tw);
   p.tiles_y = ceil_div(p.H, th);
@@ -1311,27 +1321,12 @@ static int conv_impl(const void* x, int F, int Hin, int Win, int Cin, int ldx, c
   return dispatch_gemm(tmA, Wp, ldw, p, static_cast<cudaStream_t>(stream));
 }
 
-// Tile shape (tw x th pixels) of the conv the library would launch for this shape, 0 when a 128-row tile may span
-// frames.  Mirrors the tile selection of conv_impl.
-static int conv_tile_shape(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo, int& tw, int& th) {
-  static const bool no_halo = getenv("PGT_NO_HALO") != nullptr;
-  const int H = Hin / stride, W = Win / stride;
-  const bool halo = !no_halo && stride == 1 && ((ksize == 3 && pad_lo == 1) || ksize == 2) && Cout <= 128 && Hin >= HALO_TH &&
-                    Win >= HALO_TW;      // ksize 2: an upsample phase (pgt_conv_up2x_bf16)
-  tw = 1; th = 1;
-  if (halo) { tw = HALO_TW; th = HALO_TH; }
-  else {
-    while (tw * 2 <= W && tw * 2 <= BM) tw *= 2;
-    while (th * 2 <= H && tw * th * 2 <= BM) th *= 2;
-  }
-  return tw * th == BM ? 1 : 0;
-}
-
 // 128-row tiles per frame of the conv the library would launch for this shape (0: a tile may span frames, so the
 // fused GroupNorm statistics are unavailable).
 extern "C" int pgt_conv_tiles_per_frame(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo) {
   int tw, th;
-  if (!conv_tile_shape(Hin, Win, Cout, ksize, stride, pad_lo, tw, th)) return 0;
+  conv_tile_shape(Hin, Win, Cout, ksize, stride, pad_lo, tw, th);
+  if (tw * th != BM) return 0;
   return ceil_div(Win / stride, tw) * ceil_div(Hin / stride, th);
 }
 
@@ -1339,7 +1334,8 @@ extern "C" int pgt_conv_tiles_per_frame(int Hin, int Win, int Cout, int ksize, i
 // statistics, so a tile that reaches past the frame's right or bottom edge adds rows that are not output pixels.
 extern "C" int pgt_conv_tiles_exact(int Hin, int Win, int Cout, int ksize, int stride, int pad_lo) {
   int tw, th;
-  if (!conv_tile_shape(Hin, Win, Cout, ksize, stride, pad_lo, tw, th)) return 0;
+  conv_tile_shape(Hin, Win, Cout, ksize, stride, pad_lo, tw, th);
+  if (tw * th != BM) return 0;
   const int H = Hin / stride, W = Win / stride;
   return (W % tw == 0 && H % th == 0) ? (W / tw) * (H / th) : 0;
 }

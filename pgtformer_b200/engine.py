@@ -192,8 +192,6 @@ class Engine:
     def _new(self, *shape, dtype=BF):
         return torch.empty(*shape, dtype=dtype, device=self.dev)
 
-    _fusing = False           # set per forward: SFT fusion active (w > 0)
-
     def _stats_tiles(self, H, W, cout, ksize, stride, pad_lo):
         """Tiles per frame of a conv whose epilogue emits the next GroupNorm's statistics; 0: no fused statistics.
         Fused statistics only where the conv's tile grid divides the frame: the models take frames of any multiple of
@@ -444,18 +442,59 @@ class Engine:
         return ops.assemble_cond(o0, o1, o2, self._new(Fr, H // 16, W // 16, 64))
 
     # ------------------------------------------------------------------ encoder / decoder
-    def encoder_frames(self, x):
+    res_shortcut = 'nin_shortcut'      # the 1x1 conv of a width-changing `res` block (VQGAN's ResBlock: conv_out)
+
+    def _walk(self, blocks, h, lo=0, hi=None, taps=None, outs=None, feats=None, wgt=0.0):
+        """Runs blocks[lo:hi] of a block list (spec: `_autoencoder_blocks`, VQGANEngine._blocks) on h.  Returns (h,
+        {taps[i]: output of block i}).  outs {i: tensor}: block i (`res` or `swin`) writes its output there, a slice
+        of an SFT concat buffer.  A `fuse` block runs only with feats and wgt > 0, on feats[its source].
+
+        GroupNorm statistics: a block passes gn_next to its producer exactly when the next block that runs reads its
+        input through a GroupNorm (`res`, `attn`, or the `norm` before conv_out); a `fuse` that does not run is not
+        next.  Its epilogue then writes the statistics, and that GroupNorm skips its own pass over the tensor.  (The
+        RGB conv_in and `up`, always followed by a `res`, always write them.)"""
+        fusing = feats is not None and wgt > 0
+        hi = len(blocks) if hi is None else hi
+        outs, found = outs or {}, {}
+        for i in range(lo, hi):
+            kind, p, cout = blocks[i][:3]
+            if kind == 'fuse' and not fusing:
+                continue
+            nxt = next((b[0] in ('res', 'attn', 'norm') for b in blocks[i + 1:] if fusing or b[0] != 'fuse'), False)
+            if kind == 'conv_in':
+                h = self.conv_in(h, p) if p + '.weight' == self.arch.stem else self._conv3(h, p, cout, gn_out=nxt)
+            elif kind == 'res':
+                h = self.td_resblock(h, p, cout, gn_next=nxt, out=outs.get(i), shortcut=self.res_shortcut)
+            elif kind == 'attn':
+                h = self.attn_block(h, p, gn_next=nxt)
+            elif kind == 'swin':
+                h = self.encoder_layer(h, p, blocks[i][3], blocks[i][4], gn_next=nxt, out=outs.get(i))
+            elif kind == 'down':
+                h = self._conv3(h, p + '.conv', cout, stride=2, pad_lo=0, gn_out=nxt)
+            elif kind == 'up':
+                h = self.up2x(h, p + '.conv')
+            elif kind == 'fuse':
+                h = self.fuse_sft(feats[blocks[i][3]], h, p[len('fuse_convs_dict.'):], wgt, gn_next=nxt)
+            else:
+                raise AssertionError(kind)
+            if taps and i in taps:
+                found[taps[i]] = h
+        return h, found
+
+    @staticmethod
+    def _cat_half(cat, lo, C):
+        """cat[..., lo:lo + C] of an SFT concat buffer, marked as its slice so that fuse_sft reads it in place."""
+        half = cat[..., lo:lo + C]
+        half._pgt_cat = cat
+        return half
+
+    def encoder_frames(self, x, outs=None):
         """The per-frame prefix of Encoder.forward (`archs/tdcrqvae3_arch.py:540-560`): conv_in and every level before
         the first one with attention, including the Downsample into it — nothing here looks across frames, so the
-        streaming pipeline runs it once per distinct frame.  Returns (h, feats, next level)."""
+        streaming pipeline runs it once per distinct frame.  Returns (h, {level: output}, index of the next block)."""
         a = self.arch
-        h = self.conv_in(x)
-        feats = []
-        lvl = 0
-        while lvl < a.num_levels - 1 and not a.level_has_attn[lvl]:
-            h = self._encoder_level(h, lvl, feats)
-            lvl += 1
-        return h, feats, lvl
+        h, feats = self._walk(a.enc_blocks, x, 0, a.frame_blocks, a.enc_taps, outs)
+        return h, feats, a.frame_blocks
 
     def conv_in(self, x, p='encoder.conv_in'):
         """encoder.conv_in on the fp32 NCHW frames.  Cin = 3: the kernel builds the patch rows itself; its epilogue also
@@ -467,49 +506,27 @@ class Engine:
         ops.conv_rgb(x, self.w[p + '.weight'], self.w[p + '.bias'], h, 3, 1, 1, gn_stats=stats)
         return h
 
-    def _encoder_level(self, h, lvl, feats):
+    def encoder_clips(self, h, feats, i, outs=None):
+        """The rest of Encoder.forward (`:560-573`) on clip-major frames, from block i; feats: the level outputs so
+        far.  Returns (h [F,h,w,z], the output of every level)."""
         a = self.arch
-        last = lvl == a.num_levels - 1
-        Fr, H, W, _ = h.shape
-        # a level whose output is an SFT skip tensor writes it into the [enc | dec | t] concat buffer of that fusion
-        # (not the last level: its output carries GroupNorm statistics for mid.block_1 and must stay contiguous)
-        slot = None
-        if self._fusing and lvl in a.fuse_level_key and not last:
-            cat = self._cat_slot(Fr, H, W, a.level_ch[lvl])
-            slot = cat[..., :a.level_ch[lvl]]
-        for blk in range(a.num_res_blocks):
-            # the next consumer of this level's output is a Normalize() only at the last level (mid.block_1);
-            # otherwise it is the stride-2 Downsample conv, whose own epilogue feeds the next level's norm1
-            nxt = last and blk == a.num_res_blocks - 1
-            fin = slot if blk == a.num_res_blocks - 1 else None
-            h = self.td_resblock(h, 'encoder.down.%d.block.%d' % (lvl, blk), a.level_ch[lvl],
-                                 gn_next=nxt and not a.level_has_attn[lvl], out=None if a.level_has_attn[lvl] else fin)
-            if a.level_has_attn[lvl]:
-                h = self.encoder_layer(h, 'encoder.down.%d.attn.%d' % (lvl, blk), a.num_heads[lvl], a.depths[lvl],
-                                       gn_next=nxt, out=fin)
-        if slot is not None:
-            h._pgt_cat = cat
-        feats.append(h)
-        if not last:
-            h = self._conv3(h, 'encoder.down.%d.downsample.conv' % lvl, a.level_ch[lvl], stride=2, pad_lo=0, gn_out=True)
-        return h
+        h, more = self._walk(a.enc_blocks, h, i, len(a.enc_blocks) - 2, a.enc_taps, outs)
+        (_, norm, _), (_, conv, zc) = a.enc_blocks[-2:]
+        return self._conv3(h, conv, zc, gn=norm), list(feats.values()) + list(more.values())
 
-    def encoder_clips(self, h, feats, lvl):
-        """The rest of Encoder.forward (`:560-573`) on clip-major frames."""
+    def encoder(self, x, fusing=False):
+        """Encoder.forward (`archs/tdcrqvae3_arch.py:540-573`); x fp32 NCHW -> (h [F,h,w,z], feats).  fusing: the SFT
+        fusion will read the level outputs, so each one (but the last level's, which carries GroupNorm statistics for
+        mid.block_1 and must stay contiguous) is written straight into the encoder half of its concat buffer."""
         a = self.arch
-        while lvl < a.num_levels:
-            h = self._encoder_level(h, lvl, feats)
-            lvl += 1
-        h = self.td_resblock(h, 'encoder.mid.block_1', a.level_ch[-1])
-        h = self.encoder_layer(h, 'encoder.mid.attn_1', a.num_heads[-1], a.depths[-1], gn_next=True)
-        h = self.td_resblock(h, 'encoder.mid.block_2', a.level_ch[-1], gn_next=True)
-        zc = 2 * a.z_channels if a.double_z else a.z_channels
-        return self._conv3(h, 'encoder.conv_out', zc, gn='encoder.norm_out'), feats
-
-    def encoder(self, x):
-        """Encoder.forward (`archs/tdcrqvae3_arch.py:540-573`); x fp32 NCHW -> (h [F,h,w,z], feats)."""
-        h, feats, lvl = self.encoder_frames(x)
-        return self.encoder_clips(h, feats, lvl)
+        outs = {}
+        if fusing:
+            Fr, _, H, W = x.shape
+            for i, lvl in a.enc_taps.items():
+                C = a.level_ch[lvl]
+                if lvl in a.fuse_level_key and lvl != a.num_levels - 1:
+                    outs[i] = self._cat_half(self._cat_slot(Fr, H >> lvl, W >> lvl, C), 0, C)
+        return self.encoder_clips(*self.encoder_frames(x, outs), outs)
 
     def _gather(self, t, idx):
         """t[idx] along the frame dimension, GroupNorm statistics included."""
@@ -522,33 +539,15 @@ class Engine:
 
     def decoder(self, z, feats=None, wgt=0.0):
         """Decoder.forward (`archs/tdcrqvae3_arch.py:672-707`) / the inlined variant with SFT fusion
-        (`archs/pgtformer_arch.py:680-710`).  z: [F,h,w,z_channels] bf16 -> out fp32 NCHW."""
-        a = self.arch
-        h = self._conv3(z, 'decoder.conv_in', a.level_ch[-1], gn_out=True)
-        h = self.td_resblock(h, 'decoder.mid.block_1', a.level_ch[-1])
-        h = self.encoder_layer(h, 'decoder.mid.attn_1', a.num_heads[-1], a.depths[-1], gn_next=True)
-        h = self.td_resblock(h, 'decoder.mid.block_2', a.level_ch[-1], gn_next=True)
-        for lvl in reversed(range(a.num_levels)):
-            nblk = a.num_res_blocks + 1
-            fuse = feats is not None and lvl in a.fuse_level_key and wgt > 0
-            cat = getattr(feats[lvl], '_pgt_cat', None) if fuse else None
-            for blk in range(nblk):
-                # next consumer is a Normalize(): the next block of this level, or decoder.norm_out after the very
-                # last block; after the level's last block comes the SFT concat / the upsample conv instead
-                nxt = blk < nblk - 1 or (lvl == 0 and not fuse)
-                C = a.level_ch[lvl]
-                fin = cat[..., C:2 * C] if (cat is not None and blk == nblk - 1) else None
-                h = self.td_resblock(h, 'decoder.up.%d.block.%d' % (lvl, blk), C,
-                                     gn_next=nxt and not a.level_has_attn[lvl], out=None if a.level_has_attn[lvl] else fin)
-                if a.level_has_attn[lvl]:
-                    h = self.encoder_layer(h, 'decoder.up.%d.attn.%d' % (lvl, blk), a.num_heads[lvl], a.depths[lvl],
-                                           gn_next=nxt, out=fin)
-                if fin is not None:
-                    h._pgt_cat = cat
-            if fuse:
-                h = self.fuse_sft(feats[lvl], h, a.fuse_level_key[lvl], wgt, gn_next=(lvl == 0))
-            if lvl != 0:
-                h = self.up2x(h, 'decoder.up.%d.upsample.conv' % lvl)
+        (`archs/pgtformer_arch.py:680-710`).  z: [F,h,w,z_channels] bf16 -> out fp32 NCHW.  A level whose encoder
+        output sits in an SFT concat buffer writes its own output into the decoder half."""
+        blocks = self.arch.dec_blocks
+        outs = {}
+        for i, b in enumerate(blocks):
+            cat = getattr(feats[b[3]], '_pgt_cat', None) if b[0] == 'fuse' and feats is not None and wgt > 0 else None
+            if cat is not None:
+                outs[i - 1] = self._cat_half(cat, b[2], b[2])
+        h, _ = self._walk(blocks, z, 0, len(blocks) - 2, outs=outs, feats=feats, wgt=wgt)
         return self.decoder_out(h)
 
     def up2x(self, h, p):
@@ -623,17 +622,17 @@ class Engine:
         hh, ww = H // 16, W // 16
         T, E = Fr * hh * ww, a.dim_embd
         wd = self.w
-        self._fusing = (not code_only) and float(w) > 0 and frame_index is None
         pos = self.parse_pos(x)
         # encoder
         if frame_index is None:
-            h, feats = self.encoder(x)
+            h, feats = self.encoder(x, fusing=not code_only and float(w) > 0)
         else:
             pos = self._gather(pos.view(x.shape[0], -1), frame_index).view(T, -1)
-            h, feats, lvl = self.encoder_frames(x)
+            h, feats, i = self.encoder_frames(x)
             # only the skip tensors the SFT fusion will read are worth moving (level 0 is 100 MB per clip and unused)
-            feats = [self._gather(f, frame_index) if (i in a.fuse_level_key and w > 0) else f for i, f in enumerate(feats)]
-            h, feats = self.encoder_clips(self._gather(h, frame_index), feats, lvl)
+            feats = {lvl: self._gather(f, frame_index) if (lvl in a.fuse_level_key and w > 0) else f
+                     for lvl, f in feats.items()}
+            h, feats = self.encoder_clips(self._gather(h, frame_index), feats, i)
         h = h.view(T, -1)
         lq32 = self._lin(h, 'quant_conv', a.embed_dim, out_dtype=torch.float32)
         lq = self._lin(h, 'quant_conv', a.embed_dim)
@@ -771,7 +770,6 @@ class Engine:
         encoder's latent map (H/16 x W/16 for the four-downsample encoders)."""
         a = self.arch
         x = x.to(self.dev, torch.float32).contiguous()
-        self._fusing = False                                   # the plain autoencoder has no SFT fusion
         h, _ = self.encoder(x)
         Fr, hh, ww, _ = h.shape
         z_e = self._lin(h.view(Fr * hh * ww, -1), 'quant_conv', a.embed_dim, out_dtype=torch.float32)
@@ -784,7 +782,6 @@ class Engine:
         -> fp32 NCHW [F,3,16h,16w]."""
         a = self.arch
         Fr, hh, ww, E = z_q.shape
-        self._fusing = False
         z = self._lin(z_q.to(self.dev, BF).reshape(Fr * hh * ww, E), 'post_quant_conv', a.z_channels)
         return self.decoder(z.view(Fr, hh, ww, a.z_channels))
 
@@ -794,7 +791,6 @@ class Engine:
         """RQBottleneck.embed_code (`:355-368`): int64 codes [..., D] (each in [0, n_embed], the last row being the
         padding row; the gather does no range check) -> fp32 [T, E] = the sum of the code rows of depths d0 .. d1
         (default all: embed_code; d1 = j: the 'add' mode of embed_partial_code; d0 = d1 = j: its 'select' mode)."""
-        self._fusing = False
         D = self.depth
         codes = codes.to(self.dev, torch.int64).reshape(-1, D).contiguous()
         d1 = D - 1 if d1 is None else d1
@@ -820,7 +816,6 @@ class Engine:
         D = self.depth
         if D == 1:
             return self.embed_code(codes).unsqueeze(1)
-        self._fusing = False
         codes = codes.to(self.dev, torch.int64).reshape(-1, D).contiguous()
         out = self._new(codes.shape[0], D, self.arch.embed_dim, dtype=torch.float32)
         for d in range(D):
@@ -835,7 +830,6 @@ class Engine:
         from the default CUDA generator (reproducible under torch.manual_seed, no host sync); each depth works on the
         residual the earlier codes left and writes K-slice d of p."""
         a = self.arch
-        self._fusing = False
         z = z_e.to(self.dev, torch.float32).reshape(-1, a.embed_dim).contiguous()
         T, D, K = z.shape[0], self.depth, a.n_embed
         p = self._new(T, D, K, dtype=torch.float32)

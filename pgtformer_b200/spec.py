@@ -177,6 +177,53 @@ class Arch:
         self.upsample_convs = _upsample_convs(self.num_levels)
         self.codebooks = _codebooks(self.depth)
         self.packed_apart = ('conditionnet.',)                      # BiSeNet: BatchNorms folded into its convs
+        self.enc_blocks, self.dec_blocks, self.frame_blocks, self.enc_taps = _autoencoder_blocks(self, 'swin')
+
+
+def _autoencoder_blocks(a, attn):
+    """Encoder and decoder of TDCRQVAE3 (`archs/tdcrqvae3_arch.py:540-573, 672-707`, attn='swin') or of the 2-D RQ-VAE
+    (`archs/tdrqvae_arch.py:650-680, 753-784`, attn='attn') as block lists in execution order, for Engine._walk.
+    Entries are (kind, state-dict prefix, output channels, ...): `swin` (EncoderLayer) adds its heads and depth, `fuse`
+    (PGTFormer's Fuse_sft_block after a decoder level, `archs/pgtformer_arch.py:680-710`, keyed by `fuse_level_key`) the
+    level whose encoder output it reads.  Returns (encoder blocks, decoder blocks, frame_blocks: the encoder blocks
+    before the first level with attention, which look at one frame at a time, taps: {encoder block index: level} of
+    each level's output)."""
+    fuse = getattr(a, 'fuse_level_key', {})
+
+    def attention(p, lvl):
+        if attn == 'swin':
+            return ('swin', p, a.level_ch[lvl], a.num_heads[lvl], a.depths[lvl])
+        return ('attn', p, a.level_ch[lvl])
+
+    last = a.num_levels - 1
+    enc, taps, frame_blocks = [('conv_in', 'encoder.conv_in', a.ch)], {}, None
+    for lvl in range(a.num_levels):
+        if frame_blocks is None and (a.level_has_attn[lvl] or lvl == last):
+            frame_blocks = len(enc)
+        for b in range(a.num_res_blocks):
+            enc.append(('res', 'encoder.down.%d.block.%d' % (lvl, b), a.level_ch[lvl]))
+            if a.level_has_attn[lvl]:
+                enc.append(attention('encoder.down.%d.attn.%d' % (lvl, b), lvl))
+        taps[len(enc) - 1] = lvl
+        if lvl != last:
+            enc.append(('down', 'encoder.down.%d.downsample' % lvl, a.level_ch[lvl]))
+    zc = 2 * a.z_channels if a.double_z else a.z_channels
+    enc += [('res', 'encoder.mid.block_1', a.level_ch[-1]), attention('encoder.mid.attn_1', last),
+            ('res', 'encoder.mid.block_2', a.level_ch[-1]), ('norm', 'encoder.norm_out', a.level_ch[-1]),
+            ('conv_out', 'encoder.conv_out', zc)]
+    dec = [('conv_in', 'decoder.conv_in', a.level_ch[-1]), ('res', 'decoder.mid.block_1', a.level_ch[-1]),
+           attention('decoder.mid.attn_1', last), ('res', 'decoder.mid.block_2', a.level_ch[-1])]
+    for lvl in reversed(range(a.num_levels)):
+        for b in range(a.num_res_blocks + 1):
+            dec.append(('res', 'decoder.up.%d.block.%d' % (lvl, b), a.level_ch[lvl]))
+            if a.level_has_attn[lvl]:
+                dec.append(attention('decoder.up.%d.attn.%d' % (lvl, b), lvl))
+        if lvl in fuse:
+            dec.append(('fuse', 'fuse_convs_dict.' + fuse[lvl], a.level_ch[lvl], lvl))
+        if lvl != 0:
+            dec.append(('up', 'decoder.up.%d.upsample' % lvl, a.level_ch[lvl]))
+    dec += [('norm', 'decoder.norm_out', a.level_ch[0]), ('conv_out', 'decoder.conv_out', a.out_ch)]
+    return tuple(enc), tuple(dec), frame_blocks, taps
 
 
 def _upsample_convs(num_levels):
@@ -364,6 +411,8 @@ class TDRQVAEArch:
         self.upsample_convs = _upsample_convs(self.num_levels)
         self.codebooks = _codebooks(1)
         self.packed_apart = ('tdswin_pre.', 'tdswin_post.')         # Video-Swin BasicLayers: swin3d.pack_blocks
+        self.enc_blocks, self.dec_blocks, self.frame_blocks, _ = _autoencoder_blocks(self, 'attn')
+        self.enc_taps = {}                                          # its Encoder returns h alone
 
 
 def build_tdrqvae_spec(network_g):
@@ -496,6 +545,8 @@ class RQVAEArch:
         self.upsample_convs = _upsample_convs(self.num_levels)
         self.codebooks = _codebooks(self.depth)
         self.packed_apart = ()
+        self.enc_blocks, self.dec_blocks, self.frame_blocks, _ = _autoencoder_blocks(self, 'attn')
+        self.enc_taps = {}                                          # its Encoder returns h alone
 
 
 RGB_STEM_WIDTHS = (64, 128)           # pgt_conv_rgb_bf16 3x3 output widths

@@ -16,49 +16,7 @@ from .swin3d import basic_layer_rows
 class TDRQVAEEngine(Engine):
     arch_class = TDRQVAEArch
 
-    # ------------------------------------------------------------------ blocks
-    def encoder(self, x):
-        """Encoder.forward (`archs/tdrqvae_arch.py:650-680`); x fp32 NCHW [F,3,H,W] -> (h [F,H/16,W/16,z], [])."""
-        a = self.arch
-        h = self.conv_in(x)
-        for lvl in range(a.num_levels):
-            C, last = a.level_ch[lvl], lvl == a.num_levels - 1
-            for blk in range(a.num_res_blocks):
-                # a Normalize() reads this block's output unless the stride-2 Downsample conv comes next
-                more = blk < a.num_res_blocks - 1 or last
-                h = self.td_resblock(h, 'encoder.down.%d.block.%d' % (lvl, blk), C,
-                                     gn_next=more or a.level_has_attn[lvl])
-                if a.level_has_attn[lvl]:
-                    h = self.attn_block(h, 'encoder.down.%d.attn.%d' % (lvl, blk), gn_next=more)
-            if not last:
-                h = self._conv3(h, 'encoder.down.%d.downsample.conv' % lvl, C, stride=2, pad_lo=0, gn_out=True)
-        C = a.level_ch[-1]
-        h = self.td_resblock(h, 'encoder.mid.block_1', C, gn_next=True)
-        h = self.attn_block(h, 'encoder.mid.attn_1', gn_next=True)
-        h = self.td_resblock(h, 'encoder.mid.block_2', C, gn_next=True)
-        return self._conv3(h, 'encoder.conv_out', a.z_channels, gn='encoder.norm_out'), []
-
-    def decoder(self, z, feats=None, wgt=0.0):
-        """Decoder.forward (`archs/tdrqvae_arch.py:753-784`); z [F,h,w,z_channels] bf16 -> fp32 NCHW [F,3,16h,16w]."""
-        a = self.arch
-        C = a.level_ch[-1]
-        h = self._conv3(z, 'decoder.conv_in', C, gn_out=True)
-        h = self.td_resblock(h, 'decoder.mid.block_1', C, gn_next=True)
-        h = self.attn_block(h, 'decoder.mid.attn_1', gn_next=True)
-        h = self.td_resblock(h, 'decoder.mid.block_2', C, gn_next=True)
-        nblk = a.num_res_blocks + 1
-        for lvl in reversed(range(a.num_levels)):
-            C = a.level_ch[lvl]
-            for blk in range(nblk):
-                # a Normalize() reads this block's output unless the Upsample conv comes next
-                more = blk < nblk - 1 or lvl == 0
-                h = self.td_resblock(h, 'decoder.up.%d.block.%d' % (lvl, blk), C, gn_next=more or a.level_has_attn[lvl])
-                if a.level_has_attn[lvl]:
-                    h = self.attn_block(h, 'decoder.up.%d.attn.%d' % (lvl, blk), gn_next=more)
-            if lvl != 0:
-                h = self.up2x(h, 'decoder.up.%d.upsample.conv' % lvl)
-        return self.decoder_out(h)
-
+    # ------------------------------------------------------------------ Video-Swin layers
     def tdswin(self, name, z, b, t, hh, ww, out_dtype=BF):
         """tdswin_pre / tdswin_post on the latent rows z [b*t*hh*ww, E] bf16 -> new rows of out_dtype."""
         a = self.arch
@@ -72,7 +30,6 @@ class TDRQVAEEngine(Engine):
         a = self.arch
         b, t, _, H, W = x.shape
         xs = x.to(self.dev, torch.float32).reshape(b * t, 3, H, W).contiguous()
-        self._fusing = False
         h, _ = self.encoder(xs)
         hh, ww = H // a.down, W // a.down
         T = b * t * hh * ww

@@ -22,34 +22,24 @@ class VQGANEngine(Engine):
         return VQGANArch(g, self.codeformer)
 
     # ------------------------------------------------------------------ encoder / generator
-    def _walk(self, prefix, blocks, h, lo, hi, taps=None):
-        """Runs blocks[lo:hi] of `prefix` on h; with taps (flat index -> key) returns {key: output after that block}."""
-        feats = {}
-        for i in range(lo, hi):
-            kind, cin, cout, _ = blocks[i]
-            p = '%s.blocks.%d' % (prefix, i)
-            # the next block reads this output through a GroupNorm: its statistics come from this block's epilogue
-            nxt = blocks[i + 1][0] in ('res', 'attn', 'norm') if i + 1 < len(blocks) else False
-            if kind == 'res':
-                h = self.td_resblock(h, p, cout, gn_next=nxt, shortcut='conv_out')
-            elif kind == 'attn':
-                h = self.attn_block(h, p, gn_next=nxt)
-            elif kind == 'down':
-                h = self._conv3(h, p + '.conv', cout, stride=2, pad_lo=0, gn_out=True)
-            elif kind == 'up':
-                h = self.up2x(h, p + '.conv')
-            else:
-                raise AssertionError(kind)
-            if taps is not None and i in taps:
-                feats[taps[i]] = h
-        return h, feats
+    res_shortcut = 'conv_out'
+
+    def _blocks(self, prefix, blocks, fuse=None):
+        """The flat `prefix`.blocks list as Engine._walk entries (kind, state-dict prefix, output channels), with a
+        `fuse` block (CodeFormer's Fuse_sft_block, reading the tapped encoder output of its size key) after each block
+        index in fuse."""
+        out = []
+        for i, (kind, _, cout, _) in enumerate(blocks):
+            out.append((kind, '%s.blocks.%d' % (prefix, i), cout))
+            if fuse and i in fuse:
+                out.append(('fuse', 'fuse_convs_dict.' + fuse[i], cout, fuse[i]))
+        return out
 
     def encoder(self, x, taps=None):
         """encoder.blocks[:-2] on x fp32 NCHW [b,3,H,W] -> (h bf16 [b,h,w,C] with the final GroupNorm's statistics,
         {key: tapped block output})."""
-        a = self.arch
-        h = self.conv_in(x, 'encoder.blocks.0')
-        return self._walk('encoder', a.enc_blocks, h, 1, len(a.enc_blocks) - 2, taps)
+        blocks = self._blocks('encoder', self.arch.enc_blocks)
+        return self._walk(blocks, x, 0, len(blocks) - 2, taps)
 
     def encoder_out(self, h, out, nchw=False):
         """The encoder tail: GroupNorm (no SiLU) -> conv 3x3 to emb_dim, into out (fp32 NHWC rows, fp32 NCHW with
@@ -65,26 +55,18 @@ class VQGANEngine(Engine):
         """generator.blocks on z bf16 [b,h,w,emb_dim] -> fp32 NCHW [b,3,H,W]; with feats and wgt > 0 CodeFormer's
         Fuse_sft_block after the blocks of arch.fuse_gen (`archs/codeformer_arch.py:356-363`)."""
         a = self.arch
-        blocks = a.gen_blocks
-        h = self._conv3(z, 'generator.blocks.0', blocks[0][2], gn_out=True)
-        fuse = a.fuse_gen if (feats is not None and wgt > 0) else {}
-        i = 1
-        for j in sorted(fuse) + [len(blocks) - 2]:
-            h, _ = self._walk('generator', blocks, h, i, j + 1 if j in fuse else j)
-            if j in fuse:
-                h = self.fuse(feats[fuse[j]], h, fuse[j], wgt)
-            i = j + 1
-        n = len(blocks)
+        blocks = self._blocks('generator', a.gen_blocks, getattr(a, 'fuse_gen', None))
+        h, _ = self._walk(blocks, z, 0, len(blocks) - 2, feats=feats, wgt=wgt)
+        n = len(a.gen_blocks)
         return self.decoder_out(h, 'generator.blocks.%d' % (n - 2), 'generator.blocks.%d' % (n - 1), silu=False, out_ch=3)
 
-    def fuse(self, enc, dec, key, wgt):
-        """Fuse_sft_block (`archs/codeformer_arch.py:218-226`): the concat [enc | dec] -> sft_tail; the output feeds
-        the next ResBlock's GroupNorm."""
+    def fuse_sft(self, enc, dec, key, wgt, gn_next=False):
+        """Fuse_sft_block (`archs/codeformer_arch.py:218-226`): the concat [enc | dec] -> sft_tail."""
         Fr, H, W, C = dec.shape
         cat = self._new(Fr, H, W, 2 * C)
         ops.copy2d(enc, cat[..., :C])
         ops.copy2d(dec, cat[..., C:])
-        return self.sft_tail(cat, dec, 'fuse_convs_dict.' + key, wgt, gn_next=True)
+        return self.sft_tail(cat, dec, 'fuse_convs_dict.' + key, wgt, gn_next)
 
     # ------------------------------------------------------------------ VQAutoEncoder.forward
     def _check(self, x):

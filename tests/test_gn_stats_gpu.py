@@ -93,6 +93,10 @@ def _model(name, network_g):
         if name in ('pgtformer', 'tdcrqvae3', 'tdrqvae'):
             g = dict(network_g)
             g['type'] = {'pgtformer': 'PGTFormer', 'tdcrqvae3': 'TDCRQVAE3', 'tdrqvae': 'TDRQVAE'}[name]
+        elif name == 'tdcrqvae3_r2':                     # two res blocks per level
+            g = copy.deepcopy(network_g)
+            g['type'] = 'TDCRQVAE3'
+            g['ddconfig']['num_res_blocks'] = 2
         elif name.startswith('rqvae_'):
             from oracle.make_rqvae_golden import CONFIGS
             g = copy.deepcopy(CONFIGS[name[len('rqvae_'):]])
@@ -116,7 +120,7 @@ def _run(name, m, H, W):
         frames = np.random.RandomState(2).randint(0, 256, size=(5, H, W, 3), dtype=np.uint8)
         out = VideoRestorer(m, w=1.0, adain=True, clips_per_batch=4).restore(frames)
         assert out.shape == frames.shape
-    elif name == 'tdcrqvae3':
+    elif name in ('tdcrqvae3', 'tdcrqvae3_r2'):
         _, _, code = m(_images(3, H, W, 3))
         m.decode_code(code)
     elif name == 'tdrqvae':
@@ -143,7 +147,7 @@ def _run(name, m, H, W):
 CASES = {
     ('pgtformer', 64, 64): 20, ('pgtformer', 64, 192): None, ('pgtformer', 192, 192): None,
     ('video', 64, 192): None,
-    ('tdcrqvae3', 64, 64): 30, ('tdcrqvae3', 64, 192): None,
+    ('tdcrqvae3', 64, 64): 30, ('tdcrqvae3', 64, 192): None, ('tdcrqvae3_r2', 64, 64): 48,
     ('tdrqvae', 64, 64): 35, ('tdrqvae', 64, 192): None,
     ('rqvae_r2', 128, 128): 90, ('rqvae_r2', 128, 192): None,
     ('rqvae_r1', 128, 128): 40, ('rqvae_r1', 128, 384): None,
