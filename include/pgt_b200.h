@@ -41,7 +41,10 @@ enum { PGT_OUT_NHWC = 0, PGT_OUT_NCHW = 1 };
 /* act must be PGT_ACT_RELU: y = relu(acc + bias + residual)  (ResNet BasicBlock, archs/pgtformer_arch.py:56-68) */
 enum { PGT_EPI_FLAG_RELU_AFTER_RESIDUAL = 1 };
 
-/* Fused epilogue shared by the tensor-core GEMM / implicit-GEMM conv. */
+/* Fused epilogue shared by the tensor-core GEMM / implicit-GEMM conv.  bias, out, residual and aux need only element
+ * alignment, so any view of a larger buffer may be passed (e.g. b + 1, or out[:, 1:]): the library checks the pointers
+ * and pitches and takes scalar loads / stores where 16-byte vectors or TMA would be misaligned (slower, same values).
+ * Only gn_stats needs out 16-byte aligned and ldo * element size a multiple of 16 (PGT_ERR_UNSUPPORTED otherwise). */
 typedef struct pgt_epilogue {
   const float* bias;     /* [N] fp32 or NULL                                               */
   int32_t act;           /* PGT_ACT_*                                                      */
@@ -134,8 +137,9 @@ int pgt_conv_up2x_bf16(const void* x, int F, int Hin, int Win, int Cin, int ldx,
  * folded bn1 + relu, archs/pgtformer_arch.py:95-99,110-112); Cout = 64.
  *   Wp: bf16 [Cout, ldw], K index (ky*ksize + kx)*3 + c, ldw % 8 == 0;  mean3 / std3: HOST pointers to 3 floats or
  *   NULL: the input is (x - mean) / std with zero padding applied after the normalisation, as in the reference;
- *   act: PGT_ACT_NONE or PGT_ACT_RELU;  out: bf16 [F*Ho*Wo, ldo];  gn_stats: optional GroupNorm partials of the
- *   output, fp32 [ceil(F*Ho*Wo/128)][4][32][2] (requires Ho*Wo % 128 == 0).
+ *   bias: fp32 [Cout], element alignment suffices;  act: PGT_ACT_NONE or PGT_ACT_RELU;  out: bf16 [F*Ho*Wo, ldo];
+ *   gn_stats: optional GroupNorm partials of the output, fp32 [ceil(F*Ho*Wo/128)][4][32][2] (requires
+ *   Ho*Wo % 128 == 0).
  * PGT_ERR_UNSUPPORTED for any other geometry. */
 int pgt_conv_rgb_bf16(const float* x_nchw, int F, int H, int W, int ksize, int stride, int pad, const float* mean3,
                       const float* std3, const void* Wp, int ldw, int Cout, const float* bias, int act, void* out,

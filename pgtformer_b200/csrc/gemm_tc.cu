@@ -22,7 +22,8 @@
 // so a transaction that never completes traps the launch instead of hanging it.
 //
 // Kernels in this file: gemm_tc_kernel<BN> (linear / generic implicit-GEMM conv; BN = 64, 128 or 256),
-// conv_halo_kernel<BN> (3x3 and upsample-phase convs with Cout <= 128: one halo slab serves every tap).
+// conv_halo_kernel<BN> (3x3 and upsample-phase convs with Cout <= 128: one halo slab serves every tap); each also in a
+// kVec = false instantiation for bias / output views that are not 16-byte aligned (vector_views).
 //
 // The A operand is produced by TMA in three addressing modes:
 //   LINEAR   2-D map [K, rows]
@@ -415,6 +416,8 @@ __device__ __forceinline__ DirectRow direct_row(const GemmParams& p, int m_blk, 
 }
 
 // Direct path: columns [col0, col0 + 16) of one output row, accumulators at xs (exchange row), guarded loads / stores.
+// kVec: see vector_views.
+template <bool kVec>
 __device__ __forceinline__ void epi_direct16(const GemmParams& p, const DirectRow& d, const float* xs, int col0) {
   const int ncol = min(16, p.N - col0);
   const long long orow = d.orow;
@@ -454,7 +457,7 @@ __device__ __forceinline__ void epi_direct16(const GemmParams& p, const DirectRo
       if (j < ncol) op[(((long long)d.pn * p.N + (col0 + j)) * p.H + d.py) * p.W + d.px] = f[j];
   } else if (p.out_dtype == PGT_BF16) {
     __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.out) + orow * p.ldo + col0;
-    if (ncol == 16 && ((p.ldo & 7) == 0)) {
+    if (kVec && ncol == 16 && ((p.ldo & 7) == 0)) {
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         uint4 u;
@@ -489,7 +492,7 @@ __device__ __forceinline__ float* gn_stats_ptr(const GemmParams& p, int m_blk, i
 // warpgroups write their accumulator rows into the exchange, then thread (quad, half) reads row quad * 32 + lane,
 // columns [32 half, 32 half + 32) (bf16 panels: one chunk each) or the whole panel of parity half (fp32 panels).
 // `k` counts staging items across tiles.
-template <int BN>
+template <int BN, bool kVec>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx& ctx, int warp, int lane, int tile, int& k,
                                               const float (&acc)[BN / 2]) {
   const int quad = warp & 3;                 // rows [32 quad, 32 quad + 32) of the tile
@@ -502,7 +505,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
   constexpr int SLOTS = staging_slots<BN>();
   constexpr int SLOT_SHIFT = SLOTS == 4 ? 2 : 1;
   const bool sft = SLOTS == 4 && p.epi_mode == PGT_EPI_SFT;
-  const bool bias_vec = p.bias != nullptr && (p.N % 32) == 0;   // whole chunks inside N: 128-bit bias reads
+  const bool bias_vec = kVec && p.bias != nullptr && (p.N % 32) == 0;   // whole chunks inside N: 128-bit bias reads
   const float* xrow = ctx.xch + r * XCH_LD;
 
   int n_blk, m_blk;
@@ -577,7 +580,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
         for (int sc16 = 0; sc16 < 32; sc16 += 16) {
           const int col0 = col_base + c0 + sc16;
           if (col0 >= p.N) break;
-          epi_direct16(p, drow, xrow + half * 32 + sc16, col0);
+          epi_direct16<kVec>(p, drow, xrow + half * 32 + sc16, col0);
         }
       }
       __syncwarp();
@@ -592,7 +595,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
 // epilogue_tile, so outputs and statistics are bit-identical to it.  An item (panel) is signalled to the DMA warp
 // once all its chunks are written (slot_ready counts the warpgroup's 128 threads).  `k` is the ring index of the
 // tile's first item; `bar` is a named barrier of this warpgroup's 128 threads.
-template <int BN>
+template <int BN, bool kVec>
 __device__ __forceinline__ void epilogue_tile_wg(const GemmParams& p, const EpiCtx& ctx, int wq, int bar, int tile, int k,
                                                  const float (&acc)[2][BN / 2]) {
   const int lane = lane_id();                // re-read, not kept live across the k loop (BN = 128 has no spare registers)
@@ -603,7 +606,7 @@ __device__ __forceinline__ void epilogue_tile_wg(const GemmParams& p, const EpiC
   constexpr int SLOTS = staging_slots<BN>();
   constexpr int SLOT_SHIFT = SLOTS == 4 ? 2 : 1;
   const bool sft = SLOTS == 4 && p.epi_mode == PGT_EPI_SFT;    // bf16 only: one 64-column item in two slots
-  const bool bias_vec = p.bias != nullptr && (p.N % 32) == 0;
+  const bool bias_vec = kVec && p.bias != nullptr && (p.N % 32) == 0;
   const float* xrow = ctx.xch + r * XCH_WG_LD;
 
   int n_blk, m_blk;
@@ -648,7 +651,7 @@ __device__ __forceinline__ void epilogue_tile_wg(const GemmParams& p, const EpiC
 #pragma unroll 1
         for (int sc16 = 0; sc16 < 32; sc16 += 16) {
           if (col0 + sc16 >= p.N) break;
-          epi_direct16(p, drow, xrow + sc16, col0 + sc16);
+          epi_direct16<kVec>(p, drow, xrow + sc16, col0 + sc16);
         }
       }
       __syncwarp();
@@ -662,7 +665,7 @@ __device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
   if (lane == 0) mbar_arrive(bar);
 }
 
-template <int BN>
+template <int BN, bool kVec>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
@@ -787,7 +790,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       wgmma_wait<0>();
       release_stage(&empty_bar[prev], lane);
-      epilogue_tile<BN>(p, ctx, warp, lane, tile, k, acc);
+      epilogue_tile<BN, kVec>(p, ctx, warp, lane, tile, k, acc);
     }
   }
 }
@@ -832,7 +835,7 @@ __device__ __forceinline__ void ring_skip(int& s, uint32_t& ph, int n) {
   s = t % S;
 }
 
-template <int BN>
+template <int BN, bool kVec>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
@@ -1011,7 +1014,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (++as == AS) { as = 0; aph ^= 1; }
       }
       if (j > 0) named_bar_sync(PP_EPI_BAR + wg, 256);
-      epilogue_tile_wg<BN>(p, ctx, warp & 3, PP_XCH_BAR + wg, tile, k, acc);
+      epilogue_tile_wg<BN, kVec>(p, ctx, warp & 3, PP_XCH_BAR + wg, tile, k, acc);
       if (has_next) named_bar_arrive(PP_EPI_BAR + (wg ^ 1), 256);
       k += items;
     }
@@ -1086,6 +1089,33 @@ static int setup_epilogue_maps(GemmParams& p, const CUtensorMap& placeholder, CU
   return PGT_OK;
 }
 
+// Whether the bias and the output are 16-byte aligned wherever the epilogue accesses them as vectors: the bias of an
+// N % 32 == 0 launch (float4 reads) and the bf16 NHWC output of the direct path when ldo % 8 == 0 (uint4 stores).  A view
+// starting elsewhere (b + 1, out[:, 1:]) is supported: it runs the kVec = false instantiation of the kernels, whose
+// epilogue reads and writes those one element at a time (same values).  Every other call runs kVec = true.
+static bool vector_views(const GemmParams& p) {
+  if (p.bias != nullptr && (p.N % 32) == 0 && !aligned16(p.bias)) return false;
+  if (!p.fast_epi && p.out_layout == PGT_OUT_NHWC && p.out_dtype == PGT_BF16 && (p.ldo % 8) == 0 && !aligned16(p.out))
+    return false;
+  return true;
+}
+
+template <int BN, bool kVec>
+static cudaError_t gemm_smem_once() {
+  static PerDeviceOnce once;
+  return once.run([] {
+    return cudaFuncSetAttribute(gemm_tc_kernel<BN, kVec>, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BN>::SMEM_BYTES);
+  });
+}
+
+template <int BN, bool kVec>
+static cudaError_t halo_smem_once() {
+  static PerDeviceOnce once;
+  return once.run([] {
+    return cudaFuncSetAttribute(conv_halo_kernel<BN, kVec>, cudaFuncAttributeMaxDynamicSharedMemorySize, HaloCfg<BN>::SMEM_BYTES);
+  });
+}
+
 static int encode_weight_map(CUtensorMap* tmB, const void* W, int ldw, int K, int N, int BN) {
   // rows beyond N (weight matrices are not padded to BN rows) are zero-filled by TMA
   uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
@@ -1104,8 +1134,8 @@ static int launch_gemm(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
   rc = setup_epilogue_maps(p, tmA, tmO, tmR, tmX);
   if (rc != PGT_OK) return rc;
   p.n_tiles = ceil_div(p.N, BN);
-  static PerDeviceOnce once;
-  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); }));
+  const bool vec = vector_views(p);
+  PGT_CUDA_OK((vec ? gemm_smem_once<BN, true>() : gemm_smem_once<BN, false>()));
   const int tiles = p.m_tiles * p.n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
   {
@@ -1115,7 +1145,8 @@ static int launch_gemm(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
       else snprintf(desc, sizeof(desc), "conv%d s%d F%d H%d W%d K%d N%d BN%d t%dx%dx%d e%d", p.ksize, p.mode, p.F, p.H, p.W, p.K, p.N, BN, p.tn, p.th, p.tw, p.fast_epi);
     }
     ProfScope ps(PGT_PROF_GEMM, p.flops, stream, desc);
-    gemm_tc_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
+    if (vec) gemm_tc_kernel<BN, true><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
+    else gemm_tc_kernel<BN, false><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
   }
   PGT_LAUNCH_OK();
   return PGT_OK;
@@ -1131,8 +1162,8 @@ static int launch_halo(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
   if (rc != PGT_OK) return rc;
   p.n_tiles = ceil_div(p.N, BN);
   p.b_resident = (p.ntaps * p.cin_blocks <= Cfg::B_STAGES && p.n_tiles == 1) ? 1 : 0;
-  static PerDeviceOnce once;
-  PGT_CUDA_OK(once.run([] { return cudaFuncSetAttribute(conv_halo_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES); }));
+  const bool vec = vector_views(p);
+  PGT_CUDA_OK((vec ? halo_smem_once<BN, true>() : halo_smem_once<BN, false>()));
   const int tiles = p.m_tiles * p.n_tiles;
   const int grid = tiles < num_sms() ? tiles : num_sms();
   {
@@ -1141,7 +1172,8 @@ static int launch_halo(const CUtensorMap& tmA, const void* W, int ldw, GemmParam
       snprintf(desc, sizeof(desc), "halo3 F%d H%d W%d K%d N%d BN%d e%d r%d", p.F, p.H, p.W, p.K, p.N, BN, p.fast_epi,
                p.b_resident);
     ProfScope ps(PGT_PROF_GEMM, p.flops, stream, desc);
-    conv_halo_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
+    if (vec) conv_halo_kernel<BN, true><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
+    else conv_halo_kernel<BN, false><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmO, tmR, tmX, p);
   }
   PGT_LAUNCH_OK();
   return PGT_OK;

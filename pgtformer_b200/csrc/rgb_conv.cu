@@ -86,7 +86,9 @@ __device__ __forceinline__ void rgb_build_chunks(const RgbConvParams& p, const f
   }
 }
 
-template <int KS, int STRIDE, int PAD, int N>
+// BIAS4: the bias is 16-byte aligned and read as float4 (every caller's own bias tensor); otherwise one float at a time
+// (a view such as b[1:]), in an instantiation of its own so that the aligned kernel is the same code as without it.
+template <int KS, int STRIDE, int PAD, int N, bool BIAS4>
 __global__ void __launch_bounds__(RgbCfg<KS, N>::THREADS, RgbCfg<KS, N>::PER_SM)
 rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO, const RgbConvParams p) {
   using Cfg = RgbCfg<KS, N>;
@@ -176,14 +178,19 @@ rgb_conv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
         uint32_t v[32];
         smem_row_32(xrow + hb * 32, v);
         float f[32];
-        const float4* b4 = reinterpret_cast<const float4*>(p.bias + hb * 32);
+        if (BIAS4) {
+          const float4* b4 = reinterpret_cast<const float4*>(p.bias + hb * 32);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 bb = __ldg(b4 + i);
-          f[4 * i + 0] = __uint_as_float(v[4 * i + 0]) + bb.x;
-          f[4 * i + 1] = __uint_as_float(v[4 * i + 1]) + bb.y;
-          f[4 * i + 2] = __uint_as_float(v[4 * i + 2]) + bb.z;
-          f[4 * i + 3] = __uint_as_float(v[4 * i + 3]) + bb.w;
+          for (int i = 0; i < 8; ++i) {
+            const float4 bb = __ldg(b4 + i);
+            f[4 * i + 0] = __uint_as_float(v[4 * i + 0]) + bb.x;
+            f[4 * i + 1] = __uint_as_float(v[4 * i + 1]) + bb.y;
+            f[4 * i + 2] = __uint_as_float(v[4 * i + 2]) + bb.z;
+            f[4 * i + 3] = __uint_as_float(v[4 * i + 3]) + bb.w;
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]) + __ldg(p.bias + hb * 32 + i);
         }
         if (p.relu) {
 #pragma unroll
@@ -216,22 +223,22 @@ static int rc_enc2d(CUtensorMap* map, const void* base, long long ld, long long 
   return tmap_rows_bf16(map, base, ld, rows, cols, box_rows);
 }
 
-template <int KS, int STRIDE, int PAD, int N>
+template <int KS, int STRIDE, int PAD, int N, bool BIAS4>
 static int launch_rgb(const CUtensorMap& tw, const CUtensorMap& to, const RgbConvParams& p, cudaStream_t st, const char* desc) {
   using Cfg = RgbCfg<KS, N>;
   static PerDeviceOnce once;
   PGT_CUDA_OK(once.run([] {
-    cudaError_t e = cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD, N, BIAS4>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     if (e != cudaSuccess) return e;
     // the resident-CTA count is fixed by the kernel's own budget (__launch_bounds__, shared memory), not
     // asked of the occupancy calculator: it answered 1 for the 3x3 kernel and left half of every SM idle
-    return cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD, N>, cudaFuncAttributePreferredSharedMemoryCarveout,
+    return cudaFuncSetAttribute(rgb_conv_kernel<KS, STRIDE, PAD, N, BIAS4>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                 cudaSharedmemCarveoutMaxShared);
   }));
   const int grid = p.m_tiles < num_sms() * Cfg::PER_SM ? p.m_tiles : num_sms() * Cfg::PER_SM;
   {
     ProfScope ps(PGT_PROF_GEMM, 2.0 * (double)p.M * N * Cfg::K, st, desc);
-    rgb_conv_kernel<KS, STRIDE, PAD, N><<<grid, Cfg::THREADS, Cfg::SMEM, st>>>(tw, to, p);
+    rgb_conv_kernel<KS, STRIDE, PAD, N, BIAS4><<<grid, Cfg::THREADS, Cfg::SMEM, st>>>(tw, to, p);
   }
   PGT_LAUNCH_OK();
   return PGT_OK;
@@ -269,7 +276,12 @@ extern "C" int pgt_conv_rgb_bf16(const float* x_nchw, int F, int H, int W, int k
   if (rc == PGT_OK) rc = rc_enc2d(&to, out, ldo, p.M, Cout, 128);
   if (rc != PGT_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (Cout == 128) return launch_rgb<3, 1, 1, 128>(tw, to, p, st, "rgb_conv 3x3/1 N128");
-  return ksize == 3 ? launch_rgb<3, 1, 1, 64>(tw, to, p, st, "rgb_conv 3x3/1 N64")
-                    : launch_rgb<7, 2, 3, 64>(tw, to, p, st, "rgb_conv 7x7/2 N64");
+  if (al(bias)) {
+    if (Cout == 128) return launch_rgb<3, 1, 1, 128, true>(tw, to, p, st, "rgb_conv 3x3/1 N128");
+    return ksize == 3 ? launch_rgb<3, 1, 1, 64, true>(tw, to, p, st, "rgb_conv 3x3/1 N64")
+                      : launch_rgb<7, 2, 3, 64, true>(tw, to, p, st, "rgb_conv 7x7/2 N64");
+  }
+  if (Cout == 128) return launch_rgb<3, 1, 1, 128, false>(tw, to, p, st, "rgb_conv 3x3/1 N128");
+  return ksize == 3 ? launch_rgb<3, 1, 1, 64, false>(tw, to, p, st, "rgb_conv 3x3/1 N64")
+                    : launch_rgb<7, 2, 3, 64, false>(tw, to, p, st, "rgb_conv 7x7/2 N64");
 }
