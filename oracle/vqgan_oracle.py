@@ -22,9 +22,9 @@ def res_block(sd, p, x):
     return h + x
 
 
-def block(sd, prefix, i, kind, x):
-    """One entry of Encoder.blocks / Generator.blocks (`archs/vqgan_arch.py:252-341`)."""
-    p = '%s.blocks.%d' % (prefix, i)
+def block(sd, b, x):
+    """One entry of Encoder.blocks / Generator.blocks (`archs/vqgan_arch.py:252-341`), a spec.Block."""
+    p, kind = b.prefix, b.kind
     if kind in ('conv_in', 'conv_out'):
         return conv(sd, p, x, padding=1)
     if kind == 'res':
@@ -38,22 +38,23 @@ def block(sd, prefix, i, kind, x):
     return group_norm(sd, p, x)                           # normalize(); last_silu=False adds no SiLU (:279-282)
 
 
-def encoder(sd, arch, x, taps=()):
-    """Encoder.forward (`:285-289`); returns (z NCHW, {flat index: output of that block})."""
+def encoder(sd, arch, x, taps=None):
+    """Encoder.forward (`:285-289`); returns (z NCHW, {taps[i]: output of block i})."""
     feats = {}
-    for i, (kind, *_r) in enumerate(arch.enc_blocks):
-        x = block(sd, 'encoder', i, kind, x)
-        if i in taps:
-            feats[i] = x.clone()
+    for i, b in enumerate(arch.enc_blocks):
+        x = block(sd, b, x)
+        if taps and i in taps:
+            feats[taps[i]] = x.clone()
     return x, feats
 
 
 def generator(sd, arch, x, fuse=None):
-    """Generator.forward (`:337-341`); fuse(i, x) -> x after block i (CodeFormer's SFT fusion)."""
-    for i, (kind, *_r) in enumerate(arch.gen_blocks):
-        x = block(sd, 'generator', i, kind, x)
-        if fuse is not None:
-            x = fuse(i, x)
+    """Generator.forward (`:337-341`); fuse(b, x) -> x at each `fuse` block b (CodeFormer's SFT fusion)."""
+    for b in arch.dec_blocks:
+        if b.kind != 'fuse':
+            x = block(sd, b, x)
+        elif fuse is not None:
+            x = fuse(b, x)
     return x
 
 
@@ -99,7 +100,7 @@ def codeformer_forward(sd, arch, x, w=0.0, adain_on=False, code_only=False, forc
     """CodeFormer.forward (`archs/codeformer_arch.py:303-366`): (out, logits [b, hw, K], lq_feat NCHW), or
     (logits, lq_feat) with code_only.  Codes are topk(softmax(logits), 1) as in the reference; force_codes [b, hw]
     replaces them."""
-    lq, feats = encoder(sd, arch, x, taps=tuple(arch.fuse_enc))
+    lq, feats = encoder(sd, arch, x, taps=arch.enc_taps)
     b = lq.shape[0]
     pos = sd['position_emb'].unsqueeze(1).repeat(1, b, 1)
     q = F.linear(lq.flatten(2).permute(2, 0, 1), sd['feat_emb.weight'], sd['feat_emb.bias'])
@@ -118,10 +119,6 @@ def codeformer_forward(sd, arch, x, w=0.0, adain_on=False, code_only=False, forc
     if adain_on:
         quant = adain(quant, lq)
 
-    def fuse(i, h):
-        if w > 0 and i in arch.fuse_gen:
-            key = arch.fuse_gen[i]
-            ei = [k for k, v in arch.fuse_enc.items() if v == key][0]
-            return fuse_sft(sd, 'fuse_convs_dict.' + key, feats[ei], h, w)
-        return h
+    def fuse(b, h):
+        return fuse_sft(sd, b.prefix, feats[b.src], h, w) if w > 0 else h
     return generator(sd, arch, quant, fuse), logits, lq

@@ -442,12 +442,10 @@ class Engine:
         return ops.assemble_cond(o0, o1, o2, self._new(Fr, H // 16, W // 16, 64))
 
     # ------------------------------------------------------------------ encoder / decoder
-    res_shortcut = 'nin_shortcut'      # the 1x1 conv of a width-changing `res` block (VQGAN's ResBlock: conv_out)
-
     def _walk(self, blocks, h, lo=0, hi=None, taps=None, outs=None, feats=None, wgt=0.0):
-        """Runs blocks[lo:hi] of a block list (spec: `_autoencoder_blocks`, VQGANEngine._blocks) on h.  Returns (h,
-        {taps[i]: output of block i}).  outs {i: tensor}: block i (`res` or `swin`) writes its output there, a slice
-        of an SFT concat buffer.  A `fuse` block runs only with feats and wgt > 0, on feats[its source].
+        """Runs blocks[lo:hi] of a block list (spec.Block entries) on h.  Returns (h, {taps[i]: output of block i}).
+        outs {i: tensor}: block i (`res` or `swin`) writes its output there, a slice of an SFT concat buffer.  A `fuse`
+        block runs only with feats and wgt > 0, on feats[its src].
 
         GroupNorm statistics: a block passes gn_next to its producer exactly when the next block that runs reads its
         input through a GroupNorm (`res`, `attn`, or the `norm` before conv_out); a `fuse` that does not run is not
@@ -457,24 +455,25 @@ class Engine:
         hi = len(blocks) if hi is None else hi
         outs, found = outs or {}, {}
         for i in range(lo, hi):
-            kind, p, cout = blocks[i][:3]
+            blk = blocks[i]
+            kind, p, cout = blk.kind, blk.prefix, blk.cout
             if kind == 'fuse' and not fusing:
                 continue
-            nxt = next((b[0] in ('res', 'attn', 'norm') for b in blocks[i + 1:] if fusing or b[0] != 'fuse'), False)
+            nxt = next((b.kind in ('res', 'attn', 'norm') for b in blocks[i + 1:] if fusing or b.kind != 'fuse'), False)
             if kind == 'conv_in':
                 h = self.conv_in(h, p) if p + '.weight' == self.arch.stem else self._conv3(h, p, cout, gn_out=nxt)
             elif kind == 'res':
-                h = self.td_resblock(h, p, cout, gn_next=nxt, out=outs.get(i), shortcut=self.res_shortcut)
+                h = self.td_resblock(h, p, cout, gn_next=nxt, out=outs.get(i), shortcut=self.arch.res_shortcut)
             elif kind == 'attn':
                 h = self.attn_block(h, p, gn_next=nxt)
             elif kind == 'swin':
-                h = self.encoder_layer(h, p, blocks[i][3], blocks[i][4], gn_next=nxt, out=outs.get(i))
+                h = self.encoder_layer(h, p, blk.heads, blk.depth, gn_next=nxt, out=outs.get(i))
             elif kind == 'down':
                 h = self._conv3(h, p + '.conv', cout, stride=2, pad_lo=0, gn_out=nxt)
             elif kind == 'up':
                 h = self.up2x(h, p + '.conv')
             elif kind == 'fuse':
-                h = self.fuse_sft(feats[blocks[i][3]], h, p[len('fuse_convs_dict.'):], wgt, gn_next=nxt)
+                h = self.fuse_sft(feats[blk.src], h, p[len('fuse_convs_dict.'):], wgt, gn_next=nxt)
             else:
                 raise AssertionError(kind)
             if taps and i in taps:
@@ -511,8 +510,8 @@ class Engine:
         far.  Returns (h [F,h,w,z], the output of every level)."""
         a = self.arch
         h, more = self._walk(a.enc_blocks, h, i, len(a.enc_blocks) - 2, a.enc_taps, outs)
-        (_, norm, _), (_, conv, zc) = a.enc_blocks[-2:]
-        return self._conv3(h, conv, zc, gn=norm), list(feats.values()) + list(more.values())
+        norm, conv = a.enc_blocks[-2:]
+        return self._conv3(h, conv.prefix, conv.cout, gn=norm.prefix), list(feats.values()) + list(more.values())
 
     def encoder(self, x, fusing=False):
         """Encoder.forward (`archs/tdcrqvae3_arch.py:540-573`); x fp32 NCHW -> (h [F,h,w,z], feats).  fusing: the SFT
@@ -539,16 +538,18 @@ class Engine:
 
     def decoder(self, z, feats=None, wgt=0.0):
         """Decoder.forward (`archs/tdcrqvae3_arch.py:672-707`) / the inlined variant with SFT fusion
-        (`archs/pgtformer_arch.py:680-710`).  z: [F,h,w,z_channels] bf16 -> out fp32 NCHW.  A level whose encoder
-        output sits in an SFT concat buffer writes its own output into the decoder half."""
+        (`archs/pgtformer_arch.py:680-710`), or VQGAN's Generator.forward (`archs/vqgan_arch.py:337-341`) / with
+        CodeFormer's fusion (`archs/codeformer_arch.py:356-363`).  z: [F,h,w,C] bf16 -> out fp32 NCHW.  A level whose
+        encoder output sits in an SFT concat buffer writes its own output into the decoder half."""
         blocks = self.arch.dec_blocks
         outs = {}
         for i, b in enumerate(blocks):
-            cat = getattr(feats[b[3]], '_pgt_cat', None) if b[0] == 'fuse' and feats is not None and wgt > 0 else None
+            cat = getattr(feats[b.src], '_pgt_cat', None) if b.kind == 'fuse' and feats is not None and wgt > 0 else None
             if cat is not None:
-                outs[i - 1] = self._cat_half(cat, b[2], b[2])
+                outs[i - 1] = self._cat_half(cat, b.cout, b.cout)
         h, _ = self._walk(blocks, z, 0, len(blocks) - 2, outs=outs, feats=feats, wgt=wgt)
-        return self.decoder_out(h)
+        norm, conv = blocks[-2:]
+        return self.decoder_out(h, norm.prefix, conv.prefix, conv.cout, self.arch.dec_tail_silu)
 
     def up2x(self, h, p):
         """Upsample (nearest x2 + conv3x3) as four 2x2 phase convs; the epilogue emits the next norm1's statistics."""
@@ -557,9 +558,8 @@ class Engine:
         stats = self._gn_stats(out, 16 * self._stats_tiles(H, W, C, 2, 1, 1))     # [frame][phase][tile][quadrant]
         return ops.conv_up2x(h, self.w[p + '.weight'], C, out, bias=self.w[p + '.bias'], gn_stats=stats)
 
-    def decoder_out(self, h, norm='decoder.norm_out', conv='decoder.conv_out', silu=True, out_ch=None):
+    def decoder_out(self, h, norm, conv, out_ch, silu):
         """norm (GroupNorm) + SiLU (unless silu=False) + conv -> fp32 NCHW [F, out_ch, H, W]."""
-        out_ch = self.arch.out_ch if out_ch is None else out_ch
         Fr, H, W, _ = h.shape
         out = self._new(Fr, out_ch, H, W, dtype=torch.float32)
         # norm + SiLU + conv in one kernel: the normalised 512^2 tensor never reaches HBM

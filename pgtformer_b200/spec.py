@@ -10,8 +10,12 @@ attention / Swin block / EncoderLayer / TDResnetBlock ctors), `archs/codeformer_
 `kind` drives the deterministic synthetic initialisation in weights.py.  The arch classes name what the
 kernel-layout repack (Engine._repack) cannot tell from a tensor's name and shape: the RGB stem, the upsample convs,
 the codebook key of each depth and the prefixes packed by a rule of their own.
+
+Each arch describes its encoder and decoder once, as the block lists `enc_blocks` / `dec_blocks` in execution order:
+Engine._walk runs them, `_block_list` writes their state-dict entries, and the stem and upsample convs are read off
+them.
 """
-from collections import OrderedDict
+from collections import OrderedDict, namedtuple
 
 WINDOW = (3, 4, 4)            # frames x Wh x Ww  (num_frames=3, window_sizes=[4,4])
 N_WIN_TOK = 48
@@ -60,13 +64,14 @@ def _bn(s, p, c):
     s.add(p + '.num_batches_tracked', (), 'bn_count', 'int64')
 
 
-def _td_resblock(s, p, cin, cout):
+def _res_block(s, p, cin, cout, shortcut):
+    """TDResnetBlock / ResnetBlock (1x1 shortcut `nin_shortcut`) or VQGAN's ResBlock (`conv_out`)."""
     _norm(s, p + '.norm1', cin)
     _conv(s, p + '.conv1', cin, cout, 3)
     _norm(s, p + '.norm2', cout)
     _conv(s, p + '.conv2', cout, cout, 3)
     if cin != cout:
-        _conv(s, p + '.nin_shortcut', cin, cout, 1)
+        _conv(s, '%s.%s' % (p, shortcut), cin, cout, 1)
 
 
 def _swin_block(s, p, c, heads):
@@ -124,7 +129,45 @@ def _bisenet(s, p, n_classes=19):
         _conv(s, '%s.%s.conv_out' % (p, name), mid, n_classes, 1, bias=False)
 
 
-class Arch:
+# One entry of a block list: kind is conv_in, res, attn (AttnBlock), swin (EncoderLayer: `heads` and `depth`), down, up,
+# norm, conv_out or fuse (an SFT fusion block: `src` is the key of the encoder output it reads, see Engine._walk)
+Block = namedtuple('Block', 'kind prefix cin cout heads depth src', defaults=(None, None, None))
+
+
+class _Autoencoder:
+    """What an arch's block lists decide besides the blocks themselves."""
+    res_shortcut = 'nin_shortcut'       # the 1x1 conv of a width-changing `res` block
+    dec_tail_silu = True                # the decoder's last GroupNorm is followed by SiLU
+
+    @property
+    def stem(self):
+        """The encoder's RGB conv_in."""
+        return self.enc_blocks[0].prefix + '.weight'
+
+    @property
+    def upsample_convs(self):
+        """The Upsample convs (nearest x2 + conv3x3, packed as 2x2 phase convs)."""
+        return tuple(b.prefix + '.conv.weight' for b in self.enc_blocks + self.dec_blocks if b.kind == 'up')
+
+
+def _block_list(s, a, blocks):
+    """The state-dict entries of a block list's blocks; a `fuse` block's are its model's to write."""
+    for b in blocks:
+        if b.kind in ('conv_in', 'conv_out'):
+            _conv(s, b.prefix, b.cin, b.cout, 3)
+        elif b.kind == 'res':
+            _res_block(s, b.prefix, b.cin, b.cout, a.res_shortcut)
+        elif b.kind == 'attn':
+            _attn_block(s, b.prefix, b.cin)
+        elif b.kind == 'swin':
+            _encoder_layer(s, b.prefix, b.cin, b.depth, b.heads)
+        elif b.kind in ('down', 'up'):
+            _conv(s, b.prefix + '.conv', b.cin, b.cout, 3)
+        elif b.kind == 'norm':
+            _norm(s, b.prefix, b.cin)
+
+
+class Arch(_Autoencoder):
     """Resolved architecture constants (everything the engine / oracle need besides weights)."""
 
     def __init__(self, network_g):
@@ -173,8 +216,6 @@ class Arch:
         self.fuse_level_key = {i: str(self.resolution >> i) for i in range(self.num_levels)
                                if str(self.resolution >> i) in self.connect_list}
         self.fuse_channels = {'16': 512, '32': 512, '64': 256, '128': 256, '256': 128, '512': 64}
-        self.stem = 'encoder.conv_in.weight'
-        self.upsample_convs = _upsample_convs(self.num_levels)
         self.codebooks = _codebooks(self.depth)
         self.packed_apart = ('conditionnet.',)                      # BiSeNet: BatchNorms folded into its convs
         self.enc_blocks, self.dec_blocks, self.frame_blocks, self.enc_taps = _autoencoder_blocks(self, 'swin')
@@ -182,53 +223,50 @@ class Arch:
 
 def _autoencoder_blocks(a, attn):
     """Encoder and decoder of TDCRQVAE3 (`archs/tdcrqvae3_arch.py:540-573, 672-707`, attn='swin') or of the 2-D RQ-VAE
-    (`archs/tdrqvae_arch.py:650-680, 753-784`, attn='attn') as block lists in execution order, for Engine._walk.
-    Entries are (kind, state-dict prefix, output channels, ...): `swin` (EncoderLayer) adds its heads and depth, `fuse`
-    (PGTFormer's Fuse_sft_block after a decoder level, `archs/pgtformer_arch.py:680-710`, keyed by `fuse_level_key`) the
-    level whose encoder output it reads.  Returns (encoder blocks, decoder blocks, frame_blocks: the encoder blocks
-    before the first level with attention, which look at one frame at a time, taps: {encoder block index: level} of
-    each level's output)."""
+    (`archs/tdrqvae_arch.py:587-784`, attn='attn') as block lists in execution order.  A `fuse` block is PGTFormer's
+    Fuse_sft_block after a decoder level (`archs/pgtformer_arch.py:680-710`, keyed by `fuse_level_key`); its `src` is
+    that level.  Returns (encoder blocks, decoder blocks, frame_blocks: the encoder blocks before the first level with
+    attention, which look at one frame at a time, taps: {encoder block index: level} of each level's output)."""
     fuse = getattr(a, 'fuse_level_key', {})
 
-    def attention(p, lvl):
+    def attention(p, lvl, c):
         if attn == 'swin':
-            return ('swin', p, a.level_ch[lvl], a.num_heads[lvl], a.depths[lvl])
-        return ('attn', p, a.level_ch[lvl])
+            return Block('swin', p, c, c, heads=a.num_heads[lvl], depth=a.depths[lvl])
+        return Block('attn', p, c, c)
 
     last = a.num_levels - 1
-    enc, taps, frame_blocks = [('conv_in', 'encoder.conv_in', a.ch)], {}, None
+    enc, taps, frame_blocks = [Block('conv_in', 'encoder.conv_in', a.in_channels, a.ch)], {}, None
     for lvl in range(a.num_levels):
         if frame_blocks is None and (a.level_has_attn[lvl] or lvl == last):
             frame_blocks = len(enc)
+        c = a.level_ch[lvl - 1] if lvl else a.ch                 # the reference's ch * in_ch_mult[i_level]
         for b in range(a.num_res_blocks):
-            enc.append(('res', 'encoder.down.%d.block.%d' % (lvl, b), a.level_ch[lvl]))
+            enc.append(Block('res', 'encoder.down.%d.block.%d' % (lvl, b), c, a.level_ch[lvl]))
+            c = a.level_ch[lvl]
             if a.level_has_attn[lvl]:
-                enc.append(attention('encoder.down.%d.attn.%d' % (lvl, b), lvl))
+                enc.append(attention('encoder.down.%d.attn.%d' % (lvl, b), lvl, c))
         taps[len(enc) - 1] = lvl
         if lvl != last:
-            enc.append(('down', 'encoder.down.%d.downsample' % lvl, a.level_ch[lvl]))
+            enc.append(Block('down', 'encoder.down.%d.downsample' % lvl, c, c))
     zc = 2 * a.z_channels if a.double_z else a.z_channels
-    enc += [('res', 'encoder.mid.block_1', a.level_ch[-1]), attention('encoder.mid.attn_1', last),
-            ('res', 'encoder.mid.block_2', a.level_ch[-1]), ('norm', 'encoder.norm_out', a.level_ch[-1]),
-            ('conv_out', 'encoder.conv_out', zc)]
-    dec = [('conv_in', 'decoder.conv_in', a.level_ch[-1]), ('res', 'decoder.mid.block_1', a.level_ch[-1]),
-           attention('decoder.mid.attn_1', last), ('res', 'decoder.mid.block_2', a.level_ch[-1])]
+    enc += [Block('res', 'encoder.mid.block_1', c, c), attention('encoder.mid.attn_1', last, c),
+            Block('res', 'encoder.mid.block_2', c, c), Block('norm', 'encoder.norm_out', c, c),
+            Block('conv_out', 'encoder.conv_out', c, zc)]
+    c = a.level_ch[-1]
+    dec = [Block('conv_in', 'decoder.conv_in', a.z_channels, c), Block('res', 'decoder.mid.block_1', c, c),
+           attention('decoder.mid.attn_1', last, c), Block('res', 'decoder.mid.block_2', c, c)]
     for lvl in reversed(range(a.num_levels)):
         for b in range(a.num_res_blocks + 1):
-            dec.append(('res', 'decoder.up.%d.block.%d' % (lvl, b), a.level_ch[lvl]))
+            dec.append(Block('res', 'decoder.up.%d.block.%d' % (lvl, b), c, a.level_ch[lvl]))
+            c = a.level_ch[lvl]
             if a.level_has_attn[lvl]:
-                dec.append(attention('decoder.up.%d.attn.%d' % (lvl, b), lvl))
+                dec.append(attention('decoder.up.%d.attn.%d' % (lvl, b), lvl, c))
         if lvl in fuse:
-            dec.append(('fuse', 'fuse_convs_dict.' + fuse[lvl], a.level_ch[lvl], lvl))
+            dec.append(Block('fuse', 'fuse_convs_dict.' + fuse[lvl], c, c, src=lvl))
         if lvl != 0:
-            dec.append(('up', 'decoder.up.%d.upsample' % lvl, a.level_ch[lvl]))
-    dec += [('norm', 'decoder.norm_out', a.level_ch[0]), ('conv_out', 'decoder.conv_out', a.out_ch)]
+            dec.append(Block('up', 'decoder.up.%d.upsample' % lvl, c, c))
+    dec += [Block('norm', 'decoder.norm_out', c, c), Block('conv_out', 'decoder.conv_out', c, a.out_ch)]
     return tuple(enc), tuple(dec), frame_blocks, taps
-
-
-def _upsample_convs(num_levels):
-    """The decoder's Upsample convs (nearest x2 + conv3x3, packed as 2x2 phase convs)."""
-    return tuple('decoder.up.%d.upsample.conv.weight' % lvl for lvl in range(1, num_levels))
 
 
 def _codebooks(depth):
@@ -239,42 +277,7 @@ def _codebooks(depth):
 def build_spec(network_g):
     a = Arch(network_g)
     s = Spec()
-    in_mult = (1,) + a.ch_mult
-    # ---- encoder (tdcrqvae3_arch.py:460-539)
-    _conv(s, 'encoder.conv_in', a.in_channels, a.ch, 3)
-    block_in = a.ch
-    for lvl in range(a.num_levels):
-        block_in = a.ch * in_mult[lvl]
-        block_out = a.ch * a.ch_mult[lvl]
-        for b in range(a.num_res_blocks):
-            _td_resblock(s, 'encoder.down.%d.block.%d' % (lvl, b), block_in, block_out)
-            block_in = block_out
-            if a.level_has_attn[lvl]:
-                _encoder_layer(s, 'encoder.down.%d.attn.%d' % (lvl, b), block_in, a.depths[lvl], a.num_heads[lvl])
-        if lvl != a.num_levels - 1:
-            _conv(s, 'encoder.down.%d.downsample.conv' % lvl, block_in, block_in, 3)
-    _td_resblock(s, 'encoder.mid.block_1', block_in, block_in)
-    _encoder_layer(s, 'encoder.mid.attn_1', block_in, a.depths[-1], a.num_heads[-1])
-    _td_resblock(s, 'encoder.mid.block_2', block_in, block_in)
-    _norm(s, 'encoder.norm_out', block_in)
-    _conv(s, 'encoder.conv_out', block_in, 2 * a.z_channels if a.double_z else a.z_channels, 3)
-    # ---- decoder (tdcrqvae3_arch.py:577-670)
-    block_in = a.ch * a.ch_mult[-1]
-    _conv(s, 'decoder.conv_in', a.z_channels, block_in, 3)
-    _td_resblock(s, 'decoder.mid.block_1', block_in, block_in)
-    _encoder_layer(s, 'decoder.mid.attn_1', block_in, a.depths[-1], a.num_heads[-1])
-    _td_resblock(s, 'decoder.mid.block_2', block_in, block_in)
-    for lvl in reversed(range(a.num_levels)):
-        block_out = a.ch * a.ch_mult[lvl]
-        for b in range(a.num_res_blocks + 1):
-            _td_resblock(s, 'decoder.up.%d.block.%d' % (lvl, b), block_in, block_out)
-            block_in = block_out
-            if a.level_has_attn[lvl]:
-                _encoder_layer(s, 'decoder.up.%d.attn.%d' % (lvl, b), block_in, a.depths[lvl], a.num_heads[lvl])
-        if lvl != 0:
-            _conv(s, 'decoder.up.%d.upsample.conv' % lvl, block_in, block_in, 3)
-    _norm(s, 'decoder.norm_out', block_in)
-    _conv(s, 'decoder.conv_out', block_in, a.out_ch, 3)
+    _block_list(s, a, a.enc_blocks + a.dec_blocks)          # tdcrqvae3_arch.py:460-539, 577-670
     # ---- quantiser (tdcrqvae3_arch.py:80-97,215-271): one VQEmbedding per depth, or one shared by every depth
     e = a.embed_dim
     for d in range(a.depth):
@@ -350,7 +353,7 @@ def _swin3d_layer(s, p, c, depth, heads, window, mlp_ratio=4):
         _linear(s, b + '.mlp.fc2', mlp_ratio * c, c)
 
 
-class TDRQVAEArch:
+class TDRQVAEArch(_Autoencoder):
     """Resolved constants of TDRQVAE: the 2-D RQ-VAE Encoder / Decoder (`archs/tdrqvae_arch.py:587-784`) around a
     depth-1 RQBottleneck and two Video-Swin BasicLayers.  Raises ValueError for what the reference rejects and for
     what the CUDA kernels cannot run."""
@@ -407,8 +410,6 @@ class TDRQVAEArch:
         if len(self.window_size) != 3 or min(self.window_size) < 1 or \
                 self.window_size[0] * self.window_size[1] * self.window_size[2] > SWIN_MAX_TOKENS:
             raise ValueError('Video-Swin window %s: at most %d tokens' % (self.window_size, SWIN_MAX_TOKENS))
-        self.stem = 'encoder.conv_in.weight'
-        self.upsample_convs = _upsample_convs(self.num_levels)
         self.codebooks = _codebooks(1)
         self.packed_apart = ('tdswin_pre.', 'tdswin_post.')         # Video-Swin BasicLayers: swin3d.pack_blocks
         self.enc_blocks, self.dec_blocks, self.frame_blocks, _ = _autoencoder_blocks(self, 'attn')
@@ -418,7 +419,7 @@ class TDRQVAEArch:
 def build_tdrqvae_spec(network_g):
     a = TDRQVAEArch(network_g)
     s = Spec()
-    _rqvae_autoencoder(s, a)
+    _block_list(s, a, a.enc_blocks + a.dec_blocks)          # tdrqvae_arch.py:587-751
     # ---- quantiser (:206-223, 381-394): one shared codebook of depth 1
     e = a.embed_dim
     s.add('quantizer.codebooks.0.weight', (a.n_embed + 1, e), 'codebook')
@@ -431,49 +432,7 @@ def build_tdrqvae_spec(network_g):
     return a, s
 
 
-def _rqvae_autoencoder(s, a):
-    """The 2-D RQ-VAE Encoder and Decoder TDRQVAE and RQVAE share (`archs/tdrqvae_arch.py:587-751`,
-    `archs/rqvae_arch.py:579-743`)."""
-    in_mult = (1,) + a.ch_mult
-    # ---- Encoder (tdrqvae_arch.py:587-648)
-    _conv(s, 'encoder.conv_in', a.in_channels, a.ch, 3)
-    for lvl in range(a.num_levels):
-        block_in = a.ch * in_mult[lvl]
-        block_out = a.level_ch[lvl]
-        for b in range(a.num_res_blocks):
-            _td_resblock(s, 'encoder.down.%d.block.%d' % (lvl, b), block_in, block_out)
-            block_in = block_out
-        if a.level_has_attn[lvl]:
-            for b in range(a.num_res_blocks):
-                _attn_block(s, 'encoder.down.%d.attn.%d' % (lvl, b), block_in)
-        if lvl != a.num_levels - 1:
-            _conv(s, 'encoder.down.%d.downsample.conv' % lvl, block_in, block_in, 3)
-    _td_resblock(s, 'encoder.mid.block_1', block_in, block_in)
-    _attn_block(s, 'encoder.mid.attn_1', block_in)
-    _td_resblock(s, 'encoder.mid.block_2', block_in, block_in)
-    _norm(s, 'encoder.norm_out', block_in)
-    _conv(s, 'encoder.conv_out', block_in, a.z_channels, 3)
-    # ---- Decoder (:683-751)
-    block_in = a.level_ch[-1]
-    _conv(s, 'decoder.conv_in', a.z_channels, block_in, 3)
-    _td_resblock(s, 'decoder.mid.block_1', block_in, block_in)
-    _attn_block(s, 'decoder.mid.attn_1', block_in)
-    _td_resblock(s, 'decoder.mid.block_2', block_in, block_in)
-    for lvl in reversed(range(a.num_levels)):
-        block_out = a.level_ch[lvl]
-        for b in range(a.num_res_blocks + 1):
-            _td_resblock(s, 'decoder.up.%d.block.%d' % (lvl, b), block_in, block_out)
-            block_in = block_out
-        if a.level_has_attn[lvl]:
-            for b in range(a.num_res_blocks + 1):
-                _attn_block(s, 'decoder.up.%d.attn.%d' % (lvl, b), block_in)
-        if lvl != 0:
-            _conv(s, 'decoder.up.%d.upsample.conv' % lvl, block_in, block_in, 3)
-    _norm(s, 'decoder.norm_out', block_in)
-    _conv(s, 'decoder.conv_out', block_in, a.out_ch, 3)
-
-
-class RQVAEArch:
+class RQVAEArch(_Autoencoder):
     """Resolved constants of the registered RQVAE (`archs/rqvae_arch.py:779-931`): the 2-D Encoder / Decoder around an
     RQBottleneck of depth D = code_shape[2], one codebook per depth (`n_embed` an int or a list of D sizes) or one shared
     by every depth.  Raises ValueError for what the reference rejects, for what it accepts but fails on at forward, and
@@ -541,8 +500,6 @@ class RQVAEArch:
         if self.embed_dim % 128 or self.embed_dim > 512 or any(k % 128 or k < 128 for k in self.n_embeds):
             raise ValueError('embed_dim %d, n_embed %s: the argmin takes codebooks of a multiple of 128 up to 512 '
                              'channels and a multiple of 128 codes' % (self.embed_dim, list(self.n_embeds)))
-        self.stem = 'encoder.conv_in.weight'
-        self.upsample_convs = _upsample_convs(self.num_levels)
         self.codebooks = _codebooks(self.depth)
         self.packed_apart = ()
         self.enc_blocks, self.dec_blocks, self.frame_blocks, _ = _autoencoder_blocks(self, 'attn')
@@ -555,7 +512,7 @@ RGB_STEM_WIDTHS = (64, 128)           # pgt_conv_rgb_bf16 3x3 output widths
 def build_rqvae_spec(network_g):
     a = RQVAEArch(network_g)
     s = Spec()
-    _rqvae_autoencoder(s, a)
+    _block_list(s, a, a.enc_blocks + a.dec_blocks)          # rqvae_arch.py:579-743
     # ---- RQBottleneck (rqvae_arch.py:199-216, 374-387): one VQEmbedding per depth, or one shared by every depth
     e = a.latent_shape[2]
     for d in range(a.depth):
@@ -578,22 +535,13 @@ CODEFORMER_ENC_BLOCK = {'512': 2, '256': 5, '128': 8, '64': 11, '32': 14, '16': 
 CODEFORMER_GEN_BLOCK = {'16': 6, '32': 9, '64': 12, '128': 15, '256': 18, '512': 21}        # :280
 
 
-def _res_block(s, p, cin, cout):
-    """ResBlock (`archs/vqgan_arch.py:155-178`): the 1x1 shortcut is `conv_out`."""
-    _norm(s, p + '.norm1', cin)
-    _conv(s, p + '.conv1', cin, cout, 3)
-    _norm(s, p + '.norm2', cout)
-    _conv(s, p + '.conv2', cout, cout, 3)
-    if cin != cout:
-        _conv(s, p + '.conv_out', cin, cout, 1)
-
-
-class VQGANArch:
+class VQGANArch(_Autoencoder):
     """Resolved constants of VQAutoEncoder (`archs/vqgan_arch.py:344-411`) and, with codeformer=True, CodeFormer
-    (`archs/codeformer_arch.py:229-286`).  `enc_blocks` / `gen_blocks` are the flat `encoder.blocks` / `generator.blocks`
-    ModuleLists as (kind, cin, cout, res) tuples, kind in conv_in, res, attn, down, up, norm, conv_out; `res` is the
-    constructor's curr_res (img_size-relative), which places the AttnBlocks.  Raises ValueError for what the reference
-    rejects and for what the CUDA kernels cannot run."""
+    (`archs/codeformer_arch.py:229-286`).  `enc_blocks` / `dec_blocks` are the flat `encoder.blocks` /
+    `generator.blocks` ModuleLists, CodeFormer's `fuse` blocks placed after the generator blocks they follow.  Raises
+    ValueError for what the reference rejects and for what the CUDA kernels cannot run."""
+    res_shortcut = 'conv_out'
+    dec_tail_silu = False
 
     def __init__(self, g, codeformer=False):
         g = dict(g)
@@ -625,50 +573,52 @@ class VQGANArch:
         if self.embed_dim % 32 or self.embed_dim > 512 or self.n_embed % 256:
             raise ValueError('emb_dim %d, codebook_size %d: the quantiser kernels take emb_dim a multiple of 32 up to 512 '
                              'and codebook_size a multiple of 256' % (self.embed_dim, self.n_embed))
-        enc, res = [('conv_in', 3, self.nf, self.img_size)], self.img_size
-        cin = self.nf
+        enc, gen, at = [], [], {}                                      # at: block prefix -> the constructor's curr_res
+
+        def add(blocks, name, kind, cin, cout):
+            blocks.append(Block(kind, '%s.blocks.%d' % (name, len(blocks)), cin, cout))
+            at[blocks[-1].prefix] = res
+
+        res, cin = self.img_size, self.nf
+        add(enc, 'encoder', 'conv_in', 3, cin)
         for i in range(self.num_levels):                               # Encoder.__init__ (vqgan_arch.py:252-282)
             cout = self.level_ch[i]
             for _ in range(self.res_blocks):
-                enc.append(('res', cin, cout, res))
+                add(enc, 'encoder', 'res', cin, cout)
                 cin = cout
                 if res in self.attn_resolutions:
-                    enc.append(('attn', cin, cin, res))
+                    add(enc, 'encoder', 'attn', cin, cin)
             if i != self.num_levels - 1:
-                enc.append(('down', cin, cin, res))
+                add(enc, 'encoder', 'down', cin, cin)
                 res //= 2
-        enc += [('res', cin, cin, res), ('attn', cin, cin, res), ('res', cin, cin, res), ('norm', cin, cin, res)]
+        for kind in ('res', 'attn', 'res', 'norm'):
+            add(enc, 'encoder', kind, cin, cin)
         if self.last_silu:
             raise ValueError('last_silu=True adds an nn.SiLU block the CUDA path does not run')
-        enc.append(('conv_out', cin, self.embed_dim, res))
-        gen, res = [], self.img_size // self.down                      # Generator.__init__ (:303-334)
-        cin = self.level_ch[-1]
-        gen += [('conv_in', self.embed_dim, cin, res), ('res', cin, cin, res), ('attn', cin, cin, res),
-                ('res', cin, cin, res)]
+        add(enc, 'encoder', 'conv_out', cin, self.embed_dim)
+        res, cin = self.img_size // self.down, self.level_ch[-1]       # Generator.__init__ (:303-334)
+        add(gen, 'generator', 'conv_in', self.embed_dim, cin)
+        for kind in ('res', 'attn', 'res'):
+            add(gen, 'generator', kind, cin, cin)
         for i in reversed(range(self.num_levels)):
             cout = self.level_ch[i]
             for _ in range(self.res_blocks):
-                gen.append(('res', cin, cout, res))
+                add(gen, 'generator', 'res', cin, cout)
                 cin = cout
                 if res in self.attn_resolutions:
-                    gen.append(('attn', cin, cin, res))
+                    add(gen, 'generator', 'attn', cin, cin)
             if i != 0:
-                gen.append(('up', cin, cin, res))
+                add(gen, 'generator', 'up', cin, cin)
                 res *= 2
-        gen += [('norm', cin, cin, res), ('conv_out', cin, 3, res)]
-        self.enc_blocks, self.gen_blocks = tuple(enc), tuple(gen)
-        widths = {b[1] for b in enc + gen if b[0] == 'attn'}
+        add(gen, 'generator', 'norm', cin, cin)
+        add(gen, 'generator', 'conv_out', cin, 3)
+        widths = {b.cin for b in enc + gen if b.kind == 'attn'}
         if not widths <= set(ATTN_WIDTHS):
             raise ValueError('AttnBlock widths %s: the attention kernel takes %s' % (sorted(widths), ATTN_WIDTHS))
         self.code_shape = (self.img_size // self.down, self.img_size // self.down, 1)
-        # an Upsample conv is `generator.blocks.N.conv`, a Downsample conv `encoder.blocks.N.conv`: the block list tells
-        # them apart, no name pattern does
-        self.stem = 'encoder.blocks.0.weight'
-        self.upsample_convs = tuple('%s.blocks.%d.conv.weight' % (prefix, i)
-                                    for prefix, blocks in (('encoder', enc), ('generator', gen))
-                                    for i, b in enumerate(blocks) if b[0] == 'up')
         self.codebooks = ('quantize.embedding.weight',)
         self.packed_apart = ()
+        self.enc_blocks, self.dec_blocks, self.enc_taps = tuple(enc), tuple(gen), {}
         if not codeformer:
             return
         self.dim_embd = int(g.get('dim_embd', 512))
@@ -686,7 +636,7 @@ class VQGANArch:
         if self.dim_embd % self.n_head or self.dim_embd // self.n_head != 64:
             raise ValueError('dim_embd %d with %d heads: the transformer kernel takes head width 64'
                              % (self.dim_embd, self.n_head))
-        self.fuse_enc, self.fuse_gen = {}, {}                          # flat block index -> size key
+        fuse_after = {}                                                # generator block index -> size key
         for key in self.connect_list:
             if key not in CODEFORMER_CHANNELS:
                 raise ValueError('connect_list entry %r: CodeFormer has fusion layers for %s'
@@ -695,25 +645,16 @@ class VQGANArch:
             c = CODEFORMER_CHANNELS[key]
             # the reference keys a tapped feature by its width (`codeformer_arch.py:316, 361`): the block at the table's
             # index must give the key's resolution and CodeFormer's channel count for it
-            if ei >= len(enc) or gi >= len(gen) or enc[ei][0] != 'res' or gen[gi][0] != 'res' or \
-                    enc[ei][2] != c or gen[gi][2] != c or enc[ei][3] != int(key) or gen[gi][3] != int(key):
+            if ei >= len(enc) or gi >= len(gen) or any(b.kind != 'res' or b.cout != c or at[b.prefix] != int(key)
+                                                       for b in (enc[ei], gen[gi])):
                 raise ValueError('connect_list entry %r does not fit this encoder / generator' % key)
-            self.fuse_enc[ei], self.fuse_gen[gi] = key, key
-
-
-def _vqgan_blocks(s, prefix, blocks):
-    for i, (kind, cin, cout, _) in enumerate(blocks):
-        p = '%s.blocks.%d' % (prefix, i)
-        if kind in ('conv_in', 'conv_out'):
-            _conv(s, p, cin, cout, 3)
-        elif kind == 'res':
-            _res_block(s, p, cin, cout)
-        elif kind == 'attn':
-            _attn_block(s, p, cin)
-        elif kind in ('down', 'up'):
-            _conv(s, p + '.conv', cin, cin, 3)
-        else:
-            _norm(s, p, cin)
+            self.enc_taps[ei], fuse_after[gi] = key, key
+        dec = []
+        for i, b in enumerate(gen):                                    # Fuse_sft_block after its generator block
+            dec.append(b)
+            if i in fuse_after:
+                dec.append(Block('fuse', 'fuse_convs_dict.' + fuse_after[i], b.cout, b.cout, src=fuse_after[i]))
+        self.dec_blocks = tuple(dec)
 
 
 def build_vqgan_spec(g, codeformer=False):
@@ -723,9 +664,9 @@ def build_vqgan_spec(g, codeformer=False):
     s = Spec()
     if codeformer:
         s.add('position_emb', (a.latent_size, a.dim_embd), 'pos_emb')
-    _vqgan_blocks(s, 'encoder', a.enc_blocks)
+    _block_list(s, a, a.enc_blocks)
     s.add('quantize.embedding.weight', (a.n_embed, a.embed_dim), 'codebook_nopad')
-    _vqgan_blocks(s, 'generator', a.gen_blocks)
+    _block_list(s, a, a.dec_blocks)
     if not codeformer:
         return a, s
     _linear(s, 'feat_emb', 256, a.dim_embd)
@@ -743,7 +684,7 @@ def build_vqgan_spec(g, codeformer=False):
     for key in a.connect_list:                                         # Fuse_sft_block (:200-213)
         c = CODEFORMER_CHANNELS[key]
         p = 'fuse_convs_dict.' + key
-        _res_block(s, p + '.encode_enc', 2 * c, c)
+        _res_block(s, p + '.encode_enc', 2 * c, c, a.res_shortcut)
         for br in ('scale', 'shift'):
             _conv(s, '%s.%s.0' % (p, br), c, c, 3)
             _conv(s, '%s.%s.2' % (p, br), c, c, 3)

@@ -3,9 +3,10 @@
 
 Both walk the flat `encoder.blocks` / `generator.blocks` lists of spec.VQGANArch, as the reference's forward does, on the
 blocks Engine already has: ResBlock is td_resblock with the `conv_out` shortcut, AttnBlock is attn_block, Downsample the
-stride-2 conv, Upsample up2x, the transformer global_transformer and the SFT fusion sft_tail.  Layout as in engine.py:
-channels-last bf16 feature maps [b, H, W, C]; the latent's token rows are in (image, y, x) order, which is the
-reference's b(hw) order of logits and codes.  Every op is a call into the C ABI; there is no PyTorch / CPU fallback."""
+stride-2 conv, Upsample up2x, the generator Engine.decoder, the transformer global_transformer and the SFT fusion
+sft_tail.  Layout as in engine.py: channels-last bf16 feature maps [b, H, W, C]; the latent's token rows are in
+(image, y, x) order, which is the reference's b(hw) order of logits and codes.  Every op is a call into the C ABI; there
+is no PyTorch / CPU fallback."""
 import torch
 
 from . import ops
@@ -21,44 +22,22 @@ class VQGANEngine(Engine):
     def arch_class(self, g):
         return VQGANArch(g, self.codeformer)
 
-    # ------------------------------------------------------------------ encoder / generator
-    res_shortcut = 'conv_out'
-
-    def _blocks(self, prefix, blocks, fuse=None):
-        """The flat `prefix`.blocks list as Engine._walk entries (kind, state-dict prefix, output channels), with a
-        `fuse` block (CodeFormer's Fuse_sft_block, reading the tapped encoder output of its size key) after each block
-        index in fuse."""
-        out = []
-        for i, (kind, _, cout, _) in enumerate(blocks):
-            out.append((kind, '%s.blocks.%d' % (prefix, i), cout))
-            if fuse and i in fuse:
-                out.append(('fuse', 'fuse_convs_dict.' + fuse[i], cout, fuse[i]))
-        return out
-
+    # ------------------------------------------------------------------ encoder
     def encoder(self, x, taps=None):
         """encoder.blocks[:-2] on x fp32 NCHW [b,3,H,W] -> (h bf16 [b,h,w,C] with the final GroupNorm's statistics,
         {key: tapped block output})."""
-        blocks = self._blocks('encoder', self.arch.enc_blocks)
+        blocks = self.arch.enc_blocks
         return self._walk(blocks, x, 0, len(blocks) - 2, taps)
 
     def encoder_out(self, h, out, nchw=False):
         """The encoder tail: GroupNorm (no SiLU) -> conv 3x3 to emb_dim, into out (fp32 NHWC rows, fp32 NCHW with
         nchw, or bf16 NHWC).  The GroupNorm runs on its own pass."""
-        n = len(self.arch.enc_blocks)
+        norm, conv = self.arch.enc_blocks[-2:]
         y = getattr(h, '_pgt_normed', None)
         if y is None:
-            y = self._gn(h, 'encoder.blocks.%d' % (n - 2), silu=False)
+            y = self._gn(h, norm.prefix, silu=False)
             h._pgt_normed = y
-        return self._conv3(y, 'encoder.blocks.%d' % (n - 1), self.arch.embed_dim, out=out, nchw=nchw)
-
-    def generator(self, z, feats=None, wgt=0.0):
-        """generator.blocks on z bf16 [b,h,w,emb_dim] -> fp32 NCHW [b,3,H,W]; with feats and wgt > 0 CodeFormer's
-        Fuse_sft_block after the blocks of arch.fuse_gen (`archs/codeformer_arch.py:356-363`)."""
-        a = self.arch
-        blocks = self._blocks('generator', a.gen_blocks, getattr(a, 'fuse_gen', None))
-        h, _ = self._walk(blocks, z, 0, len(blocks) - 2, feats=feats, wgt=wgt)
-        n = len(a.gen_blocks)
-        return self.decoder_out(h, 'generator.blocks.%d' % (n - 2), 'generator.blocks.%d' % (n - 1), silu=False, out_ch=3)
+        return self._conv3(y, conv.prefix, conv.cout, out=out, nchw=nchw)
 
     def fuse_sft(self, enc, dec, key, wgt, gn_next=False):
         """Fuse_sft_block (`archs/codeformer_arch.py:218-226`): the concat [enc | dec] -> sft_tail."""
@@ -117,7 +96,7 @@ class VQGANEngine(Engine):
         self.last_z = z
         if code_only:
             return zq, scalars[0], stats
-        return self.generator(zq16), scalars[0], stats
+        return self.decoder(zq16), scalars[0], stats
 
     def counted_forward(self, x, usage, code_only=False):
         """forward with the usage buffer as a positional tensor argument (the form Engine.graphed replays)."""
@@ -153,7 +132,7 @@ class CodeFormerEngine(VQGANEngine):
         L, E = hh * ww, a.embed_dim
         T = b * L
         fusing = (not code_only) and float(w) > 0
-        h, feats = self.encoder(x, a.fuse_enc if fusing else None)
+        h, feats = self.encoder(x, a.enc_taps if fusing else None)
         lq_nchw = self.encoder_out(h, self._new(b, E, hh, ww, dtype=F32), nchw=True)
         lq = self.encoder_out(h, self._new(b, hh, ww, E))
         logits = self.global_transformer(lq.view(T, E), self.pos(b), b)
@@ -169,5 +148,5 @@ class CodeFormerEngine(VQGANEngine):
             quant = self._new(T, E)
             ops.argmax_gather(logits, self.w['codebook'], codes, quant, idx_in=idx_in)
         self.last_codes = (codes if idx_in is None else idx_in).view(b, L)
-        out = self.generator(quant.view(b, hh, ww, E), feats, float(w))
+        out = self.decoder(quant.view(b, hh, ww, E), feats, float(w))
         return out, logits.view(b, L, a.n_embed), lq_nchw

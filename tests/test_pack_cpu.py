@@ -23,7 +23,6 @@ def packed(name, network_g):
     from pgtformer_b200.rqvae import RQVAEEngine
     from pgtformer_b200.tdrqvae import TDRQVAEEngine
     from pgtformer_b200.vqgan import CodeFormerEngine, VQGANEngine
-    from pgtformer_b200.weights import synth_state_dict
     if name == 'PGTFormer':
         cls, (arch, spec) = Engine, S.build_spec(network_g)
     elif name == 'TDRQVAE':
@@ -35,6 +34,12 @@ def packed(name, network_g):
         cls, (arch, spec) = VQGANEngine, S.build_vqgan_spec({})
     else:
         cls, (arch, spec) = CodeFormerEngine, S.build_codeformer_spec({})
+    return repacked(cls, arch, spec)
+
+
+def repacked(cls, arch, spec):
+    """(engine of class cls after _repack of spec's synthetic state dict on the CPU, that state dict)."""
+    from pgtformer_b200.weights import synth_state_dict
     eng = cls.__new__(cls)
     eng.arch, eng.dev, eng.w = arch, torch.device('cpu'), {}
     eng._sd = synth_state_dict(spec, 0)

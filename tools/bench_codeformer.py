@@ -32,23 +32,24 @@ def model_flops(arch, H, W, codeformer, w=0.5):
     def res(h, w_, cin, cout):
         return conv(h, w_, cin, cout, 3) + conv(h, w_, cout, cout, 3) + (conv(h, w_, cin, cout, 1) if cin != cout else 0)
 
-    def blocks(bl, scale):
+    def blocks(bl, h, w_):
         f = 0.0
-        for kind, cin, cout, r in bl:
-            h, w_ = r * H // (arch.img_size * scale), r * W // (arch.img_size * scale)
-            if kind in ('conv_in', 'conv_out'):
-                f += conv(h, w_, cin, cout, 3)
-            elif kind == 'res':
-                f += res(h, w_, cin, cout)
-            elif kind == 'attn':
+        for b in bl:                        # `fuse` blocks are counted below
+            if b.kind in ('conv_in', 'conv_out'):
+                f += conv(h, w_, b.cin, b.cout, 3)
+            elif b.kind == 'res':
+                f += res(h, w_, b.cin, b.cout)
+            elif b.kind == 'attn':
                 L = h * w_
-                f += 4 * conv(h, w_, cin, cin, 1) + 4.0 * L * L * cin
-            elif kind == 'down':
-                f += conv(h // 2, w_ // 2, cin, cin, 3)
-            elif kind == 'up':
-                f += conv(2 * h, 2 * w_, cin, cin, 3)
+                f += 4 * conv(h, w_, b.cin, b.cin, 1) + 4.0 * L * L * b.cin
+            elif b.kind == 'down':
+                h, w_ = h // 2, w_ // 2
+                f += conv(h, w_, b.cin, b.cin, 3)
+            elif b.kind == 'up':
+                h, w_ = 2 * h, 2 * w_
+                f += conv(h, w_, b.cin, b.cin, 3)
         return f
-    f = blocks(arch.enc_blocks, 1) + blocks(arch.gen_blocks, 1)
+    f = blocks(arch.enc_blocks, H, W) + blocks(arch.dec_blocks, H // arch.down, W // arch.down)
     if not codeformer:
         return f
     L, E, D = H * W // arch.down ** 2, arch.embed_dim, arch.dim_embd
