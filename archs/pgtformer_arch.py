@@ -23,7 +23,7 @@ import torch.nn as nn
 
 from pgtformer_b200.registry import ARCH_REGISTRY
 from pgtformer_b200.spec import build_spec
-from pgtformer_b200.weights import synth_tensor
+from pgtformer_b200.weights import synth_state_dict
 
 try:
     from huggingface_hub import PyTorchModelHubMixin
@@ -51,8 +51,10 @@ class _Node(nn.Module):
 
 
 def _materialise(root, spec, seed):
+    """root's module tree of spec's entries, holding synth_state_dict's tensors (each embed_ema its codebook's rows)."""
     import weakref
     rootref = weakref.ref(root)
+    sd = synth_state_dict(spec, seed)
     for name, (shape, kind, dtype) in spec.items():
         if spec.alias_of(name):
             continue
@@ -64,10 +66,7 @@ def _materialise(root, spec, seed):
                 child._pgt_root = rootref
                 node.add_module(part, child)
             node = node._modules[part]
-        t = synth_tensor(name, shape, 'codebook' if kind == 'codebook_ema' else kind, dtype, seed,
-                         window=getattr(spec, 'windows', {}).get(name))
-        if kind == 'codebook_ema':
-            t = t[:-1] if t.shape[0] == shape[0] + 1 else t
+        t = sd[name]
         if kind in ('bn_mean', 'bn_var', 'bn_count', 'rpb_index', 'zeros', 'codebook_ema'):
             node.register_buffer(parts[-1], t)
         else:
@@ -95,9 +94,6 @@ class _B200Model(nn.Module):
         self._network_g = network_g
         self.arch, self._spec = build_spec(network_g)
         _materialise(self, self._spec, seed)
-        # embed_ema mirrors the codebook rows (tdcrqvae3_arch.py:96)
-        for cb in self.quantizer.codebooks._modules.values():
-            cb.embed_ema.copy_(cb.weight.detach()[:-1])
         self._engine = None
         self.t = self.arch.tf
         self.code_shape = list(self.arch.code_shape)
@@ -146,18 +142,18 @@ class _B200Model(nn.Module):
         return getattr(eng, name)(*tensors, **scalars)
 
     # ---- code helpers shared by the codecs.  Arguments are checked on the host before any launch: bad shapes
-    # raise ValueError, codes outside [0, n_embed] IndexError (index n_embed is the codebook's padding row, which
-    # nn.Embedding accepts).
+    # raise ValueError, depth d's codes outside [0, n_embeds[d]] IndexError (index n_embeds[d] is the codebook's
+    # padding row, which nn.Embedding accepts).
     def _check_code(self, code):
         if not torch.is_tensor(code) or code.dim() != 4 or code.shape[-1] != self.code_shape[-1] or \
                 code.dtype.is_floating_point or code.dtype.is_complex or code.dtype == torch.bool:
             raise ValueError('expected integer codes [F, h, w, %d], got %s %s'
                              % (self.code_shape[-1], _shape(code), getattr(code, 'dtype', '')))
         if code.numel() > 0:
-            lo, hi = torch.aminmax(code)
-            n = self.arch.n_embed
-            if int(lo) < 0 or int(hi) > n:
-                raise IndexError('code out of range [0, %d]: min %d, max %d' % (n, int(lo), int(hi)))
+            lo, hi = torch.stack(torch.aminmax(code.reshape(-1, code.shape[-1]), dim=0)).tolist()    # one host sync
+            for d, n in enumerate(self.arch.n_embeds):
+                if lo[d] < 0 or hi[d] > n:
+                    raise IndexError('depth %d: code out of range [0, %d]: min %d, max %d' % (d, n, lo[d], hi[d]))
 
     @torch.no_grad()
     def get_code_emb_with_depth(self, code):

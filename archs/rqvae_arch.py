@@ -38,8 +38,6 @@ class RQVAE(_B200Model, PyTorchModelHubMixin):
         self._network_g = g
         self.arch, self._spec = build_rqvae_spec(g)
         _materialise(self, self._spec, 0)
-        for cb in self.quantizer.codebooks._modules.values():
-            cb.embed_ema.copy_(cb.weight.detach()[:-1])       # VQEmbedding: embed_ema = weight[:-1] (:216)
         self._engine = None
         self.code_shape = kwargs['code_shape']
         self.loss_type = loss_type
@@ -65,14 +63,6 @@ class RQVAE(_B200Model, PyTorchModelHubMixin):
     def _check_latent(self, B, h, w):
         if B == 0 or h == 0 or w == 0 or h % 4 or w % 4:
             raise ValueError('expected a latent map of multiples of 4, got [%d, %d, %d]' % (B, h, w))
-
-    def _check_code(self, code):
-        """Integer codes [B, h, w, D]; depth d's codes in [0, n_embed_d] (n_embed_d is its padding row)."""
-        super()._check_code(code)
-        for d, n in enumerate(self.arch.n_embeds):
-            c = code[..., d]
-            if c.numel() and (int(c.min()) < 0 or int(c.max()) > n):
-                raise IndexError('depth %d: code out of range [0, %d]: min %d, max %d' % (d, n, int(c.min()), int(c.max())))
 
     # ---- the reference's methods (`archs/rqvae_arch.py:828-931`)
     def forward(self, xs, code_only=False):

@@ -39,8 +39,6 @@ class TDRQVAE(_B200Model, PyTorchModelHubMixin):
         self._network_g = g
         self.arch, self._spec = build_tdrqvae_spec(g)
         _materialise(self, self._spec, 0)
-        cb = self.quantizer.codebooks._modules['0']
-        cb.embed_ema.copy_(cb.weight.detach()[:-1])           # VQEmbedding: embed_ema = weight[:-1] (:223)
         self._engine = None
         self.t = tf                                           # forward never reads it: b, t come from the input
         self.code_shape = kwargs['code_shape']

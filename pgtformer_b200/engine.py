@@ -725,8 +725,10 @@ class Engine:
         return self.w['codebooks'][d]
 
     def _n_embed(self, d=0):
-        """Codes in depth d's codebook (the rows before its padding row)."""
-        return self.arch.n_embed
+        """Codes in depth d's codebook (the rows before its padding row): arch.n_embeds[d] for the RQ archs, which list
+        one size per depth; an arch with one codebook size and no such list (VQGAN's, a bare quantiser's) has n_embed."""
+        a = self.arch
+        return a.n_embeds[d] if hasattr(a, 'n_embeds') else a.n_embed
 
     def _codebook_pack(self, d=0):
         """bf16 copy + fp32 norms of depth d's codebook (l2_argmin_tc, soft_codes), once per load and distinct codebook."""

@@ -167,6 +167,53 @@ def _block_list(s, a, blocks):
             _norm(s, b.prefix, b.cin)
 
 
+def _rq_bottleneck(a, g, per_depth_sizes=False):
+    """The RQBottleneck keys of an RQ autoencoder's config g (`archs/tdcrqvae3_arch.py:221-271, 738-752`), resolved
+    into a: embed_dim, latent_shape, code_shape, depth = code_shape[2], shared_codebook, n_embeds (codes of each depth's
+    codebook), n_embed = max(n_embeds) and the codebook key of each depth (a shared codebook's keys alias the first).
+    per_depth_sizes: n_embed may list one size per depth; otherwise it is one int for every depth."""
+    if g.get('bottleneck_type', 'rq') != 'rq':
+        raise ValueError("invalid 'bottleneck_type' (must be 'rq')")
+    a.embed_dim = int(g.get('embed_dim', 64))
+    a.latent_shape = tuple(int(v) for v in g['latent_shape'])
+    a.code_shape = tuple(int(v) for v in g['code_shape'])
+    a.shared_codebook = bool(g['shared_codebook'])
+    if not len(a.code_shape) == len(a.latent_shape) == 3:
+        raise ValueError('incompatible code shape or latent shape')
+    if any(y % x != 0 for x, y in zip(a.code_shape[:2], a.latent_shape[:2])):
+        raise ValueError('incompatible code shape or latent shape')
+    a.depth = a.code_shape[2]
+    if a.depth < 1:
+        raise ValueError('quantiser depth code_shape[2] must be >= 1, got %d' % a.depth)
+    n = g.get('n_embed', 512)
+    if per_depth_sizes and isinstance(n, (list, tuple)):
+        if a.shared_codebook:
+            raise ValueError('Shared codebooks are incompatible with list types of momentums or sizes: '
+                             'Change it into int')
+        if len(n) != a.depth:
+            raise ValueError('n_embed lists one size per code depth: %d sizes for depth %d' % (len(n), a.depth))
+        a.n_embeds = tuple(int(k) for k in n)
+    else:
+        a.n_embeds = (int(n),) * a.depth
+    a.n_embed = max(a.n_embeds)                 # rows of the padded per-depth codebook stack
+    a.codebooks = tuple('quantizer.codebooks.%d.weight' % d for d in range(a.depth))
+
+
+def _quantiser(s, a):
+    """The state-dict entries of the RQBottleneck (`archs/tdcrqvae3_arch.py:80-97, 256-269`: one VQEmbedding per depth,
+    or one shared by every depth), quant_conv and post_quant_conv."""
+    e = a.embed_dim
+    for d, k in enumerate(a.n_embeds):
+        p = 'quantizer.codebooks.%d' % d
+        s.add(p + '.weight', (k + 1, e), 'codebook')
+        s.add(p + '.cluster_size_ema', (k,), 'zeros')
+        s.add(p + '.embed_ema', (k, e), 'codebook_ema')
+        if a.shared_codebook and d > 0:
+            s.module_aliases[p] = 'quantizer.codebooks.0'
+    _conv(s, 'quant_conv', a.z_channels, e, 1)
+    _conv(s, 'post_quant_conv', e, a.z_channels, 1)
+
+
 class Arch(_Autoencoder):
     """Resolved architecture constants (everything the engine / oracle need besides weights)."""
 
@@ -174,11 +221,7 @@ class Arch(_Autoencoder):
         g = dict(network_g)
         dd = dict(g['ddconfig'])
         self.tf = int(g.get('tf', 3))
-        self.embed_dim = int(g.get('embed_dim', 64))
-        self.n_embed = int(g.get('n_embed', 512))
-        self.code_shape = tuple(g['code_shape'])
-        self.latent_shape = tuple(g['latent_shape'])
-        self.shared_codebook = bool(g.get('shared_codebook', True))       # the options files' setting
+        g.setdefault('shared_codebook', True)                            # the options files' setting
         self.dim_embd = int(g.get('dim_embd', 512))
         self.n_head = int(g.get('n_head', 8))
         self.n_layers = int(g.get('n_layers', 9))
@@ -197,17 +240,9 @@ class Arch(_Autoencoder):
         self.out_ch = int(dd['out_ch'])
         self.double_z = bool(dd.get('double_z', True))
         self.num_levels = len(self.ch_mult)
-        if g.get('bottleneck_type', 'rq') != 'rq':
-            raise ValueError("invalid 'bottleneck_type' (must be 'rq')")     # tdcrqvae3_arch.py:752
-        if not len(self.code_shape) == len(self.latent_shape) == 3:
-            raise ValueError('incompatible code shape or latent shape')      # tdcrqvae3_arch.py:232
-        if any(y % x != 0 for x, y in zip(self.code_shape[:2], self.latent_shape[:2])):
-            raise ValueError('incompatible code shape or latent shape')      # tdcrqvae3_arch.py:234
+        _rq_bottleneck(self, g)         # one n_embed for every depth: idx_pred_layer predicts depth x n_embed logits
         if self.tf != 3 or self.num_frames != 3 or any(w != (4, 4) for w in self.window_sizes):
             raise ValueError('the CUDA path is built for 3-frame clips and 4x4x3 windows')
-        if int(self.code_shape[2]) < 1:
-            raise ValueError('quantiser depth code_shape[2] must be >= 1, got %r' % (self.code_shape[2],))
-        self.depth = int(self.code_shape[2])
         # levels that carry a window-attention layer (curr_res walk of tdcrqvae3_arch.py:482-510)
         self.level_has_attn = tuple((self.resolution >> i) in self.attn_resolutions
                                     for i in range(self.num_levels))
@@ -216,7 +251,6 @@ class Arch(_Autoencoder):
         self.fuse_level_key = {i: str(self.resolution >> i) for i in range(self.num_levels)
                                if str(self.resolution >> i) in self.connect_list}
         self.fuse_channels = {'16': 512, '32': 512, '64': 256, '128': 256, '256': 128, '512': 64}
-        self.codebooks = _codebooks(self.depth)
         self.packed_apart = ('conditionnet.',)                      # BiSeNet: BatchNorms folded into its convs
         self.enc_blocks, self.dec_blocks, self.frame_blocks, self.enc_taps = _autoencoder_blocks(self, 'swin')
 
@@ -269,26 +303,11 @@ def _autoencoder_blocks(a, attn):
     return tuple(enc), tuple(dec), frame_blocks, taps
 
 
-def _codebooks(depth):
-    """The codebook key of each quantiser depth (a shared codebook's keys alias the first)."""
-    return tuple('quantizer.codebooks.%d.weight' % d for d in range(depth))
-
-
 def build_spec(network_g):
     a = Arch(network_g)
     s = Spec()
     _block_list(s, a, a.enc_blocks + a.dec_blocks)          # tdcrqvae3_arch.py:460-539, 577-670
-    # ---- quantiser (tdcrqvae3_arch.py:80-97,215-271): one VQEmbedding per depth, or one shared by every depth
-    e = a.embed_dim
-    for d in range(a.depth):
-        p = 'quantizer.codebooks.%d' % d
-        s.add(p + '.weight', (a.n_embed + 1, e), 'codebook')
-        s.add(p + '.cluster_size_ema', (a.n_embed,), 'zeros')
-        s.add(p + '.embed_ema', (a.n_embed, e), 'codebook_ema')
-        if a.shared_codebook and d > 0:
-            s.module_aliases[p] = 'quantizer.codebooks.0'
-    _conv(s, 'quant_conv', a.z_channels, e, 1)
-    _conv(s, 'post_quant_conv', e, a.z_channels, 1)
+    _quantiser(s, a)
     # ---- PGTFormer head (pgtformer_arch.py:511-550)
     _bisenet(s, 'conditionnet')
     _conv(s, 'convpos', 57, 512, 1)
@@ -362,17 +381,9 @@ class TDRQVAEArch(_Autoencoder):
         g = dict(network_g)
         dd = dict(g['ddconfig'])
         self.tf = int(g.get('tf', 7))
-        self.embed_dim = int(g.get('embed_dim', 64))
-        self.n_embed = int(g.get('n_embed', 512))
-        if g.get('bottleneck_type', 'rq') != 'rq':
-            raise ValueError("invalid 'bottleneck_type' (must be 'rq')")     # tdrqvae_arch.py:829
-        self.latent_shape = tuple(g['latent_shape'])
-        self.code_shape = tuple(g['code_shape'])
-        if not len(self.code_shape) == len(self.latent_shape) == 3:
-            raise ValueError('incompatible code shape or latent shape')      # tdrqvae_arch.py:357-360
-        if any(y % x != 0 for x, y in zip(self.code_shape[:2], self.latent_shape[:2])):
-            raise ValueError('incompatible code shape or latent shape')
-        if self.code_shape[2] != 1:
+        g.setdefault('shared_codebook', True)          # one codebook at depth 1: shared or not, the same layout
+        _rq_bottleneck(self, g)
+        if self.depth != 1:
             # the reference's TDRQVAE.forward / get_codes reshape the codes with code.view(b, t, fh, fw, 1)
             # (archs/tdrqvae_arch.py:852, 888), which fails for any deeper quantiser
             raise ValueError('TDRQVAE runs quantiser depth 1 only: the reference reshapes its codes with '
@@ -410,7 +421,6 @@ class TDRQVAEArch(_Autoencoder):
         if len(self.window_size) != 3 or min(self.window_size) < 1 or \
                 self.window_size[0] * self.window_size[1] * self.window_size[2] > SWIN_MAX_TOKENS:
             raise ValueError('Video-Swin window %s: at most %d tokens' % (self.window_size, SWIN_MAX_TOKENS))
-        self.codebooks = _codebooks(1)
         self.packed_apart = ('tdswin_pre.', 'tdswin_post.')         # Video-Swin BasicLayers: swin3d.pack_blocks
         self.enc_blocks, self.dec_blocks, self.frame_blocks, _ = _autoencoder_blocks(self, 'attn')
         self.enc_taps = {}                                          # its Encoder returns h alone
@@ -420,15 +430,9 @@ def build_tdrqvae_spec(network_g):
     a = TDRQVAEArch(network_g)
     s = Spec()
     _block_list(s, a, a.enc_blocks + a.dec_blocks)          # tdrqvae_arch.py:587-751
-    # ---- quantiser (:206-223, 381-394): one shared codebook of depth 1
-    e = a.embed_dim
-    s.add('quantizer.codebooks.0.weight', (a.n_embed + 1, e), 'codebook')
-    s.add('quantizer.codebooks.0.cluster_size_ema', (a.n_embed,), 'zeros')
-    s.add('quantizer.codebooks.0.embed_ema', (a.n_embed, e), 'codebook_ema')
-    _conv(s, 'quant_conv', a.z_channels, e, 1)
-    _conv(s, 'post_quant_conv', e, a.z_channels, 1)
+    _quantiser(s, a)                                        # :206-223, 381-394
     for p in ('tdswin_pre', 'tdswin_post'):
-        _swin3d_layer(s, p, e, a.stages_atten, a.num_head, a.window_size)
+        _swin3d_layer(s, p, a.embed_dim, a.stages_atten, a.num_head, a.window_size)
     return a, s
 
 
@@ -441,28 +445,7 @@ class RQVAEArch(_Autoencoder):
     def __init__(self, network_g):
         g = dict(network_g)
         dd = dict(g['ddconfig'])
-        if g.get('bottleneck_type', 'rq') != 'rq':
-            raise ValueError("invalid 'bottleneck_type' (must be 'rq')")     # rqvae_arch.py:820
-        self.embed_dim = int(g.get('embed_dim', 64))
-        self.latent_shape = tuple(int(v) for v in g['latent_shape'])
-        self.code_shape = tuple(int(v) for v in g['code_shape'])
-        self.shared_codebook = bool(g['shared_codebook'])
-        if not len(self.code_shape) == len(self.latent_shape) == 3:
-            raise ValueError('incompatible code shape or latent shape')      # rqvae_arch.py:350-353
-        if any(y % x != 0 for x, y in zip(self.code_shape[:2], self.latent_shape[:2])):
-            raise ValueError('incompatible code shape or latent shape')
-        self.depth = self.code_shape[2]
-        n = g.get('n_embed', 512)
-        if isinstance(n, (list, tuple)):
-            if self.shared_codebook:
-                raise ValueError('Shared codebooks are incompatible with list types of momentums or sizes: '
-                                 'Change it into int')                      # rqvae_arch.py:363-366
-            if len(n) != self.depth:
-                raise ValueError('n_embed lists one size per code depth: %d sizes for depth %d' % (len(n), self.depth))
-            self.n_embeds = tuple(int(k) for k in n)
-        else:
-            self.n_embeds = (int(n),) * self.depth
-        self.n_embed = max(self.n_embeds)                                    # rows of the padded per-depth codebook stack
+        _rq_bottleneck(self, g, per_depth_sizes=True)                       # rqvae_arch.py:350-387, 807-820
         self.ch = int(dd['ch'])
         self.ch_mult = tuple(dd['ch_mult'])
         self.num_res_blocks = int(dd['num_res_blocks'])
@@ -476,8 +459,6 @@ class RQVAEArch(_Autoencoder):
         self.down = 2 ** (self.num_levels - 1)
         self.level_ch = tuple(self.ch * m for m in self.ch_mult)
         self.level_has_attn = tuple((self.resolution >> i) in self.attn_resolutions for i in range(self.num_levels))
-        if self.depth < 1:
-            raise ValueError('quantiser depth code_shape[2] must be >= 1, got %d' % self.depth)
         if self.code_shape[:2] != self.latent_shape[:2]:
             raise ValueError('code_shape %s, latent_shape %s: code-shape divisors > 1 are not supported'
                              % (self.code_shape, self.latent_shape))
@@ -500,7 +481,6 @@ class RQVAEArch(_Autoencoder):
         if self.embed_dim % 128 or self.embed_dim > 512 or any(k % 128 or k < 128 for k in self.n_embeds):
             raise ValueError('embed_dim %d, n_embed %s: the argmin takes codebooks of a multiple of 128 up to 512 '
                              'channels and a multiple of 128 codes' % (self.embed_dim, list(self.n_embeds)))
-        self.codebooks = _codebooks(self.depth)
         self.packed_apart = ()
         self.enc_blocks, self.dec_blocks, self.frame_blocks, _ = _autoencoder_blocks(self, 'attn')
         self.enc_taps = {}                                          # its Encoder returns h alone
@@ -513,18 +493,7 @@ def build_rqvae_spec(network_g):
     a = RQVAEArch(network_g)
     s = Spec()
     _block_list(s, a, a.enc_blocks + a.dec_blocks)          # rqvae_arch.py:579-743
-    # ---- RQBottleneck (rqvae_arch.py:199-216, 374-387): one VQEmbedding per depth, or one shared by every depth
-    e = a.latent_shape[2]
-    for d in range(a.depth):
-        p = 'quantizer.codebooks.%d' % d
-        k = a.n_embeds[d]
-        s.add(p + '.weight', (k + 1, e), 'codebook')
-        s.add(p + '.cluster_size_ema', (k,), 'zeros')
-        s.add(p + '.embed_ema', (k, e), 'codebook_ema')
-        if a.shared_codebook and d > 0:
-            s.module_aliases[p] = 'quantizer.codebooks.0'
-    _conv(s, 'quant_conv', a.z_channels, a.embed_dim, 1)
-    _conv(s, 'post_quant_conv', a.embed_dim, a.z_channels, 1)
+    _quantiser(s, a)                                        # :199-216, 374-387; latent_shape[2] == embed_dim wide
     return a, s
 
 
