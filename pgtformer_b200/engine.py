@@ -206,7 +206,10 @@ class Engine:
         out is not contiguous or chunks_per_frame (32-row chunks per frame, 4 per 128-row tile) is 0."""
         if chunks_per_frame <= 0 or not ops.gn_stats_supported(out.shape[-1]) or not out.is_contiguous():
             return None
-        stats = self._new(out.shape[0] * chunks_per_frame * 64, dtype=torch.float32)
+        stats = getattr(out, '_pgt_gn_into', None)              # a live ring slot keeps them beside its features
+        if stats is None:
+            stats = self._new(out.shape[0] * chunks_per_frame * 64, dtype=torch.float32)
+        assert stats.numel() == out.shape[0] * chunks_per_frame * 64
         out._pgt_gn = (stats, chunks_per_frame)
         return stats
 
@@ -444,7 +447,8 @@ class Engine:
     # ------------------------------------------------------------------ encoder / decoder
     def _walk(self, blocks, h, lo=0, hi=None, taps=None, outs=None, feats=None, wgt=0.0):
         """Runs blocks[lo:hi] of a block list (spec.Block entries) on h.  Returns (h, {taps[i]: output of block i}).
-        outs {i: tensor}: block i (`res` or `swin`) writes its output there, a slice of an SFT concat buffer.  A `fuse`
+        outs {i: tensor}: block i (`res`, `swin` or `down`) writes its output there, a slice of an SFT concat buffer or a
+        slot of a live ring (live_ring).  A `fuse`
         block runs only with feats and wgt > 0, on feats[its src].
 
         GroupNorm statistics: a block passes gn_next to its producer exactly when the next block that runs reads its
@@ -469,7 +473,7 @@ class Engine:
             elif kind == 'swin':
                 h = self.encoder_layer(h, p, blk.heads, blk.depth, gn_next=nxt, out=outs.get(i))
             elif kind == 'down':
-                h = self._conv3(h, p + '.conv', cout, stride=2, pad_lo=0, gn_out=nxt)
+                h = self._conv3(h, p + '.conv', cout, stride=2, pad_lo=0, gn_out=nxt, out=outs.get(i))
             elif kind == 'up':
                 h = self.up2x(h, p + '.conv')
             elif kind == 'fuse':
@@ -573,12 +577,12 @@ class Engine:
         self._conv3(h, conv, out_ch, out=out, gn=norm, gn_silu=silu, nchw=True)
         return out
 
-    def parse_pos(self, x):
+    def parse_pos(self, x, out=None):
         """BiSeNet parsing features -> convpos 1x1 -> positional term [T, 512] bf16
-        (`archs/pgtformer_arch.py:606-614`)."""
+        (`archs/pgtformer_arch.py:606-614`), written into out when given."""
         Fr, _, H, W = x.shape
         cond = self.parsing_net(x)
-        return self._lin(cond.view(Fr * (H // 16) * (W // 16), 64), 'convpos', 512, K=57)
+        return self._lin(cond.view(Fr * (H // 16) * (W // 16), 64), 'convpos', 512, K=57, out=out)
 
     def global_transformer(self, lq, pos, clips):
         """feat_emb + 9 x TransformerSALayer + idx_pred_layer (`archs/pgtformer_arch.py:638-649`,
@@ -619,9 +623,7 @@ class Engine:
             Fr = frame_index.numel()
         if Fr % a.tf != 0 or H % 64 != 0 or W % 64 != 0:
             raise ValueError('expected b*3 frames with H, W multiples of 64, got %s' % (tuple(x.shape),))
-        hh, ww = H // 16, W // 16
-        T, E = Fr * hh * ww, a.dim_embd
-        wd = self.w
+        T = Fr * (H // 16) * (W // 16)
         pos = self.parse_pos(x)
         # encoder
         if frame_index is None:
@@ -633,6 +635,15 @@ class Engine:
             feats = {lvl: self._gather(f, frame_index) if (lvl in a.fuse_level_key and w > 0) else f
                      for lvl, f in feats.items()}
             h, feats = self.encoder_clips(self._gather(h, frame_index), feats, i)
+        return self._restore(h, feats, pos, w, adain, code_only, force_codes)
+
+    def _restore(self, h, feats, pos, w, adain, code_only=False, force_codes=None):
+        """forward from the encoder's output h [F,h,w,C] on: quant_conv -> global transformer -> argmax (or
+        force_codes) / AdaIN -> post_quant_conv -> decoder with SFT fusion of feats."""
+        a = self.arch
+        Fr, hh, ww, _ = h.shape
+        T = Fr * hh * ww
+        wd = self.w
         h = h.view(T, -1)
         lq32 = self._lin(h, 'quant_conv', a.embed_dim, out_dtype=torch.float32)
         lq = self._lin(h, 'quant_conv', a.embed_dim)
@@ -677,7 +688,11 @@ class Engine:
         static inputs and replays it; tensors at the indices in `writes` are ones the method updates in place, copied
         back after the replay.  Returns the graph's static outputs: consume them before the next call.  Arguments are
         checked by the caller before this: a capture never starts on an argument the method would reject, and a key
-        whose warm-up raises stores nothing."""
+        whose warm-up raises stores nothing.
+
+        A graph here is a pure function of its inputs.  The live steps (video.LiveRestorer), whose ring of per-frame
+        results persists across replays, are captured by their session instead: one graph per ring phase, all in one
+        memory pool, because each step's producers write straight into the new frame's ring slot (video._LiveSession)."""
         tensors = [t.to(self.dev) for t in tensors]
         key = (method.__name__, tuple((tuple(t.shape), t.dtype) for t in tensors), tuple(sorted(scalars.items())))
         if not hasattr(self, '_graphs'):
@@ -716,6 +731,76 @@ class Engine:
         Returned tensors are the graph's static outputs: consume them before the next call."""
         x = x.to(self.dev, torch.float32).contiguous()
         return self.graphed(self.forward, (x,), w=float(w), adain=bool(adain))
+
+    # ------------------------------------------------------------------ video: batched windows and the live ring
+    @_on_device
+    @torch.no_grad()
+    def restore_windows(self, frames_u8, index, w=1.0, adain=True, reuse_frames=True):
+        """One batch of VideoRestorer: rgb24 frames [Fd,H,W,3] uint8 on the device and the device int32 window index
+        [3n] into them -> the restored middle frames, rgb24 [n,H,W,3] uint8 on the device."""
+        Fd, H, W, _ = frames_u8.shape
+        x = ops.u8hwc_to_f32nchw(frames_u8, self._new(Fd, 3, H, W, dtype=torch.float32))
+        if reuse_frames:
+            out = self.forward(x, w=w, adain=adain, frame_index=index)[0]
+        else:
+            xc = ops.gather_frames(x, index, self._new(index.numel(), 3, H, W, dtype=torch.float32))
+            out = self.forward(xc, w=w, adain=adain)[0]
+        n = index.numel() // 3
+        return ops.f32nchw_to_u8hwc(out, torch.empty(n, H, W, 3, dtype=torch.uint8, device=self.dev), first=1, step=3)
+
+    @_on_device
+    @torch.no_grad()
+    def live_ring(self, H, W, w):
+        """The per-frame results of three frames, one slot each, for frame_step / window_step: {'pos': convpos rows
+        [3, T/3, 512], 'h': the frame blocks' output [3, ...] (with 'h_stats', the GroupNorm statistics its producer
+        writes for the next block, when it writes any), and for w > 0 'feats': {level: [3, ...]}, the skip tensors of
+        the per-frame levels the SFT fusion reads}.  Allocated here, outside any graph's memory pool, so that graphs
+        captured later can all write and read the same addresses.  Shapes are those of one run of the per-frame work."""
+        if H % 64 or W % 64:
+            raise ValueError('expected H, W multiples of 64, got %dx%d' % (H, W))
+        a = self.arch
+        x = torch.zeros(1, 3, H, W, dtype=torch.float32, device=self.dev)
+        pos = self.parse_pos(x)
+        h, feats, _ = self.encoder_frames(x)
+        ring = {'pos': self._new(3, *pos.shape), 'h': self._new(3, *h.shape[1:]), 'feats': {}}
+        gn = getattr(h, '_pgt_gn', None)
+        if gn is not None:                       # [frame][32-row chunk][32 groups][2]
+            ring['h_stats'] = self._new(3, gn[1] * 64, dtype=torch.float32)
+        if float(w) > 0:
+            ring['feats'] = {lvl: self._new(3, *f.shape[1:]) for lvl, f in feats.items() if lvl in a.fuse_level_key}
+        return ring
+
+    @_on_device
+    @torch.no_grad()
+    def frame_step(self, x1, slot, ring):
+        """The per-frame work of one fp32 frame x1 [1,3,H,W] — parse_pos and encoder_frames — written into slot `slot`
+        of ring (live_ring) by the producing kernels themselves."""
+        a = self.arch
+        self.parse_pos(x1, out=ring['pos'][slot])
+        h = ring['h'][slot:slot + 1]
+        if 'h_stats' in ring:
+            h._pgt_gn_into = ring['h_stats'][slot]
+        outs = {a.frame_blocks - 1: h}
+        outs.update({i: ring['feats'][lvl][slot:slot + 1] for i, lvl in a.enc_taps.items() if lvl in ring['feats']})
+        self.encoder_frames(x1, outs)
+
+    @_on_device
+    @torch.no_grad()
+    def window_step(self, index3, w, adain, ring, out_u8):
+        """The window (f[i-1], f[i], f[i+1]) restored from ring slots index3 (device int32 [3]): the ring's entries
+        gathered into clip order (pgt_gather_frames), then forward from encoder_clips on, exactly as
+        forward(frame_index=index3) computes it.  Writes the middle frame into out_u8 (rgb24 [1,H,W,3] uint8)."""
+        a = self.arch
+        pos = self._gather(ring['pos'], index3)
+        h = ring['h']
+        if 'h_stats' in ring:
+            h = h.view(h.shape)
+            h._pgt_gn = (ring['h_stats'].view(-1), ring['h_stats'].shape[1] // 64)
+        feats = {lvl: self._gather(ring['feats'][lvl], index3) if lvl in ring['feats'] else None
+                 for i, lvl in a.enc_taps.items() if i < a.frame_blocks}
+        h, feats = self.encoder_clips(self._gather(h, index3), feats, a.frame_blocks)
+        out = self._restore(h, feats, pos.view(-1, pos.shape[-1]), w, adain)[0]
+        return ops.f32nchw_to_u8hwc(out, out_u8, first=1, step=3)
 
     # ------------------------------------------------------------------ stage-I codec (TDCRQVAE3 methods)
     def _codebook(self, d=0):

@@ -13,6 +13,9 @@ at the ends — one window per model call, and keeps `clamp(out[0][1], 0, 1) * 2
 
 The ffmpeg pipes themselves stay in the caller's script (SURVEY section 7): `stream()` takes any iterator of rgb24
 frames and yields rgb24 frames, which is exactly what the reference's pipe loop reads and writes.
+
+`LiveRestorer` is the same loop for a source that delivers frames one at a time: each push returns the previous frame,
+each frame's per-frame work runs once into a device ring, and every step can replay from a CUDA graph.
 """
 import numpy as np
 import torch
@@ -36,32 +39,27 @@ def plan_batches(n, clips_per_batch):
 
 
 class VideoRestorer:
-    def __init__(self, model, w=1.0, adain=True, clips_per_batch=16, reuse_frames=True):
+    def __init__(self, model, w=1.0, adain=True, clips_per_batch=16, reuse_frames=True, cuda_graph=False):
+        """cuda_graph: replay each batch from a CUDA graph (Engine.graphed, one per batch shape), which removes the
+        host cost of its launches; the bytes written are the eager ones."""
         self.model = model
         self.w = float(w)
         self.adain = bool(adain)
         self.clips_per_batch = int(clips_per_batch)
         self.reuse_frames = bool(reuse_frames)
+        self.cuda_graph = bool(cuda_graph)
 
     # ------------------------------------------------------------------ one batch of windows on the device
     def _enqueue(self, frames_u8_dev, local_windows):
         """frames_u8_dev: uint8 [Fd,H,W,3] on the device (distinct frames lo..hi); local_windows: [(a,b,c)] indices
-        into it.  Returns uint8 [count,H,W,3] on the device (the restored middle frames)."""
+        into it.  Returns uint8 [count,H,W,3] on the device (the restored middle frames; with cuda_graph, the graph's
+        static output, to be consumed before the next batch)."""
         eng = self.model.engine()
-        Fd, H, W, _ = frames_u8_dev.shape
-        with torch.cuda.device(eng.dev):
-            return self._enqueue_on_device(eng, frames_u8_dev, local_windows, Fd, H, W)
-
-    def _enqueue_on_device(self, eng, frames_u8_dev, local_windows, Fd, H, W):
-        x = ops.u8hwc_to_f32nchw(frames_u8_dev, torch.empty(Fd, 3, H, W, dtype=torch.float32, device=frames_u8_dev.device))
-        idx = torch.tensor([j for win in local_windows for j in win], dtype=torch.int32).to(x.device, non_blocking=True)
-        if self.reuse_frames:
-            out = eng.forward(x, w=self.w, adain=self.adain, frame_index=idx)[0]
-        else:
-            xc = ops.gather_frames(x, idx, torch.empty(idx.numel(), 3, H, W, dtype=torch.float32, device=x.device))
-            out = eng.forward(xc, w=self.w, adain=self.adain)[0]
-        n = len(local_windows)
-        return ops.f32nchw_to_u8hwc(out, torch.empty(n, H, W, 3, dtype=torch.uint8, device=x.device), first=1, step=3)
+        idx = torch.tensor([j for win in local_windows for j in win], dtype=torch.int32).to(eng.dev, non_blocking=True)
+        if self.cuda_graph:
+            return eng.graphed(eng.restore_windows, (frames_u8_dev, idx), w=self.w, adain=self.adain,
+                               reuse_frames=self.reuse_frames)
+        return eng.restore_windows(frames_u8_dev, idx, w=self.w, adain=self.adain, reuse_frames=self.reuse_frames)
 
     def _run_batch(self, frames_u8, local_windows):
         """Host uint8 [Fd,H,W,3] + window index triples -> host uint8 [count,H,W,3] (synchronous; `stream()` uses it)."""
@@ -98,17 +96,23 @@ class VideoRestorer:
             return d, ev, host
 
         staged = stage(0)
+        copied = None
         for b, (first, cnt, lo, hi) in enumerate(plan):
             d, ev, _keep = staged
             staged = stage(b + 1) if b + 1 < len(plan) else None     # H2D of the next batch overlaps this compute
             main.wait_event(ev)
+            if self.cuda_graph and copied is not None:
+                main.wait_event(copied)                              # a replay rewrites the static output being copied
             res = self._enqueue(d, [tuple(j - lo for j in wins[i]) for i in range(first, first + cnt)])
             done = torch.cuda.Event()
             done.record(main)
             with torch.cuda.stream(copy):                            # D2H overlaps the next batch's compute
                 copy.wait_event(done)
                 out[first:first + cnt].copy_(res, non_blocking=True)
-            res.record_stream(copy)                                  # the allocator keeps `res` until the copy has run
+                copied = torch.cuda.Event()
+                copied.record(copy)
+            if not self.cuda_graph:
+                res.record_stream(copy)                              # the allocator keeps `res` until the copy has run
             d.record_stream(main)
         copy.synchronize()
         main.synchronize()
@@ -147,3 +151,204 @@ class VideoRestorer:
             if drop > 0:
                 del buf[:drop]
                 base += drop
+
+
+def _check_frame(frame, hw):
+    """A live frame, checked on the host: rgb24 [H,W,3] uint8 (numpy, or a host or CUDA torch tensor) with H and W
+    multiples of 64, and of the stream's size hw unless hw is None.  Returns it as a torch tensor or a numpy array."""
+    t = frame if torch.is_tensor(frame) else np.asarray(frame)
+    u8 = t.dtype == (torch.uint8 if torch.is_tensor(t) else np.uint8)
+    if not u8 or t.ndim != 3 or t.shape[-1] != 3:
+        raise ValueError('expected an rgb24 frame [H,W,3] uint8, got %s %s' % (tuple(t.shape), t.dtype))
+    H, W = int(t.shape[0]), int(t.shape[1])
+    if H % 64 or W % 64 or H == 0 or W == 0:
+        raise ValueError('expected H, W multiples of 64, got %dx%d' % (H, W))
+    if hw is not None and (H, W) != hw:
+        raise ValueError('frame size changed inside a stream: %dx%d after %dx%d' % ((H, W) + hw))
+    return t
+
+
+class _LiveSession:
+    """The device state of a LiveRestorer on one engine and frame size: the engine's ring of per-frame results
+    (Engine.live_ring), the rgb24 frames that produced them (u8[j % 3] holds frame j), the output frame, pinned host
+    buffers and, with cuda_graph, the captured steps.
+
+    A step is (slot s of the new frame or None, ring slots of the window or None): u8[s] -> fp32 -> frame_step into
+    ring slot s, then window_step -> out.  With cuda_graph each distinct step is captured once and replayed: every
+    address it touches (u8, ring, the window's index tensor, out) is allocated outside the graphs, so the ring carries
+    from one replay to the next.  One graph per step rather than one graph rotating through a device slot index: the
+    producing kernels write straight into the new frame's ring slot, which a kernel argument baked into a single graph
+    could not follow without one more copy of the slot per frame.  A stream uses at most 8 steps (3 steady phases, the
+    first frame, the first window, the 3 last windows or the single frame's), and all of them share one memory pool,
+    replayed one at a time on one stream, so their scratch costs one step's worth."""
+
+    def __init__(self, eng, H, W, w, adain, cuda_graph):
+        self.eng, self.hw, self.w, self.adain, self.cuda_graph = eng, (H, W), w, adain, cuda_graph
+        dev = eng.dev
+        with torch.cuda.device(dev):
+            self.ring = eng.live_ring(H, W, w)
+            self.u8 = torch.empty(3, H, W, 3, dtype=torch.uint8, device=dev)
+            self.x = torch.empty(1, 3, H, W, dtype=torch.float32, device=dev)
+            self.out = torch.empty(1, H, W, 3, dtype=torch.uint8, device=dev)
+        self.host_in = torch.empty(H, W, 3, dtype=torch.uint8).pin_memory()
+        self.host_out = torch.empty(H, W, 3, dtype=torch.uint8).pin_memory()
+        self.loaded = None                 # event: host_in has reached the device and may be overwritten
+        self.index = {}                    # window slots -> device int32 [3]
+        self.graphs = {}
+        self.pool = None
+
+    def load(self, t, slot):
+        """Frame t (uint8 [H,W,3], host or CUDA) into u8[slot] on the current stream."""
+        if torch.is_tensor(t) and t.is_cuda:
+            self.u8[slot].copy_(t, non_blocking=True)
+            return
+        if self.loaded is not None:
+            self.loaded.synchronize()      # the previous frame's H2D (its step needs no synchronisation of its own)
+        self.host_in.numpy()[...] = t.numpy() if torch.is_tensor(t) else t
+        self.u8[slot].copy_(self.host_in, non_blocking=True)
+        self.loaded = torch.cuda.Event()
+        self.loaded.record()
+
+    def _run(self, slot, win):
+        eng = self.eng
+        if slot is not None:
+            ops.u8hwc_to_f32nchw(self.u8[slot:slot + 1], self.x)
+            eng.frame_step(self.x, slot, self.ring)
+        if win is not None:
+            eng.window_step(self.index[win], self.w, self.adain, self.ring, self.out)
+
+    def step(self, slot, win):
+        """Runs one step; with a window, returns the restored frame as numpy uint8 [H,W,3] (the one synchronisation)."""
+        if win is not None and win not in self.index:
+            self.index[win] = torch.tensor(win, dtype=torch.int32).to(self.eng.dev)
+        if not self.cuda_graph:
+            self._run(slot, win)
+        else:
+            graph = self.graphs.get((slot, win))
+            if graph is None:
+                graph = self._capture(slot, win)
+            graph.replay()
+        if win is None:
+            return None
+        self.host_out.copy_(self.out[0], non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+        done.synchronize()
+        return self.host_out.numpy().copy()
+
+    def _capture(self, slot, win):
+        """Engine.graphed's warm-up (twice on a side stream: the lazy one-time set-up), then the capture, on the
+        engine's capture stream, into the session's pool.  The step's writes are idempotent, so the warm-up runs do not
+        disturb the ring."""
+        eng = self.eng
+        cur = torch.cuda.current_stream(eng.dev)
+        side = torch.cuda.Stream(device=eng.dev)
+        side.wait_stream(cur)
+        try:
+            with torch.cuda.stream(side):
+                for _ in range(2):
+                    self._run(slot, win)
+        finally:
+            cur.wait_stream(side)
+        if not hasattr(eng, 'capture_stream'):
+            eng.capture_stream = torch.cuda.Stream(device=eng.dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=self.pool, stream=eng.capture_stream):
+            self._run(slot, win)
+        self.pool = graph.pool() if self.pool is None else self.pool
+        self.graphs[slot, win] = graph
+        return graph
+
+
+class LiveRestorer:
+    """Restores a live video one frame behind its input: push(f[i+1]) returns frame i, restored from the window
+    (f[i-1], f[i], f[i+1]) of the reference's loop (window_indices), byte for byte what VideoRestorer.restore gives.
+
+    Each frame's per-frame work (BiSeNet, the frame blocks of the encoder) runs once, when it is pushed, into a ring of
+    three slots on the device; each window is gathered from the ring.  Frames are rgb24 [H,W,3] uint8 — numpy, a host
+    torch tensor or a CUDA tensor on the model's device — with H and W multiples of 64; outputs are numpy uint8.  With
+    cuda_graph every step replays from a CUDA graph (_LiveSession).  The device state belongs to the model's current
+    engine: after load_state_dict(), .to() or refresh() the next call rebuilds it, re-running the per-frame work of the
+    frames still in the window on the new weights.
+
+        live = LiveRestorer(model)
+        live.push(f0)     # None
+        live.push(f1)     # frame 0, window (0, 0, 1)
+        live.push(f2)     # frame 1, window (0, 1, 2)
+        live.flush()      # frame 2, window (1, 2, 2); then ready for a new stream
+    """
+
+    def __init__(self, model, w=1.0, adain=True, cuda_graph=True):
+        self.model = model
+        self.w = float(w)
+        self.adain = bool(adain)
+        self.cuda_graph = bool(cuda_graph)
+        self._sess = None
+        self.reset()
+
+    def reset(self):
+        """Forgets the current stream (its frames); the next push starts a new one, of any frame size."""
+        self._n = 0            # frames pushed in this stream
+        self._hw = None
+
+    # ------------------------------------------------------------------ schedule (host only)
+    @torch.no_grad()
+    def push(self, frame):
+        """Frame n of the stream in; restored frame n - 1 out (None for n = 0)."""
+        t = _check_frame(frame, self._hw)
+        if torch.is_tensor(t) and t.is_cuda and t.device != next(self.model.parameters()).device:
+            raise ValueError('frame on %s, model on %s' % (t.device, next(self.model.parameters()).device))
+        n = self._n
+        new = n % 3
+        win = None if n == 0 else (max(n - 2, 0), n - 1, n)
+        out = self._step(t, n, new, win)
+        self._n, self._hw = n + 1, (int(t.shape[0]), int(t.shape[1]))
+        return out
+
+    @torch.no_grad()
+    def flush(self):
+        """The last frame of the stream, restored from (f[n-2], f[n-1], f[n-1]) — (f0, f0, f0) for a single frame;
+        None for an empty stream.  Then ready for a new stream."""
+        n = self._n
+        try:
+            return None if n == 0 else self._step(None, n, None, (max(n - 2, 0), n - 1, n - 1))
+        finally:
+            self.reset()
+
+    def stream(self, frames):
+        """Yields restored frame i as soon as frame i + 1 (or the end of `frames`) is known."""
+        self.reset()
+        for f in frames:
+            out = self.push(f)
+            if out is not None:
+                yield out
+        out = self.flush()
+        if out is not None:
+            yield out
+
+    # ------------------------------------------------------------------ device
+    def _session(self, hw, n):
+        """The session of the model's current engine for frames of size hw; one built after the weights changed
+        mid-stream first recomputes the ring from the frames it still holds."""
+        eng = self.model.engine()
+        H, W = hw
+        old = self._sess
+        if old is not None and old.eng is eng and old.hw == (H, W):
+            return old
+        self._sess = None
+        sess = _LiveSession(eng, H, W, self.w, self.adain, self.cuda_graph)
+        if old is not None and n > 0:                # weights or device changed inside the stream
+            with torch.cuda.device(eng.dev):
+                sess.u8.copy_(old.u8)
+                for j in range(max(n - 2, 0), n):
+                    sess._run(j % 3, None)
+        self._sess = sess
+        return sess
+
+    def _step(self, t, n, new, win):
+        """t: frame n (or None at flush) going into ring slot `new`; win: frame indices of the window to restore."""
+        sess = self._session(self._hw if t is None else (int(t.shape[0]), int(t.shape[1])), n)
+        with torch.cuda.device(sess.eng.dev):
+            if t is not None:
+                sess.load(t, new)
+            return sess.step(new, None if win is None else tuple(j % 3 for j in win))
