@@ -199,16 +199,14 @@ class Engine:
         last column of tiles would add rows past the frame's edge to the statistics (pgt_conv_tiles_exact)."""
         return ops.conv_tiles_exact(H, W, cout, ksize, stride, pad_lo)
 
-    def _gn_stats(self, out, chunks_per_frame):
+    def _gn_stats(self, out, chunks_per_frame, into=None):
         """The next GroupNorm's statistics, filled by the epilogue that writes `out` (saves that GroupNorm a pass over
-        the tensor): allocates the fp32 buffer [frame][chunk][32 groups][2], attaches it as out._pgt_gn and returns it
-        for the producer's gn_stats.  None, with nothing attached, when out's channel count has no fused statistics,
-        out is not contiguous or chunks_per_frame (32-row chunks per frame, 4 per 128-row tile) is 0."""
+        the tensor): the fp32 buffer [frame][chunk][32 groups][2] (`into`, or a new one), attached as out._pgt_gn and
+        returned for the producer's gn_stats.  None, with nothing attached, when out's channel count has no fused
+        statistics, out is not contiguous or chunks_per_frame (32-row chunks per frame, 4 per 128-row tile) is 0."""
         if chunks_per_frame <= 0 or not ops.gn_stats_supported(out.shape[-1]) or not out.is_contiguous():
             return None
-        stats = getattr(out, '_pgt_gn_into', None)              # a live ring slot keeps them beside its features
-        if stats is None:
-            stats = self._new(out.shape[0] * chunks_per_frame * 64, dtype=torch.float32)
+        stats = self._new(out.shape[0] * chunks_per_frame * 64, dtype=torch.float32) if into is None else into
         assert stats.numel() == out.shape[0] * chunks_per_frame * 64
         out._pgt_gn = (stats, chunks_per_frame)
         return stats
@@ -220,9 +218,10 @@ class Engine:
                                              silu=silu)
         return ops.groupnorm_silu(x, self.w[p + '.weight'], self.w[p + '.bias'], self._new(*x.shape), silu=silu)
 
-    def _conv3(self, x, p, cout, out=None, gn_out=False, gn=None, gn_silu=True, **kw):
+    def _conv3(self, x, p, cout, out=None, gn_out=False, gn=None, gn_silu=True, gn_into=None, **kw):
         """3x3 conv; gn: name of the Normalize() that precedes it, run as a separate pass: GroupNorm, then SiLU unless
-        gn_silu=False (VQGAN's encoder tail).  gn_out: the epilogue also emits the next GroupNorm's statistics."""
+        gn_silu=False (VQGAN's encoder tail).  gn_out: the epilogue also emits the next GroupNorm's statistics, into
+        gn_into when given."""
         Fr, H, W, _ = x.shape
         stride = kw.get('stride', 1)
         if gn is not None:
@@ -231,7 +230,8 @@ class Engine:
             out = self._new(Fr, H // stride, W // stride, cout)
         stats = None
         if gn_out:
-            stats = self._gn_stats(out, 4 * self._stats_tiles(H, W, cout, kw.get('ksize', 3), stride, kw.get('pad_lo', 1)))
+            stats = self._gn_stats(out, 4 * self._stats_tiles(H, W, cout, kw.get('ksize', 3), stride, kw.get('pad_lo', 1)),
+                                   gn_into)
         return ops.conv(x, self.w[p + '.weight'], cout, out, bias=self.w.get(p + '.bias'), gn_stats=stats, **kw)
 
     def _lin(self, x, p, n, out=None, out_dtype=BF, gn_out=False, **kw):
@@ -445,11 +445,12 @@ class Engine:
         return ops.assemble_cond(o0, o1, o2, self._new(Fr, H // 16, W // 16, 64))
 
     # ------------------------------------------------------------------ encoder / decoder
-    def _walk(self, blocks, h, lo=0, hi=None, taps=None, outs=None, feats=None, wgt=0.0):
+    def _walk(self, blocks, h, lo=0, hi=None, taps=None, outs=None, feats=None, wgt=0.0, gn_outs=None):
         """Runs blocks[lo:hi] of a block list (spec.Block entries) on h.  Returns (h, {taps[i]: output of block i}).
         outs {i: tensor}: block i (`res`, `swin` or `down`) writes its output there, a slice of an SFT concat buffer or a
-        slot of a live ring (live_ring).  A `fuse`
-        block runs only with feats and wgt > 0, on feats[its src].
+        slot of a live ring (live_ring); gn_outs {i: fp32 buffer}: block i (`down`, the last of the frame blocks) writes
+        the GroupNorm statistics it emits for the next block there.  A `fuse` block runs only with feats and wgt > 0, on
+        feats[its src].
 
         GroupNorm statistics: a block passes gn_next to its producer exactly when the next block that runs reads its
         input through a GroupNorm (`res`, `attn`, or the `norm` before conv_out); a `fuse` that does not run is not
@@ -457,7 +458,7 @@ class Engine:
         RGB conv_in and `up`, always followed by a `res`, always write them.)"""
         fusing = feats is not None and wgt > 0
         hi = len(blocks) if hi is None else hi
-        outs, found = outs or {}, {}
+        outs, gn_outs, found = outs or {}, gn_outs or {}, {}
         for i in range(lo, hi):
             blk = blocks[i]
             kind, p, cout = blk.kind, blk.prefix, blk.cout
@@ -473,7 +474,8 @@ class Engine:
             elif kind == 'swin':
                 h = self.encoder_layer(h, p, blk.heads, blk.depth, gn_next=nxt, out=outs.get(i))
             elif kind == 'down':
-                h = self._conv3(h, p + '.conv', cout, stride=2, pad_lo=0, gn_out=nxt, out=outs.get(i))
+                h = self._conv3(h, p + '.conv', cout, stride=2, pad_lo=0, gn_out=nxt, out=outs.get(i),
+                                gn_into=gn_outs.get(i))
             elif kind == 'up':
                 h = self.up2x(h, p + '.conv')
             elif kind == 'fuse':
@@ -491,12 +493,12 @@ class Engine:
         half._pgt_cat = cat
         return half
 
-    def encoder_frames(self, x, outs=None):
+    def encoder_frames(self, x, outs=None, gn_outs=None):
         """The per-frame prefix of Encoder.forward (`archs/tdcrqvae3_arch.py:540-560`): conv_in and every level before
         the first one with attention, including the Downsample into it — nothing here looks across frames, so the
         streaming pipeline runs it once per distinct frame.  Returns (h, {level: output}, index of the next block)."""
         a = self.arch
-        h, feats = self._walk(a.enc_blocks, x, 0, a.frame_blocks, a.enc_taps, outs)
+        h, feats = self._walk(a.enc_blocks, x, 0, a.frame_blocks, a.enc_taps, outs, gn_outs=gn_outs)
         return h, feats, a.frame_blocks
 
     def conv_in(self, x, p='encoder.conv_in'):
@@ -532,13 +534,8 @@ class Engine:
         return self.encoder_clips(*self.encoder_frames(x, outs), outs)
 
     def _gather(self, t, idx):
-        """t[idx] along the frame dimension, GroupNorm statistics included."""
-        out = ops.gather_frames(t, idx, self._new(idx.numel(), *t.shape[1:], dtype=t.dtype))
-        gn = getattr(t, '_pgt_gn', None)
-        if gn is not None:
-            st = gn[0].view(t.shape[0], -1)
-            out._pgt_gn = (ops.gather_frames(st, idx, self._new(idx.numel(), st.shape[1], dtype=st.dtype)).view(-1), gn[1])
-        return out
+        """t[idx] along the frame dimension."""
+        return ops.gather_frames(t, idx, self._new(idx.numel(), *t.shape[1:], dtype=t.dtype))
 
     def decoder(self, z, feats=None, wgt=0.0):
         """Decoder.forward (`archs/tdcrqvae3_arch.py:672-707`) / the inlined variant with SFT fusion
@@ -623,19 +620,52 @@ class Engine:
             Fr = frame_index.numel()
         if Fr % a.tf != 0 or H % 64 != 0 or W % 64 != 0:
             raise ValueError('expected b*3 frames with H, W multiples of 64, got %s' % (tuple(x.shape),))
-        T = Fr * (H // 16) * (W // 16)
+        if frame_index is not None:
+            return self._window_tail(self._frame_pass(x, w), frame_index, w, adain, code_only, force_codes)
         pos = self.parse_pos(x)
-        # encoder
-        if frame_index is None:
-            h, feats = self.encoder(x, fusing=not code_only and float(w) > 0)
-        else:
-            pos = self._gather(pos.view(x.shape[0], -1), frame_index).view(T, -1)
-            h, feats, i = self.encoder_frames(x)
-            # only the skip tensors the SFT fusion will read are worth moving (level 0 is 100 MB per clip and unused)
-            feats = {lvl: self._gather(f, frame_index) if (lvl in a.fuse_level_key and w > 0) else f
-                     for lvl, f in feats.items()}
-            h, feats = self.encoder_clips(self._gather(h, frame_index), feats, i)
+        h, feats = self.encoder(x, fusing=not code_only and float(w) > 0)
         return self._restore(h, feats, pos, w, adain, code_only, force_codes)
+
+    def _frame_pass(self, x, w=0.0, ring=None, slot=0):
+        """The per-frame work — parse_pos and encoder_frames — of distinct fp32 frames x [n,3,H,W], as their per-frame
+        record: {'pos': convpos rows [n, T/n, 512], 'h': the frame blocks' output [n, ...], 'h_stats': the GroupNorm
+        statistics [n, chunks * 64] h's producer writes for the next block (when it writes any), 'feats': {level:
+        [n, ...]}, for w > 0 the skip tensors of the per-frame levels the SFT fusion reads (the others are never moved:
+        level 0 is 100 MB per clip and unused)}.  With ring (live_ring: the record of three frames) x is one frame, its
+        producers write straight into slot `slot` of ring, and the levels kept are those the ring has room for."""
+        a = self.arch
+        last, n = a.frame_blocks - 1, x.shape[0]
+        outs, gn_outs = {}, {}
+        if ring is None:
+            levels = list(a.fuse_level_key) if float(w) > 0 else []
+        else:
+            levels = list(ring['feats'])
+            outs = {i: ring['feats'][lvl][slot:slot + 1] for i, lvl in a.enc_taps.items() if lvl in levels}
+            outs[last] = ring['h'][slot:slot + 1]
+            if 'h_stats' in ring:
+                gn_outs[last] = ring['h_stats'][slot]
+        pos = self.parse_pos(x, out=None if ring is None else ring['pos'][slot])
+        h, feats, _ = self.encoder_frames(x, outs, gn_outs)
+        rec = {'pos': pos.view(n, -1, pos.shape[-1]), 'h': h,
+               'feats': {lvl: f for lvl, f in feats.items() if lvl in levels}}
+        gn = getattr(h, '_pgt_gn', None)
+        if gn is not None:
+            rec['h_stats'] = gn[0].view(n, -1)
+        return rec
+
+    def _window_tail(self, rec, index, w, adain, code_only=False, force_codes=None):
+        """forward from a per-frame record (_frame_pass, live_ring) on: its entries gathered into clip order by the
+        device int32 window index [b*3] (pgt_gather_frames), h's GroupNorm statistics beside h, then encoder_clips and
+        _restore, whose result it returns."""
+        a = self.arch
+        pos = self._gather(rec['pos'], index)
+        feats = {lvl: self._gather(rec['feats'][lvl], index) if lvl in rec['feats'] else None
+                 for i, lvl in a.enc_taps.items() if i < a.frame_blocks}
+        h = self._gather(rec['h'], index)
+        if 'h_stats' in rec:
+            h._pgt_gn = (self._gather(rec['h_stats'], index).view(-1), rec['h_stats'].shape[1] // 64)
+        h, feats = self.encoder_clips(h, feats, a.frame_blocks)
+        return self._restore(h, feats, pos.view(-1, pos.shape[-1]), w, adain, code_only, force_codes)
 
     def _restore(self, h, feats, pos, w, adain, code_only=False, force_codes=None):
         """forward from the encoder's output h [F,h,w,C] on: quant_conv -> global transformer -> argmax (or
@@ -691,39 +721,46 @@ class Engine:
         whose warm-up raises stores nothing.
 
         A graph here is a pure function of its inputs.  The live steps (video.LiveRestorer), whose ring of per-frame
-        results persists across replays, are captured by their session instead: one graph per ring phase, all in one
-        memory pool, because each step's producers write straight into the new frame's ring slot (video._LiveSession)."""
+        results persists across replays, are captured by their session through _capture too, but all in one memory
+        pool: one graph per ring phase, because each step's producers write straight into the new frame's ring slot
+        (video._LiveSession)."""
         tensors = [t.to(self.dev) for t in tensors]
         key = (method.__name__, tuple((tuple(t.shape), t.dtype) for t in tensors), tuple(sorted(scalars.items())))
         if not hasattr(self, '_graphs'):
             self._graphs = {}
-            self.capture_stream = torch.cuda.Stream(device=self.dev)
         entry = self._graphs.get(key)
         if entry is None:
             static = [torch.empty(t.shape, dtype=t.dtype, device=self.dev) for t in tensors]
             for s, t in zip(static, tensors):
                 s.copy_(t)
-            cur = torch.cuda.current_stream(self.dev)
-            side = torch.cuda.Stream(device=self.dev)
-            side.wait_stream(cur)
-            try:
-                with torch.cuda.stream(side):
-                    for _ in range(2):
-                        method(*static, **scalars)
-            finally:
-                cur.wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph, stream=self.capture_stream):
-                outs = method(*static, **scalars)
-            entry = (graph, static, outs)
-            self._graphs[key] = entry
-        graph, static, outs = entry
+            entry = self._graphs[key] = (static,) + self._capture(lambda: method(*static, **scalars))
+        static, graph, outs = entry
         for s, t in zip(static, tensors):
             s.copy_(t, non_blocking=True)
         graph.replay()
         for i in writes:
             tensors[i].copy_(static[i], non_blocking=True)
         return outs
+
+    def _capture(self, run, pool=None):
+        """(graph, what run() returned in it): run() twice on a side stream (the lazy one-time set-up: kernel
+        attributes, constant tables, codebook packs, workspaces), then captured as a CUDA graph on this engine's
+        capture stream, on its device, into `pool` (None: a memory pool of the graph's own)."""
+        if not hasattr(self, 'capture_stream'):
+            self.capture_stream = torch.cuda.Stream(device=self.dev)
+        cur = torch.cuda.current_stream(self.dev)
+        side = torch.cuda.Stream(device=self.dev)
+        side.wait_stream(cur)
+        try:
+            with torch.cuda.stream(side):
+                for _ in range(2):
+                    run()
+        finally:
+            cur.wait_stream(side)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, pool=pool, stream=self.capture_stream):
+            out = run()
+        return graph, out
 
     def forward_graphed(self, x, w=1.0, adain=True):
         """forward replayed from a CUDA graph captured once per (shape, w, adain) (graphed): removes the ~700
@@ -751,23 +788,14 @@ class Engine:
     @_on_device
     @torch.no_grad()
     def live_ring(self, H, W, w):
-        """The per-frame results of three frames, one slot each, for frame_step / window_step: {'pos': convpos rows
-        [3, T/3, 512], 'h': the frame blocks' output [3, ...] (with 'h_stats', the GroupNorm statistics its producer
-        writes for the next block, when it writes any), and for w > 0 'feats': {level: [3, ...]}, the skip tensors of
-        the per-frame levels the SFT fusion reads}.  Allocated here, outside any graph's memory pool, so that graphs
-        captured later can all write and read the same addresses.  Shapes are those of one run of the per-frame work."""
+        """The per-frame record (_frame_pass) of three frames, one slot each, for frame_step / window_step.  Allocated
+        here, outside any graph's memory pool, so that graphs captured later can all write and read the same
+        addresses.  Shapes are those of one run of the per-frame work."""
         if H % 64 or W % 64:
             raise ValueError('expected H, W multiples of 64, got %dx%d' % (H, W))
-        a = self.arch
-        x = torch.zeros(1, 3, H, W, dtype=torch.float32, device=self.dev)
-        pos = self.parse_pos(x)
-        h, feats, _ = self.encoder_frames(x)
-        ring = {'pos': self._new(3, *pos.shape), 'h': self._new(3, *h.shape[1:]), 'feats': {}}
-        gn = getattr(h, '_pgt_gn', None)
-        if gn is not None:                       # [frame][32-row chunk][32 groups][2]
-            ring['h_stats'] = self._new(3, gn[1] * 64, dtype=torch.float32)
-        if float(w) > 0:
-            ring['feats'] = {lvl: self._new(3, *f.shape[1:]) for lvl, f in feats.items() if lvl in a.fuse_level_key}
+        rec = self._frame_pass(torch.zeros(1, 3, H, W, dtype=torch.float32, device=self.dev), w)
+        ring = {k: self._new(3, *t.shape[1:], dtype=t.dtype) for k, t in rec.items() if k != 'feats'}
+        ring['feats'] = {lvl: self._new(3, *f.shape[1:], dtype=f.dtype) for lvl, f in rec['feats'].items()}
         return ring
 
     @_on_device
@@ -775,31 +803,14 @@ class Engine:
     def frame_step(self, x1, slot, ring):
         """The per-frame work of one fp32 frame x1 [1,3,H,W] — parse_pos and encoder_frames — written into slot `slot`
         of ring (live_ring) by the producing kernels themselves."""
-        a = self.arch
-        self.parse_pos(x1, out=ring['pos'][slot])
-        h = ring['h'][slot:slot + 1]
-        if 'h_stats' in ring:
-            h._pgt_gn_into = ring['h_stats'][slot]
-        outs = {a.frame_blocks - 1: h}
-        outs.update({i: ring['feats'][lvl][slot:slot + 1] for i, lvl in a.enc_taps.items() if lvl in ring['feats']})
-        self.encoder_frames(x1, outs)
+        self._frame_pass(x1, ring=ring, slot=slot)
 
     @_on_device
     @torch.no_grad()
     def window_step(self, index3, w, adain, ring, out_u8):
-        """The window (f[i-1], f[i], f[i+1]) restored from ring slots index3 (device int32 [3]): the ring's entries
-        gathered into clip order (pgt_gather_frames), then forward from encoder_clips on, exactly as
+        """The window (f[i-1], f[i], f[i+1]) restored from ring slots index3 (device int32 [3]), exactly as
         forward(frame_index=index3) computes it.  Writes the middle frame into out_u8 (rgb24 [1,H,W,3] uint8)."""
-        a = self.arch
-        pos = self._gather(ring['pos'], index3)
-        h = ring['h']
-        if 'h_stats' in ring:
-            h = h.view(h.shape)
-            h._pgt_gn = (ring['h_stats'].view(-1), ring['h_stats'].shape[1] // 64)
-        feats = {lvl: self._gather(ring['feats'][lvl], index3) if lvl in ring['feats'] else None
-                 for i, lvl in a.enc_taps.items() if i < a.frame_blocks}
-        h, feats = self.encoder_clips(self._gather(h, index3), feats, a.frame_blocks)
-        out = self._restore(h, feats, pos.view(-1, pos.shape[-1]), w, adain)[0]
+        out = self._window_tail(ring, index3, w, adain)[0]
         return ops.f32nchw_to_u8hwc(out, out_u8, first=1, step=3)
 
     # ------------------------------------------------------------------ stage-I codec (TDCRQVAE3 methods)

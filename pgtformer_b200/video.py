@@ -174,13 +174,13 @@ class _LiveSession:
     buffers and, with cuda_graph, the captured steps.
 
     A step is (slot s of the new frame or None, ring slots of the window or None): u8[s] -> fp32 -> frame_step into
-    ring slot s, then window_step -> out.  With cuda_graph each distinct step is captured once and replayed: every
-    address it touches (u8, ring, the window's index tensor, out) is allocated outside the graphs, so the ring carries
-    from one replay to the next.  One graph per step rather than one graph rotating through a device slot index: the
-    producing kernels write straight into the new frame's ring slot, which a kernel argument baked into a single graph
-    could not follow without one more copy of the slot per frame.  A stream uses at most 8 steps (3 steady phases, the
-    first frame, the first window, the 3 last windows or the single frame's), and all of them share one memory pool,
-    replayed one at a time on one stream, so their scratch costs one step's worth."""
+    ring slot s, then window_step -> out.  With cuda_graph each distinct step is captured once (Engine._capture) and
+    replayed: every address it touches (u8, ring, the window's index tensor, out) is allocated outside the graphs, so
+    the ring carries from one replay to the next.  One graph per step rather than one graph rotating through a device
+    slot index: the producing kernels write straight into the new frame's ring slot, which a kernel argument baked into
+    a single graph could not follow without one more copy of the slot per frame.  A stream uses at most 8 steps (3
+    steady phases, the first frame, the first window, the 3 last windows or the single frame's), and all of them share
+    one memory pool, replayed one at a time on one stream, so their scratch costs one step's worth."""
 
     def __init__(self, eng, H, W, w, adain, cuda_graph):
         self.eng, self.hw, self.w, self.adain, self.cuda_graph = eng, (H, W), w, adain, cuda_graph
@@ -225,8 +225,9 @@ class _LiveSession:
             self._run(slot, win)
         else:
             graph = self.graphs.get((slot, win))
-            if graph is None:
-                graph = self._capture(slot, win)
+            if graph is None:                  # the step's writes are idempotent: its warm-up runs leave the ring as is
+                graph = self.graphs[slot, win] = self.eng._capture(lambda: self._run(slot, win), self.pool)[0]
+                self.pool = graph.pool() if self.pool is None else self.pool
             graph.replay()
         if win is None:
             return None
@@ -235,29 +236,6 @@ class _LiveSession:
         done.record()
         done.synchronize()
         return self.host_out.numpy().copy()
-
-    def _capture(self, slot, win):
-        """Engine.graphed's warm-up (twice on a side stream: the lazy one-time set-up), then the capture, on the
-        engine's capture stream, into the session's pool.  The step's writes are idempotent, so the warm-up runs do not
-        disturb the ring."""
-        eng = self.eng
-        cur = torch.cuda.current_stream(eng.dev)
-        side = torch.cuda.Stream(device=eng.dev)
-        side.wait_stream(cur)
-        try:
-            with torch.cuda.stream(side):
-                for _ in range(2):
-                    self._run(slot, win)
-        finally:
-            cur.wait_stream(side)
-        if not hasattr(eng, 'capture_stream'):
-            eng.capture_stream = torch.cuda.Stream(device=eng.dev)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, pool=self.pool, stream=eng.capture_stream):
-            self._run(slot, win)
-        self.pool = graph.pool() if self.pool is None else self.pool
-        self.graphs[slot, win] = graph
-        return graph
 
 
 class LiveRestorer:

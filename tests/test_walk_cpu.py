@@ -2,8 +2,9 @@
 recorder that returns its output argument, checked against the rule the block walker (Engine._walk) states.
 
 Invariants, for every call of every model:
-- every GroupNorm that takes fused statistics (groupnorm_apply_stats, groupnorm_ab with stats) takes the ones the
-  producer of that very tensor wrote in its epilogue (or their frame gather, on the streaming path);
+- every GroupNorm that takes fused statistics (groupnorm_apply_stats, groupnorm_ab with stats) takes, frame by frame,
+  the ones the producer of that very tensor wrote in its epilogue (or their frame gather, on the streaming and live
+  paths, which gather frames and statistics from a batch of distinct frames or from a live ring's slots);
 - a GroupNorm whose input came straight from a conv, linear, conv_rgb, conv_up2x or swin_mlp launch computes its own
   statistics (groupnorm_silu, groupnorm_ab without stats) only where that producer could not have fused them: a tile
   grid that does not divide the frame (conv_tiles_exact), a channel count gn_stats_supported rejects, a non-contiguous
@@ -12,6 +13,7 @@ Invariants, for every call of every model:
 import contextlib
 import copy
 import inspect
+import itertools
 
 import pytest
 import torch
@@ -23,15 +25,26 @@ OPS = ('linear', 'conv', 'conv_rgb', 'conv_up2x', 'groupnorm_silu', 'groupnorm_a
        'conv_out_gn', 'layernorm', 'ln_linear', 'swin_mlp', 'window_attention', 'window_attention_tc',
        'window3d_attention', 'mha', 'argmax_gather', 'l2_argmin_tc', 'l2_argmin_tc_split', 'soft_codes', 'sample_codes',
        'rq_residual', 'rq_embed', 'vq_stats', 'adain', 'maxpool3x3s2', 'global_avgpool', 'channel_affine',
-       'assemble_cond', 'gather_frames', 'copy2d', 'regroup_frames')
+       'assemble_cond', 'gather_frames', 'copy2d', 'regroup_frames', 'f32nchw_to_u8hwc')
 # what a call returns, where that is not its `out` argument
 RETURNS = {'argmax_gather': ('idx_out', 'quant'), 'l2_argmin_tc': ('idx_out', 'quant'),
            'l2_argmin_tc_split': ('idx_out', 'quant'), 'groupnorm_ab': 'ab', 'rq_residual': 'agg',
-           'vq_stats': 'scalars', 'assemble_cond': 'cond', 'sample_codes': 'idx_out'}
+           'vq_stats': 'scalars', 'assemble_cond': 'cond', 'sample_codes': 'idx_out', 'f32nchw_to_u8hwc': 'out_u8'}
 
 
 def _key(t):
     return t.data_ptr(), tuple(t.shape), t.stride()
+
+
+def _frames(t, n):
+    """(address, shape, strides) of each of the n frames of t along its first dimension; a tensor whose first dimension
+    is not n (a flat statistics buffer) splits into n equal flat parts."""
+    if t.dim() > 1 and t.shape[0] == n:
+        step, shape, stride = t.stride(0), tuple(t.shape[1:]), t.stride()[1:]
+    else:
+        step = t.numel() // n
+        shape, stride = (step,), (1,)
+    return [(t.data_ptr() + f * step * t.element_size(), shape, stride) for f in range(n)]
 
 
 class Recorder:
@@ -44,8 +57,10 @@ class Recorder:
         # data_ptr -> (key of the tensor last written there, op, whether that op could have fused the next GroupNorm's
         # statistics); a write into a slice that starts there replaces the entry of the whole buffer
         self.producer = {}
-        self.stats_of = {}      # data_ptr of a statistics buffer -> key of the tensor it describes
-        self.gathered = {}      # key of a gathered tensor's source -> key of the gather's output
+        # frame (_frames) -> what the last write there left: a token of that write, or ('stats', token) for the
+        # GroupNorm statistics of the frame that holds that token; a frame gather moves both with the frames
+        self.held = {}
+        self.tokens = itertools.count()
 
     def could_fuse(self, name, a):
         out = a['out']
@@ -72,25 +87,29 @@ class Recorder:
                          gn_in is not None))
         x = a.get('x')
         if name in ('groupnorm_apply_stats', 'groupnorm_ab') and gn_in is not None:
-            if self.stats_of.get(gn_in.data_ptr()) != _key(x):
+            want = [('stats', self.held.get(k)) for k in _frames(x, x.shape[0])]
+            if any(w[1] is None for w in want) or [self.held.get(k) for k in _frames(gn_in, x.shape[0])] != want:
                 self.violations.append('%s on %s reads statistics of another tensor' % (name, tuple(x.shape)))
         elif name in ('groupnorm_silu', 'groupnorm_ab'):
             key, op, fusable = self.producer.get(x.data_ptr(), (None, None, False))
             if fusable and key == _key(x):
                 self.violations.append('%s recomputes the statistics of a %s output %s that could have fused them'
                                        % (name, op, tuple(x.shape)))
-        if name == 'gather_frames':
-            src = self.stats_of.get(x.data_ptr())
-            if src is not None and src in self.gathered:       # a statistics buffer follows its tensor's gather
-                self.stats_of[a['out'].data_ptr()] = self.gathered[src]
-            else:
-                self.gathered[_key(x)] = _key(a['out'])
         out = a.get('out')
         if torch.is_tensor(out):
             fusable = name in ('conv', 'linear', 'conv_rgb', 'conv_up2x', 'swin_mlp') and self.could_fuse(name, a)
             self.producer[out.data_ptr()] = (_key(out), name, fusable)
+            frames = _frames(out, out.shape[0])
+            if name == 'gather_frames':
+                src = _frames(x, x.shape[0])
+                for k, i in zip(frames, a['idx_i32'].tolist()):
+                    self.held[k] = self.held.get(src[i], ('unknown', next(self.tokens)))
+            else:
+                for k in frames:
+                    self.held[k] = next(self.tokens)
             if writes:
-                self.stats_of[a['gn_stats'].data_ptr()] = _key(out)
+                for k, s in zip(frames, _frames(a['gn_stats'], out.shape[0])):
+                    self.held[s] = ('stats', self.held[k])
 
 
 def install(monkeypatch):
@@ -143,6 +162,20 @@ def _x(*shape):
     return torch.rand(*shape, generator=torch.Generator().manual_seed(0))
 
 
+def _live(eng, H, W, w, n=4):
+    """LiveRestorer's schedule on the engine: frame j into ring slot j % 3, then the window of frame j - 1
+    (video.window_indices), and the last frame's window at the end.  Four frames reuse slot 0."""
+    from pgtformer_b200.video import window_indices
+    ring = eng.live_ring(H, W, w)
+    out = torch.empty(1, H, W, 3, dtype=torch.uint8)
+    wins = window_indices(n)
+    for j in range(n + 1):
+        if j < n:
+            eng.frame_step(_x(1, 3, H, W), j % 3, ring)
+        if j > 0:
+            eng.window_step(torch.tensor([k % 3 for k in wins[j - 1]], dtype=torch.int32), w, True, ring, out)
+
+
 def _calls(name, eng, b, H, W):
     """(label, thunk) of every call of `name` the walk is checked on, at b clips / images of H x W."""
     if name == 'PGTFormer':
@@ -150,7 +183,8 @@ def _calls(name, eng, b, H, W):
         fi = torch.tensor([0, 1, 2] + [1, 2, 3] * (b - 1), dtype=torch.int32)
         return [('w1', lambda: eng.forward(x, w=1.0)), ('w0', lambda: eng.forward(x, w=0.0)),
                 ('code_only', lambda: eng.forward(x, code_only=True)),
-                ('stream', lambda: eng.forward(_x(2 + b, 3, H, W), w=1.0, frame_index=fi))]
+                ('stream', lambda: eng.forward(_x(2 + b, 3, H, W), w=1.0, frame_index=fi)),
+                ('live_w1', lambda: _live(eng, H, W, 1.0)), ('live_w0', lambda: _live(eng, H, W, 0.0))]
     if name.startswith('TDCRQVAE3'):
         x = _x(3 * b, 3, H, W)
         z = _x(3 * b, H // 16, W // 16, eng.arch.embed_dim)
