@@ -355,10 +355,13 @@ int pgt_nhwc_bf16_to_f32(const void* x, int ldx, int F, int HW, int C, float* y,
  *   pgt_f32nchw_to_u8hwc: frames first, first+step, ... (n of them) of fp32 [*, 3, H, W] -> rgb24 [n, H, W, 3] with
  *     uint8(clamp(x, 0, 1) * 255) (apply_net_to_frames, inference.py:15-19); first = 1, step = 3 selects the middle
  *     frame of every clip.
- *   pgt_gather_frames: y[f] = x[idx[f]] for frames of frame_bytes bytes (multiple of 16); idx: DEVICE int32 [n]. */
+ *   pgt_gather_frames: y[f] = x[idx[f]] for frames of frame_bytes bytes (multiple of 16); idx: DEVICE int32 [n].
+ *   pgt_scatter_frames: y[idx[f]] = x[f], its mirror (the live pool's staging rows into each stream's ring slots);
+ *     the idx entries must be distinct. */
 int pgt_u8hwc_to_f32nchw(const void* x_u8, int F, int H, int W, float* y, void* stream);
 int pgt_f32nchw_to_u8hwc(const float* x, int first, int step, int n, int H, int W, void* y_u8, void* stream);
 int pgt_gather_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream);
+int pgt_scatter_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream);
 
 #ifdef __cplusplus
 }

@@ -97,6 +97,7 @@ SIGNATURES = {
     'pgt_u8hwc_to_f32nchw': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'pgt_f32nchw_to_u8hwc': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'pgt_gather_frames': (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
+    'pgt_scatter_frames': (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
     'pgt_copy2d': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     'pgt_regroup_frames': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
     'pgt_nchw_f32_to_nhwc_bf16': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,

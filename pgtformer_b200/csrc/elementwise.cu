@@ -194,6 +194,14 @@ __global__ void gather_frames_kernel(const uint4* __restrict__ x, size_t vec_per
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < vec_per_frame; i += (size_t)gridDim.x * blockDim.x)
     d[i] = __ldg(s + i);
 }
+
+__global__ void scatter_frames_kernel(const uint4* __restrict__ x, size_t vec_per_frame, const int* __restrict__ idx,
+                                      uint4* __restrict__ y) {
+  const uint4* s = x + (size_t)blockIdx.y * vec_per_frame;
+  uint4* d = y + (size_t)idx[blockIdx.y] * vec_per_frame;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < vec_per_frame; i += (size_t)gridDim.x * blockDim.x)
+    d[i] = __ldg(s + i);
+}
 }  // namespace pgt
 
 extern "C" int pgt_u8hwc_to_f32nchw(const void* x_u8, int F, int H, int W, float* y, void* stream) {
@@ -229,6 +237,18 @@ extern "C" int pgt_gather_frames(const void* x, long long frame_bytes, const int
   ProfScope ps(PGT_PROF_MOVE, 2.0 * (double)n * frame_bytes, static_cast<cudaStream_t>(stream), "pgt_gather_frames");
   unsigned bx = (unsigned)std::min<size_t>((vec + 255) / 256, 1024);
   pgt::gather_frames_kernel<<<dim3(bx, n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint4*>(x), vec, idx_dev, static_cast<uint4*>(y));
+  PGT_LAUNCH_OK();
+  return PGT_OK;
+}
+
+extern "C" int pgt_scatter_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream) {
+  PGT_CHECK_ARG(x && y && idx_dev && n > 0 && frame_bytes > 0 && frame_bytes % 16 == 0);
+  PGT_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0);
+  const size_t vec = (size_t)frame_bytes / 16;
+  ProfScope ps(PGT_PROF_MOVE, 2.0 * (double)n * frame_bytes, static_cast<cudaStream_t>(stream), "pgt_scatter_frames");
+  unsigned bx = (unsigned)std::min<size_t>((vec + 255) / 256, 1024);
+  pgt::scatter_frames_kernel<<<dim3(bx, n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint4*>(x), vec, idx_dev, static_cast<uint4*>(y));
   PGT_LAUNCH_OK();
   return PGT_OK;

@@ -631,20 +631,22 @@ class Engine:
         record: {'pos': convpos rows [n, T/n, 512], 'h': the frame blocks' output [n, ...], 'h_stats': the GroupNorm
         statistics [n, chunks * 64] h's producer writes for the next block (when it writes any), 'feats': {level:
         [n, ...]}, for w > 0 the skip tensors of the per-frame levels the SFT fusion reads (the others are never moved:
-        level 0 is 100 MB per clip and unused)}.  With ring (live_ring: the record of three frames) x is one frame, its
-        producers write straight into slot `slot` of ring, and the levels kept are those the ring has room for."""
+        level 0 is 100 MB per clip and unused)}.  With ring (live_ring: the record of a ring's rows) the producers write
+        the n frames straight into rows slot .. slot + n - 1 of ring, and the levels kept are those the ring has room
+        for."""
         a = self.arch
         last, n = a.frame_blocks - 1, x.shape[0]
         outs, gn_outs = {}, {}
         if ring is None:
             levels = list(a.fuse_level_key) if float(w) > 0 else []
         else:
+            rows = slice(slot, slot + n)
             levels = list(ring['feats'])
-            outs = {i: ring['feats'][lvl][slot:slot + 1] for i, lvl in a.enc_taps.items() if lvl in levels}
-            outs[last] = ring['h'][slot:slot + 1]
+            outs = {i: ring['feats'][lvl][rows] for i, lvl in a.enc_taps.items() if lvl in levels}
+            outs[last] = ring['h'][rows]
             if 'h_stats' in ring:
-                gn_outs[last] = ring['h_stats'][slot]
-        pos = self.parse_pos(x, out=None if ring is None else ring['pos'][slot])
+                gn_outs[last] = ring['h_stats'][rows].view(-1)
+        pos = self.parse_pos(x, out=None if ring is None else ring['pos'][rows].flatten(0, 1))
         h, feats, _ = self.encoder_frames(x, outs, gn_outs)
         rec = {'pos': pos.view(n, -1, pos.shape[-1]), 'h': h,
                'feats': {lvl: f for lvl, f in feats.items() if lvl in levels}}
@@ -720,10 +722,10 @@ class Engine:
         checked by the caller before this: a capture never starts on an argument the method would reject, and a key
         whose warm-up raises stores nothing.
 
-        A graph here is a pure function of its inputs.  The live steps (video.LiveRestorer), whose ring of per-frame
-        results persists across replays, are captured by their session through _capture too, but all in one memory
-        pool: one graph per ring phase, because each step's producers write straight into the new frame's ring slot
-        (video._LiveSession)."""
+        A graph here is a pure function of its inputs.  The live steps (video.LivePool, pool_step), whose ring of
+        per-frame results persists across replays, are captured by their pool through _capture too, all in one memory
+        pool: one graph per (new frames, windows) count, reading its slot and window indices from device buffers the
+        pool fills before each replay."""
         tensors = [t.to(self.dev) for t in tensors]
         key = (method.__name__, tuple((tuple(t.shape), t.dtype) for t in tensors), tuple(sorted(scalars.items())))
         if not hasattr(self, '_graphs'):
@@ -787,31 +789,56 @@ class Engine:
 
     @_on_device
     @torch.no_grad()
-    def live_ring(self, H, W, w):
-        """The per-frame record (_frame_pass) of three frames, one slot each, for frame_step / window_step.  Allocated
-        here, outside any graph's memory pool, so that graphs captured later can all write and read the same
-        addresses.  Shapes are those of one run of the per-frame work."""
+    def live_ring(self, H, W, w, streams=1):
+        """The per-frame record (_frame_pass) of 4 * streams rows, for frame_step / window_step / pool_step: row
+        3 s + (j mod 3) holds frame j of stream s, and rows 3 * streams + k are the staging rows pool_step's new frames
+        are computed into.  Allocated here, outside any graph's memory pool, so that graphs captured later can all
+        write and read the same addresses.  Shapes are those of one run of the per-frame work."""
         if H % 64 or W % 64:
             raise ValueError('expected H, W multiples of 64, got %dx%d' % (H, W))
+        rows = 4 * int(streams)
         rec = self._frame_pass(torch.zeros(1, 3, H, W, dtype=torch.float32, device=self.dev), w)
-        ring = {k: self._new(3, *t.shape[1:], dtype=t.dtype) for k, t in rec.items() if k != 'feats'}
-        ring['feats'] = {lvl: self._new(3, *f.shape[1:], dtype=f.dtype) for lvl, f in rec['feats'].items()}
+        ring = {k: self._new(rows, *t.shape[1:], dtype=t.dtype) for k, t in rec.items() if k != 'feats'}
+        ring['feats'] = {lvl: self._new(rows, *f.shape[1:], dtype=f.dtype) for lvl, f in rec['feats'].items()}
         return ring
 
-    @_on_device
-    @torch.no_grad()
-    def frame_step(self, x1, slot, ring):
-        """The per-frame work of one fp32 frame x1 [1,3,H,W] — parse_pos and encoder_frames — written into slot `slot`
-        of ring (live_ring) by the producing kernels themselves."""
-        self._frame_pass(x1, ring=ring, slot=slot)
+    @staticmethod
+    def ring_entries(ring):
+        """Every tensor of a live ring (live_ring), one row per frame: pos, h, h_stats when present, the kept feats."""
+        return [ring[k] for k in ('pos', 'h', 'h_stats') if k in ring] + list(ring['feats'].values())
 
     @_on_device
     @torch.no_grad()
-    def window_step(self, index3, w, adain, ring, out_u8):
-        """The window (f[i-1], f[i], f[i+1]) restored from ring slots index3 (device int32 [3]), exactly as
-        forward(frame_index=index3) computes it.  Writes the middle frame into out_u8 (rgb24 [1,H,W,3] uint8)."""
-        out = self._window_tail(ring, index3, w, adain)[0]
+    def frame_step(self, x, slot, ring):
+        """The per-frame work of fp32 frames x [B,3,H,W] — parse_pos and encoder_frames — written into rows
+        slot .. slot + B - 1 of ring (live_ring) by the producing kernels themselves."""
+        self._frame_pass(x, ring=ring, slot=slot)
+
+    @_on_device
+    @torch.no_grad()
+    def window_step(self, index, w, adain, ring, out_u8):
+        """The windows (f[i-1], f[i], f[i+1]) restored from the ring rows of index (device int32 [3 Bw]), exactly as
+        forward(frame_index=index) computes them.  Writes the middle frames into out_u8 (rgb24 [Bw,H,W,3] uint8)."""
+        out = self._window_tail(ring, index, w, adain)[0]
         return ops.f32nchw_to_u8hwc(out, out_u8, first=1, step=3)
+
+    @_on_device
+    @torch.no_grad()
+    def pool_step(self, u8, x, ring, slots, index, w, adain, out_u8):
+        """One step of a pool of live streams (video.LivePool) on a live_ring of S streams and its rgb24 frames u8
+        [4S,H,W,3] (the same rows).  The B = slots.numel() new frames, already in u8's staging rows 3S .. 3S + B - 1,
+        go to fp32 in x [>=B,3,H,W] and through frame_step into the ring's staging rows; every ring entry and the rgb24
+        frame are then scattered to the frames' slots (slots: device int32 [B]; h's GroupNorm statistics travel as
+        their own entry).  Then the windows of index (device int32 [3 Bw], ring rows; None for none) are restored into
+        out_u8 [Bw,H,W,3].  Nothing else is touched, so a step replays from a CUDA graph given its two index tensors."""
+        if slots is not None:
+            B, st = slots.numel(), u8.shape[0] // 4 * 3
+            xs = ops.u8hwc_to_f32nchw(u8[st:st + B], x[:B])
+            self.frame_step(xs, st, ring)
+            for t in self.ring_entries(ring) + [u8]:
+                ops.scatter_frames(t[st:st + B], slots, t)
+        if index is not None:
+            self.window_step(index, w, adain, ring, out_u8)
 
     # ------------------------------------------------------------------ stage-I codec (TDCRQVAE3 methods)
     def _codebook(self, d=0):

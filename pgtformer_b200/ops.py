@@ -560,6 +560,16 @@ def gather_frames(x, idx_i32, out):
     return out
 
 
+def scatter_frames(x, idx_i32, out):
+    """out[idx[f]] = x[f] along dim 0 (whole frames; idx: device int32, distinct entries) — gather_frames' mirror."""
+    lib = L.load()
+    assert x.is_contiguous() and out.is_contiguous() and x.dtype == out.dtype and x.shape[1:] == out.shape[1:]
+    assert idx_i32.dtype == torch.int32 and idx_i32.is_cuda and idx_i32.numel() == x.shape[0]
+    fb = x[0].numel() * x.element_size()
+    L.check(lib.pgt_scatter_frames(_p(x), fb, _p(idx_i32), x.shape[0], _p(out), _stream()))
+    return out
+
+
 def copy2d(x, out):
     lib = L.load()
     T, C, ldx = _rows(x)

@@ -15,7 +15,9 @@ The ffmpeg pipes themselves stay in the caller's script (SURVEY section 7): `str
 frames and yields rgb24 frames, which is exactly what the reference's pipe loop reads and writes.
 
 `LiveRestorer` is the same loop for a source that delivers frames one at a time: each push returns the previous frame,
-each frame's per-frame work runs once into a device ring, and every step can replay from a CUDA graph.
+each frame's per-frame work runs once into a device ring, and every step can replay from a CUDA graph.  `LivePool` runs
+many such streams on one model, batching the new frames and the windows of every stream that pushes into one step;
+`LiveRestorer` is a pool of one.
 """
 import numpy as np
 import torch
@@ -168,74 +170,209 @@ def _check_frame(frame, hw):
     return t
 
 
-class _LiveSession:
-    """The device state of a LiveRestorer on one engine and frame size: the engine's ring of per-frame results
-    (Engine.live_ring), the rgb24 frames that produced them (u8[j % 3] holds frame j), the output frame, pinned host
-    buffers and, with cuda_graph, the captured steps.
+class _PoolState:
+    """The device state of a LivePool on one engine and frame size: the engine's ring of per-frame results for S
+    streams (Engine.live_ring), the rgb24 frames that produced them (u8, the same rows: 3 s + j % 3 holds frame j of
+    stream s, and rows 3S .. 4S - 1 stage a step's new frames), the fp32 frames of a step, the output frames, the
+    device index buffer (idx[:S]: the new frames' slots, idx[S:]: the windows' ring rows), pinned host buffers and,
+    with cuda_graph, the captured steps.
 
-    A step is (slot s of the new frame or None, ring slots of the window or None): u8[s] -> fp32 -> frame_step into
-    ring slot s, then window_step -> out.  With cuda_graph each distinct step is captured once (Engine._capture) and
-    replayed: every address it touches (u8, ring, the window's index tensor, out) is allocated outside the graphs, so
-    the ring carries from one replay to the next.  One graph per step rather than one graph rotating through a device
-    slot index: the producing kernels write straight into the new frame's ring slot, which a kernel argument baked into
-    a single graph could not follow without one more copy of the slot per frame.  A stream uses at most 8 steps (3
-    steady phases, the first frame, the first window, the 3 last windows or the single frame's), and all of them share
-    one memory pool, replayed one at a time on one stream, so their scratch costs one step's worth."""
+    A step is (B new frames, Bw windows): Engine.pool_step.  With cuda_graph each distinct (B, Bw) is captured once
+    (Engine._capture) and replayed after its indices are copied into idx: every address a step touches is allocated
+    here, outside the graphs, so the ring carries from one replay to the next and one graph serves every choice of
+    streams.  B and Bw are at most S, so a pool holds at most (S + 1)^2 - 1 graphs; a single stream uses (1, 0),
+    (1, 1) and (0, 1).  They all share one memory pool, replayed one at a time on one stream, so their scratch costs
+    one step's worth."""
 
-    def __init__(self, eng, H, W, w, adain, cuda_graph):
-        self.eng, self.hw, self.w, self.adain, self.cuda_graph = eng, (H, W), w, adain, cuda_graph
+    def __init__(self, eng, S, hw, w, adain, cuda_graph):
+        self.eng, self.S, self.hw, self.w, self.adain, self.cuda_graph = eng, S, hw, w, adain, cuda_graph
+        H, W = hw
         dev = eng.dev
         with torch.cuda.device(dev):
-            self.ring = eng.live_ring(H, W, w)
-            self.u8 = torch.empty(3, H, W, 3, dtype=torch.uint8, device=dev)
-            self.x = torch.empty(1, 3, H, W, dtype=torch.float32, device=dev)
-            self.out = torch.empty(1, H, W, 3, dtype=torch.uint8, device=dev)
-        self.host_in = torch.empty(H, W, 3, dtype=torch.uint8).pin_memory()
-        self.host_out = torch.empty(H, W, 3, dtype=torch.uint8).pin_memory()
-        self.loaded = None                 # event: host_in has reached the device and may be overwritten
-        self.index = {}                    # window slots -> device int32 [3]
+            self.ring = eng.live_ring(H, W, w, S)
+            self.u8 = torch.empty(4 * S, H, W, 3, dtype=torch.uint8, device=dev)
+            self.x = torch.empty(S, 3, H, W, dtype=torch.float32, device=dev)
+            self.out = torch.empty(S, H, W, 3, dtype=torch.uint8, device=dev)
+            self.idx = torch.empty(4 * S, dtype=torch.int32, device=dev)
+        self.host_in = torch.empty(S, H, W, 3, dtype=torch.uint8).pin_memory()
+        self.host_idx = torch.zeros(4 * S, dtype=torch.int32).pin_memory()
+        self.host_out = torch.empty(S, H, W, 3, dtype=torch.uint8).pin_memory()
+        self.loaded = None                 # event: the host buffers have reached the device and may be overwritten
         self.graphs = {}
         self.pool = None
 
-    def load(self, t, slot):
-        """Frame t (uint8 [H,W,3], host or CUDA) into u8[slot] on the current stream."""
-        if torch.is_tensor(t) and t.is_cuda:
-            self.u8[slot].copy_(t, non_blocking=True)
-            return
+    def run(self, B, Bw):
+        """The step's device work, with its indices already in idx."""
+        S = self.S
+        self.eng.pool_step(self.u8, self.x, self.ring, self.idx[:B] if B else None,
+                           self.idx[S:S + 3 * Bw] if Bw else None, self.w, self.adain, self.out[:Bw])
+
+    def recompute(self, rows):
+        """The per-frame work of the rgb24 frames in u8[rows], into the same ring rows (after new weights)."""
+        for r in rows:
+            ops.u8hwc_to_f32nchw(self.u8[r:r + 1], self.x[:1])
+            self.eng.frame_step(self.x[:1], r, self.ring)
+
+    def step(self, new, wins):
+        """new: [(ring slot, frame)] of the new frames; wins: [ring rows (a, b, c)] of the windows to restore.  Runs
+        one step on the current stream; returns the restored frames, numpy uint8 [H,W,3] each (one synchronisation)."""
+        S, B, Bw = self.S, len(new), len(wins)
         if self.loaded is not None:
-            self.loaded.synchronize()      # the previous frame's H2D (its step needs no synchronisation of its own)
-        self.host_in.numpy()[...] = t.numpy() if torch.is_tensor(t) else t
-        self.u8[slot].copy_(self.host_in, non_blocking=True)
+            self.loaded.synchronize()      # the previous step's uploads (a step without windows does not wait)
+        for k, (slot, t) in enumerate(new):
+            row = self.u8[3 * S + k]
+            if torch.is_tensor(t) and t.is_cuda:
+                row.copy_(t, non_blocking=True)
+            else:
+                self.host_in[k].numpy()[...] = t.numpy() if torch.is_tensor(t) else t
+                row.copy_(self.host_in[k], non_blocking=True)
+            self.host_idx[k] = slot
+        self.host_idx[S:S + 3 * Bw] = torch.tensor([r for win in wins for r in win], dtype=torch.int32)
+        self.idx.copy_(self.host_idx, non_blocking=True)
         self.loaded = torch.cuda.Event()
         self.loaded.record()
-
-    def _run(self, slot, win):
-        eng = self.eng
-        if slot is not None:
-            ops.u8hwc_to_f32nchw(self.u8[slot:slot + 1], self.x)
-            eng.frame_step(self.x, slot, self.ring)
-        if win is not None:
-            eng.window_step(self.index[win], self.w, self.adain, self.ring, self.out)
-
-    def step(self, slot, win):
-        """Runs one step; with a window, returns the restored frame as numpy uint8 [H,W,3] (the one synchronisation)."""
-        if win is not None and win not in self.index:
-            self.index[win] = torch.tensor(win, dtype=torch.int32).to(self.eng.dev)
         if not self.cuda_graph:
-            self._run(slot, win)
+            self.run(B, Bw)
         else:
-            graph = self.graphs.get((slot, win))
-            if graph is None:                  # the step's writes are idempotent: its warm-up runs leave the ring as is
-                graph = self.graphs[slot, win] = self.eng._capture(lambda: self._run(slot, win), self.pool)[0]
+            graph = self.graphs.get((B, Bw))
+            if graph is None:              # the step's writes are idempotent: its warm-up runs leave the ring as is
+                graph = self.graphs[B, Bw] = self.eng._capture(lambda: self.run(B, Bw), self.pool)[0]
                 self.pool = graph.pool() if self.pool is None else self.pool
             graph.replay()
-        if win is None:
-            return None
-        self.host_out.copy_(self.out[0], non_blocking=True)
+        if Bw == 0:
+            return []
+        self.host_out[:Bw].copy_(self.out[:Bw], non_blocking=True)
         done = torch.cuda.Event()
         done.record()
         done.synchronize()
-        return self.host_out.numpy().copy()
+        return [f.copy() for f in self.host_out.numpy()[:Bw]]
+
+
+class LivePool:
+    """Restores several live videos on one model, each one frame behind its input, batching every stream's new frame
+    into one step: push({a: fa[i+1], b: fb[j+1]}) returns {a: frame i of a, b: frame j of b}, each restored from its
+    stream's window of the reference's loop (window_indices), byte for byte what VideoRestorer.restore gives on that
+    stream alone.
+
+    Each step runs the per-frame work (BiSeNet, the frame blocks of the encoder) of all its new frames as one batch
+    into staging rows on the device, scatters the results into each stream's three ring slots, and restores the
+    windows of every stream that has one as one batch.  Streams open, stall (a push may list any subset of the open
+    streams) and end independently.  All streams share w, adain and the frame size, which the first frame pushed while
+    the pool holds no frames sets.  Frames are rgb24 [H,W,3] uint8 — numpy, a host torch tensor or a CUDA tensor on
+    the model's device — with H and W multiples of 64; outputs are numpy uint8.  With cuda_graph each distinct
+    (new frames, windows) count replays from one CUDA graph (_PoolState), so streams that push together replay one
+    graph.  The device state belongs to the model's current engine: after load_state_dict(), .to() or refresh() the
+    next step rebuilds it, re-running the per-frame work of every open stream's frames still in a window, from the
+    rgb24 frames the pool keeps on the device.
+
+        pool = LivePool(model, max_streams=8)
+        a, b = pool.open(), pool.open()
+        pool.push({a: a0, b: b0})     # {a: None, b: None}
+        pool.push({a: a1})            # {a: frame 0 of a}
+        pool.push({a: a2, b: b1})     # {a: frame 1 of a, b: frame 0 of b}
+        pool.flush(a)                 # frame 2 of a; handle a is freed
+    """
+
+    def __init__(self, model, max_streams, w=1.0, adain=True, cuda_graph=True):
+        if int(max_streams) < 1:
+            raise ValueError('max_streams must be at least 1, got %r' % (max_streams,))
+        self.model = model
+        self.max_streams = int(max_streams)
+        self.w = float(w)
+        self.adain = bool(adain)
+        self.cuda_graph = bool(cuda_graph)
+        self._streams = {}                 # handle -> [stream index s (ring rows 3s .. 3s + 2), frames pushed]
+        self._handles = 0
+        self._hw = None
+        self._state = None
+
+    def open(self):
+        """A new stream's handle."""
+        if len(self._streams) >= self.max_streams:
+            raise ValueError('all %d streams of the pool are open' % self.max_streams)
+        s = min(set(range(self.max_streams)) - {v[0] for v in self._streams.values()})
+        h = self._handles
+        self._handles += 1
+        self._streams[h] = [s, 0]
+        return h
+
+    def close(self, handle):
+        """Frees a stream's handle without restoring its last frame."""
+        self._stream(handle)
+        del self._streams[handle]
+
+    def _stream(self, handle):
+        try:
+            return self._streams[handle]
+        except (KeyError, TypeError):
+            raise ValueError('unknown or closed stream handle %r' % (handle,)) from None
+
+    def _holds_frames(self):
+        return any(n for _, n in self._streams.values())
+
+    # ------------------------------------------------------------------ schedule (host only)
+    @torch.no_grad()
+    def push(self, frames):
+        """frames: {handle: the stream's next frame} (or (handle, frame) pairs) for any subset of the open streams.
+        Returns {handle: its stream's previous frame restored, or None for its first frame}."""
+        items = list(frames.items()) if hasattr(frames, 'items') else list(frames)
+        hw = self._hw if self._holds_frames() else None
+        checked, dev = {}, None
+        for h, f in items:
+            self._stream(h)
+            if h in checked:
+                raise ValueError('stream handle %r listed twice' % (h,))
+            t = checked[h] = _check_frame(f, hw)
+            hw = (int(t.shape[0]), int(t.shape[1]))
+            if torch.is_tensor(t) and t.is_cuda:
+                dev = dev or next(self.model.parameters()).device
+                if t.device != dev:
+                    raise ValueError('frame on %s, model on %s' % (t.device, dev))
+        if not checked:
+            return {}
+        new, wins, order = [], [], []
+        for h, t in checked.items():
+            s, n = self._streams[h]
+            new.append((3 * s + n % 3, t))
+            if n > 0:
+                wins.append(tuple(3 * s + j % 3 for j in (max(n - 2, 0), n - 1, n)))
+                order.append(h)
+        got = self._step(hw, new, wins)
+        self._hw = hw
+        for h in checked:
+            self._streams[h][1] += 1
+        out = dict.fromkeys(checked)
+        out.update(zip(order, got))
+        return out
+
+    @torch.no_grad()
+    def flush(self, handle):
+        """The stream's last frame, restored from (f[n-2], f[n-1], f[n-1]) — (f0, f0, f0) for a single frame; None for
+        a stream without frames.  Frees the handle."""
+        s, n = self._stream(handle)
+        try:
+            if n == 0:
+                return None
+            return self._step(self._hw, [], [tuple(3 * s + j % 3 for j in (max(n - 2, 0), n - 1, n - 1))])[0]
+        finally:
+            del self._streams[handle]
+
+    # ------------------------------------------------------------------ device
+    def _step(self, hw, new, wins):
+        """One step on the state of the model's current engine for frames of size hw; a state built after the weights
+        changed mid-stream first recomputes the ring from the rgb24 frames it still holds."""
+        eng = self.model.engine()
+        state = old = self._state
+        if old is None or old.eng is not eng or old.hw != hw:
+            self._state = None
+            state = _PoolState(eng, self.max_streams, hw, self.w, self.adain, self.cuda_graph)
+            if old is not None and old.hw == hw and self._holds_frames():   # weights or device changed mid-stream
+                with torch.cuda.device(eng.dev):
+                    state.u8.copy_(old.u8)
+                    state.recompute([3 * s + j % 3 for s, n in self._streams.values() for j in range(max(n - 2, 0), n)])
+            self._state = state
+        with torch.cuda.device(eng.dev):
+            return state.step(new, wins)
 
 
 class LiveRestorer:
@@ -245,7 +382,7 @@ class LiveRestorer:
     Each frame's per-frame work (BiSeNet, the frame blocks of the encoder) runs once, when it is pushed, into a ring of
     three slots on the device; each window is gathered from the ring.  Frames are rgb24 [H,W,3] uint8 — numpy, a host
     torch tensor or a CUDA tensor on the model's device — with H and W multiples of 64; outputs are numpy uint8.  With
-    cuda_graph every step replays from a CUDA graph (_LiveSession).  The device state belongs to the model's current
+    cuda_graph every step replays from a CUDA graph.  It is the one stream of a LivePool of one.  The device state belongs to the model's current
     engine: after load_state_dict(), .to() or refresh() the next call rebuilds it, re-running the per-frame work of the
     frames still in the window on the new weights.
 
@@ -261,13 +398,17 @@ class LiveRestorer:
         self.w = float(w)
         self.adain = bool(adain)
         self.cuda_graph = bool(cuda_graph)
-        self._sess = None
+        self._pool = LivePool(model, 1, w=w, adain=adain, cuda_graph=cuda_graph)
+        self._handle = None
         self.reset()
 
     def reset(self):
         """Forgets the current stream (its frames); the next push starts a new one, of any frame size."""
         self._n = 0            # frames pushed in this stream
         self._hw = None
+        if self._handle is not None:
+            self._pool.close(self._handle)
+            self._handle = None
 
     # ------------------------------------------------------------------ schedule (host only)
     @torch.no_grad()
@@ -305,28 +446,12 @@ class LiveRestorer:
             yield out
 
     # ------------------------------------------------------------------ device
-    def _session(self, hw, n):
-        """The session of the model's current engine for frames of size hw; one built after the weights changed
-        mid-stream first recomputes the ring from the frames it still holds."""
-        eng = self.model.engine()
-        H, W = hw
-        old = self._sess
-        if old is not None and old.eng is eng and old.hw == (H, W):
-            return old
-        self._sess = None
-        sess = _LiveSession(eng, H, W, self.w, self.adain, self.cuda_graph)
-        if old is not None and n > 0:                # weights or device changed inside the stream
-            with torch.cuda.device(eng.dev):
-                sess.u8.copy_(old.u8)
-                for j in range(max(n - 2, 0), n):
-                    sess._run(j % 3, None)
-        self._sess = sess
-        return sess
-
     def _step(self, t, n, new, win):
-        """t: frame n (or None at flush) going into ring slot `new`; win: frame indices of the window to restore."""
-        sess = self._session(self._hw if t is None else (int(t.shape[0]), int(t.shape[1])), n)
-        with torch.cuda.device(sess.eng.dev):
-            if t is not None:
-                sess.load(t, new)
-            return sess.step(new, None if win is None else tuple(j % 3 for j in win))
+        """t: frame n (or None at flush) going into ring slot `new`; win: frame indices of the window to restore.  The
+        one stream of the pool keeps exactly this schedule."""
+        if t is None:
+            handle, self._handle = self._handle, None
+            return self._pool.flush(handle)
+        if self._handle is None:
+            self._handle = self._pool.open()
+        return self._pool.push({self._handle: t})[self._handle]
