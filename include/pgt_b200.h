@@ -65,6 +65,8 @@ typedef struct pgt_epilogue {
                           * every 128-row tile inside one frame: pgt_conv_tiles_per_frame() > 0 (exact statistics:
                           * pgt_conv_tiles_exact() > 0), or HW % 128 == 0 for
                           * pgt_linear_bf16); consumed by pgt_groupnorm_apply_stats                         */
+  const float* sft_wf;   /* PGT_EPI_SFT, convolutions only: fp32 [F] fusion weight of each output frame, used in place
+                          * of sft_w (a batch of clips restored at different fidelity weights); NULL: sft_w for all */
 } pgt_epilogue;
 
 const char* pgt_strerror(int status);
@@ -322,6 +324,11 @@ int pgt_vq_stats(const float* z, int T, int E, int HW, const float* codebook, in
  * Replaces adaptive_instance_normalization (archs/codeformer_arch.py:15-46). */
 int pgt_adain(const void* q, int ldq, int q_dtype, const void* l, int ldl, int F, int HW, int C, float eps,
               void* y, int ldy, void* stream);
+/* The same per frame: frame f gets AdaIN where flags[f] != 0 and is q rounded to bf16 (round to nearest even, as
+ * quant.to(torch.bfloat16)) where flags[f] == 0.  flags: DEVICE int32 [F] (a batch of clips restored with and without
+ * AdaIN). */
+int pgt_adain_frames(const void* q, int ldq, int q_dtype, const void* l, int ldl, int F, int HW, int C, float eps,
+                     const int32_t* flags, void* y, int ldy, void* stream);
 
 /* ---- face-parsing branch (BiSeNet / ResNet18, archs/pgtformer_arch.py:34-397); its other convolutions run on
  * pgt_conv_bf16 / pgt_conv_up2x_bf16 / pgt_linear_bf16 with eval-mode BatchNorm folded into weights and bias.

@@ -20,7 +20,7 @@ class Epilogue(Structure):
     _fields_ = [('bias', c_void_p), ('act', c_int32), ('mode', c_int32), ('residual', c_void_p),
                 ('ldr', c_int32), ('res_dtype', c_int32), ('aux', c_void_p), ('ldaux', c_int32),
                 ('sft_w', c_float), ('out', c_void_p), ('ldo', c_int32), ('out_dtype', c_int32),
-                ('out_layout', c_int32), ('flags', c_int32), ('gn_stats', c_void_p)]
+                ('out_layout', c_int32), ('flags', c_int32), ('gn_stats', c_void_p), ('sft_wf', c_void_p)]
 
 
 # name -> (restype, argtypes); mirrors include/pgt_b200.h one to one
@@ -88,6 +88,8 @@ SIGNATURES = {
                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     'pgt_adain': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int,
                           c_void_p]),
+    'pgt_adain_frames': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p,
+                                 c_void_p, c_int, c_void_p]),
     'pgt_maxpool3x3s2': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     'pgt_global_avgpool': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     'pgt_channel_affine': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_int,

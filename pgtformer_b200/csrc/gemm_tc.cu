@@ -97,6 +97,7 @@ struct GemmParams {
   const void* aux;
   int ldaux;
   float sft_w;
+  const float* sft_wf;   // conv modes: per-frame fusion weights [F] in place of sft_w (sft_weight), or nullptr
   void* out;
   int ldo, out_dtype, out_layout;
   double flops;      // algorithmic 2*M*N*K with the un-padded K (host-side accounting only)
@@ -180,10 +181,18 @@ __device__ __forceinline__ void sts128(uint32_t a, const uint4& u) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(u.x), "r"(u.y), "r"(u.z), "r"(u.w) : "memory");
 }
 
+// SFT fusion weight of the output frame of row r of tile m_blk: sft_wf[frame], or the launch's sft_w.  Rows past the
+// last frame (F % tn != 0) are never stored and read the last frame's entry.
+__device__ __forceinline__ float sft_weight(const GemmParams& p, int m_blk, int r) {
+  if (p.sft_wf == nullptr) return p.sft_w;
+  const int f = m_blk / (p.tiles_x * p.tiles_y) * p.tn + r / (p.tw * p.th);
+  return __ldg(p.sft_wf + min(f, p.F - 1));
+}
+
 template <bool kSft>
 __device__ __forceinline__ void epi_finish(const GemmParams& p, const uint32_t (&v)[32], const float* bias32, uint32_t srow,
                                            int r, int sub, int esize, bool has_res, float* gq, int gcol,
-                                           const float4 (&pre)[8], bool use_pre) {
+                                           const float4 (&pre)[8], bool use_pre, float sw = 0.f) {
   float f[32];
   if (use_pre) {                               // bias chunk already in registers (fetched before the barrier waits)
 #pragma unroll
@@ -233,7 +242,7 @@ __device__ __forceinline__ void epi_finish(const GemmParams& p, const uint32_t (
           const float2 sa = unpack_bf16x2(ux[q].x), sb = unpack_bf16x2(ux[q].y), sc = unpack_bf16x2(ux[q].z), sd = unpack_bf16x2(ux[q].w);
           const float ss[8] = {sa.x, sa.y, sb.x, sb.y, sc.x, sc.y, sd.x, sd.y};
 #pragma unroll
-          for (int e = 0; e < 8; ++e) f[8 * q + e] = rr[e] + p.sft_w * (rr[e] * ss[e] + f[8 * q + e]);
+          for (int e = 0; e < 8; ++e) f[8 * q + e] = rr[e] + sw * (rr[e] * ss[e] + f[8 * q + e]);
         }
       } else {
 #pragma unroll
@@ -433,10 +442,11 @@ __device__ __forceinline__ void epi_direct16(const GemmParams& p, const DirectRo
       for (int j = 0; j < 16; ++j) rr[j] = (j < ncol) ? __bfloat162float(rp[j]) : 0.f;
       if (p.epi_mode == PGT_EPI_SFT) {
         const __nv_bfloat16* ap = reinterpret_cast<const __nv_bfloat16*>(p.aux) + orow * p.ldaux + col0;
+        const float sw = p.sft_wf != nullptr ? __ldg(p.sft_wf + d.pn) : p.sft_w;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const float sc = (j < ncol) ? __bfloat162float(ap[j]) : 0.f;
-          f[j] = rr[j] + p.sft_w * (rr[j] * sc + f[j]);
+          f[j] = rr[j] + sw * (rr[j] * sc + f[j]);
         }
       } else {
 #pragma unroll
@@ -536,7 +546,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const EpiCtx&
           smem_row_32(xrow + half * 32, v);
           float4 nb[8];
           epi_finish<true>(p, v, bias_vec ? p.bias + col0 : nullptr, stg + pos * 2 * PANEL_BYTES, r, half, esize, true,
-                           gn_ptr(col0), col0, nb, false);
+                           gn_ptr(col0), col0, nb, false, sft_weight(p, m_blk, r));
           fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA engine
           mbar_arrive(&ctx.slot_ready[pos]);
           ++k;
@@ -637,7 +647,7 @@ __device__ __forceinline__ void epilogue_tile_wg(const GemmParams& p, const EpiC
         float4 nb[8];
         if (sft)
           epi_finish<true>(p, v, bias_vec ? p.bias + col0 : nullptr, stg + pos * 2 * PANEL_BYTES, r, sub, esize, true,
-                           gn_stats_ptr(p, m_blk, wq, col0), col0, nb, false);
+                           gn_stats_ptr(p, m_blk, wq, col0), col0, nb, false, sft_weight(p, m_blk, r));
         else
           epi_finish<false>(p, v, bias_vec ? p.bias + col0 : nullptr, stg + pos * PANEL_BYTES, r, sub, esize,
                             p.has_res_map != 0, gn_stats_ptr(p, m_blk, wq, col0), col0, nb, false);
@@ -1208,6 +1218,7 @@ static int fill_epilogue(GemmParams& p, const pgt_epilogue* ep) {
   p.aux = ep->aux;
   p.ldaux = ep->ldaux;
   p.sft_w = ep->sft_w;
+  p.sft_wf = ep->mode == PGT_EPI_SFT ? ep->sft_wf : nullptr;
   p.out = ep->out;
   p.ldo = ep->ldo;
   p.out_dtype = ep->out_dtype;
@@ -1218,6 +1229,7 @@ static int fill_epilogue(GemmParams& p, const pgt_epilogue* ep) {
   if (p.relu_after_res && (p.act != PGT_ACT_RELU || p.epi_mode != PGT_EPI_PLAIN)) return PGT_ERR_INVALID;
   if (p.epi_mode == PGT_EPI_SFT && (p.residual == nullptr || p.aux == nullptr || p.res_dtype != PGT_BF16))
     return PGT_ERR_INVALID;
+  if (p.sft_wf != nullptr && p.mode == MODE_LINEAR) return PGT_ERR_INVALID;   // a GEMM's rows have no frames
   if (p.out_layout == PGT_OUT_NCHW && (p.out_dtype != PGT_F32 || p.mode == MODE_LINEAR)) return PGT_ERR_INVALID;
   return PGT_OK;
 }

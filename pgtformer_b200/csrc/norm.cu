@@ -321,11 +321,13 @@ layernorm_kernel(const void* __restrict__ xin, int ldx, int x_dtype, int T, cons
 
 // ---------------------------------------------------------------------------------- AdaIN
 // Block = (frame, 64-channel slab).  Thread (prow, vcol) strides over pixels accumulating fp32 (sum, sumsq)
-// for content q and style l; block reduce; second sweep applies the affine map.
+// for content q and style l; block reduce; second sweep applies the affine map.  kFlags (pgt_adain_frames): a frame
+// whose flag is 0 is only rounded to bf16.
 constexpr int ADAIN_THREADS = 256;
+template <bool kFlags>
 __global__ void __launch_bounds__(ADAIN_THREADS)
 adain_kernel(const void* __restrict__ qin, int ldq, int q_dtype, const __nv_bfloat16* __restrict__ l, int ldl, int HW,
-             int C, float eps, __nv_bfloat16* __restrict__ y, int ldy) {
+             int C, float eps, const int* __restrict__ flags, __nv_bfloat16* __restrict__ y, int ldy) {
   __shared__ float red[4][ADAIN_THREADS / 8][64];   // [stat][prow][channel]
   __shared__ float sa[64], sb[64], spiv[64];
   __shared__ double sml[64], ssl[64];
@@ -335,11 +337,6 @@ adain_kernel(const void* __restrict__ qin, int ldq, int q_dtype, const __nv_bflo
   const int prow = threadIdx.x >> 3;
   const int rows_par = ADAIN_THREADS / 8;
   const int c0 = cbase + vcol * 8;
-  float acc[4][8];
-#pragma unroll
-  for (int k = 0; k < 4; ++k)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[k][j] = 0.f;
   auto load_q = [&](int p, float (&v)[8]) {
     if (q_dtype == PGT_BF16) {
       load8_bf16(reinterpret_cast<const __nv_bfloat16*>(qin) + ((size_t)f * HW + p) * ldq + c0, v);
@@ -349,6 +346,21 @@ adain_kernel(const void* __restrict__ qin, int ldq, int q_dtype, const __nv_bflo
       v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
     }
   };
+  if constexpr (kFlags) {
+    if (flags[f] == 0) {                                // uniform over the block
+      for (int p = prow; p < HW; p += rows_par) {
+        float vq[8];
+        load_q(p, vq);
+        store8_bf16(y + ((size_t)f * HW + p) * ldy + c0, vq);
+      }
+      return;
+    }
+  }
+  float acc[4][8];
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[k][j] = 0.f;
   for (int p = prow; p < HW; p += rows_par) {
     float vq[8], vl[8];
     load_q(p, vq);
@@ -542,8 +554,19 @@ extern "C" int pgt_adain(const void* q, int ldq, int q_dtype, const void* l, int
                          void* y, int ldy, void* stream) {
   PGT_CHECK_ARG(q && l && y && F > 0 && HW > 1 && C % 64 == 0 && ldq % 8 == 0 && ldl % 8 == 0 && ldy % 8 == 0);
   ProfScope ps(PGT_PROF_MOVE, 8.0 * F * (double)HW * C, static_cast<cudaStream_t>(stream), "adain");
-  adain_kernel<<<dim3(C / 64, F), ADAIN_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
-      q, ldq, q_dtype, reinterpret_cast<const __nv_bfloat16*>(l), ldl, HW, C, eps,
+  adain_kernel<false><<<dim3(C / 64, F), ADAIN_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+      q, ldq, q_dtype, reinterpret_cast<const __nv_bfloat16*>(l), ldl, HW, C, eps, nullptr,
+      reinterpret_cast<__nv_bfloat16*>(y), ldy);
+  PGT_LAUNCH_OK();
+  return PGT_OK;
+}
+
+extern "C" int pgt_adain_frames(const void* q, int ldq, int q_dtype, const void* l, int ldl, int F, int HW, int C,
+                                float eps, const int32_t* flags, void* y, int ldy, void* stream) {
+  PGT_CHECK_ARG(q && l && y && flags && F > 0 && HW > 1 && C % 64 == 0 && ldq % 8 == 0 && ldl % 8 == 0 && ldy % 8 == 0);
+  ProfScope ps(PGT_PROF_MOVE, 8.0 * F * (double)HW * C, static_cast<cudaStream_t>(stream), "adain_frames");
+  adain_kernel<true><<<dim3(C / 64, F), ADAIN_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+      q, ldq, q_dtype, reinterpret_cast<const __nv_bfloat16*>(l), ldl, HW, C, eps, flags,
       reinterpret_cast<__nv_bfloat16*>(y), ldy);
   PGT_LAUNCH_OK();
   return PGT_OK;

@@ -218,6 +218,23 @@ void vq_stats(const at::Tensor& z, const at::Tensor& codebook, const at::Tensor&
                      scalars.data_ptr<float>(), stream_of(z)), "vq_stats");
 }
 
+void adain_frames(const at::Tensor& q, const at::Tensor& style, const at::Tensor& flags, double eps, at::Tensor out) {
+  TORCH_CHECK(q.is_cuda() && q.dim() == 3 && (q.scalar_type() == at::kFloat || q.scalar_type() == at::kBFloat16) &&
+              style.scalar_type() == at::kBFloat16 && style.sizes() == q.sizes() && out.scalar_type() == at::kBFloat16 &&
+              out.sizes() == q.sizes() && flags.scalar_type() == at::kInt && flags.is_contiguous() &&
+              flags.numel() == q.size(0), "adain_frames: fp32 / bf16 q [F, HW, C], bf16 style and out, int32 flags [F]");
+  TORCH_CHECK(style.device() == q.device() && flags.device() == q.device() && out.device() == q.device(),
+              "adain_frames: every tensor on q's device");
+  TORCH_CHECK(q.stride(1) == ld(q) && style.stride(1) == ld(style) && out.stride(1) == ld(out),
+              "adain_frames: row-pitched [F, HW, C] tensors");
+  TORCH_CHECK(q.stride(0) == q.size(1) * ld(q) && style.stride(0) == style.size(1) * ld(style) &&
+              out.stride(0) == out.size(1) * ld(out), "adain_frames: frames one after another");
+  c10::cuda::CUDAGuard guard(q.device());
+  check(pgt_adain_frames(q.data_ptr(), ld(q), q.scalar_type() == at::kBFloat16 ? PGT_BF16 : PGT_F32, style.data_ptr(),
+                         ld(style), (int)q.size(0), (int)q.size(1), (int)q.size(2), (float)eps, flags.data_ptr<int32_t>(),
+                         out.data_ptr(), ld(out), stream_of(q)), "adain_frames");
+}
+
 }  // namespace
 
 TORCH_LIBRARY(pgt, m) {
@@ -236,6 +253,7 @@ TORCH_LIBRARY(pgt, m) {
   m.def("conv_out_gn_act(Tensor x, Tensor ab, Tensor wp, int cout, Tensor? bias, bool silu, Tensor(a!) out) -> ()");
   m.def("vq_stats(Tensor z, Tensor codebook, Tensor idx, int HW, float beta, Tensor(a!) scalars, Tensor(b!)? zq_nchw, "
         "Tensor(c!)? zq_bf16, Tensor(d!)? min_enc, Tensor(e!)? scores, Tensor(f!)? usage) -> ()");
+  m.def("adain_frames(Tensor q, Tensor style, Tensor flags, float eps, Tensor(a!) out) -> ()");
 }
 
 TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
@@ -252,4 +270,5 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("rq_embed", rq_embed);
   m.impl("conv_out_gn_act", conv_out_gn_act);
   m.impl("vq_stats", vq_stats);
+  m.impl("adain_frames", adain_frames);
 }

@@ -34,6 +34,14 @@ def _on_device(fn):
     return wrapper
 
 
+def _fusing(feats, wgt):
+    """Whether the SFT fusion blocks run: with skip tensors and a weight above 0 — or a device fp32 tensor of per-frame
+    weights, which callers pass only for frames that all have w > 0 (a w = 0 frame skips the blocks, as the reference
+    does, and the next GroupNorm then reads statistics of the unrounded res-block output, which the fused path does not
+    reproduce)."""
+    return feats is not None and (torch.is_tensor(wgt) or wgt > 0)
+
+
 def _pack_conv(w):
     """OIHW fp32 -> [Cout, k*k*CinPad] bf16 (K index = tap*CinPad + c)."""
     co, ci, kh, kw = w.shape
@@ -304,7 +312,8 @@ class Engine:
 
     def fuse_sft(self, enc, dec, key, wgt, gn_next=False):
         """Fuse_sft_block (`archs/pgtformer_arch.py:460-484`); the final
-        dec + w*(dec*scale + shift) is the epilogue of the last `shift` conv."""
+        dec + w*(dec*scale + shift) is the epilogue of the last `shift` conv.  wgt: w, or a device fp32 [F] tensor of
+        one w per frame of dec."""
         p = 'fuse_convs_dict.' + key
         Fr, H, W, C = dec.shape
         b, P = Fr // 3, H * W
@@ -323,7 +332,8 @@ class Engine:
     def sft_tail(self, cat, dec, p, wgt, gn_next=False):
         """The part of Fuse_sft_block PGTFormer (`archs/pgtformer_arch.py:476-484`) and CodeFormer
         (`archs/codeformer_arch.py:218-226`) share: encode_enc (ResBlock of the concat, 1x1 conv_out shortcut) ->
-        scale / shift branches -> dec + w*(dec*scale + shift) in the epilogue of the last `shift` conv."""
+        scale / shift branches -> dec + w*(dec*scale + shift) in the epilogue of the last `shift` conv (wgt: w, or a
+        device fp32 [F] tensor of per-frame weights)."""
         C = dec.shape[-1]
         e = p + '.encode_enc'
         h = self._conv3(cat, e + '.conv1', C, gn=e + '.norm1', gn_out=True)
@@ -449,14 +459,14 @@ class Engine:
         """Runs blocks[lo:hi] of a block list (spec.Block entries) on h.  Returns (h, {taps[i]: output of block i}).
         outs {i: tensor}: block i (`res`, `swin` or `down`) writes its output there, a slice of an SFT concat buffer or a
         slot of a live ring (live_ring); gn_outs {i: fp32 buffer}: block i (`down`, the last of the frame blocks) writes
-        the GroupNorm statistics it emits for the next block there.  A `fuse` block runs only with feats and wgt > 0, on
-        feats[its src].
+        the GroupNorm statistics it emits for the next block there.  A `fuse` block runs only with feats and wgt > 0 (or
+        a device tensor of per-frame weights, see _fusing), on feats[its src].
 
         GroupNorm statistics: a block passes gn_next to its producer exactly when the next block that runs reads its
         input through a GroupNorm (`res`, `attn`, or the `norm` before conv_out); a `fuse` that does not run is not
         next.  Its epilogue then writes the statistics, and that GroupNorm skips its own pass over the tensor.  (The
         RGB conv_in and `up`, always followed by a `res`, always write them.)"""
-        fusing = feats is not None and wgt > 0
+        fusing = _fusing(feats, wgt)
         hi = len(blocks) if hi is None else hi
         outs, gn_outs, found = outs or {}, gn_outs or {}, {}
         for i in range(lo, hi):
@@ -541,11 +551,12 @@ class Engine:
         """Decoder.forward (`archs/tdcrqvae3_arch.py:672-707`) / the inlined variant with SFT fusion
         (`archs/pgtformer_arch.py:680-710`), or VQGAN's Generator.forward (`archs/vqgan_arch.py:337-341`) / with
         CodeFormer's fusion (`archs/codeformer_arch.py:356-363`).  z: [F,h,w,C] bf16 -> out fp32 NCHW.  A level whose
-        encoder output sits in an SFT concat buffer writes its own output into the decoder half."""
+        encoder output sits in an SFT concat buffer writes its own output into the decoder half.  wgt: w, or a device
+        fp32 [F] tensor of per-frame weights (_fusing)."""
         blocks = self.arch.dec_blocks
         outs = {}
         for i, b in enumerate(blocks):
-            cat = getattr(feats[b.src], '_pgt_cat', None) if b.kind == 'fuse' and feats is not None and wgt > 0 else None
+            cat = getattr(feats[b.src], '_pgt_cat', None) if b.kind == 'fuse' and _fusing(feats, wgt) else None
             if cat is not None:
                 outs[i - 1] = self._cat_half(cat, b.cout, b.cout)
         h, _ = self._walk(blocks, z, 0, len(blocks) - 2, outs=outs, feats=feats, wgt=wgt)
@@ -658,10 +669,11 @@ class Engine:
     def _window_tail(self, rec, index, w, adain, code_only=False, force_codes=None):
         """forward from a per-frame record (_frame_pass, live_ring) on: its entries gathered into clip order by the
         device int32 window index [b*3] (pgt_gather_frames), h's GroupNorm statistics beside h, then encoder_clips and
-        _restore, whose result it returns."""
+        _restore, whose result it returns.  The skip tensors are gathered only when the fusion runs (_fusing)."""
         a = self.arch
         pos = self._gather(rec['pos'], index)
-        feats = {lvl: self._gather(rec['feats'][lvl], index) if lvl in rec['feats'] else None
+        fusing = _fusing(rec['feats'], w)
+        feats = {lvl: self._gather(rec['feats'][lvl], index) if fusing and lvl in rec['feats'] else None
                  for i, lvl in a.enc_taps.items() if i < a.frame_blocks}
         h = self._gather(rec['h'], index)
         if 'h_stats' in rec:
@@ -671,7 +683,9 @@ class Engine:
 
     def _restore(self, h, feats, pos, w, adain, code_only=False, force_codes=None):
         """forward from the encoder's output h [F,h,w,C] on: quant_conv -> global transformer -> argmax (or
-        force_codes) / AdaIN -> post_quant_conv -> decoder with SFT fusion of feats."""
+        force_codes) / AdaIN -> post_quant_conv -> decoder with SFT fusion of feats.  Per frame (the live pool's
+        batches of streams with their own settings): w may be a device fp32 [F] tensor of weights, all > 0 (_fusing),
+        and adain a device int32 [F] tensor of flags (pgt_adain_frames: AdaIN where set, a bf16 rounding elsewhere)."""
         a = self.arch
         Fr, hh, ww, _ = h.shape
         T = Fr * hh * ww
@@ -699,12 +713,15 @@ class Engine:
                 codes = idx_in
             ops.rq_embed(codes, 0, D - 1, wd['codebooks'], quant, ldi=D, ldd=1)
         self.last_codes = codes.view(Fr, hh, ww, D)
-        if adain:
+        if torch.is_tensor(adain):
+            quant = ops.adain(quant.view(Fr, hh * ww, -1), lq.view(Fr, hh * ww, -1), self._new(Fr, hh * ww, a.embed_dim),
+                              flags=adain)
+        elif adain:
             quant = ops.adain(quant.view(Fr, hh * ww, -1), lq.view(Fr, hh * ww, -1), self._new(Fr, hh * ww, a.embed_dim))
         else:
             quant = quant.to(BF)
         z = self._lin(quant.reshape(T, a.embed_dim), 'post_quant_conv', a.z_channels)
-        out = self.decoder(z.view(Fr, hh, ww, a.z_channels), feats, float(w))
+        out = self.decoder(z.view(Fr, hh, ww, a.z_channels), feats, w if torch.is_tensor(w) else float(w))
         return out, logits5, lq_nhwc
 
     @_on_device
@@ -818,7 +835,8 @@ class Engine:
     @torch.no_grad()
     def window_step(self, index, w, adain, ring, out_u8):
         """The windows (f[i-1], f[i], f[i+1]) restored from the ring rows of index (device int32 [3 Bw]), exactly as
-        forward(frame_index=index) computes them.  Writes the middle frames into out_u8 (rgb24 [Bw,H,W,3] uint8)."""
+        forward(frame_index=index) computes them.  Writes the middle frames into out_u8 (rgb24 [Bw,H,W,3] uint8).  w and
+        adain: scalars, or device tensors of one value per frame of index (_restore)."""
         out = self._window_tail(ring, index, w, adain)[0]
         return ops.f32nchw_to_u8hwc(out, out_u8, first=1, step=3)
 
@@ -830,7 +848,8 @@ class Engine:
         go to fp32 in x [>=B,3,H,W] and through frame_step into the ring's staging rows; every ring entry and the rgb24
         frame are then scattered to the frames' slots (slots: device int32 [B]; h's GroupNorm statistics travel as
         their own entry).  Then the windows of index (device int32 [3 Bw], ring rows; None for none) are restored into
-        out_u8 [Bw,H,W,3].  Nothing else is touched, so a step replays from a CUDA graph given its two index tensors."""
+        out_u8 [Bw,H,W,3], with w and adain as window_step takes them.  Nothing else is touched, so a step replays from a
+        CUDA graph given its index tensors (and its per-frame settings)."""
         if slots is not None:
             B, st = slots.numel(), u8.shape[0] // 4 * 3
             xs = ops.u8hwc_to_f32nchw(u8[st:st + B], x[:B])

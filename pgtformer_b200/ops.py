@@ -48,6 +48,8 @@ def _rows(t):
 
 def make_epilogue(out, bias=None, act=ACT_NONE, residual=None, sft_scale=None, sft_w=0.0, nchw=False,
                   relu_after_res=False, gn_stats=None):
+    """sft_w: the SFT fusion weight, a number or (convolutions only) a device fp32 tensor of one weight per output
+    frame."""
     ep = Epilogue()
     ep.flags = 1 if relu_after_res else 0
     if gn_stats is not None:
@@ -64,7 +66,12 @@ def make_epilogue(out, bias=None, act=ACT_NONE, residual=None, sft_scale=None, s
     if sft_scale is not None:
         _, _, lda = _rows(sft_scale)
         assert sft_scale.dtype == torch.bfloat16
-        ep.aux, ep.ldaux, ep.sft_w = sft_scale.data_ptr(), lda, float(sft_w)
+        ep.aux, ep.ldaux = sft_scale.data_ptr(), lda
+        if torch.is_tensor(sft_w):
+            assert sft_w.dtype == torch.float32 and sft_w.is_contiguous() and sft_w.device == out.device
+            ep.sft_wf = sft_w.data_ptr()
+        else:
+            ep.sft_w = float(sft_w)
     ep.out = out.data_ptr()
     ep.out_dtype = _dt(out)
     if nchw:
@@ -97,9 +104,11 @@ def linear(a, w, out, bias=None, act=ACT_NONE, residual=None, K=None, N=None, re
 
 def conv(x, wp, cout, out, ksize=3, stride=1, pad_lo=1, bias=None, act=ACT_NONE, residual=None, sft_scale=None,
          sft_w=0.0, nchw=False, relu_after_res=False, gn_stats=None):
-    """Implicit-GEMM conv on [F,H,W,Cin] bf16 with packed weights wp [>=cout, k*k*CinPad]."""
+    """Implicit-GEMM conv on [F,H,W,Cin] bf16 with packed weights wp [>=cout, k*k*CinPad]; sft_w: a number or a
+    device fp32 [F] tensor of per-frame weights."""
     lib = L.load()
     F, H, W, Cin = x.shape
+    assert not torch.is_tensor(sft_w) or sft_w.numel() == F
     assert x.dtype == torch.bfloat16 and x.stride(3) == 1 and x.stride(1) == W * x.stride(2) and \
         (F == 1 or x.stride(0) == H * x.stride(1))
     ep = make_epilogue(out, bias, act, residual, sft_scale, sft_w, nchw, relu_after_res, gn_stats)
@@ -488,13 +497,20 @@ def vq_stats(z, codebook, idx, HW, beta, scalars, zq_nchw=None, zq_bf16=None, mi
     return scalars
 
 
-def adain(q, style, out, eps=1e-5):
+def adain(q, style, out, eps=1e-5, flags=None):
+    """AdaIN of q [F, HW(, ...), C] against style into bf16 out; flags (device int32 [F]): frames whose flag is 0 are
+    q rounded to bf16 instead (pgt_adain_frames)."""
     lib = L.load()
     F = q.shape[0]
     C = q.shape[-1]
     HW = q.shape[1] * q.shape[2] if q.dim() == 4 else q.shape[1]
-    L.check(lib.pgt_adain(_p(q), _rows(q)[2], _dt(q), _p(style), _rows(style)[2], F, HW, C, eps, _p(out),
-                          _rows(out)[2], _stream()))
+    if flags is None:
+        L.check(lib.pgt_adain(_p(q), _rows(q)[2], _dt(q), _p(style), _rows(style)[2], F, HW, C, eps, _p(out),
+                              _rows(out)[2], _stream()))
+        return out
+    assert flags.dtype == torch.int32 and flags.is_contiguous() and flags.numel() == F and flags.device == q.device
+    L.check(lib.pgt_adain_frames(_p(q), _rows(q)[2], _dt(q), _p(style), _rows(style)[2], F, HW, C, eps, _p(flags),
+                                 _p(out), _rows(out)[2], _stream()))
     return out
 
 

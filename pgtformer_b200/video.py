@@ -19,6 +19,8 @@ each frame's per-frame work runs once into a device ring, and every step can rep
 many such streams on one model, batching the new frames and the windows of every stream that pushes into one step;
 `LiveRestorer` is a pool of one.
 """
+import math
+
 import numpy as np
 import torch
 
@@ -155,6 +157,14 @@ class VideoRestorer:
                 base += drop
 
 
+def _check_w(w):
+    """A fidelity weight from the caller, as a float: NaN and infinities raise ValueError."""
+    w = float(w)
+    if not math.isfinite(w):
+        raise ValueError('w must be finite, got %r' % (w,))
+    return w
+
+
 def _check_frame(frame, hw):
     """A live frame, checked on the host: rgb24 [H,W,3] uint8 (numpy, or a host or CUDA torch tensor) with H and W
     multiples of 64, and of the stream's size hw unless hw is None.  Returns it as a torch tensor or a numpy array."""
@@ -172,40 +182,48 @@ def _check_frame(frame, hw):
 
 class _PoolState:
     """The device state of a LivePool on one engine and frame size: the engine's ring of per-frame results for S
-    streams (Engine.live_ring), the rgb24 frames that produced them (u8, the same rows: 3 s + j % 3 holds frame j of
-    stream s, and rows 3S .. 4S - 1 stage a step's new frames), the fp32 frames of a step, the output frames, the
-    device index buffer (idx[:S]: the new frames' slots, idx[S:]: the windows' ring rows), pinned host buffers and,
-    with cuda_graph, the captured steps.
+    streams (Engine.live_ring; with feats, the SFT skip tensors too), the rgb24 frames that produced them (u8, the same
+    rows: 3 s + j % 3 holds frame j of stream s, and rows 3S .. 4S - 1 stage a step's new frames), the fp32 frames of a
+    step, the output frames, the device step inputs, pinned host buffers and, with cuda_graph, the captured steps.
 
-    A step is (B new frames, Bw windows): Engine.pool_step.  With cuda_graph each distinct (B, Bw) is captured once
-    (Engine._capture) and replayed after its indices are copied into idx: every address a step touches is allocated
-    here, outside the graphs, so the ring carries from one replay to the next and one graph serves every choice of
-    streams.  B and Bw are at most S, so a pool holds at most (S + 1)^2 - 1 graphs; a single stream uses (1, 0),
-    (1, 1) and (0, 1).  They all share one memory pool, replayed one at a time on one stream, so their scratch costs
-    one step's worth."""
+    The step inputs are one int32 buffer, uploaded by one copy: idx[:S] the new frames' slots; idx[S:4S] the windows'
+    ring rows, three per window; idx[4S:7S] the fusion weight of each of those frames (fp32 bits) and idx[7S:10S] its
+    AdaIN flag.  A step is (B new frames, Bw windows, the first Bw0 of them restored without the SFT fusion):
+    Engine.pool_step runs the new frames and those Bw0 windows, Engine.window_step the others with their per-frame
+    weights (all > 0).  With cuda_graph each distinct step is captured once (Engine._capture) and replayed after its
+    inputs are copied into idx: every address a step touches is allocated here, outside the graphs, so the ring carries
+    from one replay to the next and one graph serves every choice of streams and every mix of their settings.  The key
+    is (B, Bw), or (B, Bw, Bw0) when Bw0 > 0; B and Bw are at most S, so a pool holds at most (S + 1)^2 (S + 2) / 2 - 1
+    graphs, and a pool whose streams all take the same path at most (S + 1)^2 - 1; a single stream with w > 0 uses
+    (1, 0), (1, 1) and (0, 1).  They all share one memory pool, replayed one at a time on one stream, so their scratch
+    costs one step's worth."""
 
-    def __init__(self, eng, S, hw, w, adain, cuda_graph):
-        self.eng, self.S, self.hw, self.w, self.adain, self.cuda_graph = eng, S, hw, w, adain, cuda_graph
+    def __init__(self, eng, S, hw, feats, cuda_graph):
+        self.eng, self.S, self.hw, self.feats, self.cuda_graph = eng, S, hw, feats, cuda_graph
         H, W = hw
         dev = eng.dev
         with torch.cuda.device(dev):
-            self.ring = eng.live_ring(H, W, w, S)
+            self.ring = eng.live_ring(H, W, 1.0 if feats else 0.0, S)
             self.u8 = torch.empty(4 * S, H, W, 3, dtype=torch.uint8, device=dev)
             self.x = torch.empty(S, 3, H, W, dtype=torch.float32, device=dev)
             self.out = torch.empty(S, H, W, 3, dtype=torch.uint8, device=dev)
-            self.idx = torch.empty(4 * S, dtype=torch.int32, device=dev)
+            self.idx = torch.empty(10 * S, dtype=torch.int32, device=dev)
         self.host_in = torch.empty(S, H, W, 3, dtype=torch.uint8).pin_memory()
-        self.host_idx = torch.zeros(4 * S, dtype=torch.int32).pin_memory()
+        self.host_idx = torch.zeros(10 * S, dtype=torch.int32).pin_memory()
         self.host_out = torch.empty(S, H, W, 3, dtype=torch.uint8).pin_memory()
         self.loaded = None                 # event: the host buffers have reached the device and may be overwritten
         self.graphs = {}
         self.pool = None
 
-    def run(self, B, Bw):
-        """The step's device work, with its indices already in idx."""
-        S = self.S
-        self.eng.pool_step(self.u8, self.x, self.ring, self.idx[:B] if B else None,
-                           self.idx[S:S + 3 * Bw] if Bw else None, self.w, self.adain, self.out[:Bw])
+    def run(self, B, Bw, Bw0=0):
+        """The step's device work, with its inputs already in idx."""
+        S, n0 = self.S, 3 * Bw0
+        rows, flags = self.idx[S:S + 3 * Bw], self.idx[7 * S:7 * S + 3 * Bw]
+        self.eng.pool_step(self.u8, self.x, self.ring, self.idx[:B] if B else None, rows[:n0] if Bw0 else None, 0.0,
+                           flags[:n0], self.out[:Bw0])
+        if Bw > Bw0:
+            wgt = self.idx[4 * S + n0:4 * S + 3 * Bw].view(torch.float32)
+            self.eng.window_step(rows[n0:], wgt, flags[n0:], self.ring, self.out[Bw0:Bw])
 
     def recompute(self, rows):
         """The per-frame work of the rgb24 frames in u8[rows], into the same ring rows (after new weights)."""
@@ -213,10 +231,13 @@ class _PoolState:
             ops.u8hwc_to_f32nchw(self.u8[r:r + 1], self.x[:1])
             self.eng.frame_step(self.x[:1], r, self.ring)
 
-    def step(self, new, wins):
-        """new: [(ring slot, frame)] of the new frames; wins: [ring rows (a, b, c)] of the windows to restore.  Runs
-        one step on the current stream; returns the restored frames, numpy uint8 [H,W,3] each (one synchronisation)."""
+    def step(self, new, wins, conf):
+        """new: [(ring slot, frame)] of the new frames; wins: [ring rows (a, b, c)] of the windows to restore; conf:
+        [(w, adain)] of each window.  Runs one step on the current stream; returns the restored frames in the order of
+        wins, numpy uint8 [H,W,3] each (one synchronisation)."""
         S, B, Bw = self.S, len(new), len(wins)
+        order = [k for k in range(Bw) if not conf[k][0] > 0] + [k for k in range(Bw) if conf[k][0] > 0]
+        Bw0 = sum(not w > 0 for w, _ in conf)
         if self.loaded is not None:
             self.loaded.synchronize()      # the previous step's uploads (a step without windows does not wait)
         for k, (slot, t) in enumerate(new):
@@ -227,16 +248,21 @@ class _PoolState:
                 self.host_in[k].numpy()[...] = t.numpy() if torch.is_tensor(t) else t
                 row.copy_(self.host_in[k], non_blocking=True)
             self.host_idx[k] = slot
-        self.host_idx[S:S + 3 * Bw] = torch.tensor([r for win in wins for r in win], dtype=torch.int32)
+        self.host_idx[S:S + 3 * Bw] = torch.tensor([r for k in order for r in wins[k]], dtype=torch.int32)
+        self.host_idx[4 * S:4 * S + 3 * Bw].view(torch.float32)[:] = torch.tensor(
+            [max(conf[k][0], 0.0) for k in order for _ in range(3)], dtype=torch.float32)
+        self.host_idx[7 * S:7 * S + 3 * Bw] = torch.tensor([int(conf[k][1]) for k in order for _ in range(3)],
+                                                           dtype=torch.int32)
         self.idx.copy_(self.host_idx, non_blocking=True)
         self.loaded = torch.cuda.Event()
         self.loaded.record()
         if not self.cuda_graph:
-            self.run(B, Bw)
+            self.run(B, Bw, Bw0)
         else:
-            graph = self.graphs.get((B, Bw))
+            key = (B, Bw, Bw0) if Bw0 else (B, Bw)
+            graph = self.graphs.get(key)
             if graph is None:              # the step's writes are idempotent: its warm-up runs leave the ring as is
-                graph = self.graphs[B, Bw] = self.eng._capture(lambda: self.run(B, Bw), self.pool)[0]
+                graph = self.graphs[key] = self.eng._capture(lambda: self.run(B, Bw, Bw0), self.pool)[0]
                 self.pool = graph.pool() if self.pool is None else self.pool
             graph.replay()
         if Bw == 0:
@@ -245,7 +271,9 @@ class _PoolState:
         done = torch.cuda.Event()
         done.record()
         done.synchronize()
-        return [f.copy() for f in self.host_out.numpy()[:Bw]]
+        got = self.host_out.numpy()
+        back = {k: i for i, k in enumerate(order)}
+        return [got[back[k]].copy() for k in range(Bw)]
 
 
 class LivePool:
@@ -257,44 +285,60 @@ class LivePool:
     Each step runs the per-frame work (BiSeNet, the frame blocks of the encoder) of all its new frames as one batch
     into staging rows on the device, scatters the results into each stream's three ring slots, and restores the
     windows of every stream that has one as one batch.  Streams open, stall (a push may list any subset of the open
-    streams) and end independently.  All streams share w, adain and the frame size, which the first frame pushed while
-    the pool holds no frames sets.  Frames are rgb24 [H,W,3] uint8 — numpy, a host torch tensor or a CUDA tensor on
-    the model's device — with H and W multiples of 64; outputs are numpy uint8.  With cuda_graph each distinct
-    (new frames, windows) count replays from one CUDA graph (_PoolState), so streams that push together replay one
-    graph.  The device state belongs to the model's current engine: after load_state_dict(), .to() or refresh() the
-    next step rebuilds it, re-running the per-frame work of every open stream's frames still in a window, from the
-    rgb24 frames the pool keeps on the device.
+    streams) and end independently.  Each stream has its own fidelity weight w and AdaIN switch (open, configure),
+    and may change them between any two calls; all share the frame size, which the first frame pushed while the pool
+    holds no frames sets.  Frames are rgb24 [H,W,3] uint8 — numpy, a host torch tensor or a CUDA tensor on the model's
+    device — with H and W multiples of 64; outputs are numpy uint8.  With cuda_graph each distinct (new frames,
+    windows, windows without fusion) count replays from one CUDA graph (_PoolState), so streams that push together
+    replay one graph whatever their settings.  The device state belongs to the model's current engine: after
+    load_state_dict(), .to() or refresh() the next step rebuilds it, re-running the per-frame work of every open
+    stream's frames still in a window, from the rgb24 frames the pool keeps on the device.  It is rebuilt the same way
+    the first time an open stream has w > 0 on a ring built without the SFT skip tensors (a pool of w = 0 streams does
+    not move them); a ring that has them keeps them until the state is rebuilt for another reason.
 
         pool = LivePool(model, max_streams=8)
-        a, b = pool.open(), pool.open()
+        a, b = pool.open(), pool.open(w=0.5, adain=False)
         pool.push({a: a0, b: b0})     # {a: None, b: None}
         pool.push({a: a1})            # {a: frame 0 of a}
+        pool.configure(a, w=0.0)      # from frame 1 of a on
         pool.push({a: a2, b: b1})     # {a: frame 1 of a, b: frame 0 of b}
         pool.flush(a)                 # frame 2 of a; handle a is freed
     """
 
     def __init__(self, model, max_streams, w=1.0, adain=True, cuda_graph=True):
+        """w, adain: the settings of streams opened without their own."""
         if int(max_streams) < 1:
             raise ValueError('max_streams must be at least 1, got %r' % (max_streams,))
         self.model = model
         self.max_streams = int(max_streams)
-        self.w = float(w)
+        self.w = _check_w(w)
         self.adain = bool(adain)
         self.cuda_graph = bool(cuda_graph)
         self._streams = {}                 # handle -> [stream index s (ring rows 3s .. 3s + 2), frames pushed]
+        self._conf = {}                    # stream index s -> (w, adain) of the stream open there
         self._handles = 0
         self._hw = None
         self._state = None
 
-    def open(self):
-        """A new stream's handle."""
+    def open(self, w=None, adain=None):
+        """A new stream's handle; w and adain default to the pool's."""
+        conf = (self.w if w is None else _check_w(w), self.adain if adain is None else bool(adain))
         if len(self._streams) >= self.max_streams:
             raise ValueError('all %d streams of the pool are open' % self.max_streams)
         s = min(set(range(self.max_streams)) - {v[0] for v in self._streams.values()})
         h = self._handles
         self._handles += 1
         self._streams[h] = [s, 0]
+        self._conf[s] = conf
         return h
+
+    def configure(self, handle, w=None, adain=None):
+        """Changes an open stream's w and / or adain: every window restored after this call uses them, including
+        the frame its next push or flush returns.  A negative w restores as w = 0 does (no fusion), as in the
+        reference."""
+        s, _ = self._stream(handle)
+        cw, ca = self._conf[s]
+        self._conf[s] = (cw if w is None else _check_w(w), ca if adain is None else bool(adain))
 
     def close(self, handle):
         """Frees a stream's handle without restoring its last frame."""
@@ -359,20 +403,24 @@ class LivePool:
 
     # ------------------------------------------------------------------ device
     def _step(self, hw, new, wins):
-        """One step on the state of the model's current engine for frames of size hw; a state built after the weights
-        changed mid-stream first recomputes the ring from the rgb24 frames it still holds."""
+        """One step on the state of the model's current engine for frames of size hw, each window restored with the
+        settings of its stream; a state built mid-stream (new weights or device, or a ring without the SFT skip tensors
+        when a stream has w > 0) first recomputes the ring from the rgb24 frames it still holds.  A state with the skip
+        tensors keeps them while no stream needs them: dropping them would cost a rebuild and new graph captures at
+        every crossing."""
         eng = self.model.engine()
+        feats = any(self._conf[s][0] > 0 for s, _ in self._streams.values())
         state = old = self._state
-        if old is None or old.eng is not eng or old.hw != hw:
+        if old is None or old.eng is not eng or old.hw != hw or (feats and not old.feats):
             self._state = None
-            state = _PoolState(eng, self.max_streams, hw, self.w, self.adain, self.cuda_graph)
-            if old is not None and old.hw == hw and self._holds_frames():   # weights or device changed mid-stream
+            state = _PoolState(eng, self.max_streams, hw, feats, self.cuda_graph)
+            if old is not None and old.hw == hw and self._holds_frames():
                 with torch.cuda.device(eng.dev):
                     state.u8.copy_(old.u8)
                     state.recompute([3 * s + j % 3 for s, n in self._streams.values() for j in range(max(n - 2, 0), n)])
             self._state = state
         with torch.cuda.device(eng.dev):
-            return state.step(new, wins)
+            return state.step(new, wins, [self._conf[win[0] // 3] for win in wins])
 
 
 class LiveRestorer:
@@ -382,7 +430,8 @@ class LiveRestorer:
     Each frame's per-frame work (BiSeNet, the frame blocks of the encoder) runs once, when it is pushed, into a ring of
     three slots on the device; each window is gathered from the ring.  Frames are rgb24 [H,W,3] uint8 — numpy, a host
     torch tensor or a CUDA tensor on the model's device — with H and W multiples of 64; outputs are numpy uint8.  With
-    cuda_graph every step replays from a CUDA graph.  It is the one stream of a LivePool of one.  The device state belongs to the model's current
+    cuda_graph every step replays from a CUDA graph.  configure() changes w and adain between any two calls.  It is the
+    one stream of a LivePool of one.  The device state belongs to the model's current
     engine: after load_state_dict(), .to() or refresh() the next call rebuilds it, re-running the per-frame work of the
     frames still in the window on the new weights.
 
@@ -395,12 +444,22 @@ class LiveRestorer:
 
     def __init__(self, model, w=1.0, adain=True, cuda_graph=True):
         self.model = model
-        self.w = float(w)
+        self.w = _check_w(w)
         self.adain = bool(adain)
         self.cuda_graph = bool(cuda_graph)
         self._pool = LivePool(model, 1, w=w, adain=adain, cuda_graph=cuda_graph)
         self._handle = None
         self.reset()
+
+    def configure(self, w=None, adain=None):
+        """Changes w and / or adain for every window restored after this call, including the frame the next push or
+        flush returns, and for the streams after a reset."""
+        w = self.w if w is None else _check_w(w)
+        adain = self.adain if adain is None else bool(adain)
+        if self._handle is not None:
+            self._pool.configure(self._handle, w, adain)
+        self.w = self._pool.w = w
+        self.adain = self._pool.adain = adain
 
     def reset(self):
         """Forgets the current stream (its frames); the next push starts a new one, of any frame size."""
