@@ -364,8 +364,16 @@ int pgt_nhwc_bf16_to_f32(const void* x, int ldx, int F, int HW, int C, float* y,
  *     frame of every clip.
  *   pgt_gather_frames: y[f] = x[idx[f]] for frames of frame_bytes bytes (multiple of 16); idx: DEVICE int32 [n].
  *   pgt_scatter_frames: y[idx[f]] = x[f], its mirror (the live pool's staging rows into each stream's ring slots);
- *     the idx entries must be distinct. */
+ *     the idx entries must be distinct.
+ *   pgt_u8hwc_resize_to_f32nchw: rgb24 source frames of any size -> fp32 [F, 3, H, W] (H, W multiples of 64; y 16-byte
+ *     aligned): (float)(v / 255.0), then F.interpolate(mode='bilinear', align_corners=True) to H x W as torch
+ *     computes it on an AVX2 / AVX512 host (the low-resolution test input, data/vfhq_full_dataset.py:1046-1051).
+ *     sizes_dev NULL: every frame is h x w, packed one after another from x_u8.  Otherwise DEVICE int32 [F, 3] of
+ *     each frame's (h, w, byte offset from x_u8), all >= 1 (offset >= 0); h, w then bound the table's frames and
+ *     only size the profile's byte count.  pgt_u8hwc_to_f32nchw is kept for frames already at the model's size. */
 int pgt_u8hwc_to_f32nchw(const void* x_u8, int F, int H, int W, float* y, void* stream);
+int pgt_u8hwc_resize_to_f32nchw(const void* x_u8, int F, int h, int w, const int32_t* sizes_dev, int H, int W, float* y,
+                                void* stream);
 int pgt_f32nchw_to_u8hwc(const float* x, int first, int step, int n, int H, int W, void* y_u8, void* stream);
 int pgt_gather_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream);
 int pgt_scatter_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream);

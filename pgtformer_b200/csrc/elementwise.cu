@@ -202,6 +202,71 @@ __global__ void scatter_frames_kernel(const uint4* __restrict__ x, size_t vec_pe
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < vec_per_frame; i += (size_t)gridDim.x * blockDim.x)
     d[i] = __ldg(s + i);
 }
+
+// The low-resolution input of the reference's test set (data/vfhq_full_dataset.py:1046-1051): rgb24 frames of any
+// size, (float)(v / 255.0), then F.interpolate(mode='bilinear', align_corners=True) to the model's H x W.  One output
+// axis position o maps to source rows i0, i1 with weights l0, l1 exactly as torch's CPU kernel computes them, every
+// step in fp32: scale = (in - 1) / (out - 1) (0 for out = 1), src = scale * o, i0 = min(floor(src), in - 1),
+// i1 = i0 + (i0 < in - 1), l1 = clamp(src - i0, 0, 1), l0 = 1 - l1.
+struct LerpAxis {
+  int i0, i1;
+  float l0, l1;
+};
+
+__device__ __forceinline__ LerpAxis lerp_axis(int in, int out, int o) {
+  const float scale = out > 1 ? __fdiv_rn((float)(in - 1), (float)(out - 1)) : 0.f;
+  const float src = __fmul_rn(scale, (float)o);
+  LerpAxis a;
+  a.i0 = min((int)floorf(src), in - 1);
+  a.i1 = a.i0 + (a.i0 < in - 1 ? 1 : 0);
+  a.l1 = fminf(fmaxf(__fsub_rn(src, (float)a.i0), 0.f), 1.f);
+  a.l0 = __fsub_rn(1.f, a.l1);
+  return a;
+}
+
+// Each thread writes four consecutive pixels of one output row (W % 4 == 0), all three planes, as float4 stores.
+// The combination is the one torch's AVX2 / AVX512 kernel evaluates, fma(h0, fma(w0, a, w1 b), h1 fma(w0, c, w1 d)),
+// spelled with explicit intrinsics so that no contraction choice of the compiler changes a bit.
+__global__ void u8hwc_resize_kernel(const uint8_t* __restrict__ x, int h, int w, const int* __restrict__ sizes, int H,
+                                    int W, size_t total, float* __restrict__ y) {
+  __shared__ float unit[256];
+  for (int v = threadIdx.x; v < 256; v += blockDim.x) unit[v] = __double2float_rn(__ddiv_rn((double)v, 255.0));
+  __syncthreads();
+  const int qw = W >> 2;
+  const size_t HW = (size_t)H * W;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t row = i / qw;
+    const int ox = (int)(i - row * qw) << 2;
+    const int f = (int)(row / H), oy = (int)(row - (size_t)f * H);
+    int fh = h, fw = w;
+    size_t off = (size_t)f * h * w * 3;
+    if (sizes != nullptr) {
+      fh = __ldg(sizes + 3 * f);
+      fw = __ldg(sizes + 3 * f + 1);
+      off = (size_t)(unsigned)__ldg(sizes + 3 * f + 2);
+    }
+    const LerpAxis ay = lerp_axis(fh, H, oy);
+    const uint8_t* r0 = x + off + (size_t)ay.i0 * fw * 3;
+    const uint8_t* r1 = x + off + (size_t)ay.i1 * fw * 3;
+    float o[3][4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const LerpAxis ax = lerp_axis(fw, W, ox + k);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float a = unit[r0[ax.i0 * 3 + c]], b = unit[r0[ax.i1 * 3 + c]];
+        const float cc = unit[r1[ax.i0 * 3 + c]], d = unit[r1[ax.i1 * 3 + c]];
+        const float top = __fmaf_rn(ax.l0, a, __fmul_rn(ax.l1, b));
+        const float bot = __fmaf_rn(ax.l0, cc, __fmul_rn(ax.l1, d));
+        o[c][k] = __fmaf_rn(ay.l0, top, __fmul_rn(ay.l1, bot));
+      }
+    }
+    float* dst = y + (size_t)f * 3 * HW + (size_t)oy * W + ox;
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      *reinterpret_cast<float4*>(dst + c * HW) = make_float4(o[c][0], o[c][1], o[c][2], o[c][3]);
+  }
+}
 }  // namespace pgt
 
 extern "C" int pgt_u8hwc_to_f32nchw(const void* x_u8, int F, int H, int W, float* y, void* stream) {
@@ -216,6 +281,19 @@ extern "C" int pgt_u8hwc_to_f32nchw(const void* x_u8, int F, int H, int W, float
   ProfScope ps(PGT_PROF_MOVE, 15.0 * (double)total, static_cast<cudaStream_t>(stream), "pgt_u8hwc_to_f32nchw");
   pgt::u8hwc_to_f32nchw_kernel<<<ew_grid(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint8_t*>(x_u8), HW, total, y);
+  PGT_LAUNCH_OK();
+  return PGT_OK;
+}
+
+extern "C" int pgt_u8hwc_resize_to_f32nchw(const void* x_u8, int F, int h, int w, const int32_t* sizes_dev, int H,
+                                           int W, float* y, void* stream) {
+  PGT_CHECK_ARG(x_u8 && y && F > 0 && h > 0 && w > 0 && H > 0 && W > 0 && H % 64 == 0 && W % 64 == 0);
+  PGT_CHECK_ARG((reinterpret_cast<uintptr_t>(y) & 15) == 0);
+  const size_t total = (size_t)F * H * (W / 4);
+  ProfScope ps(PGT_PROF_MOVE, 12.0 * F * (double)H * W + 3.0 * F * (double)h * w, static_cast<cudaStream_t>(stream),
+               "pgt_u8hwc_resize_to_f32nchw");
+  pgt::u8hwc_resize_kernel<<<ew_grid(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint8_t*>(x_u8), h, w, sizes_dev, H, W, total, y);
   PGT_LAUNCH_OK();
   return PGT_OK;
 }

@@ -235,6 +235,26 @@ void adain_frames(const at::Tensor& q, const at::Tensor& style, const at::Tensor
                          out.data_ptr(), ld(out), stream_of(q)), "adain_frames");
 }
 
+void u8hwc_resize_to_f32nchw(const at::Tensor& x, int64_t h, int64_t w, const c10::optional<at::Tensor>& sizes,
+                             at::Tensor out) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kByte && x.is_contiguous() && out.scalar_type() == at::kFloat &&
+              out.is_contiguous() && out.dim() == 4 && out.size(1) == 3,
+              "u8hwc_resize_to_f32nchw: contiguous uint8 x, contiguous fp32 out [F, 3, H, W]");
+  TORCH_CHECK(out.device() == x.device(), "u8hwc_resize_to_f32nchw: x and out on one device");
+  const int64_t F = out.size(0);
+  const int32_t* sp = nullptr;
+  if (sizes.has_value()) {
+    TORCH_CHECK(sizes->scalar_type() == at::kInt && sizes->is_contiguous() && sizes->numel() == 3 * F &&
+                sizes->device() == x.device(), "u8hwc_resize_to_f32nchw: int32 sizes [F, 3] on x's device");
+    sp = sizes->data_ptr<int32_t>();
+  } else {
+    TORCH_CHECK(x.numel() >= F * h * w * 3, "u8hwc_resize_to_f32nchw: x holds fewer than F h w 3 bytes");
+  }
+  c10::cuda::CUDAGuard guard(x.device());
+  check(pgt_u8hwc_resize_to_f32nchw(x.data_ptr(), (int)F, (int)h, (int)w, sp, (int)out.size(2), (int)out.size(3),
+                                    out.data_ptr<float>(), stream_of(x)), "u8hwc_resize_to_f32nchw");
+}
+
 }  // namespace
 
 TORCH_LIBRARY(pgt, m) {
@@ -254,6 +274,7 @@ TORCH_LIBRARY(pgt, m) {
   m.def("vq_stats(Tensor z, Tensor codebook, Tensor idx, int HW, float beta, Tensor(a!) scalars, Tensor(b!)? zq_nchw, "
         "Tensor(c!)? zq_bf16, Tensor(d!)? min_enc, Tensor(e!)? scores, Tensor(f!)? usage) -> ()");
   m.def("adain_frames(Tensor q, Tensor style, Tensor flags, float eps, Tensor(a!) out) -> ()");
+  m.def("u8hwc_resize_to_f32nchw(Tensor x, int h, int w, Tensor? sizes, Tensor(a!) out) -> ()");
 }
 
 TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
@@ -271,4 +292,5 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("conv_out_gn_act", conv_out_gn_act);
   m.impl("vq_stats", vq_stats);
   m.impl("adain_frames", adain_frames);
+  m.impl("u8hwc_resize_to_f32nchw", u8hwc_resize_to_f32nchw);
 }

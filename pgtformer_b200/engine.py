@@ -791,11 +791,18 @@ class Engine:
     # ------------------------------------------------------------------ video: batched windows and the live ring
     @_on_device
     @torch.no_grad()
-    def restore_windows(self, frames_u8, index, w=1.0, adain=True, reuse_frames=True):
+    def restore_windows(self, frames_u8, index, w=1.0, adain=True, reuse_frames=True, size=None):
         """One batch of VideoRestorer: rgb24 frames [Fd,H,W,3] uint8 on the device and the device int32 window index
-        [3n] into them -> the restored middle frames, rgb24 [n,H,W,3] uint8 on the device."""
-        Fd, H, W, _ = frames_u8.shape
-        x = ops.u8hwc_to_f32nchw(frames_u8, self._new(Fd, 3, H, W, dtype=torch.float32))
+        [3n] into them -> the restored middle frames, rgb24 [n,H,W,3] uint8 on the device.  size = (H, W): the frames
+        are [Fd,h,w,3] sources of any size, upsampled to H x W as the reference's test set does
+        (ops.u8hwc_resize_to_f32nchw)."""
+        Fd, h, w_src, _ = frames_u8.shape
+        if size is None:
+            H, W = h, w_src
+            x = ops.u8hwc_to_f32nchw(frames_u8, self._new(Fd, 3, H, W, dtype=torch.float32))
+        else:
+            H, W = size
+            x = ops.u8hwc_resize_to_f32nchw(frames_u8, self._new(Fd, 3, H, W, dtype=torch.float32), (h, w_src))
         if reuse_frames:
             out = self.forward(x, w=w, adain=adain, frame_index=index)[0]
         else:
@@ -842,17 +849,22 @@ class Engine:
 
     @_on_device
     @torch.no_grad()
-    def pool_step(self, u8, x, ring, slots, index, w, adain, out_u8):
+    def pool_step(self, u8, x, ring, slots, index, w, adain, out_u8, sizes=None):
         """One step of a pool of live streams (video.LivePool) on a live_ring of S streams and its rgb24 frames u8
         [4S,H,W,3] (the same rows).  The B = slots.numel() new frames, already in u8's staging rows 3S .. 3S + B - 1,
         go to fp32 in x [>=B,3,H,W] and through frame_step into the ring's staging rows; every ring entry and the rgb24
         frame are then scattered to the frames' slots (slots: device int32 [B]; h's GroupNorm statistics travel as
         their own entry).  Then the windows of index (device int32 [3 Bw], ring rows; None for none) are restored into
-        out_u8 [Bw,H,W,3], with w and adain as window_step takes them.  Nothing else is touched, so a step replays from a
-        CUDA graph given its index tensors (and its per-frame settings)."""
+        out_u8 [Bw,H,W,3], with w and adain as window_step takes them.  sizes (device int32 [B, 3]): the staging rows
+        hold source frames of (h, w) at a byte offset from row 3S, each upsampled to H x W
+        (ops.u8hwc_resize_to_f32nchw); None: frames at H x W.  Nothing else is touched, so a step replays from a CUDA
+        graph given its index tensors (and its per-frame settings and source sizes)."""
         if slots is not None:
             B, st = slots.numel(), u8.shape[0] // 4 * 3
-            xs = ops.u8hwc_to_f32nchw(u8[st:st + B], x[:B])
+            if sizes is None:
+                xs = ops.u8hwc_to_f32nchw(u8[st:st + B], x[:B])
+            else:
+                xs = ops.u8hwc_resize_to_f32nchw(u8[st:st + B], x[:B], tuple(u8.shape[1:3]), sizes)
             self.frame_step(xs, st, ring)
             for t in self.ring_entries(ring) + [u8]:
                 ops.scatter_frames(t[st:st + B], slots, t)

@@ -556,6 +556,26 @@ def u8hwc_to_f32nchw(x_u8, out):
     return out
 
 
+def u8hwc_resize_to_f32nchw(x_u8, out, hw, sizes=None):
+    """rgb24 source frames -> fp32 out [F,3,H,W]: (float)(v / 255.0), then bilinear with align_corners=True to H x W,
+    bit for bit what F.interpolate gives on an AVX2 / AVX512 host (data/vfhq_full_dataset.py:1046-1051).  x_u8: uint8
+    on the device holding the frames.  sizes None: every frame is hw = (h, w), packed one after another from x_u8's
+    first byte.  sizes: device int32 [F, 3] of each frame's (h, w, byte offset from x_u8's first byte); hw then bounds
+    them and only sizes the profile's byte count."""
+    lib = L.load()
+    F, C, H, W = out.shape
+    h, w = hw
+    assert x_u8.dtype == torch.uint8 and x_u8.is_contiguous() and x_u8.is_cuda
+    assert C == 3 and out.dtype == torch.float32 and out.is_contiguous() and out.device == x_u8.device
+    if sizes is None:
+        assert x_u8.numel() >= F * h * w * 3
+    else:
+        assert sizes.dtype == torch.int32 and sizes.is_contiguous() and sizes.numel() == 3 * F and \
+            sizes.device == x_u8.device
+    L.check(lib.pgt_u8hwc_resize_to_f32nchw(_p(x_u8), F, h, w, _p(sizes), H, W, _p(out), _stream()))
+    return out
+
+
 def f32nchw_to_u8hwc(x, out_u8, first=0, step=1):
     """uint8(clamp(x, 0, 1) * 255) of frames first, first+step, ... -> rgb24 [n,H,W,3] (inference.py:15-19)."""
     lib = L.load()

@@ -43,6 +43,11 @@ def plan_batches(n, clips_per_batch):
 
 
 class VideoRestorer:
+    """restore() and stream() take size = (H, W), multiples of 64: frames of any size are then restored at H x W, each
+    upsampled on the device as the reference's test set feeds its low-resolution frames to the model (bilinear,
+    align_corners=True; ops.u8hwc_resize_to_f32nchw); the pinned host buffers and the host-to-device copies carry the
+    source frames, and outputs are rgb24 at H x W.  size is checked when the call is made, before any device work."""
+
     def __init__(self, model, w=1.0, adain=True, clips_per_batch=16, reuse_frames=True, cuda_graph=False):
         """cuda_graph: replay each batch from a CUDA graph (Engine.graphed, one per batch shape), which removes the
         host cost of its launches; the bytes written are the eager ones."""
@@ -54,34 +59,38 @@ class VideoRestorer:
         self.cuda_graph = bool(cuda_graph)
 
     # ------------------------------------------------------------------ one batch of windows on the device
-    def _enqueue(self, frames_u8_dev, local_windows):
+    def _enqueue(self, frames_u8_dev, local_windows, size=None):
         """frames_u8_dev: uint8 [Fd,H,W,3] on the device (distinct frames lo..hi); local_windows: [(a,b,c)] indices
         into it.  Returns uint8 [count,H,W,3] on the device (the restored middle frames; with cuda_graph, the graph's
-        static output, to be consumed before the next batch)."""
+        static output, to be consumed before the next batch); with size, [count,*size,3]."""
         eng = self.model.engine()
         idx = torch.tensor([j for win in local_windows for j in win], dtype=torch.int32).to(eng.dev, non_blocking=True)
         if self.cuda_graph:
             return eng.graphed(eng.restore_windows, (frames_u8_dev, idx), w=self.w, adain=self.adain,
-                               reuse_frames=self.reuse_frames)
-        return eng.restore_windows(frames_u8_dev, idx, w=self.w, adain=self.adain, reuse_frames=self.reuse_frames)
+                               reuse_frames=self.reuse_frames, size=size)
+        return eng.restore_windows(frames_u8_dev, idx, w=self.w, adain=self.adain, reuse_frames=self.reuse_frames,
+                                   size=size)
 
-    def _run_batch(self, frames_u8, local_windows):
+    def _run_batch(self, frames_u8, local_windows, size=None):
         """Host uint8 [Fd,H,W,3] + window index triples -> host uint8 [count,H,W,3] (synchronous; `stream()` uses it)."""
         dev = self.model.engine().dev
         d = torch.from_numpy(np.ascontiguousarray(frames_u8)).pin_memory().to(dev, non_blocking=True)
-        return self._enqueue(d, local_windows).cpu().numpy()
+        return self._enqueue(d, local_windows, size).cpu().numpy()
 
     # ------------------------------------------------------------------ whole sequence in memory
     @torch.no_grad()
-    def restore(self, frames_u8):
-        """frames_u8: uint8 [N,H,W,3] (numpy or torch, host).  Returns numpy uint8 [N,H,W,3]."""
+    def restore(self, frames_u8, size=None):
+        """frames_u8: uint8 [N,H,W,3] (numpy or torch, host).  Returns numpy uint8 [N,H,W,3] ([N,*size,3] with
+        size)."""
+        size = _check_size(size)
         frames = torch.as_tensor(np.ascontiguousarray(frames_u8)) if not torch.is_tensor(frames_u8) else frames_u8
         if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3:
             raise ValueError('expected rgb24 frames [N,H,W,3] uint8, got %s %s' % (tuple(frames.shape), frames.dtype))
         n = frames.shape[0]
+        shape = (n,) + (size or tuple(frames.shape[1:3])) + (3,)
         if n == 0:
-            return np.zeros((0,) + tuple(frames.shape[1:]), np.uint8)
-        out = torch.empty(frames.shape, dtype=torch.uint8).pin_memory()
+            return np.zeros(shape, np.uint8)
+        out = torch.empty(shape, dtype=torch.uint8).pin_memory()
         dev = self.model.engine().dev
         main = torch.cuda.current_stream(dev)
         copy = torch.cuda.Stream(dev)
@@ -107,7 +116,7 @@ class VideoRestorer:
             main.wait_event(ev)
             if self.cuda_graph and copied is not None:
                 main.wait_event(copied)                              # a replay rewrites the static output being copied
-            res = self._enqueue(d, [tuple(j - lo for j in wins[i]) for i in range(first, first + cnt)])
+            res = self._enqueue(d, [tuple(j - lo for j in wins[i]) for i in range(first, first + cnt)], size)
             done = torch.cuda.Event()
             done.record(main)
             with torch.cuda.stream(copy):                            # D2H overlaps the next batch's compute
@@ -123,10 +132,14 @@ class VideoRestorer:
         return out.numpy()
 
     # ------------------------------------------------------------------ iterator in, iterator out (bounded memory)
-    @torch.no_grad()
-    def stream(self, frame_iter):
+    def stream(self, frame_iter, size=None):
         """Yields restored rgb24 frames for an iterator of rgb24 frames [H,W,3] uint8, `clips_per_batch` windows per
         launch; the last frame of a batch needs its successor, so output lags the input by one batch."""
+        return self._stream(frame_iter, _check_size(size))
+
+    @torch.no_grad()
+    def _stream(self, frame_iter, size):
+        run_batch = self._run_batch if size is None else lambda f, wins: self._run_batch(f, wins, size)
         buf, base, total_in, emitted = [], 0, 0, 0       # buf[k] is frame base + k
         it = iter(frame_iter)
         ended = False
@@ -147,7 +160,7 @@ class VideoRestorer:
             lo = max(emitted - 1, 0)
             hi = min(emitted + cnt, n_known - 1)
             local = [(max(i - 1, 0) - lo, i - lo, min(i + 1, n_known - 1) - lo) for i in range(emitted, emitted + cnt)]
-            res = self._run_batch(np.stack(buf[lo - base:hi - base + 1]), local)
+            res = run_batch(np.stack(buf[lo - base:hi - base + 1]), local)
             for k in range(cnt):
                 yield res[k]
             emitted += cnt
@@ -165,16 +178,35 @@ def _check_w(w):
     return w
 
 
-def _check_frame(frame, hw):
+def _check_size(size):
+    """The model size (H, W) a video is restored at, as a tuple of ints (None stays None): multiples of 64, else
+    ValueError."""
+    if size is None:
+        return None
+    try:
+        H, W = (int(v) for v in size)
+    except (TypeError, ValueError):
+        raise ValueError('size must be (H, W), got %r' % (size,)) from None
+    if H <= 0 or W <= 0 or H % 64 or W % 64:
+        raise ValueError('size must be multiples of 64, got %dx%d' % (H, W))
+    return H, W
+
+
+def _check_frame(frame, hw, size=None):
     """A live frame, checked on the host: rgb24 [H,W,3] uint8 (numpy, or a host or CUDA torch tensor) with H and W
-    multiples of 64, and of the stream's size hw unless hw is None.  Returns it as a torch tensor or a numpy array."""
+    multiples of 64, and of the stream's size hw unless hw is None.  With the model size `size` = (H, W) the frame is
+    a source of any h, w >= 1 with h w <= H W (it is staged in a row of H W 3 bytes).  Returns it as a torch tensor or
+    a numpy array."""
     t = frame if torch.is_tensor(frame) else np.asarray(frame)
     u8 = t.dtype == (torch.uint8 if torch.is_tensor(t) else np.uint8)
     if not u8 or t.ndim != 3 or t.shape[-1] != 3:
         raise ValueError('expected an rgb24 frame [H,W,3] uint8, got %s %s' % (tuple(t.shape), t.dtype))
     H, W = int(t.shape[0]), int(t.shape[1])
-    if H % 64 or W % 64 or H == 0 or W == 0:
+    if size is None and (H % 64 or W % 64 or H == 0 or W == 0):
         raise ValueError('expected H, W multiples of 64, got %dx%d' % (H, W))
+    if size is not None and (H == 0 or W == 0 or H * W > size[0] * size[1]):
+        raise ValueError('expected a source frame of at most %d pixels (the model size %dx%d), got %dx%d'
+                         % ((size[0] * size[1],) + size + (H, W)))
     if hw is not None and (H, W) != hw:
         raise ValueError('frame size changed inside a stream: %dx%d after %dx%d' % ((H, W) + hw))
     return t
@@ -186,30 +218,33 @@ class _PoolState:
     rows: 3 s + j % 3 holds frame j of stream s, and rows 3S .. 4S - 1 stage a step's new frames), the fp32 frames of a
     step, the output frames, the device step inputs, pinned host buffers and, with cuda_graph, the captured steps.
 
-    The step inputs are one int32 buffer, uploaded by one copy: idx[:S] the new frames' slots; idx[S:4S] the windows'
-    ring rows, three per window; idx[4S:7S] the fusion weight of each of those frames (fp32 bits) and idx[7S:10S] its
-    AdaIN flag.  A step is (B new frames, Bw windows, the first Bw0 of them restored without the SFT fusion):
-    Engine.pool_step runs the new frames and those Bw0 windows, Engine.window_step the others with their per-frame
-    weights (all > 0).  With cuda_graph each distinct step is captured once (Engine._capture) and replayed after its
-    inputs are copied into idx: every address a step touches is allocated here, outside the graphs, so the ring carries
-    from one replay to the next and one graph serves every choice of streams and every mix of their settings.  The key
-    is (B, Bw), or (B, Bw, Bw0) when Bw0 > 0; B and Bw are at most S, so a pool holds at most (S + 1)^2 (S + 2) / 2 - 1
-    graphs, and a pool whose streams all take the same path at most (S + 1)^2 - 1; a single stream with w > 0 uses
-    (1, 0), (1, 1) and (0, 1).  They all share one memory pool, replayed one at a time on one stream, so their scratch
-    costs one step's worth."""
+    The step inputs are one int32 buffer, uploaded by one copy: idx[:S] the new frames' slots; idx[S:4S] the
+    windows' ring rows, three per window; idx[4S:7S] the fusion weight of each of those frames (fp32 bits) and
+    idx[7S:10S] its AdaIN flag.  In a pool of source frames (lr), idx[10S:13S] holds each new frame's (h, w, byte
+    offset from staging row 3S): its rgb24 row holds the source frame packed from the row's first byte, and the step
+    upsamples it to the model size hw (Engine.pool_step).  A step is (B new frames, Bw windows, the first Bw0 of them
+    restored without the SFT fusion): Engine.pool_step runs the new frames and those Bw0 windows, Engine.window_step
+    the others with their per-frame weights (all > 0).  With cuda_graph each distinct step is captured once
+    (Engine._capture) and replayed after its inputs are copied into idx: every address a step touches is allocated
+    here, outside the graphs, so the ring carries from one replay to the next and one graph serves every choice of
+    streams and every mix of their settings.  The key is (B, Bw), or (B, Bw, Bw0) when Bw0 > 0; B and Bw are at most
+    S, so a pool holds at most (S + 1)^2 (S + 2) / 2 - 1 graphs, and a pool whose streams all take the same path at
+    most (S + 1)^2 - 1; a single stream with w > 0 uses (1, 0), (1, 1) and (0, 1).  They all share one memory pool,
+    replayed one at a time on one stream, so their scratch costs one step's worth."""
 
-    def __init__(self, eng, S, hw, feats, cuda_graph):
-        self.eng, self.S, self.hw, self.feats, self.cuda_graph = eng, S, hw, feats, cuda_graph
+    def __init__(self, eng, S, hw, feats, cuda_graph, lr=False):
+        self.eng, self.S, self.hw, self.feats, self.cuda_graph, self.lr = eng, S, hw, feats, cuda_graph, lr
         H, W = hw
+        n_idx = 13 * S if lr else 10 * S
         dev = eng.dev
         with torch.cuda.device(dev):
             self.ring = eng.live_ring(H, W, 1.0 if feats else 0.0, S)
             self.u8 = torch.empty(4 * S, H, W, 3, dtype=torch.uint8, device=dev)
             self.x = torch.empty(S, 3, H, W, dtype=torch.float32, device=dev)
             self.out = torch.empty(S, H, W, 3, dtype=torch.uint8, device=dev)
-            self.idx = torch.empty(10 * S, dtype=torch.int32, device=dev)
+            self.idx = torch.empty(n_idx, dtype=torch.int32, device=dev)
         self.host_in = torch.empty(S, H, W, 3, dtype=torch.uint8).pin_memory()
-        self.host_idx = torch.zeros(10 * S, dtype=torch.int32).pin_memory()
+        self.host_idx = torch.zeros(n_idx, dtype=torch.int32).pin_memory()
         self.host_out = torch.empty(S, H, W, 3, dtype=torch.uint8).pin_memory()
         self.loaded = None                 # event: the host buffers have reached the device and may be overwritten
         self.graphs = {}
@@ -219,16 +254,21 @@ class _PoolState:
         """The step's device work, with its inputs already in idx."""
         S, n0 = self.S, 3 * Bw0
         rows, flags = self.idx[S:S + 3 * Bw], self.idx[7 * S:7 * S + 3 * Bw]
+        kw = {'sizes': self.idx[10 * S:10 * S + 3 * B]} if self.lr and B else {}
         self.eng.pool_step(self.u8, self.x, self.ring, self.idx[:B] if B else None, rows[:n0] if Bw0 else None, 0.0,
-                           flags[:n0], self.out[:Bw0])
+                           flags[:n0], self.out[:Bw0], **kw)
         if Bw > Bw0:
             wgt = self.idx[4 * S + n0:4 * S + 3 * Bw].view(torch.float32)
             self.eng.window_step(rows[n0:], wgt, flags[n0:], self.ring, self.out[Bw0:Bw])
 
-    def recompute(self, rows):
-        """The per-frame work of the rgb24 frames in u8[rows], into the same ring rows (after new weights)."""
-        for r in rows:
-            ops.u8hwc_to_f32nchw(self.u8[r:r + 1], self.x[:1])
+    def recompute(self, rows, srcs=None):
+        """The per-frame work of the rgb24 frames in u8[rows], into the same ring rows (after new weights); srcs: the
+        (h, w) of each row's source frame in a pool of source frames (lr), upsampled again."""
+        for k, r in enumerate(rows):
+            if self.lr:
+                ops.u8hwc_resize_to_f32nchw(self.u8[r:r + 1], self.x[:1], srcs[k])
+            else:
+                ops.u8hwc_to_f32nchw(self.u8[r:r + 1], self.x[:1])
             self.eng.frame_step(self.x[:1], r, self.ring)
 
     def step(self, new, wins, conf):
@@ -241,12 +281,16 @@ class _PoolState:
         if self.loaded is not None:
             self.loaded.synchronize()      # the previous step's uploads (a step without windows does not wait)
         for k, (slot, t) in enumerate(new):
-            row = self.u8[3 * S + k]
+            row, host = self.u8[3 * S + k], self.host_in[k]
+            if self.lr:                    # the source frame, packed from the row's first byte
+                h, w = int(t.shape[0]), int(t.shape[1])
+                row, host = row.view(-1)[:h * w * 3].view(h, w, 3), host.view(-1)[:h * w * 3].view(h, w, 3)
+                self.host_idx[10 * S + 3 * k:10 * S + 3 * k + 3] = torch.tensor([h, w, k * self.u8[0].numel()])
             if torch.is_tensor(t) and t.is_cuda:
                 row.copy_(t, non_blocking=True)
             else:
-                self.host_in[k].numpy()[...] = t.numpy() if torch.is_tensor(t) else t
-                row.copy_(self.host_in[k], non_blocking=True)
+                host.numpy()[...] = t.numpy() if torch.is_tensor(t) else t
+                row.copy_(host, non_blocking=True)
             self.host_idx[k] = slot
         self.host_idx[S:S + 3 * Bw] = torch.tensor([r for k in order for r in wins[k]], dtype=torch.int32)
         self.host_idx[4 * S:4 * S + 3 * Bw].view(torch.float32)[:] = torch.tensor(
@@ -296,6 +340,12 @@ class LivePool:
     the first time an open stream has w > 0 on a ring built without the SFT skip tensors (a pool of w = 0 streams does
     not move them); a ring that has them keeps them until the state is rebuilt for another reason.
 
+    size = (H, W), multiples of 64: streams of low-resolution sources, restored at H x W.  Each new frame is upsampled
+    on the device as the reference's test set feeds its low-resolution frames to the model (bilinear,
+    align_corners=True; ops.u8hwc_resize_to_f32nchw), and only its source bytes cross to the device.  Each stream's
+    source size, any h x w with h w <= H W, is set by its first frame; streams of different source sizes share steps
+    and graphs.  Outputs are rgb24 at H x W.
+
         pool = LivePool(model, max_streams=8)
         a, b = pool.open(), pool.open(w=0.5, adain=False)
         pool.push({a: a0, b: b0})     # {a: None, b: None}
@@ -305,10 +355,14 @@ class LivePool:
         pool.flush(a)                 # frame 2 of a; handle a is freed
     """
 
-    def __init__(self, model, max_streams, w=1.0, adain=True, cuda_graph=True):
+    def __init__(self, model, max_streams, w=1.0, adain=True, cuda_graph=True, size=None):
         """w, adain: the settings of streams opened without their own."""
         if int(max_streams) < 1:
             raise ValueError('max_streams must be at least 1, got %r' % (max_streams,))
+        self.size = _check_size(size)
+        if self.size is not None and int(max_streams) * self.size[0] * self.size[1] * 3 >= 2 ** 31:
+            raise ValueError('%d streams of %dx%d frames overflow the int32 staging offsets'
+                             % ((int(max_streams),) + self.size))
         self.model = model
         self.max_streams = int(max_streams)
         self.w = _check_w(w)
@@ -316,6 +370,7 @@ class LivePool:
         self.cuda_graph = bool(cuda_graph)
         self._streams = {}                 # handle -> [stream index s (ring rows 3s .. 3s + 2), frames pushed]
         self._conf = {}                    # stream index s -> (w, adain) of the stream open there
+        self._src = {}                     # stream index s -> (h, w) of its source frames (with size)
         self._handles = 0
         self._hw = None
         self._state = None
@@ -330,6 +385,7 @@ class LivePool:
         self._handles += 1
         self._streams[h] = [s, 0]
         self._conf[s] = conf
+        self._src.pop(s, None)
         return h
 
     def configure(self, handle, w=None, adain=None):
@@ -363,11 +419,14 @@ class LivePool:
         hw = self._hw if self._holds_frames() else None
         checked, dev = {}, None
         for h, f in items:
-            self._stream(h)
+            s, n = self._stream(h)
             if h in checked:
                 raise ValueError('stream handle %r listed twice' % (h,))
-            t = checked[h] = _check_frame(f, hw)
-            hw = (int(t.shape[0]), int(t.shape[1]))
+            if self.size is None:
+                t = checked[h] = _check_frame(f, hw)
+                hw = (int(t.shape[0]), int(t.shape[1]))
+            else:                          # each stream keeps the source size of its first frame
+                t = checked[h] = _check_frame(f, self._src[s] if n else None, self.size)
             if torch.is_tensor(t) and t.is_cuda:
                 dev = dev or next(self.model.parameters()).device
                 if t.device != dev:
@@ -381,10 +440,13 @@ class LivePool:
             if n > 0:
                 wins.append(tuple(3 * s + j % 3 for j in (max(n - 2, 0), n - 1, n)))
                 order.append(h)
+        hw = hw or self.size
         got = self._step(hw, new, wins)
         self._hw = hw
-        for h in checked:
+        for h, t in checked.items():
             self._streams[h][1] += 1
+            if self.size is not None:
+                self._src[self._streams[h][0]] = (int(t.shape[0]), int(t.shape[1]))
         out = dict.fromkeys(checked)
         out.update(zip(order, got))
         return out
@@ -413,11 +475,12 @@ class LivePool:
         state = old = self._state
         if old is None or old.eng is not eng or old.hw != hw or (feats and not old.feats):
             self._state = None
-            state = _PoolState(eng, self.max_streams, hw, feats, self.cuda_graph)
+            state = _PoolState(eng, self.max_streams, hw, feats, self.cuda_graph, self.size is not None)
             if old is not None and old.hw == hw and self._holds_frames():
+                live = [(s, j) for s, n in self._streams.values() for j in range(max(n - 2, 0), n)]
                 with torch.cuda.device(eng.dev):
                     state.u8.copy_(old.u8)
-                    state.recompute([3 * s + j % 3 for s, n in self._streams.values() for j in range(max(n - 2, 0), n)])
+                    state.recompute([3 * s + j % 3 for s, j in live], [self._src.get(s) for s, _ in live])
             self._state = state
         with torch.cuda.device(eng.dev):
             return state.step(new, wins, [self._conf[win[0] // 3] for win in wins])
@@ -433,7 +496,8 @@ class LiveRestorer:
     cuda_graph every step replays from a CUDA graph.  configure() changes w and adain between any two calls.  It is the
     one stream of a LivePool of one.  The device state belongs to the model's current
     engine: after load_state_dict(), .to() or refresh() the next call rebuilds it, re-running the per-frame work of the
-    frames still in the window on the new weights.
+    frames still in the window on the new weights.  size = (H, W): a low-resolution source of any h x w with
+    h w <= H W, restored at H x W as LivePool(size=...) does.
 
         live = LiveRestorer(model)
         live.push(f0)     # None
@@ -442,12 +506,13 @@ class LiveRestorer:
         live.flush()      # frame 2, window (1, 2, 2); then ready for a new stream
     """
 
-    def __init__(self, model, w=1.0, adain=True, cuda_graph=True):
+    def __init__(self, model, w=1.0, adain=True, cuda_graph=True, size=None):
         self.model = model
         self.w = _check_w(w)
         self.adain = bool(adain)
         self.cuda_graph = bool(cuda_graph)
-        self._pool = LivePool(model, 1, w=w, adain=adain, cuda_graph=cuda_graph)
+        self._pool = LivePool(model, 1, w=w, adain=adain, cuda_graph=cuda_graph, size=size)
+        self.size = self._pool.size
         self._handle = None
         self.reset()
 
@@ -473,7 +538,7 @@ class LiveRestorer:
     @torch.no_grad()
     def push(self, frame):
         """Frame n of the stream in; restored frame n - 1 out (None for n = 0)."""
-        t = _check_frame(frame, self._hw)
+        t = _check_frame(frame, self._hw, self.size)
         if torch.is_tensor(t) and t.is_cuda and t.device != next(self.model.parameters()).device:
             raise ValueError('frame on %s, model on %s' % (t.device, next(self.model.parameters()).device))
         n = self._n
