@@ -378,6 +378,19 @@ int pgt_f32nchw_to_u8hwc(const float* x, int first, int step, int n, int H, int 
 int pgt_gather_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream);
 int pgt_scatter_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream);
 
+/* ---- full-reference scores of restored frames (metrics.cu): basicsr's calculate_psnr / calculate_ssim with
+ * crop_border 0 and test_y_channel false over the rgb frame, as the reference's test configuration scores
+ * (options/release_test_stage_IIII_dont_need_align_version.yml, val.metrics; restated in oracle/metrics_oracle.py).
+ * a_u8, b_u8: F contiguous rgb24 frame pairs [F, H, W, 3], H, W >= 11 (any size).  Per frame:
+ *   sse[f]: uint64, the exact integer sum of (a - b)^2 over all H W 3 values (PSNR = 10 log10(255^2 H W 3 / sse));
+ *   ssim[3 f + c]: fp64, channel c's SSIM map mean: 11 x 11 Gaussian window (sigma 1.5) over the valid region
+ *     [5, H - 5) x [5, W - 5), C1 = (0.01 255)^2, C2 = (0.03 255)^2; filtered fields, map and sums in fp64.
+ * ws: pgt_frame_scores_ws_doubles(F, H, W) doubles of per-tile partials, summed by a second launch in a fixed order:
+ * no floating-point atomics, so the same inputs give the same bits on every run, eager or replayed from a graph. */
+long long pgt_frame_scores_ws_doubles(int F, int H, int W);
+int pgt_frame_scores(const void* a_u8, const void* b_u8, int F, int H, int W, double* ws, uint64_t* sse, double* ssim,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif

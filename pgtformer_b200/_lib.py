@@ -102,6 +102,8 @@ SIGNATURES = {
     'pgt_f32nchw_to_u8hwc': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'pgt_gather_frames': (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
     'pgt_scatter_frames': (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
+    'pgt_frame_scores_ws_doubles': (c_int64, [c_int, c_int, c_int]),
+    'pgt_frame_scores': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     'pgt_copy2d': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     'pgt_regroup_frames': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
     'pgt_nchw_f32_to_nhwc_bf16': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,

@@ -255,6 +255,24 @@ void u8hwc_resize_to_f32nchw(const at::Tensor& x, int64_t h, int64_t w, const c1
                                     out.data_ptr<float>(), stream_of(x)), "u8hwc_resize_to_f32nchw");
 }
 
+void frame_scores(const at::Tensor& a, const at::Tensor& b, at::Tensor sse, at::Tensor ssim) {
+  TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kByte && a.is_contiguous() && a.dim() == 4 && a.size(3) == 3 &&
+              b.scalar_type() == at::kByte && b.is_contiguous() && b.sizes() == a.sizes(),
+              "frame_scores: contiguous rgb24 frames a, b [F, H, W, 3] uint8 of one shape");
+  const int64_t F = a.size(0);
+  TORCH_CHECK(sse.scalar_type() == at::kLong && sse.is_contiguous() && sse.numel() == F &&
+              ssim.scalar_type() == at::kDouble && ssim.is_contiguous() && ssim.numel() == 3 * F,
+              "frame_scores: int64 sse [F], fp64 ssim [F, 3]");
+  TORCH_CHECK(b.device() == a.device() && sse.device() == a.device() && ssim.device() == a.device(),
+              "frame_scores: every tensor on a's device");
+  c10::cuda::CUDAGuard guard(a.device());
+  const int H = (int)a.size(1), W = (int)a.size(2);
+  auto ws = at::empty({std::max<int64_t>(pgt_frame_scores_ws_doubles((int)F, H, W), 1)}, a.options().dtype(at::kDouble));
+  check(pgt_frame_scores(a.data_ptr(), b.data_ptr(), (int)F, H, W, ws.data_ptr<double>(),
+                         reinterpret_cast<uint64_t*>(sse.data_ptr<int64_t>()), ssim.data_ptr<double>(), stream_of(a)),
+        "frame_scores");
+}
+
 }  // namespace
 
 TORCH_LIBRARY(pgt, m) {
@@ -275,6 +293,7 @@ TORCH_LIBRARY(pgt, m) {
         "Tensor(c!)? zq_bf16, Tensor(d!)? min_enc, Tensor(e!)? scores, Tensor(f!)? usage) -> ()");
   m.def("adain_frames(Tensor q, Tensor style, Tensor flags, float eps, Tensor(a!) out) -> ()");
   m.def("u8hwc_resize_to_f32nchw(Tensor x, int h, int w, Tensor? sizes, Tensor(a!) out) -> ()");
+  m.def("frame_scores(Tensor a, Tensor b, Tensor(a!) sse, Tensor(b!) ssim) -> ()");
 }
 
 TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
@@ -293,4 +312,5 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("vq_stats", vq_stats);
   m.impl("adain_frames", adain_frames);
   m.impl("u8hwc_resize_to_f32nchw", u8hwc_resize_to_f32nchw);
+  m.impl("frame_scores", frame_scores);
 }

@@ -813,6 +813,14 @@ class Engine:
 
     @_on_device
     @torch.no_grad()
+    def restore_and_score(self, frames_u8, index, gt_u8, w=1.0, adain=True, reuse_frames=True, size=None):
+        """restore_windows, then the restored frames scored against gt_u8 (rgb24 [n,H,W,3] uint8 on the device) before
+        they leave it (ops.frame_scores) -> (restored, sse int64 [n], per-channel ssim fp64 [n,3])."""
+        out = self.restore_windows(frames_u8, index, w=w, adain=adain, reuse_frames=reuse_frames, size=size)
+        return (out,) + ops.frame_scores(out, gt_u8)
+
+    @_on_device
+    @torch.no_grad()
     def live_ring(self, H, W, w, streams=1):
         """The per-frame record (_frame_pass) of 4 * streams rows, for frame_step / window_step / pool_step: row
         3 s + (j mod 3) holds frame j of stream s, and rows 3 * streams + k are the staging rows pool_step's new frames

@@ -606,6 +606,26 @@ def scatter_frames(x, idx_i32, out):
     return out
 
 
+def frame_scores(a_u8, b_u8, sse=None, ssim=None):
+    """PSNR / SSIM sums of F rgb24 frame pairs a_u8, b_u8 [F,H,W,3] uint8 on the device, H, W >= 11 (pgt_frame_scores):
+    sse int64 [F], the exact sum of (a - b)^2 over all H W 3 values, and ssim fp64 [F,3], each channel's SSIM map mean
+    (basicsr's calculate_ssim with crop_border 0; oracle/metrics_oracle.py).  Deterministic, and capture-safe: the
+    workspace comes from the current allocator (a graph's own pool under capture)."""
+    lib = L.load()
+    F, H, W, C = a_u8.shape
+    assert C == 3 and a_u8.dtype == torch.uint8 and a_u8.is_contiguous() and a_u8.is_cuda
+    assert b_u8.shape == a_u8.shape and b_u8.dtype == torch.uint8 and b_u8.is_contiguous() and b_u8.device == a_u8.device
+    if sse is None:
+        sse = torch.empty(F, dtype=torch.int64, device=a_u8.device)
+    if ssim is None:
+        ssim = torch.empty(F, 3, dtype=torch.float64, device=a_u8.device)
+    assert sse.dtype == torch.int64 and sse.is_contiguous() and sse.numel() == F and sse.device == a_u8.device
+    assert ssim.dtype == torch.float64 and ssim.is_contiguous() and ssim.numel() == 3 * F and ssim.device == a_u8.device
+    ws = torch.empty(max(int(lib.pgt_frame_scores_ws_doubles(F, H, W)), 1), dtype=torch.float64, device=a_u8.device)
+    L.check(lib.pgt_frame_scores(_p(a_u8), _p(b_u8), F, H, W, _p(ws), _p(sse), _p(ssim), _stream(a_u8)))
+    return sse, ssim
+
+
 def copy2d(x, out):
     lib = L.load()
     T, C, ldx = _rows(x)

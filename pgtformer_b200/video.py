@@ -24,7 +24,7 @@ import math
 import numpy as np
 import torch
 
-from . import ops
+from . import metrics, ops
 
 
 def window_indices(n):
@@ -59,12 +59,18 @@ class VideoRestorer:
         self.cuda_graph = bool(cuda_graph)
 
     # ------------------------------------------------------------------ one batch of windows on the device
-    def _enqueue(self, frames_u8_dev, local_windows, size=None):
+    def _enqueue(self, frames_u8_dev, local_windows, size=None, gt=None):
         """frames_u8_dev: uint8 [Fd,H,W,3] on the device (distinct frames lo..hi); local_windows: [(a,b,c)] indices
         into it.  Returns uint8 [count,H,W,3] on the device (the restored middle frames; with cuda_graph, the graph's
-        static output, to be consumed before the next batch); with size, [count,*size,3]."""
+        static output, to be consumed before the next batch); with size, [count,*size,3].  With gt (their ground
+        truth, uint8 [count,*,3] on the device): (restored, sse, per-channel ssim) of Engine.restore_and_score."""
         eng = self.model.engine()
         idx = torch.tensor([j for win in local_windows for j in win], dtype=torch.int32).to(eng.dev, non_blocking=True)
+        if gt is not None:
+            kw = dict(w=self.w, adain=self.adain, reuse_frames=self.reuse_frames, size=size)
+            if self.cuda_graph:
+                return eng.graphed(eng.restore_and_score, (frames_u8_dev, idx, gt), **kw)
+            return eng.restore_and_score(frames_u8_dev, idx, gt, **kw)
         if self.cuda_graph:
             return eng.graphed(eng.restore_windows, (frames_u8_dev, idx), w=self.w, adain=self.adain,
                                reuse_frames=self.reuse_frames, size=size)
@@ -78,19 +84,41 @@ class VideoRestorer:
         return self._enqueue(d, local_windows, size).cpu().numpy()
 
     # ------------------------------------------------------------------ whole sequence in memory
-    @torch.no_grad()
     def restore(self, frames_u8, size=None):
         """frames_u8: uint8 [N,H,W,3] (numpy or torch, host).  Returns numpy uint8 [N,H,W,3] ([N,*size,3] with
         size)."""
+        return self._restore(_check_video(frames_u8), _check_size(size))
+
+    def evaluate(self, frames_u8, gt_u8, size=None):
+        """restore(frames_u8, size), scored against the ground truth gt_u8 (uint8 [N,*out_size,3], numpy or host
+        torch; out_size is size, or the frames' own size) as the reference's test configuration scores it
+        (pgtformer_b200.metrics.score).  -> (restored, {'psnr': float64 [N], 'ssim': float64 [N]}), restored exactly
+        what restore returns.  Each batch's ground truth is staged with its input frames and the restored batch is
+        scored on the device before its copy back; the scores are the same bits with cuda_graph.  Arguments are
+        checked before any device work."""
         size = _check_size(size)
-        frames = torch.as_tensor(np.ascontiguousarray(frames_u8)) if not torch.is_tensor(frames_u8) else frames_u8
-        if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3:
-            raise ValueError('expected rgb24 frames [N,H,W,3] uint8, got %s %s' % (tuple(frames.shape), frames.dtype))
+        frames = _check_video(frames_u8)
+        gt = metrics.check_frames(gt_u8, 'gt_u8')
+        shape = (frames.shape[0],) + (size or tuple(frames.shape[1:3])) + (3,)
+        if gt.is_cuda or tuple(gt.shape) != shape:
+            raise ValueError('gt_u8: expected host frames %s, got %s%s'
+                             % (shape, tuple(gt.shape), ' on %s' % gt.device if gt.is_cuda else ''))
+        out, sse, ssim = self._restore(frames, size, gt)
+        return out, metrics.finish(sse, ssim, shape[1:3])
+
+    @torch.no_grad()
+    def _restore(self, frames, size, gt=None):
+        """restore() on checked arguments; with gt (host uint8 [N,*out_size,3]): (restored, sse int64 [N], ssim
+        float64 [N,3]), each batch scored on the device (Engine.restore_and_score)."""
         n = frames.shape[0]
         shape = (n,) + (size or tuple(frames.shape[1:3])) + (3,)
         if n == 0:
-            return np.zeros(shape, np.uint8)
+            out = np.zeros(shape, np.uint8)
+            return out if gt is None else (out, np.zeros(0, np.int64), np.zeros((0, 3)))
         out = torch.empty(shape, dtype=torch.uint8).pin_memory()
+        if gt is not None:
+            sse = torch.empty(n, dtype=torch.int64).pin_memory()
+            ssim = torch.empty(n, 3, dtype=torch.float64).pin_memory()
         dev = self.model.engine().dev
         main = torch.cuda.current_stream(dev)
         copy = torch.cuda.Stream(dev)
@@ -98,38 +126,49 @@ class VideoRestorer:
         staged = None                                  # frames of the NEXT batch already on their way
         plan = plan_batches(n, self.clips_per_batch)
 
+        def pinned(t):
+            t = t.contiguous()
+            return t if t.is_pinned() else t.pin_memory()
+
         def stage(b):
             first, cnt, lo, hi = plan[b]
-            host = frames[lo:hi + 1].contiguous()
-            host = host if host.is_pinned() else host.pin_memory()
+            host = pinned(frames[lo:hi + 1])
+            host_gt = pinned(gt[first:first + cnt]) if gt is not None else None
             with torch.cuda.stream(copy):
                 d = host.to(dev, non_blocking=True)
+                gd = host_gt.to(dev, non_blocking=True) if gt is not None else None
                 ev = torch.cuda.Event()
                 ev.record(copy)
-            return d, ev, host
+            return d, gd, ev, (host, host_gt)
 
         staged = stage(0)
         copied = None
         for b, (first, cnt, lo, hi) in enumerate(plan):
-            d, ev, _keep = staged
+            d, gd, ev, _keep = staged
             staged = stage(b + 1) if b + 1 < len(plan) else None     # H2D of the next batch overlaps this compute
             main.wait_event(ev)
             if self.cuda_graph and copied is not None:
                 main.wait_event(copied)                              # a replay rewrites the static output being copied
-            res = self._enqueue(d, [tuple(j - lo for j in wins[i]) for i in range(first, first + cnt)], size)
+            res = self._enqueue(d, [tuple(j - lo for j in wins[i]) for i in range(first, first + cnt)], size, gd)
+            res, scores = (res, ()) if gd is None else (res[0], res[1:])
             done = torch.cuda.Event()
             done.record(main)
             with torch.cuda.stream(copy):                            # D2H overlaps the next batch's compute
                 copy.wait_event(done)
                 out[first:first + cnt].copy_(res, non_blocking=True)
+                for host, t in zip((sse, ssim) if scores else (), scores):
+                    host[first:first + cnt].copy_(t, non_blocking=True)
                 copied = torch.cuda.Event()
                 copied.record(copy)
             if not self.cuda_graph:
-                res.record_stream(copy)                              # the allocator keeps `res` until the copy has run
+                for t in (res,) + scores:
+                    t.record_stream(copy)                            # the allocator keeps `t` until the copy has run
             d.record_stream(main)
+            if gd is not None:
+                gd.record_stream(main)
         copy.synchronize()
         main.synchronize()
-        return out.numpy()
+        return out.numpy() if gt is None else (out.numpy(), sse.numpy(), ssim.numpy())
 
     # ------------------------------------------------------------------ iterator in, iterator out (bounded memory)
     def stream(self, frame_iter, size=None):
@@ -176,6 +215,14 @@ def _check_w(w):
     if not math.isfinite(w):
         raise ValueError('w must be finite, got %r' % (w,))
     return w
+
+
+def _check_video(frames_u8):
+    """A whole video from the caller, rgb24 [N,H,W,3] uint8 (numpy or host torch), as a torch tensor; else ValueError."""
+    frames = torch.as_tensor(np.ascontiguousarray(frames_u8)) if not torch.is_tensor(frames_u8) else frames_u8
+    if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3:
+        raise ValueError('expected rgb24 frames [N,H,W,3] uint8, got %s %s' % (tuple(frames.shape), frames.dtype))
+    return frames
 
 
 def _check_size(size):
