@@ -370,10 +370,26 @@ int pgt_nhwc_bf16_to_f32(const void* x, int ldx, int F, int HW, int C, float* y,
  *     computes it on an AVX2 / AVX512 host (the low-resolution test input, data/vfhq_full_dataset.py:1046-1051).
  *     sizes_dev NULL: every frame is h x w, packed one after another from x_u8.  Otherwise DEVICE int32 [F, 3] of
  *     each frame's (h, w, byte offset from x_u8), all >= 1 (offset >= 0); h, w then bound the table's frames and
- *     only size the profile's byte count.  pgt_u8hwc_to_f32nchw is kept for frames already at the model's size. */
+ *     only size the profile's byte count.  pgt_u8hwc_to_f32nchw is kept for frames already at the model's size.
+ *   pgt_f32nchw_resize_to_f32nchw: the same bilinear resize (align_corners=True, the same fma form) of fp32 frames
+ *     [F, 3, h, w] to [F, 3, H, W] (H, W multiples of 64; y 16-byte aligned): the second step of the test set's `lr`
+ *     degradation (data/vfhq_full_dataset.py:1017-1024), whose low-resolution frames stay fp32. */
 int pgt_u8hwc_to_f32nchw(const void* x_u8, int F, int H, int W, float* y, void* stream);
 int pgt_u8hwc_resize_to_f32nchw(const void* x_u8, int F, int h, int w, const int32_t* sizes_dev, int H, int W, float* y,
                                 void* stream);
+int pgt_f32nchw_resize_to_f32nchw(const float* x, int F, int h, int w, int H, int W, float* y, void* stream);
+
+/* ---- the `lr` degradation of the reference's test set (degrade.cu; data/vfhq_full_dataset.py:983-988): basicsr's
+ * antialiased bicubic imresize (basicsr/utils/matlab_functions.py) of F rgb24 frames [F, h, w, 3], x = (float)(v /
+ * 255.0), to fp32 [F, 3, oh, ow], the H pass first into fp32 and the W pass on it, both in one launch.  Each output
+ * of a pass is the fp32 value nearest to the exact sum of its fp32 products w x (ties to even), whatever the tiling.
+ * Tap tables (built and checked on the host by pgtformer_b200/degrade.py, the only builder): DEVICE fp32 weights
+ * wts [out, K] and int32 indices idx [out, K], already mirrored into [0, in); each row's indices span at most
+ * K + 1 consecutive source samples before mirroring, and consecutive rows advance by at most K / 4, which sizes the
+ * shared-memory footprint.  Outputs are not clamped: bicubic overshoot below 0 and above 1 is kept. */
+int pgt_imresize_u8hwc_to_f32nchw(const void* x_u8, int F, int h, int w, const float* wts_h, const int32_t* idx_h,
+                                  int Kh, int oh, const float* wts_w, const int32_t* idx_w, int Kw, int ow, float* y,
+                                  void* stream);
 int pgt_f32nchw_to_u8hwc(const float* x, int first, int step, int n, int H, int W, void* y_u8, void* stream);
 int pgt_gather_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream);
 int pgt_scatter_frames(const void* x, long long frame_bytes, const int* idx_dev, int n, void* y, void* stream);

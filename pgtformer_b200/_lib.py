@@ -99,6 +99,9 @@ SIGNATURES = {
     'pgt_u8hwc_to_f32nchw': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'pgt_u8hwc_resize_to_f32nchw': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p,
                                             c_void_p]),
+    'pgt_f32nchw_resize_to_f32nchw': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    'pgt_imresize_u8hwc_to_f32nchw': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                                              c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     'pgt_f32nchw_to_u8hwc': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'pgt_gather_frames': (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),
     'pgt_scatter_frames': (c_int, [c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p]),

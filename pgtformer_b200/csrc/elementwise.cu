@@ -224,38 +224,68 @@ __device__ __forceinline__ LerpAxis lerp_axis(int in, int out, int o) {
   return a;
 }
 
+// The source of a resize: frame f's size and (c, y, x) sample as the fp32 value the interpolation reads.
+//   U8Frames: rgb24 frames, (float)(v / 255.0) through the CTA's table `unit`; every frame h x w packed one after
+//     another, or each frame's (h, w, byte offset) from a device int32 table.
+//   F32Planes: fp32 frames [F, 3, h, w] (the output of pgt_imresize_u8hwc_to_f32nchw); `unit` is not read.
+struct U8Frames {
+  static constexpr bool kUnit = true;
+  const uint8_t* x;
+  int h, w;
+  const int* sizes;
+  struct Frame {
+    const uint8_t* p;
+    int h, w;
+  };
+  __device__ __forceinline__ Frame frame(int f) const {
+    if (sizes == nullptr) return {x + (size_t)f * h * w * 3, h, w};
+    return {x + (size_t)(unsigned)__ldg(sizes + 3 * f + 2), __ldg(sizes + 3 * f), __ldg(sizes + 3 * f + 1)};
+  }
+  __device__ __forceinline__ float at(const Frame& fr, const float* unit, int c, int y, int xx) const {
+    return unit[fr.p[((size_t)y * fr.w + xx) * 3 + c]];
+  }
+};
+
+struct F32Planes {
+  static constexpr bool kUnit = false;
+  const float* x;
+  int h, w;
+  struct Frame {
+    const float* p;
+    int h, w;
+  };
+  __device__ __forceinline__ Frame frame(int f) const { return {x + (size_t)f * 3 * h * w, h, w}; }
+  __device__ __forceinline__ float at(const Frame& fr, const float*, int c, int y, int xx) const {
+    return __ldg(fr.p + ((size_t)c * fr.h + y) * fr.w + xx);
+  }
+};
+
 // Each thread writes four consecutive pixels of one output row (W % 4 == 0), all three planes, as float4 stores.
 // The combination is the one torch's AVX2 / AVX512 kernel evaluates, fma(h0, fma(w0, a, w1 b), h1 fma(w0, c, w1 d)),
 // spelled with explicit intrinsics so that no contraction choice of the compiler changes a bit.
-__global__ void u8hwc_resize_kernel(const uint8_t* __restrict__ x, int h, int w, const int* __restrict__ sizes, int H,
-                                    int W, size_t total, float* __restrict__ y) {
-  __shared__ float unit[256];
-  for (int v = threadIdx.x; v < 256; v += blockDim.x) unit[v] = __double2float_rn(__ddiv_rn((double)v, 255.0));
-  __syncthreads();
+template <class Src>
+__global__ void resize_kernel(Src src, int H, int W, size_t total, float* __restrict__ y) {
+  __shared__ float unit[Src::kUnit ? 256 : 1];
+  if (Src::kUnit) {
+    for (int v = threadIdx.x; v < 256; v += blockDim.x) unit[v] = __double2float_rn(__ddiv_rn((double)v, 255.0));
+    __syncthreads();
+  }
   const int qw = W >> 2;
   const size_t HW = (size_t)H * W;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const size_t row = i / qw;
     const int ox = (int)(i - row * qw) << 2;
     const int f = (int)(row / H), oy = (int)(row - (size_t)f * H);
-    int fh = h, fw = w;
-    size_t off = (size_t)f * h * w * 3;
-    if (sizes != nullptr) {
-      fh = __ldg(sizes + 3 * f);
-      fw = __ldg(sizes + 3 * f + 1);
-      off = (size_t)(unsigned)__ldg(sizes + 3 * f + 2);
-    }
-    const LerpAxis ay = lerp_axis(fh, H, oy);
-    const uint8_t* r0 = x + off + (size_t)ay.i0 * fw * 3;
-    const uint8_t* r1 = x + off + (size_t)ay.i1 * fw * 3;
+    const typename Src::Frame fr = src.frame(f);
+    const LerpAxis ay = lerp_axis(fr.h, H, oy);
     float o[3][4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const LerpAxis ax = lerp_axis(fw, W, ox + k);
+      const LerpAxis ax = lerp_axis(fr.w, W, ox + k);
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        const float a = unit[r0[ax.i0 * 3 + c]], b = unit[r0[ax.i1 * 3 + c]];
-        const float cc = unit[r1[ax.i0 * 3 + c]], d = unit[r1[ax.i1 * 3 + c]];
+        const float a = src.at(fr, unit, c, ay.i0, ax.i0), b = src.at(fr, unit, c, ay.i0, ax.i1);
+        const float cc = src.at(fr, unit, c, ay.i1, ax.i0), d = src.at(fr, unit, c, ay.i1, ax.i1);
         const float top = __fmaf_rn(ax.l0, a, __fmul_rn(ax.l1, b));
         const float bot = __fmaf_rn(ax.l0, cc, __fmul_rn(ax.l1, d));
         o[c][k] = __fmaf_rn(ay.l0, top, __fmul_rn(ay.l1, bot));
@@ -292,8 +322,21 @@ extern "C" int pgt_u8hwc_resize_to_f32nchw(const void* x_u8, int F, int h, int w
   const size_t total = (size_t)F * H * (W / 4);
   ProfScope ps(PGT_PROF_MOVE, 12.0 * F * (double)H * W + 3.0 * F * (double)h * w, static_cast<cudaStream_t>(stream),
                "pgt_u8hwc_resize_to_f32nchw");
-  pgt::u8hwc_resize_kernel<<<ew_grid(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint8_t*>(x_u8), h, w, sizes_dev, H, W, total, y);
+  pgt::resize_kernel<<<ew_grid(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      pgt::U8Frames{static_cast<const uint8_t*>(x_u8), h, w, sizes_dev}, H, W, total, y);
+  PGT_LAUNCH_OK();
+  return PGT_OK;
+}
+
+extern "C" int pgt_f32nchw_resize_to_f32nchw(const float* x, int F, int h, int w, int H, int W, float* y,
+                                             void* stream) {
+  PGT_CHECK_ARG(x && y && F > 0 && h > 0 && w > 0 && H > 0 && W > 0 && H % 64 == 0 && W % 64 == 0);
+  PGT_CHECK_ARG((reinterpret_cast<uintptr_t>(y) & 15) == 0);
+  const size_t total = (size_t)F * H * (W / 4);
+  ProfScope ps(PGT_PROF_MOVE, 12.0 * F * (double)H * W + 12.0 * F * (double)h * w, static_cast<cudaStream_t>(stream),
+               "pgt_f32nchw_resize_to_f32nchw");
+  pgt::resize_kernel<<<ew_grid(total, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      pgt::F32Planes{x, h, w}, H, W, total, y);
   PGT_LAUNCH_OK();
   return PGT_OK;
 }

@@ -255,6 +255,39 @@ void u8hwc_resize_to_f32nchw(const at::Tensor& x, int64_t h, int64_t w, const c1
                                     out.data_ptr<float>(), stream_of(x)), "u8hwc_resize_to_f32nchw");
 }
 
+void f32nchw_resize_to_f32nchw(const at::Tensor& x, at::Tensor out) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kFloat && x.is_contiguous() && x.dim() == 4 && x.size(1) == 3 &&
+              out.scalar_type() == at::kFloat && out.is_contiguous() && out.dim() == 4 && out.size(1) == 3 &&
+              out.size(0) == x.size(0), "f32nchw_resize_to_f32nchw: contiguous fp32 x [F, 3, h, w], out [F, 3, H, W]");
+  TORCH_CHECK(out.device() == x.device(), "f32nchw_resize_to_f32nchw: x and out on one device");
+  c10::cuda::CUDAGuard guard(x.device());
+  check(pgt_f32nchw_resize_to_f32nchw(x.data_ptr<float>(), (int)x.size(0), (int)x.size(2), (int)x.size(3),
+                                      (int)out.size(2), (int)out.size(3), out.data_ptr<float>(), stream_of(x)),
+        "f32nchw_resize_to_f32nchw");
+}
+
+void imresize_u8hwc_to_f32nchw(const at::Tensor& x, const at::Tensor& wts_h, const at::Tensor& idx_h,
+                               const at::Tensor& wts_w, const at::Tensor& idx_w, at::Tensor out) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kByte && x.is_contiguous() && x.dim() == 4 && x.size(3) == 3 &&
+              out.scalar_type() == at::kFloat && out.is_contiguous() && out.dim() == 4 && out.size(1) == 3 &&
+              out.size(0) == x.size(0), "imresize_u8hwc_to_f32nchw: contiguous rgb24 x [F, h, w, 3], fp32 out "
+              "[F, 3, oh, ow]");
+  for (const at::Tensor* t : {&wts_h, &idx_h, &wts_w, &idx_w})
+    TORCH_CHECK(t->is_contiguous() && t->dim() == 2 && t->device() == x.device(),
+                "imresize_u8hwc_to_f32nchw: contiguous [out, K] tap tables on x's device");
+  TORCH_CHECK(wts_h.scalar_type() == at::kFloat && wts_w.scalar_type() == at::kFloat &&
+              idx_h.scalar_type() == at::kInt && idx_w.scalar_type() == at::kInt && wts_h.sizes() == idx_h.sizes() &&
+              wts_w.sizes() == idx_w.sizes() && wts_h.size(0) == out.size(2) && wts_w.size(0) == out.size(3),
+              "imresize_u8hwc_to_f32nchw: fp32 weights and int32 indices [oh, Kh], [ow, Kw]");
+  TORCH_CHECK(out.device() == x.device(), "imresize_u8hwc_to_f32nchw: x and out on one device");
+  c10::cuda::CUDAGuard guard(x.device());
+  check(pgt_imresize_u8hwc_to_f32nchw(x.data_ptr(), (int)x.size(0), (int)x.size(1), (int)x.size(2),
+                                      wts_h.data_ptr<float>(), idx_h.data_ptr<int32_t>(), (int)wts_h.size(1),
+                                      (int)out.size(2), wts_w.data_ptr<float>(), idx_w.data_ptr<int32_t>(),
+                                      (int)wts_w.size(1), (int)out.size(3), out.data_ptr<float>(), stream_of(x)),
+        "imresize_u8hwc_to_f32nchw");
+}
+
 void frame_scores(const at::Tensor& a, const at::Tensor& b, at::Tensor sse, at::Tensor ssim) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kByte && a.is_contiguous() && a.dim() == 4 && a.size(3) == 3 &&
               b.scalar_type() == at::kByte && b.is_contiguous() && b.sizes() == a.sizes(),
@@ -294,6 +327,9 @@ TORCH_LIBRARY(pgt, m) {
   m.def("adain_frames(Tensor q, Tensor style, Tensor flags, float eps, Tensor(a!) out) -> ()");
   m.def("u8hwc_resize_to_f32nchw(Tensor x, int h, int w, Tensor? sizes, Tensor(a!) out) -> ()");
   m.def("frame_scores(Tensor a, Tensor b, Tensor(a!) sse, Tensor(b!) ssim) -> ()");
+  m.def("f32nchw_resize_to_f32nchw(Tensor x, Tensor(a!) out) -> ()");
+  m.def("imresize_u8hwc_to_f32nchw(Tensor x, Tensor wts_h, Tensor idx_h, Tensor wts_w, Tensor idx_w, Tensor(a!) out) "
+        "-> ()");
 }
 
 TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
@@ -313,4 +349,6 @@ TORCH_LIBRARY_IMPL(pgt, CUDA, m) {
   m.impl("adain_frames", adain_frames);
   m.impl("u8hwc_resize_to_f32nchw", u8hwc_resize_to_f32nchw);
   m.impl("frame_scores", frame_scores);
+  m.impl("f32nchw_resize_to_f32nchw", f32nchw_resize_to_f32nchw);
+  m.impl("imresize_u8hwc_to_f32nchw", imresize_u8hwc_to_f32nchw);
 }

@@ -14,7 +14,7 @@ into the C ABI; there is no PyTorch / cuDNN / CPU fallback: without the CUDA lib
 import torch
 import torch.nn.functional as F  # noqa: F401  (load-time weight padding only)
 
-from . import ops
+from . import degrade, ops
 from .spec import Arch
 from .swin3d import pack_blocks
 
@@ -791,13 +791,20 @@ class Engine:
     # ------------------------------------------------------------------ video: batched windows and the live ring
     @_on_device
     @torch.no_grad()
-    def restore_windows(self, frames_u8, index, w=1.0, adain=True, reuse_frames=True, size=None):
+    def restore_windows(self, frames_u8, index, w=1.0, adain=True, reuse_frames=True, size=None, downscale=None):
         """One batch of VideoRestorer: rgb24 frames [Fd,H,W,3] uint8 on the device and the device int32 window index
         [3n] into them -> the restored middle frames, rgb24 [n,H,W,3] uint8 on the device.  size = (H, W): the frames
         are [Fd,h,w,3] sources of any size, upsampled to H x W as the reference's test set does
-        (ops.u8hwc_resize_to_f32nchw)."""
+        (ops.u8hwc_resize_to_f32nchw).  downscale (with size): the frames are ground truth, degraded as the test set's
+        `lr` protocol does, basicsr's imresize by that scale into fp32 (degrade.resize), then bilinear to H x W
+        (ops.f32nchw_resize_to_f32nchw); the caller has checked the scale against the frames (degrade.plan)."""
         Fd, h, w_src, _ = frames_u8.shape
-        if size is None:
+        if downscale is not None:
+            H, W = size
+            lo = degrade.resize(frames_u8, downscale, self._new(Fd, 3, *degrade.out_size((h, w_src), downscale),
+                                                                dtype=torch.float32))
+            x = ops.f32nchw_resize_to_f32nchw(lo, self._new(Fd, 3, H, W, dtype=torch.float32))
+        elif size is None:
             H, W = h, w_src
             x = ops.u8hwc_to_f32nchw(frames_u8, self._new(Fd, 3, H, W, dtype=torch.float32))
         else:
@@ -813,10 +820,12 @@ class Engine:
 
     @_on_device
     @torch.no_grad()
-    def restore_and_score(self, frames_u8, index, gt_u8, w=1.0, adain=True, reuse_frames=True, size=None):
+    def restore_and_score(self, frames_u8, index, gt_u8, w=1.0, adain=True, reuse_frames=True, size=None,
+                          downscale=None):
         """restore_windows, then the restored frames scored against gt_u8 (rgb24 [n,H,W,3] uint8 on the device) before
         they leave it (ops.frame_scores) -> (restored, sse int64 [n], per-channel ssim fp64 [n,3])."""
-        out = self.restore_windows(frames_u8, index, w=w, adain=adain, reuse_frames=reuse_frames, size=size)
+        out = self.restore_windows(frames_u8, index, w=w, adain=adain, reuse_frames=reuse_frames, size=size,
+                                   downscale=downscale)
         return (out,) + ops.frame_scores(out, gt_u8)
 
     @_on_device

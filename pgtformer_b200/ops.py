@@ -576,6 +576,35 @@ def u8hwc_resize_to_f32nchw(x_u8, out, hw, sizes=None):
     return out
 
 
+def f32nchw_resize_to_f32nchw(x, out):
+    """fp32 frames x [F,3,h,w] -> fp32 out [F,3,H,W] (H, W multiples of 64): bilinear with align_corners=True in the
+    fma form of u8hwc_resize_to_f32nchw, the second step of the test set's `lr` degradation
+    (data/vfhq_full_dataset.py:1017-1024)."""
+    lib = L.load()
+    F, C, h, w = x.shape
+    assert C == 3 and x.dtype == torch.float32 and x.is_contiguous() and x.is_cuda
+    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape[:2]) == (F, 3) and \
+        out.device == x.device
+    L.check(lib.pgt_f32nchw_resize_to_f32nchw(_p(x), F, h, w, out.shape[2], out.shape[3], _p(out), _stream()))
+    return out
+
+
+def imresize_u8hwc_to_f32nchw(x_u8, taps_h, taps_w, out):
+    """rgb24 frames x_u8 [F,h,w,3] on the device -> fp32 out [F,3,oh,ow]: basicsr's antialiased bicubic imresize of
+    (float)(v / 255.0), each pass rounded once from its exact sum (pgt_imresize_u8hwc_to_f32nchw).  taps_h, taps_w:
+    (weights fp32, indices int32), each [out, K] on the device, as pgtformer_b200.degrade builds them."""
+    lib = L.load()
+    F, h, w, C = x_u8.shape
+    (wh, ih), (ww, iw) = taps_h, taps_w
+    assert C == 3 and x_u8.dtype == torch.uint8 and x_u8.is_contiguous() and x_u8.is_cuda
+    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (F, 3, wh.shape[0], ww.shape[0])
+    for t, dt in ((wh, torch.float32), (ih, torch.int32), (ww, torch.float32), (iw, torch.int32)):
+        assert t.dtype == dt and t.dim() == 2 and t.is_contiguous() and t.device == x_u8.device
+    L.check(lib.pgt_imresize_u8hwc_to_f32nchw(_p(x_u8), F, h, w, _p(wh), _p(ih), wh.shape[1], wh.shape[0], _p(ww),
+                                              _p(iw), ww.shape[1], ww.shape[0], _p(out), _stream()))
+    return out
+
+
 def f32nchw_to_u8hwc(x, out_u8, first=0, step=1):
     """uint8(clamp(x, 0, 1) * 255) of frames first, first+step, ... -> rgb24 [n,H,W,3] (inference.py:15-19)."""
     lib = L.load()

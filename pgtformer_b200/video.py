@@ -24,7 +24,7 @@ import math
 import numpy as np
 import torch
 
-from . import metrics, ops
+from . import degrade, metrics, ops
 
 
 def window_indices(n):
@@ -46,7 +46,13 @@ class VideoRestorer:
     """restore() and stream() take size = (H, W), multiples of 64: frames of any size are then restored at H x W, each
     upsampled on the device as the reference's test set feeds its low-resolution frames to the model (bilinear,
     align_corners=True; ops.u8hwc_resize_to_f32nchw); the pinned host buffers and the host-to-device copies carry the
-    source frames, and outputs are rgb24 at H x W.  size is checked when the call is made, before any device work."""
+    source frames, and outputs are rgb24 at H x W.  size is checked when the call is made, before any device work.
+
+    restore(), evaluate() and stream() take downscale = s, 0 < s < 1: the frames are then ground truth, degraded on the
+    device as the reference's test set builds its `lr` input (basicsr's antialiased bicubic imresize by s of v / 255.0,
+    kept fp32 and unclamped, then bilinear to H x W; pgtformer_b200.degrade), and restored at size, or at the frames'
+    own size (multiples of 64) when size is None.  Only the ground-truth bytes cross to the device.  The `lr` protocol
+    on 512^2 ground truth is VideoRestorer(model).evaluate(gt, gt, downscale=0.25)."""
 
     def __init__(self, model, w=1.0, adain=True, clips_per_batch=16, reuse_frames=True, cuda_graph=False):
         """cuda_graph: replay each batch from a CUDA graph (Engine.graphed, one per batch shape), which removes the
@@ -59,55 +65,59 @@ class VideoRestorer:
         self.cuda_graph = bool(cuda_graph)
 
     # ------------------------------------------------------------------ one batch of windows on the device
-    def _enqueue(self, frames_u8_dev, local_windows, size=None, gt=None):
+    def _enqueue(self, frames_u8_dev, local_windows, size=None, gt=None, downscale=None):
         """frames_u8_dev: uint8 [Fd,H,W,3] on the device (distinct frames lo..hi); local_windows: [(a,b,c)] indices
         into it.  Returns uint8 [count,H,W,3] on the device (the restored middle frames; with cuda_graph, the graph's
         static output, to be consumed before the next batch); with size, [count,*size,3].  With gt (their ground
-        truth, uint8 [count,*,3] on the device): (restored, sse, per-channel ssim) of Engine.restore_and_score."""
+        truth, uint8 [count,*,3] on the device): (restored, sse, per-channel ssim) of Engine.restore_and_score.
+        downscale (with size): the frames are ground truth, degraded as the `lr` protocol does."""
         eng = self.model.engine()
         idx = torch.tensor([j for win in local_windows for j in win], dtype=torch.int32).to(eng.dev, non_blocking=True)
+        kw = dict(w=self.w, adain=self.adain, reuse_frames=self.reuse_frames, size=size)
+        if downscale is not None:
+            kw['downscale'] = downscale
         if gt is not None:
-            kw = dict(w=self.w, adain=self.adain, reuse_frames=self.reuse_frames, size=size)
             if self.cuda_graph:
                 return eng.graphed(eng.restore_and_score, (frames_u8_dev, idx, gt), **kw)
             return eng.restore_and_score(frames_u8_dev, idx, gt, **kw)
         if self.cuda_graph:
-            return eng.graphed(eng.restore_windows, (frames_u8_dev, idx), w=self.w, adain=self.adain,
-                               reuse_frames=self.reuse_frames, size=size)
-        return eng.restore_windows(frames_u8_dev, idx, w=self.w, adain=self.adain, reuse_frames=self.reuse_frames,
-                                   size=size)
+            return eng.graphed(eng.restore_windows, (frames_u8_dev, idx), **kw)
+        return eng.restore_windows(frames_u8_dev, idx, **kw)
 
-    def _run_batch(self, frames_u8, local_windows, size=None):
+    def _run_batch(self, frames_u8, local_windows, size=None, downscale=None):
         """Host uint8 [Fd,H,W,3] + window index triples -> host uint8 [count,H,W,3] (synchronous; `stream()` uses it)."""
         dev = self.model.engine().dev
         d = torch.from_numpy(np.ascontiguousarray(frames_u8)).pin_memory().to(dev, non_blocking=True)
-        return self._enqueue(d, local_windows, size).cpu().numpy()
+        return self._enqueue(d, local_windows, size, downscale=downscale).cpu().numpy()
 
     # ------------------------------------------------------------------ whole sequence in memory
-    def restore(self, frames_u8, size=None):
+    def restore(self, frames_u8, size=None, downscale=None):
         """frames_u8: uint8 [N,H,W,3] (numpy or torch, host).  Returns numpy uint8 [N,H,W,3] ([N,*size,3] with
-        size)."""
-        return self._restore(_check_video(frames_u8), _check_size(size))
+        size).  downscale: the frames are ground truth, degraded by the `lr` protocol first (class docstring)."""
+        frames = _check_video(frames_u8)
+        size, downscale = _check_downscale(downscale, frames.shape[1:3], _check_size(size))
+        return self._restore(frames, size, downscale=downscale)
 
-    def evaluate(self, frames_u8, gt_u8, size=None):
+    def evaluate(self, frames_u8, gt_u8, size=None, downscale=None):
         """restore(frames_u8, size), scored against the ground truth gt_u8 (uint8 [N,*out_size,3], numpy or host
         torch; out_size is size, or the frames' own size) as the reference's test configuration scores it
         (pgtformer_b200.metrics.score).  -> (restored, {'psnr': float64 [N], 'ssim': float64 [N]}), restored exactly
         what restore returns.  Each batch's ground truth is staged with its input frames and the restored batch is
         scored on the device before its copy back; the scores are the same bits with cuda_graph.  Arguments are
-        checked before any device work."""
-        size = _check_size(size)
+        checked before any device work.  downscale: frames_u8 is ground truth, degraded by the `lr` protocol first
+        (class docstring), so evaluate(gt, gt, downscale=0.25) is that protocol end to end."""
         frames = _check_video(frames_u8)
+        size, downscale = _check_downscale(downscale, frames.shape[1:3], _check_size(size))
         gt = metrics.check_frames(gt_u8, 'gt_u8')
         shape = (frames.shape[0],) + (size or tuple(frames.shape[1:3])) + (3,)
         if gt.is_cuda or tuple(gt.shape) != shape:
             raise ValueError('gt_u8: expected host frames %s, got %s%s'
                              % (shape, tuple(gt.shape), ' on %s' % gt.device if gt.is_cuda else ''))
-        out, sse, ssim = self._restore(frames, size, gt)
+        out, sse, ssim = self._restore(frames, size, gt, downscale)
         return out, metrics.finish(sse, ssim, shape[1:3])
 
     @torch.no_grad()
-    def _restore(self, frames, size, gt=None):
+    def _restore(self, frames, size, gt=None, downscale=None):
         """restore() on checked arguments; with gt (host uint8 [N,*out_size,3]): (restored, sse int64 [N], ssim
         float64 [N,3]), each batch scored on the device (Engine.restore_and_score)."""
         n = frames.shape[0]
@@ -149,7 +159,8 @@ class VideoRestorer:
             main.wait_event(ev)
             if self.cuda_graph and copied is not None:
                 main.wait_event(copied)                              # a replay rewrites the static output being copied
-            res = self._enqueue(d, [tuple(j - lo for j in wins[i]) for i in range(first, first + cnt)], size, gd)
+            res = self._enqueue(d, [tuple(j - lo for j in wins[i]) for i in range(first, first + cnt)], size, gd,
+                                downscale)
             res, scores = (res, ()) if gd is None else (res[0], res[1:])
             done = torch.cuda.Event()
             done.record(main)
@@ -171,14 +182,27 @@ class VideoRestorer:
         return out.numpy() if gt is None else (out.numpy(), sse.numpy(), ssim.numpy())
 
     # ------------------------------------------------------------------ iterator in, iterator out (bounded memory)
-    def stream(self, frame_iter, size=None):
+    def stream(self, frame_iter, size=None, downscale=None):
         """Yields restored rgb24 frames for an iterator of rgb24 frames [H,W,3] uint8, `clips_per_batch` windows per
-        launch; the last frame of a batch needs its successor, so output lags the input by one batch."""
-        return self._stream(frame_iter, _check_size(size))
+        launch; the last frame of a batch needs its successor, so output lags the input by one batch.  downscale: the
+        frames are ground truth, degraded by the `lr` protocol first (class docstring); the scale is checked now and
+        against the first frame's size before it reaches the device."""
+        size = _check_size(size)
+        if downscale is not None:
+            downscale = degrade.check_scale(downscale)
+        return self._stream(frame_iter, size, downscale)
 
     @torch.no_grad()
-    def _stream(self, frame_iter, size):
-        run_batch = self._run_batch if size is None else lambda f, wins: self._run_batch(f, wins, size)
+    def _stream(self, frame_iter, size, downscale=None):
+        if downscale is None:
+            run_batch = self._run_batch if size is None else lambda f, wins: self._run_batch(f, wins, size)
+        else:
+            checked = []                                  # the model size, once the first frame has been seen
+
+            def run_batch(f, wins):
+                if not checked:
+                    checked.append(_check_downscale(downscale, f.shape[1:3], size)[0])
+                return self._run_batch(f, wins, checked[0], downscale)
         buf, base, total_in, emitted = [], 0, 0, 0       # buf[k] is frame base + k
         it = iter(frame_iter)
         ended = False
@@ -223,6 +247,17 @@ def _check_video(frames_u8):
     if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3:
         raise ValueError('expected rgb24 frames [N,H,W,3] uint8, got %s %s' % (tuple(frames.shape), frames.dtype))
     return frames
+
+
+def _check_downscale(downscale, hw, size):
+    """(model size, scale) for frames of hw = (h, w) degraded by `downscale`: the scale checked against the frames
+    (degrade.plan) and the size (already checked) or, when None, the frames' own size, which must be multiples of
+    64.  downscale None: (size, None).  Anything else raises ValueError."""
+    if downscale is None:
+        return size, None
+    hw = (int(hw[0]), int(hw[1]))
+    degrade.plan(hw, downscale)
+    return _check_size(size or hw), degrade.check_scale(downscale)
 
 
 def _check_size(size):
